@@ -10,7 +10,8 @@ five MSMs (A, B-in-G1, B-in-G2, H, L) plus the O(1) final assembly, through the 
       are sharded by index range over the ranks (SURVEY.md section 8e), 5 partial points per rank are all-gathered over NCCL,
       every rank assembles the same proof.  Strong scaling: the proof size is fixed as N grows.
 
-Output: ONE JSON line on rank 0 (contract in the task statement) with `roofline`, `cpu_baseline`, `e2e`, `clocks`.
+Output: ONE JSON line on rank 0 with `roofline`, `cpu_baseline`, `e2e`, `clocks`.  `--dump-outputs DIR` also writes the
+proof of the last timed step as DIR/proof_{a,b,c}.npy, so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -24,6 +25,7 @@ import time
 import numpy as np
 
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")   # before CUDA is initialised: see groth16_b200/__init__.py
+sys.dont_write_bytecode = True   # the benchmark may run from a read-only tree: it writes nothing there
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
@@ -59,7 +61,9 @@ def parse():
                          "and additionally measures the replicas, reported under the secondary key \"replicas\"")
     ap.add_argument("--check-oracle", action="store_true",
                     help="N > 1: rank 0 also proves once with the CPU oracle and compares bit for bit (N = 1 always does, as its cpu_baseline)")
-    ap.add_argument("--record", default="", help="also append the JSON line to this file (profiles/r02_bench_*.json)")
+    ap.add_argument("--record", default="", help="also append the JSON line to this file")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the proof of the last timed step to DIR/proof_{a,b,c}.npy (float64 values of its 32-bit limbs)")
     return ap.parse_args()
 
 
@@ -72,13 +76,12 @@ def workload_name(a):
 
 # ------------------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe).
+    """nvidia-smi clocks / throttle reasons during the timed region.
 
     The nvidia-smi process is started BEFORE the warm-up steps: its start-up (process spawn, NVML attaching to every GPU of
     the box) takes driver-wide locks for hundreds of milliseconds, which inside a 0.3 s timed region of an 8-GPU sharded
-    run stalled kernel launches on all ranks (profiles/r02_bench_h_bls12_381_20_n8.json: `value` 77 proofs/s under the
-    sampler against 137 for the unsampled host-input run of the same process).  Every sample is stamped on arrival and only
-    those that fall between mark_begin() and mark_end() are reported."""
+    run stalled kernel launches on all ranks.  Every sample is stamped on arrival and only those that fall between
+    mark_begin() and mark_end() are reported."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -172,7 +175,7 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured)"
         except Exception:
             pass
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet 3.35 TB/s (not measured)"
 
 
 def ncu_summary():
@@ -291,6 +294,16 @@ def emit(a, line):
             f.write(out + "\n")
 
 
+def dump_proof(out_dir, proof, nq):
+    """The proof buffer as g16_prove returns it (A, B, C as affine Montgomery limbs), split into its 32-bit halves so that
+    float64 holds every value exactly."""
+    os.makedirs(out_dir, exist_ok=True)
+    limbs = proof.view(np.uint32).astype(np.float64)
+    parts = {"proof_a": limbs[:4 * nq], "proof_b": limbs[4 * nq:12 * nq], "proof_c": limbs[12 * nq:]}
+    for name, arr in parts.items():
+        np.save(os.path.join(out_dir, name + ".npy"), arr)
+
+
 # ------------------------------------------------------------------------------------------------------------------
 def kernel_rev():
     """hash of the kernel sources a committed ncu capture must have been taken with to describe the running code"""
@@ -331,10 +344,12 @@ def run_cuda(a):
     key_bytes = nvars * 8 * nq * (4 * 2 + 4)              # a, b_g1, h, l (G1) + b_g2, packed affine, one copy
     mem_total = torch.cuda.get_device_properties(dev).total_memory
     share = world if want_shard else 1
+    # the key may take 35 % of device memory: at 2^24 constraints the plain MSM pipelines of one proof (sorted arrays, level-0
+    # partial sums; ~24 GB), the setup's export buffers, the circuit and the NTT tables need the rest of an 80 GB H100
     ne = 1
-    while ne < 16 and key_bytes * ((16 + ne - 1) // ne) / share > 0.5 * mem_total:
+    while ne < 16 and key_bytes * ((16 + ne - 1) // ne) / share > 0.35 * mem_total:
         ne *= 2
-    big = key_bytes * 16 > 0.5 * mem_total                # the unsharded key with all copies does not fit one GPU
+    big = key_bytes * 16 > 0.35 * mem_total               # the unsharded key with all copies does not fit one GPU
     if os.environ.get("G16_BENCH_FORCE_BIG"):              # exercise the large-key path (mint without copies, re-load) at any size
         big = True
     residency = {"key_bytes_one_copy": int(key_bytes), "msm_ne": ne, "copies": (16 + ne - 1) // ne,
@@ -448,12 +463,13 @@ def run_cuda(a):
             self.run_steps(z_dev.data_ptr(), ON_DEV, max(a.warmup, 3))
             first = self.step(z_dev.data_ptr(), ON_DEV).copy()
             dt, dev_ms, launches, clocks = self.timed(z_dev.data_ptr(), ON_DEV, a.steps, sampler)
+            last = proof.copy()   # what the last timed step returned
             lat = self.latency(z_dev.data_ptr(), ON_DEV)
             self.run_steps(z_pinned.data_ptr(), 0, 2)
             assert np.array_equal(first, proof), "resident-input and host-input proofs differ"
             dt_e, _, _, _ = self.timed(z_pinned.data_ptr(), 0, a.steps)
             tm_e = g.timings()
-            return {"proof": first, "value": units * a.steps / dt, "ms_per_step": 1e3 * dt / a.steps,
+            return {"proof": first, "last": last, "value": units * a.steps / dt, "ms_per_step": 1e3 * dt / a.steps,
                     "device_ms_per_step": statistics.mean(dev_ms), "latency_ms_single_proof": lat, "launches": int(launches),
                     "clocks": clocks, "inflight": self.inflight,
                     "e2e": {"value": units * a.steps / dt_e, "unit": "proofs/s", "h2d_bytes_per_step": int(tm_e["h2d_bytes"]),
@@ -462,8 +478,7 @@ def run_cuda(a):
     sampler = ClockSampler(local) if rank == 0 else None
     secondary = None
     # Two proofs in flight (software pipeline over the two proof slots of a context) up to 2^20: the next proof's sort and
-    # first rounds fill the latency-bound tail of the previous one (bucket reduction, host finish) -- +3.7 % on one GPU
-    # (gpurun_out/bench_r02p_*.json: 35.8 vs 34.5 proofs/s), more on the small per-rank shards.  Larger circuits keep one proof
+    # first rounds fill the latency-bound tail of the previous one (bucket reduction, host finish).  Larger circuits keep one proof
     # in flight: the second slot's work lists would compete with the precomputed multiples for HBM.
     auto_inflight = 1 if (big or a.log_n > 20) else 2
     if want_shard:
@@ -520,7 +535,7 @@ def run_cuda(a):
             mul = 2 * nl * nl                    # IMAD.WIDE per Montgomery product (288 for 12 limbs, 128 for 8)
             per_entry = cfg["imad_per_g1_entry_mul"] * mul
             e_g1 = sum(entries[k] for k in g1k)
-            sm_clk = (main["clocks"] or {}).get("sm_mhz") or 1965.0
+            sm_clk = (main["clocks"] or {}).get("sm_mhz") or 1980.0   # H100 SXM maximum SM clock when nvidia-smi gives none
             pipe_peak = torch.cuda.get_device_properties(dev).multi_processor_count * INT_PIPE_LANES_PER_CLK_SM * sm_clk * 1e6
             imad_rate = e_g1 * per_entry / (t_g1 * 1e-3) if t_g1 > 0 else 0.0
             roof = {"kernel": cfg["g1_accum_stage"], "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s",
@@ -591,6 +606,8 @@ def run_cuda(a):
             line["kernels"] = kern
         if cpu:
             line["cpu_baseline"] = cpu
+        if a.dump_outputs:
+            dump_proof(a.dump_outputs, main["last"], nq)
         emit(a, line)
     if world > 1:
         dist.barrier()

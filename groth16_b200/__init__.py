@@ -1,4 +1,4 @@
-"""groth16_b200 -- B200-native (sm_100a) Groth16 proving hot path: NTT witness map + five MSMs behind the
+"""groth16_b200 -- H100-native (sm_90a) Groth16 proving hot path: NTT witness map + five MSMs behind the
 ark-groth16 `create_proof_with_reduction_and_matrices` interface.  See DESIGN.md / INTEGRATION.md."""
 import os as _os
 

@@ -66,8 +66,8 @@ int g16_ctx_create(int curve, int device, g16_ctx** out) {
   if (!out) return fail(G16_ERR_BAD_ARGUMENT, "null out pointer");
   *out = nullptr;
   // A proof uses 6 streams per slot (witness map + five MSMs), two slots, plus the exchange stream.  With the default of 8
-  // hardware work queues several of them share a queue and serialise behind each other: measured, the H MSM started only
-  // when the L MSM had finished (profiles/r02j_shard*.jsonl vs r02k_shard*.jsonl).  The variable is read when the CUDA
+  // hardware work queues several of them share a queue and serialise behind each other: the H MSM would start only
+  // when the L MSM has finished.  The variable is read when the CUDA
   // context is created, so this only helps when we get here before the host process touches the device; the Python package
   // and bench.py also set it at import.  An explicit setting by the user is respected.
   setenv("CUDA_DEVICE_MAX_CONNECTIONS", "32", 0);

@@ -239,10 +239,9 @@ struct Engine : IEngine {
   int cfg_ne = 1;         // effective windows with precomputed bases; 0 = no precomputation
   int cfg_maxcopies = MSM_MAX_COPIES;
   struct Tune {
-    // defaults from the round-2 sweeps on a B200 at 2^20 (profiles/r02_sweep_*.jsonl): 38.3 ms per proof without rounds,
-    // 29.6 ms with these
+    // defaults from sweeps of a full proof at 2^20 (tools/sweep.py)
     int ba_g1 = 4;        // batched-affine rounds before the XYZZ accumulation, G1 MSMs with >= 2^18 entries
-    int ba_g2 = 5;        // same for the G2 MSM
+    int ba_g2 = 4;        // same for the G2 MSM (on an H100 a fifth round costs more than it saves)
     int ba_m = 32;        // additions per thread and round
     int ba_G = 16;        // thread products per inversion
     int ba_gcd = 1;       // safegcd inversion
@@ -255,12 +254,8 @@ struct Engine : IEngine {
     int ba_cap_fwd_g2 = 0, ba_cap_bwd_g2 = 0;
     // Smallest MSM (in bucket entries) that runs the rounds, and how many: a round halves a list whose buckets hold
     // `entries / buckets` slots on average and pads every bucket to 2^R slots, so R is the smallest value with
-    // 11 * 2^R >= that average, capped by ba_g1 / ba_g2 (4 / 5 at
-    // 2^20 pairs on one GPU, 3 on the 2.1 M-entry shards of an 8-way proof, 2 on its 1.0 M-entry A / B shards).  Round 2
-    // first kept the plain XYZZ accumulation below 4 M entries because one proof at a time is latency-bound there
-    // (profiles/r02g_shard8.jsonl); with two proofs in flight -- how the sharded arm runs -- the rounds' smaller
-    // multiplier footprint wins: 8.64 -> 7.37 ms per 8-way shard, 11.03 -> 10.73 ms per 4-way shard, and the
-    // one-at-a-time latency does not lose either (8.86 -> 8.46 ms; profiles/r02q_shard*.jsonl).
+    // 11 * 2^R >= that average, capped by ba_g1 / ba_g2 (4 / 4 at
+    // 2^20 pairs on one GPU, 3 on the 2.1 M-entry shards of an 8-way proof, 2 on its 1.0 M-entry A / B shards).
     long long ba_min_g1 = 1ll << 19;
     long long ba_min_g2 = 1ll << 19;
     int ba_adaptive = 1;  // 0: exactly ba_g1 / ba_g2 rounds whatever the bucket occupancy (tests)
@@ -276,7 +271,7 @@ struct Engine : IEngine {
     return g;
   }
   // entries per level-0 thread, from the number of resident accumulation threads of this device
-  int sm_count = 148;
+  int sm_count = 132;
   int proof_slots = NSLOTS;   // slots the caller will use (g16_set_option "proof_slots" 1 halves the workspace the key must leave room for)
   bool ba_allowed = true;   // cleared by pk_load / setup when the rounds' work lists would not fit in device memory
   uint32_t ba_allowed_mask = 0x1f;   // per MSM (bit m): the work lists of MSM m fit next to the key and the other MSMs' lists
@@ -305,7 +300,7 @@ struct Engine : IEngine {
   }
   int wm_first_opt = 0;        // g16_set_option "wm_first": 1 / 0 / -1 = automatic (sharded keys).  Off: with enough hardware work
                                // queues (CUDA_DEVICE_MAX_CONNECTIONS, see api.cu) the witness map is not held up, and delaying the
-                               // other accumulations then only idles the GPU (profiles/r02k_shard*.jsonl)
+                               // other accumulations then only idles the GPU
   bool share_b_sort = false;   // set when a key is made resident: b_g1_query and b_g2_query have the same identity pattern
   bool share_b_sort_wanted = true;
   void refresh_geoms() {   // after a knob changed: same shards, new launch geometry
@@ -332,15 +327,27 @@ struct Engine : IEngine {
     return G16_OK;
   }
   // Work lists of the batched-affine rounds for all five MSMs of one proof slot; the rounds are switched off for this
-  // key when two slots' worth would not fit next to the resident key (e.g. 2^24 constraints on one GPU).
+  // key when two slots' worth would not fit next to the resident key (e.g. 2^24 constraints on one 80 GB GPU).
   void decide_ba_memory() {
     ba_allowed = true;
     ba_allowed_mask = 0x1f;
     refresh_geoms();
     size_t fr = 0, tot = 0;
     if (cudaMemGetInfo(&fr, &tot) != cudaSuccess) return;
-    // greedy, G1 MSMs first (their lists are half the size of the G2 ones): keep the rounds for an MSM while the lists of all
-    // MSMs granted so far fit `proof_slots` times into the free memory, with 10 GB to spare for everything else
+    // The plain pipeline of every MSM (sorted index / key arrays, level-0 partial sums) is allocated whatever is decided
+    // here: at 2^24 constraints it alone is ~16 GB per proof slot, so it is set aside before any work list is granted.
+    uint64_t plain = 0;
+    for (int m : {M_H, M_L, M_A, M_B1, M_B2}) {
+      if (q[m].hi <= q[m].lo) continue;
+      MsmGeom g = q[m].geom;
+      g.ba = g.ba_pad = 0;
+      MsmBaPlan bp;
+      bp.make(g);
+      plain += bp.len[0] * 8 + 2 * bp.l0_threads(g) * (4 + (m == M_B2 ? sizeof(XYZZ<Fq2>) : sizeof(XYZZ<Fq>)));
+    }
+    // greedy, G1 MSMs first (their lists are half the size of the G2 ones): keep the rounds for an MSM while the plain
+    // pipelines and the lists of all MSMs granted so far fit `proof_slots` times into the free memory, with 10 GB to spare
+    // for everything else (NTT domain and work vectors, CUDA context)
     const uint64_t margin = 10ull << 30;
     uint64_t used = 0;
     uint32_t mask = 0;
@@ -348,8 +355,9 @@ struct Engine : IEngine {
       if (q[m].hi <= q[m].lo) { mask |= 1u << m; continue; }
       MsmBaPlan bp;
       bp.make(q[m].geom);
-      const uint64_t need = ((m == M_B2) ? bp.template extra_bytes<Fq2>() : bp.template extra_bytes<Fq>()) + bp.len[0] * 8;
-      if ((uint64_t)proof_slots * (used + need) + margin <= fr) { used += need; mask |= 1u << m; }
+      const uint64_t need = ((m == M_B2) ? bp.template extra_bytes<Fq2>() : bp.template extra_bytes<Fq>()) +
+                            (bp.len[0] - q[m].geom.max_entries) * 8;   // bucket padding of the sorted arrays
+      if ((uint64_t)proof_slots * (plain + used + need) + margin <= fr) { used += need; mask |= 1u << m; }
     }
     ba_allowed_mask = mask;
     refresh_geoms();
@@ -423,7 +431,8 @@ struct Engine : IEngine {
     G16_CUDA(cudaSetDevice(dev));
     cudaDeviceProp prop;
     G16_CUDA(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major < 10) return fail(G16_ERR_CUDA, "device is not sm_100-class (this library ships sm_100a code only)");
+    if (prop.major != 9 || prop.minor != 0)
+      return fail(G16_ERR_CUDA, "device is not sm_90 (this library ships sm_90a code only, for the H100)");
     sm_count = prop.multiProcessorCount;
     pool.reset(new HostPool(7));
     if (const char* v = getenv("G16_MSM_C")) cfg_c = atoi(v);
@@ -567,11 +576,10 @@ struct Engine : IEngine {
 
   // One transform: the TMA-tiled passes (ntt_tma.cuh) from 2^14 points up, the generic passes (ntt.cuh) below that or
   // when the tensor-map encoder is unavailable / switched off (g16_set_option "ntt_tma" 0).
-  // Measured on a B200 (profiles/r02_sweep_c.jsonl, r02_bench_bls12_377_22_synthetic.json): the TMA plan halves the
-  // passes' DRAM traffic but loses on time -- at 2^20 its 128 KB tiles are only 256 CTAs for 148 SMs (1.7 waves, one CTA
-  // per SM, no overlap of load / butterflies / store): witness map 2.61 ms against 2.03 ms with the generic passes, and
-  // 9.9 ms against 8.1 ms at 2^22.  It is therefore OFF by default and selectable (g16_set_option "ntt_tma" 1) --
-  // DESIGN.md section 3 has the analysis.  1 = from 2^14 points, 0 / -1 = generic passes.
+  // Measured on an H100 (tools/sweep.py, BLS12-381 at 2^20): the TMA plan halves the passes' DRAM traffic but loses on
+  // time -- its 128 KB tiles are only 256 CTAs for 132 SMs (1.9 waves, one CTA per SM, no overlap of load / butterflies /
+  // store): witness map 2.61 ms against 2.30 ms with the generic passes.  It is therefore OFF by default and selectable
+  // (g16_set_option "ntt_tma" 1) -- DESIGN.md section 3 has the analysis.  1 = from 2^14 points, 0 / -1 = generic passes.
   int use_ntt_tma = 0;
   void ntt_any(cudaStream_t st, const NttDomain<Fr>& d, bool inverse, const Fr* src, Fr* work, Fr* dst, int load_mode, const Fr* ltab,
                const Fr* in_b, const Fr* in_c, const Fr& load_cst, int store_mode, const Fr* stab, const Fr& store_cst) {

@@ -1,4 +1,4 @@
-// fp.cuh -- prime-field arithmetic in Montgomery form, 32-bit limbs, for sm_100a.
+// fp.cuh -- prime-field arithmetic in Montgomery form, 32-bit limbs, for sm_90a.
 //
 // Replaces ark-ff 0.5.0 `Fp<MontBackend<_,N>,N>` (un-vendored dependency of /root/reference; used at
 // prover.rs:64,71,82 `into_bigint`, r1cs_to_qap.rs:28-67,201-232 and inside every curve operation).  The memory

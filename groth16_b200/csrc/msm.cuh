@@ -1,4 +1,4 @@
-// msm.cuh -- variable-base multi-scalar multiplication on sm_100a (Pippenger, signed digits, sort-by-bucket).
+// msm.cuh -- variable-base multi-scalar multiplication on sm_90a (Pippenger, signed digits, sort-by-bucket).
 //
 // Replaces ark-ec 0.5.0 `VariableBaseMSM::msm_bigint` as called at /root/reference/src/prover.rs:66 (H query),
 // :74 (L query) and :262 (A, B-in-G1, B-in-G2 via calculate_coeff).  The group element returned is identical to
@@ -277,7 +277,7 @@ __device__ __forceinline__ Affine<F> load_affine(const Affine<F>* __restrict__ b
 // Level 0: grid covers T0 = ceil(max_entries / K0) threads; threads past the real entry count only clear their slots.
 // Register budget: 3 resident blocks per SM for single-field points (G1), 2 for Fq2 points (G2).  (Staging the gathered
 // bases through shared memory with cp.async was measured and is slower: with 3 warps per scheduler the gather latency
-// is already hidden and the kernel is bound by the IMAD.WIDE pipe, profiles/.  Also measured and slower: the running sum
+// is already hidden and the kernel is bound by the IMAD.WIDE pipe.  Also measured and slower: the running sum
 // kept in shared memory for one more resident block per SM; lazily reduced double-width products.)
 template <class F>
 struct MsmAccumCfg { static constexpr int MIN_BLOCKS = sizeof(F) <= 48 ? 3 : 2; };

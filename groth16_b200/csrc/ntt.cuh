@@ -1,4 +1,4 @@
-// ntt.cuh -- radix-2 NTT / iNTT over Fr and the R1CS->QAP witness map on sm_100a.
+// ntt.cuh -- radix-2 NTT / iNTT over Fr and the R1CS->QAP witness map on sm_90a.
 //
 // Replaces ark-poly 0.5.0 `Radix2EvaluationDomain::{fft,ifft}_in_place`, `get_coset`, `mul_polynomials_in_
 // evaluation_domain` and `evaluate_vanishing_polynomial` as called from

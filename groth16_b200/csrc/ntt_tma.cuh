@@ -1,4 +1,4 @@
-// ntt_tma.cuh -- radix-2 NTT passes on 128 KB shared-memory tiles moved by TMA (sm_100a), for transforms of 2^14 points up.
+// ntt_tma.cuh -- radix-2 NTT passes on 128 KB shared-memory tiles moved by TMA (sm_90a), for transforms of 2^14 points up.
 //
 // Same mathematics and conventions as ntt.cuh (ark-poly Radix2EvaluationDomain as called at
 // /root/reference/src/r1cs_to_qap.rs:201-207,220-221,232; natural order in and out, L decimation-in-frequency stages), a

@@ -1,4 +1,4 @@
-/* g16b200.h -- C ABI of libg16b200.so: the B200-native Groth16 proving hot path (NTT witness map + five MSMs).
+/* g16b200.h -- C ABI of libg16b200.so: the H100-native Groth16 proving hot path (NTT witness map + five MSMs).
  *
  * Drop-in boundary for ark-groth16 0.5.0 (/root/reference).  Every entry point names the reference interface it
  * replaces; INTEGRATION.md shows the Rust `extern "C"` binding a maintainer would add.
@@ -34,7 +34,7 @@ enum {
   G16_OK = 0,
   G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE = 1, /* SynthesisError::PolynomialDegreeTooLarge, r1cs_to_qap.rs:134,179 */
   G16_ERR_BAD_ARGUMENT = 2,                /* null pointer / inconsistent length / unknown curve               */
-  G16_ERR_CUDA = 3,                        /* CUDA failure or no usable sm_100 device; see g16_last_error()    */
+  G16_ERR_CUDA = 3,                        /* CUDA failure or no usable sm_90 device; see g16_last_error()     */
   G16_ERR_MALFORMED_KEY = 4                /* SynthesisError::MalformedVerifyingKey-class length mismatch      */
 };
 

@@ -1,4 +1,4 @@
-//! `ark-groth16-b200`: ark-groth16 0.5's prover API on top of `libg16b200.so` (B200 / sm_100a CUDA kernels).
+//! `ark-groth16-b200`: ark-groth16 0.5's prover API on top of `libg16b200.so` (H100 / sm_90a CUDA kernels).
 //!
 //! What is replaced (file:line of arkworks-rs/groth16 @ d570ee5):
 //!   * `Groth16::<E>::create_proof_with_reduction_and_matrices`   src/prover.rs:26-51   -> [`B200Prover::create_proof_with_reduction_and_matrices`]
@@ -501,7 +501,7 @@ impl<E: SwPairing> CircuitSpecificSetupSNARK<E::ScalarField> for Groth16B200<E> 
 #[cfg(test)]
 mod tests {
     //! The reference's own round trip (src/test.rs:45-72) with the GPU prover and ark's verifier, plus bit-equality with
-    //! ark's CPU prover for fixed (r, s).  Needs a B200 and libg16b200.so at run time.
+    //! ark's CPU prover for fixed (r, s).  Needs an H100 and libg16b200.so at run time.
     use super::*;
     use ark_bls12_381::{Bls12_381, Fr};
     use ark_relations::{lc, r1cs::Variable};

@@ -11,7 +11,7 @@ for p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 def _newest(paths):
@@ -22,10 +22,10 @@ def _ensure_built():
     """The shared libraries are build artefacts (git-ignored): build them on demand so that a fresh checkout can run the
     CPU tier (ABI symbol check, oracle pinning) without a separate build step, and never test a stale .so silently.
 
-    In a development tree `make` is the staleness check (headers tracked through the -MMD dependency files).  A gpurun
-    snapshot ships the built libraries WITHOUT the object files (.gpurunignore): there `make` would recompile everything
-    (~2 min of nvcc on the GPU box) just to relink the same code, so the shipped library is used as it is when it is at least
-    as new as every source it is built from, and rebuilt otherwise."""
+    In a development tree `make` is the staleness check (headers tracked through the -MMD dependency files).  A tree copied
+    to a GPU machine with the built libraries but WITHOUT the object files would make `make` recompile everything (minutes
+    of nvcc) just to relink the same code, so there the copied library is used as it is when it is at least as new as every
+    source it is built from, and rebuilt otherwise."""
     import glob
     import shutil
     import subprocess

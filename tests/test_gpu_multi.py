@@ -1,5 +1,5 @@
-"""Multi-GPU tier (needs >= 2 B200s on the box; skipped otherwise): one process per GPU under torchrun, NCCL inside the
-library.  `gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu` runs it; the N > 1 host logic is also
+"""Multi-GPU tier (needs >= 2 H100s on the box; skipped otherwise): one process per GPU under torchrun, NCCL inside the
+library.  `python -m pytest tests/test_gpu_multi.py -m gpu` on a multi-GPU box runs it; the N > 1 host logic is also
 covered on CPU with gloo (tests/test_dist_cpu.py)."""
 import os
 import subprocess

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on a B200 with `pytest -m gpu`): every C-ABI entry point against the CPU oracle.
+"""GPU parity tests (run on an H100 with `pytest -m gpu`): every C-ABI entry point against the CPU oracle.
 
 Bar: bit-exact (integer arithmetic throughout).  Reference behaviour cited per test."""
 import numpy as np

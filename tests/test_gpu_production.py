@@ -1,4 +1,4 @@
-"""GPU parity at the PRODUCTION kernel geometry (run on a B200 with `pytest -m gpu`).
+"""GPU parity at the PRODUCTION kernel geometry (run on an H100 with `pytest -m gpu`).
 
 test_gpu_parity.py stops at 2^15-pair MSMs / 2^13-point NTTs / 2^14-constraint proofs, where the MSM picks c = 11 and
 the NTT plan has two passes.  What bench.py ships is different code paths: c = 16 with ONE bucket set and 16

@@ -139,7 +139,7 @@ def test_msm_reduction_plan_host(tmp_path):
     if shutil.which("nvcc") is None:
         pytest.skip("nvcc not available")
     exe = str(tmp_path / "msm_plan_check")
-    subprocess.check_call(["nvcc", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-o", exe,
+    subprocess.check_call(["nvcc", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-o", exe,
                            os.path.join(ROOT, "tests", "host", "msm_plan_check.cu")])
     out = subprocess.run([exe], capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
@@ -154,7 +154,7 @@ def test_batched_affine_rounds_host(tmp_path):
     if shutil.which("nvcc") is None:
         pytest.skip("nvcc not available")
     exe = str(tmp_path / "ba_check")
-    subprocess.check_call(["nvcc", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-o", exe,
+    subprocess.check_call(["nvcc", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-o", exe,
                            os.path.join(ROOT, "tests", "host", "ba_check.cu")])
     out = subprocess.run([exe], capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr

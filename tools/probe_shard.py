@@ -23,7 +23,7 @@ ON = _lib.ASSIGNMENT_ON_DEVICE
 lines = []
 GRID = json.loads(os.environ["G16_PROBE_GRID"]) if os.environ.get("G16_PROBE_GRID") else [{}, {"msm_ba": 0, "msm_ba_g2": 0}]
 for opts in GRID:
-    base = {"msm_ba": 4, "msm_ba_g2": 5, "ba_m": 32, "ba_g": 16, "ba_min_entries_g1": 1 << 19, "ba_min_entries_g2": 1 << 19, "wm_first": -1}
+    base = {"msm_ba": 4, "msm_ba_g2": 4, "ba_m": 32, "ba_g": 16, "ba_min_entries_g1": 1 << 19, "ba_min_entries_g2": 1 << 19, "wm_first": -1}
     base.update(opts)
     for k, v in base.items():
         g.set_option(k, v)
@@ -64,7 +64,7 @@ for opts in GRID:
             "timeline_begin": {k: round(v, 2) for k, v in tm["msm_begin_ms"].items()}, "timeline_end": {k: round(v, 2) for k, v in tm["msm_end_ms"].items()}}
     print(json.dumps(line), flush=True)
     lines.append(line)
-for k, v in {"msm_ba": 4, "msm_ba_g2": 5, "ba_m": 32, "ba_g": 16, "ba_min_entries_g1": 1 << 19, "ba_min_entries_g2": 1 << 19}.items():
+for k, v in {"msm_ba": 4, "msm_ba_g2": 4, "ba_m": 32, "ba_g": 16, "ba_min_entries_g1": 1 << 19, "ba_min_entries_g2": 1 << 19}.items():
     g.set_option(k, v)
 g.prove_partial_raw(r, zd.data_ptr(), ON | _lib.SERIAL_MSMS, out)
 torch.cuda.synchronize()

@@ -37,7 +37,7 @@ DEFAULT_GRID = [
     {"msm_ba": 4, "msm_ba_g2": 0, "acc_k0_g2": 16},
     {"msm_ba": 4, "msm_ba_g2": 0, "acc_k0_g2": 64},
 ]
-BASE = {"msm_ba": 4, "msm_ba_g2": 5, "ba_m": 32, "ba_g": 16, "ba_inv_gcd": 1, "acc_k0_g1": 0, "acc_k0_g2": 0, "acc_block": 128,
+BASE = {"msm_ba": 4, "msm_ba_g2": 4, "ba_m": 32, "ba_g": 16, "ba_inv_gcd": 1, "acc_k0_g1": 0, "acc_k0_g2": 0, "acc_block": 128,
         "share_b_sort": 1, "ba_occ_g1": 0, "ba_occ_g2": 0, "ntt_tma": -1,
         "ba_cap_fwd_g1": 0, "ba_cap_bwd_g1": 0, "ba_cap_fwd_g2": 0, "ba_cap_bwd_g2": 0}
 

@@ -1,4 +1,4 @@
-// tools/ubench_pipes.cu -- which execution pipes bound 384-bit modular arithmetic on a B200 (sm_100a)?
+// tools/ubench_pipes.cu -- which execution pipes bound 384-bit modular arithmetic on an H100 (sm_90a)?
 // Measures, with all SMs full of warps and long independent dependency chains per thread:
 //   imad_wide   mad.wide.u32 (IMAD.WIDE.U32)            the instruction the Montgomery products are made of
 //   imad_lo     mad.lo.u32   (IMAD)                      32-bit multiply-add
