@@ -13,6 +13,7 @@
 #pragma once
 #include <cstdint>
 #include <cstring>
+#include <type_traits>
 #include "g16_constants.h"
 
 namespace g16 {
@@ -58,6 +59,12 @@ inline void madc_hi(uint32_t& r, uint32_t a, uint32_t b, uint32_t c) { r = (uint
 // ------------------------------------------------------------------------------------------------
 // Fp<P>: P supplies N, INV32, mod(i), one(i), r2(i)
 // ------------------------------------------------------------------------------------------------
+// Curve base fields (Fq): their device products are out-of-line calls, see Fp::mul.  Scalar fields stay inlined.
+template <class P>
+constexpr bool is_base_field() {
+  return std::is_same<P, BLS381_FqP>::value || std::is_same<P, BN254_FqP>::value || std::is_same<P, BLS377_FqP>::value;
+}
+
 template <class P>
 struct alignas(16) Fp {
   static constexpr int N = P::N;
@@ -206,7 +213,7 @@ struct alignas(16) Fp {
     cmad_row_mod<0>(E, m);
     ptx::addc(O[N - 1], O[N - 1], 0);
   }
-  G16_HD static Fp mul(const Fp& a, const Fp& b) {
+  G16_HD static Fp mont_mul(const Fp& a, const Fp& b) {
     static_assert(N % 2 == 0, "even limb count required");
     uint32_t ev[N], od[N];
     mont_step<true>(ev, od, a.v, b.v[0]);
@@ -225,7 +232,7 @@ struct alignas(16) Fp {
     return reduce_once(r);
   }
 #else
-  G16_HD static Fp mul(const Fp& a, const Fp& b) {
+  G16_HD static Fp mont_mul(const Fp& a, const Fp& b) {
     constexpr int W = N / 2;
     uint64_t x[W], y[W], p[W], t[W + 2];
     memcpy(x, a.v, sizeof(x));
@@ -249,6 +256,19 @@ struct alignas(16) Fp {
     return reduce_once(r);
   }
 #endif
+#ifdef __CUDACC__
+  // One out-of-line product body per base field and kernel; operands and result travel in registers (no local memory).
+  // Inlined at every call, the MSM kernels' straight-line bodies (an Fq2 bucket addition alone is >100 KB of SASS) run out
+  // of registers and spill; called, the G2 kernels stop spilling and the proof is shorter (DESIGN.md section 3).  It is
+  // not the instruction cache: a 185 KB straight-line loop of products runs within 1 % of a single product at 8 warps/SM.
+  static __device__ __noinline__ Fp mont_mul_call(Fp a, Fp b) { return mont_mul(a, b); }
+#endif
+  G16_HD static Fp mul(const Fp& a, const Fp& b) {
+#ifdef __CUDA_ARCH__
+    if constexpr (is_base_field<P>()) return mont_mul_call(a, b);
+#endif
+    return mont_mul(a, b);
+  }
   G16_HD static Fp sqr(const Fp& a) { return mul(a, a); }
 
   // r in [0, 2p) -> [0, p)

@@ -5,8 +5,11 @@
 //   dfma        fma.rz.f64   (DFMA)                      the alternative multiplier: 52-bit limbs in doubles
 //   iadd3       add.u32 chains                           carry-propagation side work (ALU pipe)
 //   mix_*       two of them interleaved in one thread    do the pipes overlap (separate issue ports) or serialise?
-// Output: one JSON line per test: {"test":..., "lane_ops_per_clk_per_sm":..., "gops":...}.  Used once per round to decide whether a
-// floating-point limb representation is worth building (DESIGN.md section 6); not part of the product.
+//   fq_mul_*    the library's BLS12-381 Fq product, alone and in loop bodies of growing code size (fq_mul_body)
+// Output: one JSON line per test: {"test":..., "lane_ops_per_clk_per_sm":..., "gops":...}.  Used to decide whether a
+// floating-point limb representation is worth building, and how large a hot loop may grow (DESIGN.md sections 3 and 6);
+// not part of the product.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 --expt-relaxed-constexpr tools/ubench_pipes.cu -o tools/ubench_pipes
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -48,36 +51,80 @@ __global__ void __launch_bounds__(128) mulchain(uint32_t* out, int iters) {
   for (int c = 0; c < CHAINS; c++) { x[c] = F::one(); x[c].v[0] += threadIdx.x + c; }
   for (int it = 0; it < iters; it++) {
 #pragma unroll
-    for (int c = 0; c < CHAINS; c++) x[c] = F::mul(x[c], y);
+    for (int c = 0; c < CHAINS; c++) x[c] = F::mont_mul(x[c], y);   // the inlined body (F::mul is a call on the device)
   }
   uint32_t s = 0;
   for (int c = 0; c < CHAINS; c++) s += x[c].v[3];
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
-template <int CHAINS>
-static void run_mul(int warps_per_sm, int sms, double mhz) {
+// Code-size sweep: one dependent product chain whose loop body is K fully inlined copies of the product (about 7 KB of
+// SASS each), or, with CALL, K calls of the one out-of-line body the library's base-field products use.  The arithmetic is
+// the same for every K; only the size of the straight-line body each warp runs through changes, so a drop in rate with K
+// is instruction fetch (the SM's instruction caches are smaller than the larger bodies; NVIDIA does not publish sizes).
+template <int K, bool CALL>
+__global__ void __launch_bounds__(128) mulbody(uint32_t* out, int iters) {
+  using F = g16::Fp<g16::BLS381_FqP>;
+  F x = F::one(), y = F::r2();
+  x.v[0] += threadIdx.x;
+#pragma unroll 1
+  for (int it = 0; it < iters; it++) {
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+      if constexpr (CALL) x = F::mont_mul_call(x, y);
+      else x = F::mont_mul(x, y);
+    }
+  }
+  out[blockIdx.x * blockDim.x + threadIdx.x] = x.v[3];
+}
+
+// Milliseconds of the second of two launches of kern<<<sms * warps_per_sm / 4, 128>>>(out, iters), with exactly
+// warps_per_sm / 4 blocks resident per SM (forced by the dynamic shared memory request).
+static float time_resident(void (*kern)(uint32_t*, int), int warps_per_sm, int sms, int iters, int* blocks_out) {
   const int blocks_per_sm = warps_per_sm / 4;
-  const int smem = (227 * 1024) / blocks_per_sm - 1024;   // forces exactly blocks_per_sm resident blocks
-  cudaFuncSetAttribute(mulchain<CHAINS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  const int blocks = sms * blocks_per_sm, iters = 2000;
+  const int smem = (227 * 1024) / blocks_per_sm - 1024;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  const int blocks = sms * blocks_per_sm;
   uint32_t* out;
   cudaMalloc(&out, (size_t)blocks * 128 * 4);
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);
-  mulchain<CHAINS><<<blocks, 128, smem>>>(out, iters);
+  kern<<<blocks, 128, smem>>>(out, iters);
   cudaDeviceSynchronize();
   cudaEventRecord(e0);
-  mulchain<CHAINS><<<blocks, 128, smem>>>(out, iters);
+  kern<<<blocks, 128, smem>>>(out, iters);
   cudaEventRecord(e1);
   cudaEventSynchronize(e1);
   float ms = 0;
   cudaEventElapsedTime(&ms, e0, e1);
+  cudaFree(out);
+  *blocks_out = blocks;
+  return ms;
+}
+
+template <int K, bool CALL>
+static void run_body(int warps_per_sm, int sms, double mhz) {
+  const int iters = 4096 / K;   // 4096 products per thread for every K
+  int blocks = 0;
+  const float ms = time_resident(mulbody<K, CALL>, warps_per_sm, sms, iters, &blocks);
+  const double muls = (double)blocks * 128 * iters * K / (ms * 1e-3);
+  cudaFuncAttributes fa;
+  cudaFuncGetAttributes(&fa, mulbody<K, CALL>);
+  printf("{\"test\": \"fq_mul_body\", \"copies\": %d, \"call\": %s, \"warps_per_sm\": %d, \"regs\": %d, \"local_bytes\": %zu, \"ms\": %.4f, "
+         "\"muls_per_s\": %.4e, \"imad_wide_lanes_per_clk_per_sm\": %.2f, \"err\": \"%s\"}\n",
+         K, CALL ? "true" : "false", warps_per_sm, fa.numRegs, fa.localSizeBytes, ms, muls, muls * 288 / (mhz * 1e6) / sms,
+         cudaGetErrorString(cudaGetLastError()));
+}
+
+template <int CHAINS>
+static void run_mul(int warps_per_sm, int sms, double mhz) {
+  const int iters = 2000;
+  int blocks = 0;
+  const float ms = time_resident(mulchain<CHAINS>, warps_per_sm, sms, iters, &blocks);
   const double muls = (double)blocks * 128 * iters * CHAINS / (ms * 1e-3);
   printf("{\"test\": \"fq_mul_bls381\", \"chains_per_thread\": %d, \"warps_per_sm\": %d, \"ms\": %.4f, \"muls_per_s\": %.4e, \"imad_wide_per_s\": %.4e, "
          "\"imad_wide_lanes_per_clk_per_sm\": %.2f, \"err\": \"%s\"}\n",
          CHAINS, warps_per_sm, ms, muls, muls * 288, muls * 288 / (mhz * 1e6) / sms, cudaGetErrorString(cudaGetLastError()));
-  cudaFree(out);
 }
 
 template <int MODE>
@@ -119,5 +166,15 @@ int main() {
   run<6>("mix_dfma_iadd", 2, p.multiProcessorCount, mhz);
   for (int w : {4, 8, 12, 16, 24, 32, 48}) run_mul<1>(w, p.multiProcessorCount, mhz);
   for (int w : {4, 8, 12, 16, 24}) run_mul<2>(w, p.multiProcessorCount, mhz);
+  for (int w : {8, 12}) {
+    const int sms = p.multiProcessorCount;
+    run_body<1, false>(w, sms, mhz);
+    run_body<2, false>(w, sms, mhz);
+    run_body<4, false>(w, sms, mhz);
+    run_body<8, false>(w, sms, mhz);
+    run_body<16, false>(w, sms, mhz);
+    run_body<32, false>(w, sms, mhz);
+    run_body<32, true>(w, sms, mhz);
+  }
   return 0;
 }
