@@ -73,6 +73,7 @@ SIGNATURES = [
     ("g16_synthetic_r1cs", C.c_int, [C.c_int, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("g16_get_config", C.c_int, [C.c_void_p, C.POINTER(Config)]),
     ("g16_set_option", C.c_int, [C.c_void_p, C.c_char_p, C.c_int64]),
+    ("g16_get_option", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_int64)]),
 ]
 
 G16_OK = 0

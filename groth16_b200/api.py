@@ -418,6 +418,12 @@ class Groth16:
         """MSM launch-geometry knobs (g16_set_option; results never depend on them)."""
         _check(self._lib.g16_set_option(self._ctx, key.encode(), int(value)))
 
+    def get_option(self, key: str) -> int:
+        """g16_get_option: the value `key` holds now; set_option(key, get_option(key)) changes nothing."""
+        v = C.c_int64()
+        _check(self._lib.g16_get_option(self._ctx, key.encode(), C.byref(v)))
+        return int(v.value)
+
     def config(self) -> dict:
         """Launch geometry of the resident key's MSMs plus two derived figures bench.py reports: the field products per
         bucket entry of the G1 accumulation stage (XYZZ mixed addition = 10; batched-affine addition = 6 + the combine's

@@ -218,5 +218,13 @@ int g16_set_option(g16_ctx* ctx, const char* key, int64_t value) {
   if (!key) return fail(G16_ERR_BAD_ARGUMENT, "null key");
   return ctx->eng->set_option(key, (long long)value);
 }
+int g16_get_option(const g16_ctx* ctx, const char* key, int64_t* value) {
+  CTX_OR_FAIL(ctx);
+  if (!key || !value) return fail(G16_ERR_BAD_ARGUMENT, "null key / out");
+  long long v = 0;
+  const int rc = ctx->eng->get_option(key, &v);
+  if (rc == G16_OK) *value = (int64_t)v;
+  return rc;
+}
 
 }  // extern "C"

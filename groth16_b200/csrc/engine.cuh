@@ -148,6 +148,7 @@ struct IEngine {
   virtual int sharded_submit(int slot, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags) = 0;
   virtual int sharded_wait(int slot, uint64_t* proof) = 0;
   virtual int set_option(const char* key, long long value) = 0;
+  virtual int get_option(const char* key, long long* value) const = 0;
   virtual int get_config(g16_config* out) const = 0;
   g16_timings tm{};
 };
@@ -365,6 +366,18 @@ struct Engine : IEngine {
   int set_option(const char* key, long long v) override {
     if (any_busy()) return fail(G16_ERR_BAD_ARGUMENT, "a proof is in flight");
     const std::string k(key ? key : "");
+    // values the launch geometry cannot honour are refused rather than silently replaced
+    auto out_of_range = [&](long long lo, long long hi) {
+      return fail(G16_ERR_BAD_ARGUMENT, "option " + k + " = " + std::to_string(v) + " outside [" + std::to_string(lo) + ", " +
+                                            std::to_string(hi) + "]");
+    };
+    if ((k == "msm_ba" || k == "msm_ba_g2") && (v < 0 || v > MSM_BA_MAX_ROUNDS)) return out_of_range(0, MSM_BA_MAX_ROUNDS);
+    if ((k == "acc_k0_g1" || k == "acc_k0_g2") && v != 0 && (v < 4 || v > 1024))
+      return fail(G16_ERR_BAD_ARGUMENT, "option " + k + " must be 0 (automatic) or in [4, 1024]");
+    if (k == "acc_block" && v != 32 && v != 64 && v != 128) return fail(G16_ERR_BAD_ARGUMENT, "option acc_block must be 32, 64 or 128");
+    if (k == "msm_ne" && (v < 0 || v > 32)) return out_of_range(0, 32);
+    if (k == "msm_c" && (v < 0 || v > 24)) return out_of_range(0, 24);
+    if (k == "msm_maxcopies" && (v < 1 || v > MSM_MAX_COPIES)) return out_of_range(1, MSM_MAX_COPIES);
     if (k == "msm_ba") tune.ba_g1 = (int)v;
     else if (k == "msm_ba_g2") tune.ba_g2 = (int)v;
     else if (k == "ba_m") tune.ba_m = (int)std::max(1ll, std::min(v, 256ll));
@@ -387,12 +400,44 @@ struct Engine : IEngine {
     else if (k == "wm_split") { split_wm_wanted = v != 0; return G16_OK; }
     else if (k == "proof_slots") { proof_slots = v <= 1 ? 1 : NSLOTS; if (have_pk) decide_ba_memory(); return G16_OK; }
     // residency knobs: take effect at the NEXT g16_pk_load / g16_setup (they decide how many precomputed multiples a key keeps)
-    else if (k == "msm_ne") { cfg_ne = (int)std::max(0ll, std::min(v, 32ll)); return G16_OK; }
-    else if (k == "msm_c") { cfg_c = (v < 0 || v > 24) ? 0 : (int)v; return G16_OK; }
-    else if (k == "msm_maxcopies") { cfg_maxcopies = (int)std::max(1ll, std::min(v, (long long)MSM_MAX_COPIES)); return G16_OK; }
+    else if (k == "msm_ne") { cfg_ne = (int)v; return G16_OK; }
+    else if (k == "msm_c") { cfg_c = (int)v; return G16_OK; }
+    else if (k == "msm_maxcopies") { cfg_maxcopies = (int)v; return G16_OK; }
     else if (k == "share_b_sort") { share_b_sort_wanted = v != 0; if (have_pk) { int rc = decide_b_sort_sharing(); if (rc) return rc; } }
     else return fail(G16_ERR_BAD_ARGUMENT, "unknown option: " + k);
     refresh_geoms();
+    return G16_OK;
+  }
+  // the value an option holds now, in the form g16_set_option accepts (set_option(k, get_option(k)) changes nothing)
+  int get_option(const char* key, long long* out) const override {
+    if (!out) return fail(G16_ERR_BAD_ARGUMENT, "null out");
+    const std::string k(key ? key : "");
+    if (k == "msm_ba") *out = tune.ba_g1;
+    else if (k == "msm_ba_g2") *out = tune.ba_g2;
+    else if (k == "ba_m") *out = tune.ba_m;
+    else if (k == "ba_g") *out = tune.ba_G;
+    else if (k == "ba_inv_gcd") *out = tune.ba_gcd;
+    else if (k == "acc_k0_g1") *out = tune.k0_g1;
+    else if (k == "acc_k0_g2") *out = tune.k0_g2;
+    else if (k == "acc_block") *out = tune.acc_block;
+    else if (k == "ba_occ_g2") *out = tune.ba_occ_g2;
+    else if (k == "ba_occ_g1") *out = tune.ba_occ_g1;
+    else if (k == "ba_cap_fwd_g1") *out = tune.ba_cap_fwd_g1;
+    else if (k == "ba_cap_bwd_g1") *out = tune.ba_cap_bwd_g1;
+    else if (k == "ba_cap_fwd_g2") *out = tune.ba_cap_fwd_g2;
+    else if (k == "ba_cap_bwd_g2") *out = tune.ba_cap_bwd_g2;
+    else if (k == "ba_adaptive") *out = tune.ba_adaptive;
+    else if (k == "ba_min_entries_g1") *out = tune.ba_min_g1;
+    else if (k == "ba_min_entries_g2") *out = tune.ba_min_g2;
+    else if (k == "ntt_tma") *out = use_ntt_tma;
+    else if (k == "wm_first") *out = wm_first_opt;
+    else if (k == "wm_split") *out = split_wm_wanted ? 1 : 0;
+    else if (k == "proof_slots") *out = proof_slots;
+    else if (k == "msm_ne") *out = cfg_ne;
+    else if (k == "msm_c") *out = cfg_c;
+    else if (k == "msm_maxcopies") *out = cfg_maxcopies;
+    else if (k == "share_b_sort") *out = share_b_sort_wanted ? 1 : 0;
+    else return fail(G16_ERR_BAD_ARGUMENT, "unknown option: " + k);
     return G16_OK;
   }
   int get_config(g16_config* o) const override {

@@ -601,9 +601,10 @@ struct MsmBaPlan {
     k0_final = g.k0 >> R;
     if (k0_final < 8) k0_final = g.k0 < 8 ? g.k0 : 8;
   }
-  // threads of the level-0 accumulation
+  // threads of the level-0 accumulation.  Without rounds the list is still padded when it is shared with an MSM that runs
+  // them (pad > 0): the threads must cover the padded length len[0], not just max_entries
   uint64_t l0_threads(const MsmGeom& g) const {
-    return R > 0 ? (len[R] + k0_final - 1) / k0_final : (g.max_entries + g.k0 - 1) / g.k0;
+    return R > 0 ? (len[R] + k0_final - 1) / k0_final : (len[0] + g.k0 - 1) / g.k0;
   }
   // device bytes the rounds need on top of the plain pipeline (per MSM and proof slot)
   template <class F>

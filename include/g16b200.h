@@ -212,8 +212,12 @@ int g16_get_config(const g16_ctx* ctx, g16_config* out);
  * "msm_ba" rounds, 1 = at most that many, fewer for sparsely filled buckets), "ba_cap_fwd_g1", "ba_cap_bwd_g1", "ba_cap_fwd_g2", "ba_cap_bwd_g2", "ntt_tma", "wm_split", "proof_slots", and -- effective at the next
  * g16_pk_load / g16_setup -- "msm_ne", "msm_c", "msm_maxcopies" (the G16_* environment
  * variables of INTEGRATION.md section 6, read once at g16_ctx_create, in lower case without the prefix).  Takes effect
- * from the next proof; results never depend on these knobs. */
+ * from the next proof; results never depend on these knobs.  Accepted ranges: "msm_ba", "msm_ba_g2" 0 .. 6; "acc_k0_g1",
+ * "acc_k0_g2" 0 (automatic) or 4 .. 1024; "acc_block" 32, 64 or 128; "msm_ne" 0 .. 32; "msm_c" 0 (automatic) .. 24;
+ * "msm_maxcopies" 1 .. 20.  A value outside its range is refused with G16_ERR_BAD_ARGUMENT and changes nothing. */
 int g16_set_option(g16_ctx* ctx, const char* key, int64_t value);
+/* The value an option holds now (same keys; feeding it back to g16_set_option restores the option exactly). */
+int g16_get_option(const g16_ctx* ctx, const char* key, int64_t* value);
 uint32_t g16_domain_log(const g16_ctx* ctx); /* log2 of the resident circuit's domain size */
 
 /* ---- benchmark / test helper (no reference counterpart: arkworks users bring their own circuits) -----------------

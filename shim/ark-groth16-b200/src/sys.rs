@@ -136,4 +136,5 @@ extern "C" {
     pub fn g16_synthetic_r1cs(curve: c_int, log_n: u32, seed: u64, a_col: *mut u32, a_val: *mut u64, b_col: *mut u32, c_col: *mut u32, full_assignment: *mut u64) -> c_int;
     pub fn g16_get_config(ctx: *const g16_ctx, out: *mut g16_config) -> c_int;
     pub fn g16_set_option(ctx: *mut g16_ctx, key: *const c_char, value: i64) -> c_int;
+    pub fn g16_get_option(ctx: *const g16_ctx, key: *const c_char, value: *mut i64) -> c_int;
 }

@@ -3,6 +3,7 @@
 // MsmHostRed::T / msm_finish, against the definition  sum_e 2^(c e) * sum_b (b + 1) * bucket[e][b].
 // The device kernel msm_sum_strided is replaced here by a literal host evaluation of the same sums.
 #include <cstdio>
+#include <utility>
 #include <vector>
 #include "../../groth16_b200/csrc/msm.cuh"
 using namespace g16;
@@ -27,8 +28,13 @@ int main() {
   uint64_t seed = 12345;
   auto rnd = [&]() { seed = seed * 6364136223846793005ull + 1442695040888963407ull; return (uint32_t)(seed >> 40); };
   int bad = 0, cases = 0;
-  for (int m : {2, 3, 5, 6, 7, 8, 10, 11, 13}) {
-    for (int ne : {1, 3}) {
+  // up to the production shape: 2^15 buckets per window, 1 .. 16 effective windows (the bucket sets of bench.py's plans)
+  const std::vector<std::pair<int, std::vector<int>>> shapes = {{2, {1, 3}}, {3, {1, 3}}, {5, {1, 3}}, {6, {1, 3}}, {7, {1, 3}},
+                                                                {8, {1, 3}}, {10, {1, 3}}, {11, {1, 3}}, {13, {1, 3}},
+                                                                {14, {1, 2, 8, 16}}, {15, {1, 2, 8, 16}}};
+  for (const auto& shape : shapes) {
+    const int m = shape.first;
+    for (int ne : shape.second) {
       cases++;
       const int c = m + 1;
       MsmGeom g{};
@@ -38,7 +44,7 @@ int main() {
       const MsmRedPlan& pl = ws.plan;
       const size_t B = g.B;
       std::vector<Pt> buckets(B * ne), inner(pl.inner_pts * ne + 1), leaf(pl.leaf_pts * ne + 1);
-      std::vector<uint64_t> weight(ne, 0);   // sum (b+1) s_b per window (fits: B <= 8192, s <= 7)
+      std::vector<uint64_t> weight(ne, 0);   // sum (b+1) s_b per window (fits: B <= 2^15, s <= 7: < 7 * 2^29)
       for (int w = 0; w < ne; w++)
         for (size_t b = 0; b < B; b++) {
           const uint32_t s = (rnd() % 3 == 0) ? 0 : rnd() % 8;
@@ -90,8 +96,16 @@ int main() {
     }
   }
   // geometry helpers
-  MsmGeom g16 = msm_geom(1u << 20, 255, 16, 1);
-  if (!(g16.W == 16 && g16.copies == 16 && g16.B == 32768 && g16.nkeys == 32768)) { bad++; fprintf(stderr, "geom c=16 mismatch\n"); }
+  // c = 16 at 2^20 pairs for every bucket-set count of bench.py's residency plans (and a ragged one), all three scalar widths
+  for (int bits : {255, 254, 253})
+    for (int ne : {1, 2, 3, 4, 8, 16}) {
+      const MsmGeom g = msm_geom(1u << 20, bits, 16, ne);
+      if (!(g.c == 16 && g.W == 16 && g.ne == ne && g.copies == (16 + ne - 1) / ne && g.B == 32768 && g.nkeys == 32768u * ne &&
+            g.max_entries == (16ull << 20))) {
+        bad++;
+        fprintf(stderr, "geom c=16 bits=%d ne=%d mismatch\n", bits, ne);
+      }
+    }
   MsmGeom g3 = msm_geom(17, 254, 0, 0);
   if (!(g3.c == 3 && g3.ne == g3.W && g3.copies == 1 && g3.W == 85)) { bad++; fprintf(stderr, "geom small mismatch\n"); }
   if (msm_pick_k0(16u << 20, 56832, 8) != 64 || msm_pick_k0(2u << 20, 56832, 8) != 16 || msm_level_threads(2048, 4) != 512) { bad++; fprintf(stderr, "k0 / level mismatch\n"); }

@@ -1,0 +1,492 @@
+"""GPU parity over every MSM geometry the prover can run (run on an H100 with `pytest -m gpu`).
+
+The tuning knobs of include/g16b200.h change speed, never results.  test_gpu_production.py checks that for the default
+single-GPU plan only (c = 16, one bucket set, 16 precomputed multiples, equal batched-affine rounds on G1 and G2).  Here one
+2^17-constraint key per curve (every query >= 2^16 pairs, so c = 16 is chosen) and ONE oracle proof per curve serve a matrix
+of residency plans, uneven rounds, accumulation knobs, schedules and sharded keys: every configuration re-loads the key,
+asserts through g16_get_config that the geometry it asked for was reached, proves, and must match the oracle bit for bit.
+Further: adversarial bases (duplicates, opposite pairs, identity runs) and signed-digit edge scalars at the resident
+geometry, partial MSMs against the oracle's msm_bigint; the stand-alone g16_msm_g1 / g2 at c = 12 .. 16 and c = 17 / 20."""
+import contextlib
+from dataclasses import dataclass
+
+import numpy as np
+import pytest
+
+import orc
+import pyref as P
+from groth16_b200 import Groth16, _lib
+from groth16_b200.params import GENERATORS
+from groth16_b200.workload import synthetic_r1cs
+from util import ALL_CURVES
+
+pytestmark = pytest.mark.gpu
+
+LOG_N = 17
+TOXIC = (0x1111111111111111111111, 0x2222222222222222222223, 0x3333333333333333333335, 0x4444444444444444444447,
+         0x5555555555555555555559)
+THREADS = 16
+OPTIONS = ("msm_ne", "msm_c", "msm_maxcopies", "msm_ba", "msm_ba_g2", "ba_adaptive", "ba_min_entries_g1", "ba_min_entries_g2",
+           "acc_k0_g1", "acc_k0_g2", "acc_block", "share_b_sort", "wm_first", "proof_slots")
+M_H, M_L, M_A, M_B1, M_B2 = range(5)
+
+
+# ---- the launch geometry the library should pick (Engine::pick_geom / with_k0, msm_geom, msm_pick_k0) -----------------
+def _pick_c(n):
+    return min(max((n - 1).bit_length() - 4, 3), 16)
+
+
+def _geom(n, bits, c, ne):
+    c = c if c > 0 else _pick_c(n)
+    w = (bits + c) // c
+    ne = w if (ne <= 0 or ne > w) else ne
+    return dict(c=c, W=w, ne=ne, copies=-(-w // ne), nkeys=ne << (c - 1), entries=n * w)
+
+
+def _resident_geom(n, bits, o):
+    if o["msm_ne"] <= 0:
+        return _geom(n, bits, o["msm_c"], 0)
+    c = o["msm_c"] if o["msm_c"] > 0 else (16 if n >= 1 << 16 else 0)
+    ne = o["msm_ne"]
+    g = _geom(n, bits, c, ne)
+    while g["copies"] > o["msm_maxcopies"]:
+        ne += 1
+        g = _geom(n, bits, c, ne)
+    return g
+
+
+def _k0(g, sm_count, g2, o):
+    k0, kmin = 64, (16 if g2 else 8)
+    while k0 > kmin and g["entries"] // k0 < sm_count * 128 * (2 if g2 else 3) * 2:
+        k0 >>= 1
+    if g2 and k0 > 32:
+        k0 = 32
+    k = o["acc_k0_g2" if g2 else "acc_k0_g1"]
+    return k if 4 <= k <= 1024 else k0
+
+
+def _rounds(g, g2, o):
+    r = o["msm_ba_g2" if g2 else "msm_ba"]
+    fit, per = 0, g["entries"] // g["nkeys"]
+    while (11 << fit) < per:
+        fit += 1
+    if not o["ba_adaptive"]:
+        fit = r
+    big = g["entries"] >= max(1 << 18, o["ba_min_entries_g2" if g2 else "ba_min_entries_g1"])
+    return min(r, fit, 6) if r > 0 and big else 0
+
+
+# ---- per-curve state: one engine, one key, one oracle proof ----------------------------------------------------------------
+@dataclass
+class Case:
+    curve: str
+    g: Groth16
+    m: object
+    z: np.ndarray
+    pk: object
+    r: np.ndarray
+    s: np.ndarray
+    want: np.ndarray
+    defaults: dict
+    config0: dict
+
+    @property
+    def bits(self):
+        return self.g.curve.r.bit_length()
+
+    def pairs(self, rank=0, world=1):
+        """(H, B2) pairs owned by `rank`: H has domain - 1 pairs, B-in-G2 one per variable but the constant One"""
+        nv = self.m.num_instance_variables + self.m.num_witness_variables
+        own = lambda n: (n - rank + world - 1) // world
+        return own((1 << LOG_N) - 1), own(nv - 1)
+
+    def expected(self, opts, rank=0, world=1):
+        o = dict(self.defaults, **opts)
+        nh, nb = self.pairs(rank, world)
+        gh, gb = _resident_geom(nh, self.bits, o), _resident_geom(nb, self.bits, o)
+        sm = self.config0["sm_count"]
+        return dict(c=gh["c"], ne=gh["ne"], copies=gh["copies"], k0_g1=_k0(gh, sm, False, o), k0_g2=_k0(gb, sm, True, o),
+                    ba_rounds_g1=_rounds(gh, False, o), ba_rounds_g2=_rounds(gb, True, o))
+
+
+_CASES = {}
+
+
+def case(curve) -> Case:
+    if curve not in _CASES:
+        g = Groth16(curve, 0)
+        defaults = {k: g.get_option(k) for k in OPTIONS}
+        cd = g.codec
+        G = GENERATORS[curve]
+        m, z, _ = synthetic_r1cs(curve, LOG_N, seed=21)
+        g.set_option("msm_ne", 0)          # mint without precomputed multiples (bench.py's big-key flow), export, re-load
+        try:
+            pk = g.generate_parameters_with_qap(m, *TOXIC, G["g1"], G["g2"], export=True)
+        finally:
+            g.set_option("msm_ne", defaults["msm_ne"])
+        g.load_proving_key(pk)
+        r, s = np.ascontiguousarray(cd.fr.enc1(0x1234567 + cd.c.cid)), np.ascontiguousarray(cd.fr.enc1(0x7654321))
+        want, _ = orc.prove(cd.c.cid, cd.nq, pk, m, z, r, s, threads=THREADS)
+        _CASES[curve] = Case(curve, g, m, z, pk, r, s, want, defaults, g.config())
+    return _CASES[curve]
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _engines():
+    yield
+    for cs in _CASES.values():
+        assert {k: cs.g.get_option(k) for k in OPTIONS} == cs.defaults, cs.curve   # every configuration restored its knobs
+        cs.g.close()
+    _CASES.clear()
+
+
+@contextlib.contextmanager
+def knobs(cs, **opts):
+    """set options for one configuration; whatever happens, put back the values the context started with"""
+    try:
+        for k, v in opts.items():
+            cs.g.set_option(k, v)
+        yield
+    finally:
+        for k, v in cs.defaults.items():
+            cs.g.set_option(k, v)
+
+
+def load(cs, opts, rank=0, world=1, pk=None):
+    """re-load the key under the current options and check that the intended geometry is what the library runs"""
+    cs.g.load_proving_key(cs.pk if pk is None else pk, rank, world)
+    cfg = cs.g.config()
+    want = cs.expected(opts, rank, world)
+    assert {k: cfg[k] for k in want} == want, (cs.curve, opts, rank, world)
+    assert (cfg["rank"], cfg["world"]) == (rank, world)
+    return cfg
+
+
+def prove(cs, flags=0):
+    m = cs.m
+    pf = cs.g.create_proof_with_reduction_and_matrices(None, cs.r, cs.s, None, m.num_instance_variables, m.num_constraints,
+                                                        cs.z, flags=flags)
+    return np.concatenate([pf.a, pf.b, pf.c])
+
+
+def run_config(curve, opts, check=None, flags=0):
+    cs = case(curve)
+    with knobs(cs, **opts):
+        cfg = load(cs, opts)
+        if check:
+            check(cfg)
+        assert np.array_equal(prove(cs, flags), cs.want), (curve, opts)
+
+
+# ---- residency plans ------------------------------------------------------------------------------------------------------
+RESIDENCY = ([dict(msm_ne=ne) for ne in (0, 1, 2, 3, 5, 8, 16)] +
+             [dict(msm_ne=1, msm_maxcopies=mc) for mc in (1, 3)] +
+             [dict(msm_ne=1, msm_c=c) for c in (12, 13, 14)])
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("opts", RESIDENCY, ids=lambda o: "-".join(f"{k}{v}" for k, v in o.items()))
+def test_residency_plan(curve, opts):
+    """msm_ne 0 (no copies, c from n), 1 .. 16 effective windows (3 and 5 leave a ragged last copy), a copies cap that forces
+    ne up, and c = 12 / 13 / 14 (22 windows: above the 20-copy cap, so ne = 2; 20 windows: exactly on the cap; 19)."""
+    def check(cfg):
+        if opts.get("msm_ne") == 0:
+            assert cfg["copies"] == 1 and cfg["c"] == 13
+        elif "msm_maxcopies" in opts:
+            assert cfg["copies"] <= opts["msm_maxcopies"] and cfg["ne"] == {1: 16, 3: 6}[opts["msm_maxcopies"]]
+        elif "msm_c" in opts:
+            assert (cfg["c"], cfg["ne"], cfg["copies"]) == {12: (12, 2, 11), 13: (13, 1, 20), 14: (14, 1, 19)}[opts["msm_c"]]
+        else:
+            assert cfg["ne"] == opts["msm_ne"] and cfg["copies"] == -(-16 // opts["msm_ne"])
+    run_config(curve, opts, check)
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+def test_big_key_flow(curve):
+    """bench.py's large-key flow verbatim: setup with msm_ne 0 and proof_slots 1, export, msm_ne 8, re-load, prove.  And the
+    export must not depend on the residency plan: a setup run directly under msm_ne 2 exports the same key (and proves
+    right from the setup-resident key)."""
+    cs = case(curve)
+    g, m = cs.g, cs.m
+    G = GENERATORS[curve]
+    fields = ("a_query", "b_g1_query", "b_g2_query", "h_query", "l_query", "beta_g1", "delta_g1")
+    vk_fields = ("alpha_g1", "beta_g2", "gamma_g2", "delta_g2", "gamma_abc_g1")
+
+    def same_key(a, b):
+        for f in fields:
+            assert np.array_equal(getattr(a, f), getattr(b, f)), f
+        for f in vk_fields:
+            assert np.array_equal(getattr(a.vk, f), getattr(b.vk, f)), f
+
+    try:
+        with knobs(cs, msm_ne=0, proof_slots=1):
+            pk0 = g.generate_parameters_with_qap(m, *TOXIC, G["g1"], G["g2"], export=True)
+            same_key(pk0, cs.pk)
+            g.set_option("msm_ne", 8)
+            load(cs, dict(msm_ne=8, proof_slots=1), pk=pk0)
+            assert np.array_equal(prove(cs), cs.want)
+        with knobs(cs, msm_ne=2):
+            pk2 = g.generate_parameters_with_qap(m, *TOXIC, G["g1"], G["g2"], export=True)
+            cfg = g.config()
+            assert (cfg["ne"], cfg["copies"]) == (2, 8)
+            assert np.array_equal(prove(cs), cs.want)
+            same_key(pk2, cs.pk)
+    finally:
+        g.load_matrices(m)
+        g.load_proving_key(cs.pk)
+
+
+# ---- uneven batched-affine rounds (the shapes of the 2^24 memory guard) ---------------------------------------------------
+UNEVEN = [dict(msm_ba=b1, msm_ba_g2=b2, ba_adaptive=0, share_b_sort=sh)
+          for (b1, b2) in ((4, 0), (0, 4), (4, 2), (2, 4)) for sh in (1, 0)] + \
+         [dict(msm_ba=4, msm_ba_g2=0, ba_adaptive=0, share_b_sort=1, msm_ne=8)]
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("opts", UNEVEN, ids=lambda o: "-".join(f"{k}{v}" for k, v in o.items()))
+def test_uneven_rounds(curve, opts):
+    """B in G1 and B in G2 with different round counts: with share_b_sort 1 they still share one sorted list, padded for the
+    larger count (ba_pad = max), so the MSM with fewer rounds (or none) walks a list longer than its own entries."""
+    def check(cfg):
+        assert (cfg["ba_rounds_g1"], cfg["ba_rounds_g2"]) == (opts["msm_ba"], opts["msm_ba_g2"])
+        assert cfg["ba_rounds_g1"] != cfg["ba_rounds_g2"]
+    run_config(curve, opts, check)
+
+
+# ---- accumulation knobs ---------------------------------------------------------------------------------------------------
+ACCUM = [("acc_k0_g1", v) for v in (4, 24, 128, 1024)] + [("acc_k0_g2", v) for v in (4, 48, 256)] + \
+        [("acc_block", v) for v in (32, 64)]
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("rounds", [1, 0], ids=["rounds", "no_rounds"])
+@pytest.mark.parametrize("knob,value", ACCUM)
+def test_accumulation_knobs(curve, rounds, knob, value):
+    """sorted entries per level-0 thread (any value in 4 .. 1024, powers of two or not, above MSM_K0_MAX too; with rounds the
+    last list runs k0 >> R) and the level-0 block size, with and without the batched-affine rounds"""
+    opts = {knob: value} if rounds else {knob: value, "msm_ba": 0, "msm_ba_g2": 0}
+
+    def check(cfg):
+        assert cfg[{"acc_k0_g1": "k0_g1", "acc_k0_g2": "k0_g2", "acc_block": "acc_block"}[knob]] == value
+        assert (cfg["ba_rounds_g1"] > 0 and cfg["ba_rounds_g2"] > 0) if rounds else (cfg["ba_rounds_g1"] == cfg["ba_rounds_g2"] == 0)
+    run_config(curve, opts, check)
+
+
+def test_knobs_out_of_range_are_refused():
+    """a value the kernels cannot honour is an error, not a silent replacement, and leaves the option unchanged"""
+    cs = case("bn254")
+    bad = [("acc_k0_g1", 3), ("acc_k0_g1", 1025), ("acc_k0_g2", -1), ("acc_k0_g2", 2048), ("acc_block", 100), ("acc_block", 256),
+           ("acc_block", 0), ("msm_ne", -1), ("msm_ne", 33), ("msm_c", -2), ("msm_c", 25), ("msm_maxcopies", 0),
+           ("msm_maxcopies", 21), ("msm_ba", 7), ("msm_ba_g2", -1)]
+    for k, v in bad:
+        before = cs.g.get_option(k)
+        with pytest.raises(ValueError):
+            cs.g.set_option(k, v)
+        assert cs.g.get_option(k) == before, k
+    with pytest.raises(ValueError):
+        cs.g.get_option("no_such_option")
+
+
+# ---- schedules ------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("curve", ALL_CURVES)
+def test_schedules(curve):
+    """witness map first, one proof slot (memory guard recomputed), serialised MSMs and two pipelined proofs under ne = 8"""
+    run_config(curve, dict(wm_first=1))
+    run_config(curve, dict(proof_slots=1))
+    run_config(curve, dict(msm_ne=8), flags=_lib.SERIAL_MSMS)
+    cs = case(curve)
+    with knobs(cs, msm_ne=8):
+        load(cs, dict(msm_ne=8))
+        nq = cs.g.nq
+        outs = [np.zeros(8 * nq, dtype=np.uint64) for _ in range(2)]
+        for slot in (0, 1):
+            cs.g.prove_submit_raw(slot, cs.r, cs.s, cs.z.ctypes.data, 0)
+        for slot in (0, 1):
+            cs.g.prove_wait_raw(slot, outs[slot])
+        for o in outs:
+            assert np.array_equal(o, cs.want)
+
+
+# ---- sharded keys ---------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("world,opts", [(2, {}), (3, {}), (8, {}), (2, dict(msm_ne=4))], ids=["w2", "w3", "w8", "w2-ne4"])
+def test_sharded_key(curve, world, opts):
+    """every rank's round-robin share at its own geometry (2 ranks: rank 0's H shard has 2^16 pairs and runs c = 16, rank 1's
+    has 2^16 - 1 and falls back to the size rule, c = 12), partial sums assembled into the oracle's proof"""
+    cs = case(curve)
+    g = cs.g
+    parts = []
+    try:
+        with knobs(cs, **opts):
+            for rank in range(world):
+                cfg = load(cs, opts, rank, world)
+                if world == 2 and not opts:
+                    assert cfg["c"] == (16 if rank == 0 else 12)
+                out = np.zeros(g.partial_limbs(), dtype=np.uint64)
+                g.prove_partial_raw(cs.r, cs.z.ctypes.data, 0, out)
+                parts.append(out)
+        pf = g.prove_assemble(cs.r, cs.s, np.stack(parts))
+        assert np.array_equal(np.concatenate([pf.a, pf.b, pf.c]), cs.want)
+    finally:
+        g.load_proving_key(cs.pk)
+
+
+# ---- adversarial bases and signed-digit edge scalars at the resident geometry ----------------------------------------------
+def edge_scalars(r, c):
+    """canonical scalars at the signed-digit boundaries of c-bit windows"""
+    bits = r.bit_length()
+    B = 1 << (c - 1)
+    out = {0, 1, r - 1, r - 2, (r - 1) // 2, 1 << (bits - 1)}
+    for digit in (B, B + 1, B - 1, (1 << c) - 1):
+        v = 0
+        for k in range(bits // c + 2):
+            v += digit << (c * k)
+            out.add(v % r)
+            if v < r:
+                out.add(v)
+    for k in range(1, bits // c + 2):
+        out.add(((1 << (c * k)) - 1) % r)
+        out.add((1 << (c * k)) % r)
+    return sorted(out)
+
+
+def _neg_points(cd, cx, arr, g2):
+    pts = cd.dec_g2(arr) if g2 else cd.dec_g1(arr)
+    G = cx.G2 if g2 else cx.G1
+    return cd.enc_g2([G.neg(p) for p in pts]) if g2 else cd.enc_g1([G.neg(p) for p in pts])
+
+
+_ADV = {}
+
+
+def adversarial(curve):
+    """key with duplicate / opposite base pairs (equal scalars: the pair meets in one bucket in every window) and identity
+    runs longer than a batched-affine tile in all five queries, an assignment of edge scalars for c = 13 and c = 16, and the
+    oracle's five MSMs over it"""
+    if curve in _ADV:
+        return _ADV[curve]
+    cs = case(curve)
+    cd = cs.g.codec
+    cx = P.ctx(curve)
+    cid, nq = cd.c.cid, cd.nq
+    ni = cs.m.num_instance_variables
+    nv = ni + cs.m.num_witness_variables
+    z = cs.z.copy()
+    edges = edge_scalars(cd.c.r, 16) + edge_scalars(cd.c.r, 13)
+    z[4000:4000 + len(edges)] = cd.fr.enc(edges)
+    rs = np.random.RandomState(5)
+    q = {f: np.array(getattr(cs.pk, f), copy=True) for f in ("a_query", "b_g1_query", "b_g2_query", "h_query", "l_query")}
+
+    # base pairs (i, i + 1): duplicates from 1000, opposites from 2000; the same positions in every query, so that b_g1 and
+    # b_g2 keep one identity pattern (shared sorted list).  Scalars: a / b base k <-> z[k], l base k <-> z[ni + k]; the h
+    # scalars come from the witness map.
+    dup = np.arange(1000, 1600, 2)
+    opp = np.arange(2000, 2600, 2)
+    for name, Q in q.items():
+        Q[dup + 1] = Q[dup]
+        Q[opp + 1] = _neg_points(cd, cx, Q[opp], name == "b_g2_query")
+        Q[3000:3000 + 700] = 0                  # identity runs
+        Q[5000:5000 + 3] = 0
+    for first in (1000, 2000):
+        for k in range(first, first + 600, 2):
+            for off in (0, ni):
+                v = edges[(k // 2) % len(edges)] if k % 4 == 0 else int(rs.randint(1, 1 << 62))
+                z[k + off] = z[k + 1 + off] = cd.fr.enc1(v % cd.c.r)
+    pk = type(cs.pk)(cs.pk.vk, cs.pk.beta_g1, cs.pk.delta_g1, q["a_query"], q["b_g1_query"], q["b_g2_query"], q["h_query"],
+                     q["l_query"])
+    zc = cd.fr.bigint(cd.fr.dec(z))
+    h = orc.witness_map(cid, cs.m, z, threads=THREADS)
+    want = [orc.msm_g1(cid, nq, q["h_query"], cd.fr.bigint(cd.fr.dec(h)), THREADS),
+            orc.msm_g1(cid, nq, q["l_query"], zc[ni:], THREADS),
+            orc.msm_g1(cid, nq, q["a_query"].reshape(nv, -1)[1:], zc[1:], THREADS),
+            orc.msm_g1(cid, nq, q["b_g1_query"].reshape(nv, -1)[1:], zc[1:], THREADS),
+            orc.msm_g2(cid, nq, q["b_g2_query"].reshape(nv, -1)[1:], zc[1:], THREADS)]
+    _ADV[curve] = (pk, np.ascontiguousarray(z), want)
+    return _ADV[curve]
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("ne", [0, 1, 8])
+@pytest.mark.parametrize("rounds", [1, 0], ids=["rounds", "no_rounds"])
+def test_adversarial_partials(curve, ne, rounds):
+    """tangent (P + P) and cancellation (P - P) cases inside one bucket of the device rounds, G1 and G2, identity runs, and
+    the carry chains of edge scalars at c = 13 (ne 0) and c = 16: every partial MSM against the oracle's msm_bigint"""
+    cs = case(curve)
+    pk, z, want = adversarial(curve)
+    nq = cs.g.nq
+    opts = dict(msm_ne=ne, ba_adaptive=0, msm_ba=4 if rounds else 0, msm_ba_g2=4 if rounds else 0)
+    try:
+        with knobs(cs, **opts):
+            cfg = load(cs, opts, pk=pk)
+            assert cfg["c"] == (13 if ne == 0 else 16)
+            out = np.zeros(cs.g.partial_limbs(), dtype=np.uint64)
+            cs.g.prove_partial_raw(cs.r, z.ctypes.data, 0, out)
+    finally:
+        cs.g.load_proving_key(cs.pk)
+    for k, w in enumerate(want):
+        width = (4 if k == M_B2 else 2) * nq
+        got = out[2 * nq * k:2 * nq * k + width]
+        if not w[width:].any():                 # identity: projective Z = 0, affine all-zero
+            assert not got.any(), (curve, ne, rounds, k)
+        else:
+            assert np.array_equal(got, w[:width]), (curve, ne, rounds, k)
+
+
+# ---- stand-alone g16_msm_g1 / g2 above 2^15 pairs ---------------------------------------------------------------------------
+def _msm_inputs(curve, n, c, g2=False):
+    """n bases taken from the module key (tiled when n exceeds it), with duplicates, opposites and identities; edge scalars
+    for c-bit windows, equal scalars on the duplicate / opposite pairs, uniform-looking canonical scalars elsewhere"""
+    cs = case(curve)
+    cd = cs.g.codec
+    cx = P.ctx(curve)
+    if g2:
+        src = np.asarray(cs.pk.b_g2_query)
+    else:
+        src = np.concatenate([np.asarray(cs.pk.h_query), np.asarray(cs.pk.l_query)])
+    bases = np.ascontiguousarray(np.resize(src, (n, src.shape[1])))
+    bases[101:401:2] = bases[100:400:2]
+    bases[501:801:2] = _neg_points(cd, cx, bases[500:800:2], g2)
+    bases[900:1200] = 0
+    rs = np.random.RandomState(n + c)
+    sc = rs.randint(0, 1 << 62, size=(n, 4), dtype=np.int64).astype(np.uint64)
+    sc[:, 3] &= np.uint64((1 << 58) - 1)
+    edges = edge_scalars(cd.c.r, c)
+    sc[2000:2000 + len(edges)] = cd.fr.bigint(edges)
+    sc[101:401:2] = sc[100:400:2]
+    sc[501:801:2] = sc[500:800:2]
+    sc[3000:3100] = 0
+    return bases, np.ascontiguousarray(sc)
+
+
+def _check_msm(curve, n, c_expect, g2=False, msm_c=0):
+    cs = case(curve)
+    cd = cs.g.codec
+    bases, sc = _msm_inputs(curve, n, c_expect, g2)
+    assert msm_c or _pick_c(n) == c_expect
+    with knobs(cs, msm_c=msm_c):
+        got = cs.g.msm_g2(bases, sc) if g2 else cs.g.msm_g1(bases, sc)
+    want = (orc.msm_g2 if g2 else orc.msm_g1)(cd.c.cid, cd.nq, bases, sc, THREADS)
+    assert np.array_equal(got, want), (curve, n, c_expect, g2)
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("n,c", [((1 << 16) - 1, 12), ((1 << 16) + 1, 13), ((1 << 17) + 3, 14)])
+def test_standalone_msm_g1(curve, n, c):
+    """no precomputation: W bucket sets of 2^(c-1) buckets each, scans over many blocks"""
+    _check_msm(curve, n, c)
+
+
+def test_standalone_msm_g1_c16():
+    """2^20 pairs: c = 16, 16 bucket sets of 2^15 buckets, batched-affine rounds on a caller-supplied base array"""
+    _check_msm("bls12_381", 1 << 20, 16)
+
+
+def test_standalone_msm_g2():
+    _check_msm("bls12_377", (1 << 16) + 1, 13, g2=True)
+
+
+@pytest.mark.parametrize("msm_c", [17, 20])
+def test_standalone_msm_wide_windows(msm_c):
+    """msm_c above 16 (the header allows 24): at c = 20 there are 13 x 2^19 keys, 1664 scan blocks, and msm_scan_tops loops
+    over its 1024-wide block scan twice"""
+    _check_msm("bn254", 1 << 16, msm_c, msm_c=msm_c)

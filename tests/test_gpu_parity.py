@@ -307,7 +307,8 @@ def test_msm_skewed_scalars_large():
     _skewed_msm_check()
 
 
-LEAN_DEFAULT = (0, 0)   # Engine::Tune::ba_occ_g1 / ba_occ_g2
+_BA_OPTIONS = ("msm_ba", "msm_ba_g2", "ba_min_entries_g1", "ba_min_entries_g2", "ba_adaptive", "ba_m", "ba_g", "ba_inv_gcd",
+               "ba_occ_g1", "ba_occ_g2", "ba_cap_fwd_g1", "ba_cap_bwd_g1", "ba_cap_fwd_g2", "ba_cap_bwd_g2")
 
 
 def _set_ba(rounds_g1, rounds_g2, min_entries=0, **kw):
@@ -334,18 +335,17 @@ def test_batched_affine_rounds(rounds, m, G, gcd, lean):
     import orc
     from groth16_b200.params import GENERATORS
     from groth16_b200.workload import dummy_r1cs, synthetic_r1cs
+    saved = {name: {k: engine(name).get_option(k) for k in _BA_OPTIONS} for name in ALL_CURVES}   # whatever the engines hold now
     try:
         cap = 1 if lean == 2 else 0
         _set_ba(rounds, rounds, ba_m=m, ba_g=G, ba_inv_gcd=gcd, ba_occ_g1=int(lean == 1), ba_occ_g2=int(lean == 1),
                 ba_cap_fwd_g1=cap, ba_cap_bwd_g1=cap, ba_cap_fwd_g2=cap, ba_cap_bwd_g2=cap)
         _ba_body(orc, GENERATORS, dummy_r1cs, synthetic_r1cs)
     finally:
-        _set_ba(4, 5, ba_m=32, ba_g=16, ba_inv_gcd=1, ba_occ_g1=LEAN_DEFAULT[0], ba_occ_g2=LEAN_DEFAULT[1],
-                ba_cap_fwd_g1=0, ba_cap_bwd_g1=0, ba_cap_fwd_g2=0, ba_cap_bwd_g2=0)   # the library defaults (Engine::Tune) ...
-        for name in ALL_CURVES:
-            engine(name).set_option("ba_min_entries_g1", 1 << 19)
-            engine(name).set_option("ba_min_entries_g2", 1 << 19)
-            engine(name).set_option("ba_adaptive", 1)
+        for name, opts in saved.items():
+            for k, v in opts.items():
+                engine(name).set_option(k, v)
+        assert {k: engine("bn254").get_option(k) for k in _BA_OPTIONS} == saved["bn254"]
 
 
 def _ba_body(orc, GENERATORS, dummy_r1cs, synthetic_r1cs):

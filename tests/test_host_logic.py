@@ -134,7 +134,8 @@ def test_ec_host_backend(tmp_path):
 def test_msm_reduction_plan_host(tmp_path):
     """msm.cuh: the bucket-reduction plan (row / column sum tree, array layout) and its host recombination
     (MsmHostRed::T, msm_finish), the window / copies geometry and the entries-per-thread rule -- built by nvcc, executed on
-    the CPU only, for bucket counts 2^2 .. 2^13 and 1 or 3 effective windows."""
+    the CPU only, for bucket counts 2^2 .. 2^13 with 1 or 3 effective windows and 2^14 / 2^15 (the production bucket count)
+    with 1, 2, 8 or 16."""
     import shutil
     if shutil.which("nvcc") is None:
         pytest.skip("nvcc not available")
@@ -143,7 +144,7 @@ def test_msm_reduction_plan_host(tmp_path):
                            os.path.join(ROOT, "tests", "host", "msm_plan_check.cu")])
     out = subprocess.run([exe], capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
-    assert "18 cases, 0 mismatches" in out.stdout
+    assert "26 cases, 0 mismatches" in out.stdout
 
 
 def test_batched_affine_rounds_host(tmp_path):
