@@ -36,7 +36,7 @@ class Timings(C.Structure):
 
 class Config(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("c", "ne", "copies", "k0_g1", "k0_g2", "ba_rounds_g1", "ba_rounds_g2", "ba_m", "ba_g",
-                                         "ba_inv_gcd", "acc_block", "sm_count", "rank", "world", "ba_lean_g1", "ba_lean_g2")] + [("reserved", C.c_int32 * 2)]
+                                         "ba_inv_gcd", "acc_block", "sm_count", "rank", "world")] + [("reserved", C.c_int32 * 4)]
 
 
 # every symbol include/g16b200.h declares: (name, restype, argtypes)

@@ -8,7 +8,10 @@
 #include <nvtx3/nvToolsExt.h>       // header-only NVTX v3: no-ops unless a profiler injects itself
 #include <nvtx3/nvToolsExtCudaRt.h>
 #include <algorithm>
+#include <cctype>
+#include <cerrno>
 #include <chrono>
+#include <climits>
 #include <cstdlib>
 #include <cstdio>
 #include <condition_variable>
@@ -22,7 +25,7 @@
 #include "../../include/g16b200.h"
 #include "ec.cuh"
 #include "msm.cuh"
-#include "ntt_tma.cuh"
+#include "ntt.cuh"
 
 namespace g16 {
 
@@ -233,77 +236,126 @@ struct Engine : IEngine {
     uint64_t lo = 0, hi = 0;   // this rank owns pairs lo, lo + world, lo + 2 world, ... : hi - lo of them (lo = rank)
     MsmGeom geom{};
   } q[5];
-  // MSM tuning knobs: defaults below, overridden at context creation by the environment (G16_MSM_C, G16_MSM_NE,
-  // G16_MSM_MAXCOPIES, G16_MSM_BA, G16_MSM_BA_G2, G16_BA_M, G16_BA_G, G16_BA_INV_GCD, G16_ACC_K0_G1, G16_ACC_K0_G2,
-  // G16_ACC_BLOCK) and at run time by g16_set_option (same names, lower case, without the G16_ prefix).
-  int cfg_c = 0;          // 0 = pick from n
-  int cfg_ne = 1;         // effective windows with precomputed bases; 0 = no precomputation
-  int cfg_maxcopies = MSM_MAX_COPIES;
+  // Tuning options: defaults below (from sweeps of a full proof at 2^20, tools/sweep.py), overridden at context creation by
+  // the environment and at run time by g16_set_option.  options() lists them.
   struct Tune {
-    // defaults from sweeps of a full proof at 2^20 (tools/sweep.py)
-    int ba_g1 = 4;        // batched-affine rounds before the XYZZ accumulation, G1 MSMs with >= 2^18 entries
-    int ba_g2 = 4;        // same for the G2 MSM (on an H100 a fifth round costs more than it saves)
-    int ba_m = 32;        // additions per thread and round
-    int ba_G = 16;        // thread products per inversion
-    int ba_gcd = 1;       // safegcd inversion
-    int k0_g1 = 0;        // sorted entries per accumulation thread (0 = automatic)
-    int k0_g2 = 0;
-    int acc_block = 128;
-    int ba_occ_g2 = 0;    // != 0: register-lean Fq2 round kernels, 3 resident blocks per SM (168 registers; msm_ba.cuh)
-    int ba_occ_g1 = 0;    // != 0: register-lean G1 round kernels, 5 resident blocks per SM
-    int ba_cap_fwd_g1 = 0, ba_cap_bwd_g1 = 0;   // blocks per SM of a forward / backward round launch (0 = one block per tile)
-    int ba_cap_fwd_g2 = 0, ba_cap_bwd_g2 = 0;
+    long long c = 0;          // window bits; 0 = pick from n
+    long long ne = 1;         // effective windows with precomputed bases; 0 = no precomputation
+    long long maxcopies = MSM_MAX_COPIES;
+    long long ba_g1 = 4;      // batched-affine rounds before the XYZZ accumulation, G1 MSMs with >= 2^18 entries
+    long long ba_g2 = 4;      // same for the G2 MSM (on an H100 a fifth round costs more than it saves)
+    long long ba_m = 32;      // additions per thread and round
+    long long ba_G = 16;      // thread products per inversion
+    long long ba_gcd = 1;     // safegcd inversion
+    long long k0_g1 = 0;      // sorted entries per accumulation thread (0 = automatic)
+    long long k0_g2 = 0;
+    long long acc_block = 128;
     // Smallest MSM (in bucket entries) that runs the rounds, and how many: a round halves a list whose buckets hold
     // `entries / buckets` slots on average and pads every bucket to 2^R slots, so R is the smallest value with
     // 11 * 2^R >= that average, capped by ba_g1 / ba_g2 (4 / 4 at
     // 2^20 pairs on one GPU, 3 on the 2.1 M-entry shards of an 8-way proof, 2 on its 1.0 M-entry A / B shards).
     long long ba_min_g1 = 1ll << 19;
     long long ba_min_g2 = 1ll << 19;
-    int ba_adaptive = 1;  // 0: exactly ba_g1 / ba_g2 rounds whatever the bucket occupancy (tests)
+    long long ba_adaptive = 1;   // 0: exactly ba_g1 / ba_g2 rounds whatever the bucket occupancy (tests)
+    long long share_b_sort = 1;  // let B-in-G2 borrow B-in-G1's sorted list when the keys allow it
+    // 1 / 0 / -1 = automatic (sharded keys): hold the MSM accumulations back until the witness map is done.  Off: with
+    // enough hardware work queues (CUDA_DEVICE_MAX_CONNECTIONS, see api.cu) the witness map is not held up, and delaying
+    // the other accumulations then only idles the GPU
+    long long wm_first = 0;
+    long long wm_split = 1;      // sharded proofs with a communicator: spread the witness map over the ranks
+    long long proof_slots = NSLOTS;   // slots the caller will use (1 halves the workspace the key must leave room for)
   } tune;
+  // What a change of an option must redo.
+  enum OptEffect {
+    OPT_GEOM,        // re-derive the launch geometry of the resident key now
+    OPT_NEXT_KEY,    // nothing: read at the next g16_pk_load / g16_setup
+    OPT_B_SORT,      // re-decide whether B-in-G2 borrows B-in-G1's sorted list
+    OPT_BA_MEMORY,   // re-decide which MSMs' round work lists fit in device memory
+    OPT_NONE         // nothing: read by every proof
+  };
+  struct OptRange { long long lo, hi; };
+  struct Option {
+    const char* name;          // g16_set_option key; the environment variable is G16_<NAME IN UPPER CASE>
+    long long Tune::*value;
+    std::vector<OptRange> ok;  // accepted values: the union of these closed ranges
+    OptEffect effect;
+  };
+  static const std::vector<Option>& options() {
+    static const std::vector<Option> t = {
+        {"msm_ne", &Tune::ne, {{0, 32}}, OPT_NEXT_KEY},
+        {"msm_c", &Tune::c, {{0, 24}}, OPT_NEXT_KEY},
+        {"msm_maxcopies", &Tune::maxcopies, {{1, MSM_MAX_COPIES}}, OPT_NEXT_KEY},
+        {"msm_ba", &Tune::ba_g1, {{0, MSM_BA_MAX_ROUNDS}}, OPT_GEOM},
+        {"msm_ba_g2", &Tune::ba_g2, {{0, MSM_BA_MAX_ROUNDS}}, OPT_GEOM},
+        {"ba_m", &Tune::ba_m, {{1, 256}}, OPT_GEOM},
+        {"ba_g", &Tune::ba_G, {{1, 4096}}, OPT_GEOM},
+        {"ba_min_entries_g1", &Tune::ba_min_g1, {{0, LLONG_MAX}}, OPT_GEOM},
+        {"ba_min_entries_g2", &Tune::ba_min_g2, {{0, LLONG_MAX}}, OPT_GEOM},
+        {"acc_k0_g1", &Tune::k0_g1, {{0, 0}, {4, 1024}}, OPT_GEOM},
+        {"acc_k0_g2", &Tune::k0_g2, {{0, 0}, {4, 1024}}, OPT_GEOM},
+        {"acc_block", &Tune::acc_block, {{32, 32}, {64, 64}, {128, 128}}, OPT_GEOM},
+        {"ba_inv_gcd", &Tune::ba_gcd, {{0, 1}}, OPT_GEOM},
+        {"ba_adaptive", &Tune::ba_adaptive, {{0, 1}}, OPT_GEOM},
+        {"share_b_sort", &Tune::share_b_sort, {{0, 1}}, OPT_B_SORT},
+        {"wm_first", &Tune::wm_first, {{-1, 1}}, OPT_NONE},
+        {"wm_split", &Tune::wm_split, {{0, 1}}, OPT_NONE},
+        {"proof_slots", &Tune::proof_slots, {{1, NSLOTS}}, OPT_BA_MEMORY},
+    };
+    return t;
+  }
+  static const Option* find_option(const std::string& name) {
+    for (const Option& o : options())
+      if (name == o.name) return &o;
+    return nullptr;
+  }
+  static bool accepts(const Option& o, long long v) {
+    for (const OptRange& r : o.ok)
+      if (v >= r.lo && v <= r.hi) return true;
+    return false;
+  }
+  static std::string accepted(const Option& o) {   // e.g. "0, 4 .. 1024"
+    std::string s;
+    for (const OptRange& r : o.ok) {
+      s += (s.empty() ? "" : ", ") + std::to_string(r.lo);
+      if (r.hi > r.lo) s += " .. " + (r.hi == LLONG_MAX ? std::string() : std::to_string(r.hi));
+    }
+    return s;
+  }
   MsmGeom pick_geom(uint64_t cnt) const {
-    if (cfg_ne <= 0) return msm_geom(cnt, FR_BITS, cfg_c, 0);
+    if (tune.ne <= 0) return msm_geom(cnt, FR_BITS, (int)tune.c, 0);
     // with all windows sharing one bucket set the bucket count is 2^(c-1) whatever the size: c = 16 from 2^16 pairs up
     // (also for the per-rank shards of a multi-GPU run), the size-based rule below that
-    const int c = cfg_c > 0 ? cfg_c : (cnt >= (1u << 16) ? 16 : 0);
-    MsmGeom g = msm_geom(cnt, FR_BITS, c, cfg_ne);
-    int ne = cfg_ne;
-    while (g.copies > cfg_maxcopies) g = msm_geom(cnt, FR_BITS, c, ++ne);
+    const int c = tune.c > 0 ? (int)tune.c : (cnt >= (1u << 16) ? 16 : 0);
+    int ne = (int)tune.ne;
+    MsmGeom g = msm_geom(cnt, FR_BITS, c, ne);
+    while (g.copies > tune.maxcopies) g = msm_geom(cnt, FR_BITS, c, ++ne);
     return g;
   }
   // entries per level-0 thread, from the number of resident accumulation threads of this device
   int sm_count = 132;
-  int proof_slots = NSLOTS;   // slots the caller will use (g16_set_option "proof_slots" 1 halves the workspace the key must leave room for)
   bool ba_allowed = true;   // cleared by pk_load / setup when the rounds' work lists would not fit in device memory
   uint32_t ba_allowed_mask = 0x1f;   // per MSM (bit m): the work lists of MSM m fit next to the key and the other MSMs' lists
   MsmGeom with_k0(MsmGeom g, bool g2, int m = -1) const {
     g.k0 = msm_pick_k0(g.max_entries, (uint64_t)sm_count * 128 * (g2 ? 2 : 3), g2 ? 16 : 8);
     // G2 additions are ~3x longer: 32 entries per thread (twice the thread count) shortens the last partial wave (-13 %)
     if (g2 && g.k0 > 32) g.k0 = 32;
-    const int k = g2 ? tune.k0_g2 : tune.k0_g1;
+    const int k = (int)(g2 ? tune.k0_g2 : tune.k0_g1);
     if (k >= 4 && k <= 1024) g.k0 = k;
     // batched-affine pre-reduction (msm_ba.cuh) for MSMs with at least 2^18 entries
-    const int r = g2 ? tune.ba_g2 : tune.ba_g1;
+    const int r = (int)(g2 ? tune.ba_g2 : tune.ba_g1);
     const bool allowed = ba_allowed && (m < 0 || ((ba_allowed_mask >> m) & 1));
     const uint64_t min_entries = (uint64_t)std::max(1ll << 18, g2 ? tune.ba_min_g2 : tune.ba_min_g1);
     int r_fit = 0;   // smallest R with 11 * 2^R >= average entries per bucket
     for (uint64_t per_bucket = g.max_entries / std::max<uint64_t>(1, g.nkeys); (11ull << r_fit) < per_bucket; r_fit++) {}
     if (!tune.ba_adaptive) r_fit = r;
     g.ba = (allowed && r > 0 && g.max_entries >= min_entries) ? std::min(std::min(r, r_fit), (int)MSM_BA_MAX_ROUNDS) : 0;
-    g.ba_m = tune.ba_m;
-    g.ba_G = tune.ba_G;
-    g.ba_gcd = tune.ba_gcd;
-    g.acc_block = tune.acc_block;
-    g.ba_occ = g2 ? tune.ba_occ_g2 : tune.ba_occ_g1;
-    g.ba_grid_fwd = sm_count * (g2 ? tune.ba_cap_fwd_g2 : tune.ba_cap_fwd_g1);
-    g.ba_grid_bwd = sm_count * (g2 ? tune.ba_cap_bwd_g2 : tune.ba_cap_bwd_g1);
+    g.ba_m = (int)tune.ba_m;
+    g.ba_G = (int)tune.ba_G;
+    g.ba_gcd = (int)tune.ba_gcd;
+    g.acc_block = (int)tune.acc_block;
     return g;
   }
-  int wm_first_opt = 0;        // g16_set_option "wm_first": 1 / 0 / -1 = automatic (sharded keys).  Off: with enough hardware work
-                               // queues (CUDA_DEVICE_MAX_CONNECTIONS, see api.cu) the witness map is not held up, and delaying the
-                               // other accumulations then only idles the GPU
   bool share_b_sort = false;   // set when a key is made resident: b_g1_query and b_g2_query have the same identity pattern
-  bool share_b_sort_wanted = true;
   void refresh_geoms() {   // after a knob changed: same shards, new launch geometry
     for (int m = 0; m < 5; m++)
       if (q[m].hi > q[m].lo) q[m].geom = with_k0(q[m].geom, m == M_B2, m);
@@ -318,7 +370,7 @@ struct Engine : IEngine {
     share_b_sort = false;
     const Query &x = q[M_B1], &y = q[M_B2];
     const uint64_t cnt = x.hi - x.lo;
-    if (share_b_sort_wanted && cnt > 0 && cnt == y.hi - y.lo && x.lo == y.lo && x.geom.c == y.geom.c && x.geom.ne == y.geom.ne &&
+    if (tune.share_b_sort && cnt > 0 && cnt == y.hi - y.lo && x.lo == y.lo && x.geom.c == y.geom.c && x.geom.ne == y.geom.ne &&
         x.geom.copies == y.geom.copies) {
       std::vector<uint8_t> mx(cnt), my(cnt);
       G16_CUDA(cudaMemcpy(mx.data(), x.mask.p, cnt, cudaMemcpyDeviceToHost));
@@ -358,7 +410,7 @@ struct Engine : IEngine {
       bp.make(q[m].geom);
       const uint64_t need = ((m == M_B2) ? bp.template extra_bytes<Fq2>() : bp.template extra_bytes<Fq>()) +
                             (bp.len[0] - q[m].geom.max_entries) * 8;   // bucket padding of the sorted arrays
-      if ((uint64_t)proof_slots * (plain + used + need) + margin <= fr) { used += need; mask |= 1u << m; }
+      if ((uint64_t)tune.proof_slots * (plain + used + need) + margin <= fr) { used += need; mask |= 1u << m; }
     }
     ba_allowed_mask = mask;
     refresh_geoms();
@@ -366,78 +418,29 @@ struct Engine : IEngine {
   int set_option(const char* key, long long v) override {
     if (any_busy()) return fail(G16_ERR_BAD_ARGUMENT, "a proof is in flight");
     const std::string k(key ? key : "");
-    // values the launch geometry cannot honour are refused rather than silently replaced
-    auto out_of_range = [&](long long lo, long long hi) {
-      return fail(G16_ERR_BAD_ARGUMENT, "option " + k + " = " + std::to_string(v) + " outside [" + std::to_string(lo) + ", " +
-                                            std::to_string(hi) + "]");
-    };
-    if ((k == "msm_ba" || k == "msm_ba_g2") && (v < 0 || v > MSM_BA_MAX_ROUNDS)) return out_of_range(0, MSM_BA_MAX_ROUNDS);
-    if ((k == "acc_k0_g1" || k == "acc_k0_g2") && v != 0 && (v < 4 || v > 1024))
-      return fail(G16_ERR_BAD_ARGUMENT, "option " + k + " must be 0 (automatic) or in [4, 1024]");
-    if (k == "acc_block" && v != 32 && v != 64 && v != 128) return fail(G16_ERR_BAD_ARGUMENT, "option acc_block must be 32, 64 or 128");
-    if (k == "msm_ne" && (v < 0 || v > 32)) return out_of_range(0, 32);
-    if (k == "msm_c" && (v < 0 || v > 24)) return out_of_range(0, 24);
-    if (k == "msm_maxcopies" && (v < 1 || v > MSM_MAX_COPIES)) return out_of_range(1, MSM_MAX_COPIES);
-    if (k == "msm_ba") tune.ba_g1 = (int)v;
-    else if (k == "msm_ba_g2") tune.ba_g2 = (int)v;
-    else if (k == "ba_m") tune.ba_m = (int)std::max(1ll, std::min(v, 256ll));
-    else if (k == "ba_g") tune.ba_G = (int)std::max(1ll, std::min(v, 4096ll));
-    else if (k == "ba_inv_gcd") tune.ba_gcd = v ? 1 : 0;
-    else if (k == "acc_k0_g1") tune.k0_g1 = (int)v;
-    else if (k == "acc_k0_g2") tune.k0_g2 = (int)v;
-    else if (k == "acc_block") tune.acc_block = (int)v;
-    else if (k == "ba_occ_g2") tune.ba_occ_g2 = v != 0 ? 3 : 0;
-    else if (k == "ba_occ_g1") tune.ba_occ_g1 = v != 0 ? 5 : 0;
-    else if (k == "ba_cap_fwd_g1") tune.ba_cap_fwd_g1 = (int)std::max(0ll, std::min(v, 16ll));
-    else if (k == "ba_cap_bwd_g1") tune.ba_cap_bwd_g1 = (int)std::max(0ll, std::min(v, 16ll));
-    else if (k == "ba_cap_fwd_g2") tune.ba_cap_fwd_g2 = (int)std::max(0ll, std::min(v, 16ll));
-    else if (k == "ba_cap_bwd_g2") tune.ba_cap_bwd_g2 = (int)std::max(0ll, std::min(v, 16ll));
-    else if (k == "ba_adaptive") tune.ba_adaptive = v ? 1 : 0;
-    else if (k == "ba_min_entries_g1") tune.ba_min_g1 = std::max(0ll, v);
-    else if (k == "ba_min_entries_g2") tune.ba_min_g2 = std::max(0ll, v);
-    else if (k == "ntt_tma") { use_ntt_tma = v < 0 ? -1 : (v != 0 ? 1 : 0); return G16_OK; }
-    else if (k == "wm_first") { wm_first_opt = v < 0 ? -1 : (v ? 1 : 0); return G16_OK; }
-    else if (k == "wm_split") { split_wm_wanted = v != 0; return G16_OK; }
-    else if (k == "proof_slots") { proof_slots = v <= 1 ? 1 : NSLOTS; if (have_pk) decide_ba_memory(); return G16_OK; }
-    // residency knobs: take effect at the NEXT g16_pk_load / g16_setup (they decide how many precomputed multiples a key keeps)
-    else if (k == "msm_ne") { cfg_ne = (int)v; return G16_OK; }
-    else if (k == "msm_c") { cfg_c = (int)v; return G16_OK; }
-    else if (k == "msm_maxcopies") { cfg_maxcopies = (int)v; return G16_OK; }
-    else if (k == "share_b_sort") { share_b_sort_wanted = v != 0; if (have_pk) { int rc = decide_b_sort_sharing(); if (rc) return rc; } }
-    else return fail(G16_ERR_BAD_ARGUMENT, "unknown option: " + k);
-    refresh_geoms();
+    const Option* o = find_option(k);
+    if (!o) return fail(G16_ERR_BAD_ARGUMENT, "unknown option: " + k);
+    if (!accepts(*o, v))
+      return fail(G16_ERR_BAD_ARGUMENT, "option " + k + " = " + std::to_string(v) + " is not one of " + accepted(*o));
+    tune.*o->value = v;
+    switch (o->effect) {
+      case OPT_GEOM: refresh_geoms(); break;
+      case OPT_B_SORT:
+        if (have_pk) { int rc = decide_b_sort_sharing(); if (rc) return rc; }
+        refresh_geoms();
+        break;
+      case OPT_BA_MEMORY: if (have_pk) decide_ba_memory(); break;
+      case OPT_NEXT_KEY: case OPT_NONE: break;
+    }
     return G16_OK;
   }
   // the value an option holds now, in the form g16_set_option accepts (set_option(k, get_option(k)) changes nothing)
   int get_option(const char* key, long long* out) const override {
     if (!out) return fail(G16_ERR_BAD_ARGUMENT, "null out");
     const std::string k(key ? key : "");
-    if (k == "msm_ba") *out = tune.ba_g1;
-    else if (k == "msm_ba_g2") *out = tune.ba_g2;
-    else if (k == "ba_m") *out = tune.ba_m;
-    else if (k == "ba_g") *out = tune.ba_G;
-    else if (k == "ba_inv_gcd") *out = tune.ba_gcd;
-    else if (k == "acc_k0_g1") *out = tune.k0_g1;
-    else if (k == "acc_k0_g2") *out = tune.k0_g2;
-    else if (k == "acc_block") *out = tune.acc_block;
-    else if (k == "ba_occ_g2") *out = tune.ba_occ_g2;
-    else if (k == "ba_occ_g1") *out = tune.ba_occ_g1;
-    else if (k == "ba_cap_fwd_g1") *out = tune.ba_cap_fwd_g1;
-    else if (k == "ba_cap_bwd_g1") *out = tune.ba_cap_bwd_g1;
-    else if (k == "ba_cap_fwd_g2") *out = tune.ba_cap_fwd_g2;
-    else if (k == "ba_cap_bwd_g2") *out = tune.ba_cap_bwd_g2;
-    else if (k == "ba_adaptive") *out = tune.ba_adaptive;
-    else if (k == "ba_min_entries_g1") *out = tune.ba_min_g1;
-    else if (k == "ba_min_entries_g2") *out = tune.ba_min_g2;
-    else if (k == "ntt_tma") *out = use_ntt_tma;
-    else if (k == "wm_first") *out = wm_first_opt;
-    else if (k == "wm_split") *out = split_wm_wanted ? 1 : 0;
-    else if (k == "proof_slots") *out = proof_slots;
-    else if (k == "msm_ne") *out = cfg_ne;
-    else if (k == "msm_c") *out = cfg_c;
-    else if (k == "msm_maxcopies") *out = cfg_maxcopies;
-    else if (k == "share_b_sort") *out = share_b_sort_wanted ? 1 : 0;
-    else return fail(G16_ERR_BAD_ARGUMENT, "unknown option: " + k);
+    const Option* o = find_option(k);
+    if (!o) return fail(G16_ERR_BAD_ARGUMENT, "unknown option: " + k);
+    *out = tune.*o->value;
     return G16_OK;
   }
   int get_config(g16_config* o) const override {
@@ -448,10 +451,9 @@ struct Engine : IEngine {
     o->c = g1.c; o->ne = g1.ne; o->copies = g1.copies;
     o->k0_g1 = g1.k0; o->k0_g2 = g2.k0;
     o->ba_rounds_g1 = g1.ba; o->ba_rounds_g2 = g2.ba;
-    o->ba_m = tune.ba_m; o->ba_g = tune.ba_G; o->ba_inv_gcd = tune.ba_gcd; o->acc_block = tune.acc_block;
+    o->ba_m = (int32_t)tune.ba_m; o->ba_g = (int32_t)tune.ba_G; o->ba_inv_gcd = (int32_t)tune.ba_gcd; o->acc_block = (int32_t)tune.acc_block;
     o->sm_count = sm_count;
     o->world = (int32_t)world; o->rank = (int32_t)rank;
-    o->ba_lean_g1 = g1.ba_occ != 0; o->ba_lean_g2 = g2.ba_occ != 0;
     return G16_OK;
   }
   template <class F>
@@ -479,28 +481,19 @@ struct Engine : IEngine {
     if (prop.major != 9 || prop.minor != 0)
       return fail(G16_ERR_CUDA, "device is not sm_90 (this library ships sm_90a code only, for the H100)");
     sm_count = prop.multiProcessorCount;
+    for (const Option& o : options()) {
+      std::string var = "G16_";
+      for (const char* p = o.name; *p; p++) var += (char)toupper(*p);
+      const char* s = getenv(var.c_str());
+      if (!s) continue;
+      char* end = nullptr;
+      errno = 0;
+      const long long v = strtoll(s, &end, 10);
+      if (end == s || *end || errno || !accepts(o, v))
+        return fail(G16_ERR_BAD_ARGUMENT, var + "=\"" + s + "\" is not one of " + accepted(o));
+      tune.*o.value = v;
+    }
     pool.reset(new HostPool(7));
-    if (const char* v = getenv("G16_MSM_C")) cfg_c = atoi(v);
-    if (const char* v = getenv("G16_MSM_NE")) cfg_ne = atoi(v);
-    if (const char* v = getenv("G16_MSM_MAXCOPIES")) cfg_maxcopies = std::max(1, std::min(atoi(v), (int)MSM_MAX_COPIES));
-    auto env_int = [](const char* name, int& dst, int lo, int hi) {
-      if (const char* v = getenv(name)) { const int x = atoi(v); if (x >= lo && x <= hi) dst = x; }
-    };
-    env_int("G16_MSM_BA", tune.ba_g1, 0, MSM_BA_MAX_ROUNDS);
-    env_int("G16_MSM_BA_G2", tune.ba_g2, 0, MSM_BA_MAX_ROUNDS);
-    env_int("G16_BA_M", tune.ba_m, 1, 256);
-    env_int("G16_BA_G", tune.ba_G, 1, 4096);
-    env_int("G16_BA_INV_GCD", tune.ba_gcd, 0, 1);
-    env_int("G16_ACC_K0_G1", tune.k0_g1, 4, 1024);
-    env_int("G16_ACC_K0_G2", tune.k0_g2, 4, 1024);
-    env_int("G16_ACC_BLOCK", tune.acc_block, 32, 128);
-    env_int("G16_BA_OCC_G2", tune.ba_occ_g2, 0, 3);
-    env_int("G16_BA_OCC_G1", tune.ba_occ_g1, 0, 5);
-    env_int("G16_BA_CAP_FWD_G1", tune.ba_cap_fwd_g1, 0, 16);
-    env_int("G16_BA_CAP_BWD_G1", tune.ba_cap_bwd_g1, 0, 16);
-    env_int("G16_BA_CAP_FWD_G2", tune.ba_cap_fwd_g2, 0, 16);
-    env_int("G16_BA_CAP_BWD_G2", tune.ba_cap_bwd_g2, 0, 16);
-    if (cfg_c < 0 || cfg_c > 24) cfg_c = 0;
     // Stream priorities (greatest first): the witness map (H's MSM waits for it), then the G2 MSM (longest latency-bound
     // tail: its point additions cost ~3x a G1 addition), then H (starts last), then L / A / B-in-G1.  The heavy
     // accumulation kernels of the low-priority streams fill the machine while the high-priority tails trickle through.
@@ -619,18 +612,9 @@ struct Engine : IEngine {
     return d;
   }
 
-  // One transform: the TMA-tiled passes (ntt_tma.cuh) from 2^14 points up, the generic passes (ntt.cuh) below that or
-  // when the tensor-map encoder is unavailable / switched off (g16_set_option "ntt_tma" 0).
-  // Measured on an H100 (tools/sweep.py, BLS12-381 at 2^20): the TMA plan halves the passes' DRAM traffic but loses on
-  // time -- its 128 KB tiles are only 256 CTAs for 132 SMs (1.9 waves, one CTA per SM, no overlap of load / butterflies /
-  // store): witness map 2.61 ms against 2.30 ms with the generic passes.  It is therefore OFF by default and selectable
-  // (g16_set_option "ntt_tma" 1) -- DESIGN.md section 3 has the analysis.  1 = from 2^14 points, 0 / -1 = generic passes.
-  int use_ntt_tma = 0;
+  // one transform (ntt.cuh), counted in ntt_launches
   void ntt_any(cudaStream_t st, const NttDomain<Fr>& d, bool inverse, const Fr* src, Fr* work, Fr* dst, int load_mode, const Fr* ltab,
                const Fr* in_b, const Fr* in_c, const Fr& load_cst, int store_mode, const Fr* stab, const Fr& store_cst) {
-    const bool tma = use_ntt_tma > 0;
-    if (tma && ntt2_run<Fr>(st, d, inverse, src, work, dst, load_mode, ltab, in_b, in_c, load_cst, store_mode, stab, store_cst, &ntt_launches))
-      return;
     ntt_run<Fr>(st, d, inverse, src, work, dst, load_mode, ltab, in_b, in_c, load_cst, store_mode, stab, store_cst, &ntt_launches);
   }
 
@@ -745,7 +729,7 @@ struct Engine : IEngine {
       G16_CUDA(cudaMemcpyAsync(db.p, bases, n * sizeof(Affine<F>), cudaMemcpyHostToDevice, S0.st_main));
       G16_CUDA(cudaMemcpyAsync(ds.p, scalars, n * 32, cudaMemcpyHostToDevice, S0.st_main));
       G16_CUDA(msm_prepare_query<F>(S0.st_main, db.template as<Affine<F>>(), (uint32_t)n, 1, 0, dm.template as<uint8_t>()));
-      const MsmGeom g = with_k0(msm_geom(n, FR_BITS, cfg_c, 0), sizeof(F) > 48);   // caller-supplied bases: no precomputed copies
+      const MsmGeom g = with_k0(msm_geom(n, FR_BITS, (int)tune.c, 0), sizeof(F) > 48);   // caller-supplied bases: no precomputed copies
       cudaError_t e = msm_enqueue<F, Fr>(S0.st_main, ws, g, db.template as<Affine<F>>(), dm.template as<uint8_t>(), ds.template as<uint32_t>(), 1, false, &ctr, nullptr, nullptr, nullptr, nullptr, nullptr);
       if (e != cudaSuccess) { db.release(); ds.release(); dm.release(); return fail(G16_ERR_CUDA, std::string("msm_enqueue: ") + cudaGetErrorString(e)); }
       e = cudaStreamSynchronize(S0.st_main);
@@ -1098,7 +1082,7 @@ struct Engine : IEngine {
         const bool share = share_b_sort && sl.run[M_B1] && sl.run[M_B2];
         // "witness map first" (option, off by default): the MSMs that do not need h sort their entries at once but start
         // accumulating only when the witness map is done, so that their register-heavy blocks do not slow the NTT kernels.
-        const bool wm_first = !sl.serial && (wm_first_opt > 0 || (wm_first_opt < 0 && world > 1));
+        const bool wm_first = !sl.serial && (tune.wm_first > 0 || (tune.wm_first < 0 && world > 1));
         cudaEvent_t gate = (wm_first && m != M_H) ? sl.ev_h : nullptr;
         if (m == M_B2 && share) { sl.b_sorted = MsmSorted{}; sl.b_sorted.ready = sl.ev_bsort; }
         if (m == M_B2) e = msm_enqueue<Fq2, Fr>(st, sl.ws2, sl.geom[m], q[m].bases.template as<A2>(), q[m].mask.template as<uint8_t>(), sc, world, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], share ? &sl.b_sorted : nullptr, nullptr, gate);
@@ -1304,7 +1288,6 @@ struct Engine : IEngine {
   // finishes the same proof (EC addition is exactly associative and commutative: bit-identical for any world size).
   void* nccl_comm = nullptr;      // all-gather of the partial proof points (stream st_comm)
   void* nccl_comm_wm = nullptr;   // witness-map exchange (send / recv / broadcast on the proof slot's main stream)
-  bool split_wm_wanted = true;    // g16_set_option "wm_split"
   uint32_t comm_rank = 0, comm_world = 0;
   cudaStream_t st_comm = nullptr;
   DevBuf d_comm_send, d_comm_recv;
@@ -1359,7 +1342,7 @@ struct Engine : IEngine {
     if (!s) return fail(G16_ERR_BAD_ARGUMENT, "null buffer");
     if (!nccl_comm) return fail(G16_ERR_BAD_ARGUMENT, "g16_comm_init must precede g16_prove_sharded");
     if (comm_world != world || comm_rank != rank) return fail(G16_ERR_BAD_ARGUMENT, "the key's (rank, world) differs from the communicator's");
-    slots[slot].split_wm = split_wm_wanted && comm_world > 1;
+    slots[slot].split_wm = tune.wm_split && comm_world > 1;
     const int rc = submit(slots[slot], r, s, z, flags);
     slots[slot].split_wm = false;
     return rc;
@@ -1452,7 +1435,6 @@ struct Engine : IEngine {
 // extern-template declarations for one curve: put before make_engine<CP> is instantiated (engine_<curve>.cu)
 #define G16_CURVE_KERNELS(X, CP)                                                                  \
   G16_NTT_TEMPLATES(X, Fp<CP::FrP>)                                                               \
-  G16_NTT2_TEMPLATES(X, Fp<CP::FrP>)                                                              \
   G16_MSM_TEMPLATES(X, Fp<CP::FqP>, Fp<CP::FrP>)                                                  \
   G16_MSM_TEMPLATES(X, G16_FQ2(CP), Fp<CP::FrP>)
 #define G16_FQ2(CP) Fp2<CP::FqP, CP::FQ2_NONRESIDUE_NEG>

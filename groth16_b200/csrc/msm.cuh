@@ -45,9 +45,6 @@ struct MsmGeom {
   int ba_G;          // batched-affine: thread products per field inversion
   int ba_gcd;        // batched-affine: 1 = safegcd inversion, 0 = Fermat
   int acc_block;     // threads per block of the level-0 accumulation (32 / 64 / 128)
-  int ba_grid_fwd;   // batched-affine forward / backward launches: at most this many blocks, which pull 128-thread tiles from a
-  int ba_grid_bwd;   // counter (0 = one block per tile).  Leaves block slots to the kernels of the other MSM streams.
-  int ba_occ;        // batched-affine kernels: 0 = plain bodies (4 / 2 resident blocks per SM), != 0 = register-lean bodies (5 / 3)
 };
 
 static constexpr int MSM_K0_MAX = 64;
@@ -85,8 +82,6 @@ inline MsmGeom msm_geom(uint64_t n, int scalar_bits, int c_override = 0, int ne_
   g.ba_G = 16;
   g.ba_gcd = 1;
   g.acc_block = 128;
-  g.ba_occ = 0;
-  g.ba_grid_fwd = g.ba_grid_bwd = 0;
   return g;
 }
 
@@ -649,7 +644,7 @@ struct MsmWorkspace {
     G16_TRY(pp0.reserve(S1 * sizeof(XYZZ<F>)));
     G16_TRY(pk1.reserve(S2 * 4 + 16));
     G16_TRY(pp1.reserve(S2 * sizeof(XYZZ<F>)));
-    G16_TRY(pending.reserve(128 * 4));   // [0, 64): level counters, [64, 128): tile counters of the capped round launches
+    G16_TRY(pending.reserve(64 * 4));   // one partial-list counter per accumulation level
     if (plan_m != g.c - 1 || plan_ne != g.ne) {
       plan.make(g.c - 1);
       plan_m = g.c - 1;
@@ -712,7 +707,7 @@ cudaError_t msm_enqueue(cudaStream_t st, MsmWorkspace<F>& ws, const MsmGeom& g, 
   uint32_t* pending = ws.pending.template as<uint32_t>();
   XYZZ<F>* buckets = ws.buckets.template as<XYZZ<F>>();
   unsigned long long nl = 0;
-  cudaMemsetAsync(pending, 0, 128 * 4, st);
+  cudaMemsetAsync(pending, 0, 64 * 4, st);
   cudaMemsetAsync(buckets, 0, (size_t)g.nkeys * sizeof(XYZZ<F>), st);
   const MsmBaPlan& bp = ws.bap;
   const uint32_t* total0 = offsets + g.nkeys;
@@ -765,21 +760,11 @@ cudaError_t msm_enqueue(cudaStream_t st, MsmWorkspace<F>& ws, const MsmGeom& g, 
       a.prod = ws.ba_prod.template as<F>();
       a.pre2 = ws.ba_pre2.template as<F>();
       a.out = lists[r & 1];
-      a.tile_fwd = g.ba_grid_fwd > 0 ? pending + 64 + 2 * r : nullptr;
-      a.tile_bwd = g.ba_grid_bwd > 0 ? pending + 64 + 2 * r + 1 : nullptr;
       const uint64_t T = ba_threads(bp.len[r + 1], a.m), lanes = (T + a.G - 1) / a.G;
       const unsigned nblk = (unsigned)((T + 127) / 128);
-      // register-lean round kernels (msm_ba.cuh): more resident warps instead of operands held in registers
-      constexpr int LEAN = BaLeanOcc<F>::value;
-      const unsigned nblk_f = a.tile_fwd ? std::min(nblk, (unsigned)g.ba_grid_fwd) : nblk;
-      const unsigned nblk_b = a.tile_bwd ? std::min(nblk, (unsigned)g.ba_grid_bwd) : nblk;
-      if (a.tile_fwd) ba_forward_tiles_kernel<F><<<nblk_f, 128, 0, st>>>(a);
-      else if (g.ba_occ != 0) ba_forward_kernel<F, LEAN><<<nblk, 128, 0, st>>>(a);
-      else ba_forward_kernel<F><<<nblk, 128, 0, st>>>(a);
+      ba_forward_kernel<F><<<nblk, 128, 0, st>>>(a);
       ba_combine_kernel<F><<<(unsigned)((lanes + 31) / 32), 32, 0, st>>>(a);
-      if (a.tile_bwd) ba_backward_tiles_kernel<F><<<nblk_b, 128, 0, st>>>(a);
-      else if (g.ba_occ != 0) ba_backward_kernel<F, LEAN><<<nblk, 128, 0, st>>>(a);
-      else ba_backward_kernel<F><<<nblk, 128, 0, st>>>(a);
+      ba_backward_kernel<F><<<nblk, 128, 0, st>>>(a);
       nl += 3;
     }
     acc_bases = lists[(bp.R - 1) & 1];

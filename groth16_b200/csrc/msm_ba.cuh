@@ -46,8 +46,6 @@ struct BaRound {
   F* prod;                   // [threads]  thread product, then its inverse
   F* pre2;                   // [threads]  running product of the lane before thread t
   Affine<F>* out;            // [outputs]
-  uint32_t* tile_fwd;        // capped grids (msm.cuh, MsmGeom::ba_grid): tile counters of this round's forward / backward launch,
-  uint32_t* tile_bwd;        // zeroed once per MSM; nullptr = one block per tile of 128 threads
 };
 
 G16_HD uint64_t ba_threads(uint64_t outputs, uint32_t m) { return (outputs + m - 1) / m; }
@@ -60,25 +58,6 @@ G16_HD F ba_ld(const F* p) {
   uint4* d = reinterpret_cast<uint4*>(&v);
 #pragma unroll
   for (int j = 0; j < (int)(sizeof(F) / 16); j++) d[j] = __ldg(s + j);
-  return v;
-#else
-  return *p;
-#endif
-}
-
-// A second read of an operand that was already read by this thread.  The register-lean bodies below drop coordinates as soon
-// as they are consumed and fetch them again (an L1 / L2 hit) when they are needed a second time; the volatile asm keeps the
-// compiler from merging the two reads and carrying the first value across the multiplications in between.
-template <class F>
-G16_HD F ba_ld_again(const F* p) {
-#ifdef __CUDA_ARCH__
-  F v;
-  uint32_t* d = reinterpret_cast<uint32_t*>(&v);
-#pragma unroll
-  for (int j = 0; j < (int)(sizeof(F) / 16); j++)
-    asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(d[4 * j]), "=r"(d[4 * j + 1]), "=r"(d[4 * j + 2]), "=r"(d[4 * j + 3])
-                 : "l"(reinterpret_cast<const uint4*>(p) + j));
   return v;
 #else
   return *p;
@@ -106,14 +85,6 @@ template <class F>
 G16_HD F ba_y(const BaSrc<F>& s) {
   if (!s.p) return F::zero();
   F y = ba_ld(&s.p->y);
-  return s.neg ? F::neg(y) : y;
-}
-template <class F>
-G16_HD F ba_x_again(const BaSrc<F>& s) { return s.p ? ba_ld_again(&s.p->x) : F::zero(); }
-template <class F>
-G16_HD F ba_y_again(const BaSrc<F>& s) {
-  if (!s.p) return F::zero();
-  F y = ba_ld_again(&s.p->y);
   return s.neg ? F::neg(y) : y;
 }
 
@@ -163,29 +134,6 @@ G16_HD void ba_forward(const BaRound<F>& a, uint64_t t) {
       if (!more) break;
       j = jn; s1 = n1; s2 = n2; x1 = nx1; x2 = nx2;
     }
-  }
-  a.prod[t] = run;
-}
-
-// Register-lean forward body (Fq2 points at 3 resident blocks per SM): no software prefetch of the next pair -- the extra
-// resident warps hide the gather latency instead of 48 more live registers.  Same outputs as ba_forward.
-template <class F>
-G16_HD void ba_forward_lean(const BaRound<F>& a, uint64_t t) {
-  const uint64_t M = (uint64_t)(*a.total0) >> a.shift;
-  const uint64_t T = ba_threads(M, a.m);
-  if (t >= T) return;
-  F run = F::one();
-  uint64_t j = t;
-  for (uint32_t k = 0; k < a.m && j < M; k++, j += T) {
-    const BaSrc<F> s1 = ba_src(a, 2 * j), s2 = ba_src(a, 2 * j + 1);
-    F d;
-    int kind;
-    {
-      const F x1 = ba_x(s1), x2 = ba_x(s2);
-      kind = ba_kind(s1, s2, x1, x2, d);
-    }
-    a.pre[j] = run;
-    if (kind <= BA_TANGENT) run = F::mul(run, d);
   }
   a.prod[t] = run;
 }
@@ -268,113 +216,22 @@ G16_HD void ba_backward(const BaRound<F>& a, uint64_t t) {
   }
 }
 
-// Register-lean backward body: at most the running inverse and two operands are live across any multiplication.
-// x1, x2 and y1 are read a second time (ba_ld_again) where the plain body keeps them in registers, and x3 is stored before
-// y3 is formed.  For Fq2 points this fits 168 registers (3 resident blocks per SM, 12 warps) without local-memory traffic,
-// where the plain body needs 254 (2 blocks, 8 warps).  `out` never aliases `in` (ping-pong lists), so the early store is safe.
-template <class F>
-G16_HD void ba_backward_lean(const BaRound<F>& a, uint64_t t) {
-  const uint64_t M = (uint64_t)(*a.total0) >> a.shift;
-  const uint64_t T = ba_threads(M, a.m);
-  if (t >= T) return;
-  F run_inv = a.prod[t];
-  uint32_t kn = 0;
-  while (kn < a.m && (uint64_t)kn * T + t < M) kn++;
-  for (uint32_t k = kn; k-- > 0;) {
-    const uint64_t j = (uint64_t)k * T + t;
-    const BaSrc<F> s1 = ba_src(a, 2 * j), s2 = ba_src(a, 2 * j + 1);
-    Affine<F>* o = a.out + j;
-    F d;
-    int kind;
-    {
-      const F x1 = ba_x(s1), x2 = ba_x(s2);
-      kind = ba_kind(s1, s2, x1, x2, d);
-    }
-    if (kind <= BA_TANGENT) {
-      F lam = F::mul(run_inv, ba_ld(a.pre + j));   // 1 / d
-      run_inv = F::mul(run_inv, d);
-      if (kind == BA_CHORD) {
-        lam = F::mul(F::sub(ba_y(s2), ba_y(s1)), lam);
-      } else {
-        const F xx = F::sqr(ba_x_again(s1));
-        lam = F::mul(F::add(F::dbl(xx), xx), lam);
-      }
-      F w = F::sqr(lam);
-      {
-        const F x1 = ba_x_again(s1);
-        w = F::sub(w, x1);
-        w = F::sub(w, kind == BA_CHORD ? ba_x_again(s2) : x1);   // x3
-        o->x = w;
-        w = F::sub(x1, w);                                       // x1 - x3
-      }
-      w = F::mul(lam, w);
-      o->y = F::sub(w, ba_y_again(s1));
-    } else if (kind == BA_FIRST) {
-      o->x = ba_x_again(s1);
-      o->y = ba_y(s1);
-    } else if (kind == BA_SECOND) {
-      o->x = ba_x_again(s2);
-      o->y = ba_y(s2);
-    } else {
-      *o = Affine<F>::inf();
-    }
-  }
-}
-
 #ifdef __CUDACC__
-// Resident blocks per SM the register allocation aims at.  Plain bodies (OCC = 0): single-field points ask for 3 and get 4
-// (~125 registers); Fq2 points 2 = the whole backward body in 254 registers (8 warps per SM).  Register-lean bodies
-// (OCC = BaLeanOcc<F>::value): Fq2 points 3 blocks (168 registers, 12 warps), single-field points 5 (102 registers, 20 warps).
-// Selected per MSM (MsmGeom::ba_occ).
-template <class F, int OCC>
-struct BaCfg { static constexpr int MIN_BLOCKS = OCC > 0 ? OCC : (sizeof(F) <= 48 ? 3 : 2); };
+// Resident blocks per SM the register allocation aims at: single-field points ask for 3 and get 4 (~125 registers); Fq2
+// points 2 = the whole backward body in 254 registers (8 warps per SM).
 template <class F>
-struct BaLeanOcc { static constexpr int value = sizeof(F) <= 48 ? 5 : 3; };
-// Capped grids.  The block scheduler hands a grid's blocks out in launch order: a round kernel with thousands of blocks
-// owns every SM until its tail, so the memory-bound forward pass of one MSM and the multiplier-bound backward pass of
-// another (five MSM streams per proof) run one after the other instead of side by side.  With a cap the kernel is launched
-// with `cap x SMs` blocks which pull tiles of 128 threads from a counter (dynamic, so the last wave stays balanced); the
-// free block slots of every SM go to the kernels of the other streams.  Same work split (thread t owns outputs k*T + t),
-// hence the same prod[] / pre[] layout for the combine kernel.
-__device__ __forceinline__ bool ba_next_tile(uint32_t* ctr, uint64_t ntiles, uint32_t& tile) {
-  __shared__ uint32_t sh_tile;
-  __syncthreads();                       // everybody has read the previous tile
-  if (threadIdx.x == 0) sh_tile = atomicAdd(ctr, 1u);
-  __syncthreads();
-  tile = sh_tile;
-  return tile < ntiles;
-}
+struct BaCfg { static constexpr int MIN_BLOCKS = sizeof(F) <= 48 ? 3 : 2; };
 template <class F>
-__device__ __forceinline__ uint64_t ba_ntiles(const BaRound<F>& a) {
-  const uint64_t M = (uint64_t)(*a.total0) >> a.shift;
-  return (ba_threads(M, a.m) + 127) / 128;
-}
-template <class F, int OCC = 0>
-__global__ void __launch_bounds__(128, BaCfg<F, OCC>::MIN_BLOCKS) ba_forward_kernel(BaRound<F> a) {
-  if constexpr (OCC > 0) ba_forward_lean<F>(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
-  else ba_forward<F>(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
+__global__ void __launch_bounds__(128, BaCfg<F>::MIN_BLOCKS) ba_forward_kernel(BaRound<F> a) {
+  ba_forward<F>(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
 }
 template <class F>
 __global__ void __launch_bounds__(32) ba_combine_kernel(BaRound<F> a) {
   ba_combine<F>(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
 }
-template <class F, int OCC = 0>
-__global__ void __launch_bounds__(128, BaCfg<F, OCC>::MIN_BLOCKS) ba_backward_kernel(BaRound<F> a) {
-  if constexpr (OCC > 0) ba_backward_lean<F>(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
-  else ba_backward<F>(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
-}
-// the capped-grid forms (separate kernels: the tile loop must not cost the one-block-per-tile kernels any registers)
 template <class F>
-__global__ void __launch_bounds__(128, BaCfg<F, 0>::MIN_BLOCKS) ba_forward_tiles_kernel(BaRound<F> a) {
-  const uint64_t nt = ba_ntiles(a);
-  uint32_t tile;
-  while (ba_next_tile(a.tile_fwd, nt, tile)) ba_forward<F>(a, (uint64_t)tile * 128 + threadIdx.x);
-}
-template <class F>
-__global__ void __launch_bounds__(128, BaCfg<F, 0>::MIN_BLOCKS) ba_backward_tiles_kernel(BaRound<F> a) {
-  const uint64_t nt = ba_ntiles(a);
-  uint32_t tile;
-  while (ba_next_tile(a.tile_bwd, nt, tile)) ba_backward<F>(a, (uint64_t)tile * 128 + threadIdx.x);
+__global__ void __launch_bounds__(128, BaCfg<F>::MIN_BLOCKS) ba_backward_kernel(BaRound<F> a) {
+  ba_backward<F>(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);
 }
 #endif  // __CUDACC__
 

@@ -203,18 +203,20 @@ typedef struct {
   int32_t ba_m, ba_g, ba_inv_gcd;     /* additions per thread and round; products per inversion; 1 = safegcd      */
   int32_t acc_block, sm_count;
   int32_t rank, world;
-  int32_t ba_lean_g1, ba_lean_g2;     /* != 0: register-lean round kernels (more resident warps per SM)           */
-  int32_t reserved[2];
+  int32_t reserved[4];
 } g16_config;
 int g16_get_config(const g16_ctx* ctx, g16_config* out);
-/* key: "msm_ba", "msm_ba_g2", "ba_m", "ba_g", "ba_inv_gcd", "acc_k0_g1", "acc_k0_g2", "acc_block", "share_b_sort", "ba_occ_g1", "ba_occ_g2",
- * "ba_min_entries_g1", "ba_min_entries_g2" (smallest MSM, in bucket entries, that runs the rounds), "ba_adaptive" (0 = exactly
- * "msm_ba" rounds, 1 = at most that many, fewer for sparsely filled buckets), "ba_cap_fwd_g1", "ba_cap_bwd_g1", "ba_cap_fwd_g2", "ba_cap_bwd_g2", "ntt_tma", "wm_split", "proof_slots", and -- effective at the next
- * g16_pk_load / g16_setup -- "msm_ne", "msm_c", "msm_maxcopies" (the G16_* environment
- * variables of INTEGRATION.md section 6, read once at g16_ctx_create, in lower case without the prefix).  Takes effect
- * from the next proof; results never depend on these knobs.  Accepted ranges: "msm_ba", "msm_ba_g2" 0 .. 6; "acc_k0_g1",
- * "acc_k0_g2" 0 (automatic) or 4 .. 1024; "acc_block" 32, 64 or 128; "msm_ne" 0 .. 32; "msm_c" 0 (automatic) .. 24;
- * "msm_maxcopies" 1 .. 20.  A value outside its range is refused with G16_ERR_BAD_ARGUMENT and changes nothing. */
+/* Tuning options (INTEGRATION.md section 6) and the values each accepts:
+ *   "msm_ne" 0 .. 32            "msm_c" 0 (automatic) .. 24          "msm_maxcopies" 1 .. 20
+ *   "msm_ba", "msm_ba_g2" 0 .. 6                                      "ba_m" 1 .. 256          "ba_g" 1 .. 4096
+ *   "ba_min_entries_g1", "ba_min_entries_g2" >= 0 (smallest MSM, in bucket entries, that runs the rounds)
+ *   "acc_k0_g1", "acc_k0_g2" 0 (automatic) or 4 .. 1024               "acc_block" 32, 64 or 128
+ *   "ba_inv_gcd", "ba_adaptive" (0 = exactly "msm_ba" rounds, 1 = fewer for sparsely filled buckets), "share_b_sort",
+ *   "wm_split" 0 or 1           "wm_first" -1 (automatic), 0 or 1    "proof_slots" 1 or 2
+ * "msm_ne", "msm_c" and "msm_maxcopies" take effect at the next g16_pk_load / g16_setup, the others from the next proof;
+ * results never depend on them.  A value outside its set is refused with G16_ERR_BAD_ARGUMENT and changes nothing.
+ * g16_ctx_create reads the environment variable G16_<KEY IN UPPER CASE> of every option; a value there that is not a
+ * whole number in the option's set makes it fail with G16_ERR_BAD_ARGUMENT. */
 int g16_set_option(g16_ctx* ctx, const char* key, int64_t value);
 /* The value an option holds now (same keys; feeding it back to g16_set_option restores the option exactly). */
 int g16_get_option(const g16_ctx* ctx, const char* key, int64_t* value);

@@ -98,9 +98,7 @@ pub struct g16_config {
     pub sm_count: i32,
     pub rank: i32,
     pub world: i32,
-    pub ba_lean_g1: i32,
-    pub ba_lean_g2: i32,
-    pub reserved: [i32; 2],
+    pub reserved: [i32; 4],
 }
 
 extern "C" {

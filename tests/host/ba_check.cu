@@ -21,8 +21,7 @@ static bool same_pt(const XYZZ<F>& a, const XYZZ<F>& b) {
 }
 
 template <class F>
-static int run_case(const Affine<F>& G, uint32_t nkeys, uint32_t nbase, uint32_t avg, int R, uint32_t m, uint32_t Gc, const char* name, uint32_t gcd = 0,
-                    bool lean = false) {
+static int run_case(const Affine<F>& G, uint32_t nkeys, uint32_t nbase, uint32_t avg, int R, uint32_t m, uint32_t Gc, const char* name, uint32_t gcd = 0) {
   int bad = 0;
   // base table: k * G, a few identities
   std::vector<Affine<F>> bases(nbase);
@@ -78,11 +77,10 @@ static int run_case(const Affine<F>& G, uint32_t nkeys, uint32_t nbase, uint32_t
     a.m = m; a.G = Gc; a.inv_gcd = gcd;   // (the plan may pick a smaller m for short lists; any m must work)
     a.pre = pre.data(); a.prod = prod.data(); a.pre2 = pre2.data();
     a.out = lists[r & 1].data();
-    a.tile_fwd = a.tile_bwd = nullptr;
     const uint64_t Tmax = ba_threads(bp.len[r + 1], m) + 3;   // over-launch like the kernels do
-    for (uint64_t t = 0; t < Tmax; t++) lean ? ba_forward_lean<F>(a, t) : ba_forward<F>(a, t);
+    for (uint64_t t = 0; t < Tmax; t++) ba_forward<F>(a, t);
     for (uint64_t l = 0; l < (Tmax + Gc - 1) / Gc + 2; l++) ba_combine<F>(a, l);
-    for (uint64_t t = 0; t < Tmax; t++) lean ? ba_backward_lean<F>(a, t) : ba_backward<F>(a, t);
+    for (uint64_t t = 0; t < Tmax; t++) ba_backward<F>(a, t);
   }
   // last list: slot j belongs to the bucket of sorted slot j << R (the key msm_accum_l0 reads)
   const std::vector<Affine<F>>& fin = lists[(R - 1) & 1];
@@ -112,10 +110,6 @@ int main() {
     bad += run_case<F>(G, 37, 50, 12, 3, 4, 3, "bn254-g1-safegcd", 1); cases++;
     bad += run_case<F>(G, 5, 3, 40, 5, 8, 64, "bn254-g1-dense-safegcd", 1); cases++;
     bad += run_case<F>(G, 64, 200, 3, 4, 16, 64, "bn254-g1-sparse-R4", 1); cases++;
-    // the register-lean bodies (ba_forward_lean / ba_backward_lean) must give the same lists
-    bad += run_case<F>(G, 37, 50, 12, 3, 4, 3, "bn254-g1-lean", 1, true); cases++;
-    bad += run_case<F>(G, 5, 3, 40, 5, 8, 64, "bn254-g1-dense-lean", 1, true); cases++;
-    bad += run_case<F>(G, 1, 9, 100, 6, 32, 64, "bn254-g1-onebucket-lean", 0, true); cases++;
   }
   {
     using B = Fp<BLS381_FqP>;
@@ -126,8 +120,6 @@ int main() {
     bad += run_case<F>(G, 3, 4, 20, 3, 16, 64, "bls381-g2-dense"); cases++;
     bad += run_case<F>(G, 19, 20, 6, 2, 4, 5, "bls381-g2-safegcd", 1); cases++;
     bad += run_case<F>(G, 19, 20, 6, 4, 4, 5, "bls381-g2-R4", 1); cases++;
-    bad += run_case<F>(G, 19, 20, 6, 4, 4, 5, "bls381-g2-R4-lean", 1, true); cases++;
-    bad += run_case<F>(G, 3, 4, 20, 3, 16, 64, "bls381-g2-dense-lean", 0, true); cases++;
   }
   {
     using B = Fp<BLS377_FqP>;
@@ -136,7 +128,6 @@ int main() {
     const Affine<F> G{{small(2), small(9)}, {small(4), small(1)}};
     bad += run_case<F>(G, 7, 6, 10, 2, 4, 2, "bls377-g2"); cases++;
     bad += run_case<F>(G, 7, 6, 10, 3, 2, 2, "bls377-g2-R3", 1); cases++;
-    bad += run_case<F>(G, 7, 6, 10, 3, 2, 2, "bls377-g2-R3-lean", 1, true); cases++;
   }
   printf("%d cases, %d mismatches\n", cases, bad);
   return bad ? 1 : 0;

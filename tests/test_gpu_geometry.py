@@ -272,19 +272,61 @@ def test_accumulation_knobs(curve, rounds, knob, value):
     run_config(curve, opts, check)
 
 
+INT64_MAX = (1 << 63) - 1
+# every option of g16_set_option and the values it accepts, as the union of closed ranges (include/g16b200.h)
+ACCEPTED = {"msm_ne": [(0, 32)], "msm_c": [(0, 24)], "msm_maxcopies": [(1, 20)], "msm_ba": [(0, 6)], "msm_ba_g2": [(0, 6)],
+            "ba_m": [(1, 256)], "ba_g": [(1, 4096)], "ba_min_entries_g1": [(0, INT64_MAX)],
+            "ba_min_entries_g2": [(0, INT64_MAX)], "acc_k0_g1": [(0, 0), (4, 1024)], "acc_k0_g2": [(0, 0), (4, 1024)],
+            "acc_block": [(32, 32), (64, 64), (128, 128)], "ba_inv_gcd": [(0, 1)], "ba_adaptive": [(0, 1)],
+            "share_b_sort": [(0, 1)], "wm_split": [(0, 1)], "wm_first": [(-1, 1)], "proof_slots": [(1, 2)]}
+
+
 def test_knobs_out_of_range_are_refused():
-    """a value the kernels cannot honour is an error, not a silent replacement, and leaves the option unchanged"""
+    """a value the kernels cannot honour is an error, not a silent replacement, and leaves the option unchanged: for every
+    option the values just outside its set (below, above, and in each gap of a discrete set); every endpoint of the set
+    is accepted and reads back unchanged"""
     cs = case("bn254")
-    bad = [("acc_k0_g1", 3), ("acc_k0_g1", 1025), ("acc_k0_g2", -1), ("acc_k0_g2", 2048), ("acc_block", 100), ("acc_block", 256),
-           ("acc_block", 0), ("msm_ne", -1), ("msm_ne", 33), ("msm_c", -2), ("msm_c", 25), ("msm_maxcopies", 0),
-           ("msm_maxcopies", 21), ("msm_ba", 7), ("msm_ba_g2", -1)]
-    for k, v in bad:
-        before = cs.g.get_option(k)
-        with pytest.raises(ValueError):
+    saved = {k: cs.g.get_option(k) for k in ACCEPTED}
+    try:
+        for k, ranges in ACCEPTED.items():
+            bad = {ranges[0][0] - 1, ranges[-1][1] + 1} | {v for (_, hi), (lo, _) in zip(ranges, ranges[1:]) for v in (hi + 1, lo - 1)}
+            for v in sorted(b for b in bad if b <= INT64_MAX):
+                before = cs.g.get_option(k)
+                with pytest.raises(ValueError):
+                    cs.g.set_option(k, v)
+                assert cs.g.get_option(k) == before, (k, v)
+            for v in sorted({e for r in ranges for e in r}):
+                cs.g.set_option(k, v)
+                assert cs.g.get_option(k) == v, (k, v)
+            cs.g.set_option(k, saved[k])
+    finally:
+        for k, v in saved.items():
             cs.g.set_option(k, v)
-        assert cs.g.get_option(k) == before, k
     with pytest.raises(ValueError):
         cs.g.get_option("no_such_option")
+
+
+def test_options_from_environment():
+    """g16_ctx_create reads G16_<OPTION> for every option; a value outside the option's set makes it fail, naming the
+    variable"""
+    import os
+    keep = {k: os.environ.get(k) for k in ("G16_ACC_BLOCK", "G16_WM_SPLIT")}
+    try:
+        os.environ.update(G16_ACC_BLOCK="64", G16_WM_SPLIT="0")
+        g = Groth16("bn254", 0)
+        try:
+            assert (g.get_option("acc_block"), g.get_option("wm_split")) == (64, 0)
+        finally:
+            g.close()
+        os.environ["G16_ACC_BLOCK"] = "100"
+        with pytest.raises(ValueError, match="G16_ACC_BLOCK"):
+            Groth16("bn254", 0)
+    finally:
+        for k, v in keep.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
 
 
 # ---- schedules ------------------------------------------------------------------------------------------------------------

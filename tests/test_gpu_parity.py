@@ -307,8 +307,7 @@ def test_msm_skewed_scalars_large():
     _skewed_msm_check()
 
 
-_BA_OPTIONS = ("msm_ba", "msm_ba_g2", "ba_min_entries_g1", "ba_min_entries_g2", "ba_adaptive", "ba_m", "ba_g", "ba_inv_gcd",
-               "ba_occ_g1", "ba_occ_g2", "ba_cap_fwd_g1", "ba_cap_bwd_g1", "ba_cap_fwd_g2", "ba_cap_bwd_g2")
+_BA_OPTIONS = ("msm_ba", "msm_ba_g2", "ba_min_entries_g1", "ba_min_entries_g2", "ba_adaptive", "ba_m", "ba_g", "ba_inv_gcd")
 
 
 def _set_ba(rounds_g1, rounds_g2, min_entries=0, **kw):
@@ -323,13 +322,12 @@ def _set_ba(rounds_g1, rounds_g2, min_entries=0, **kw):
             g.set_option(k, v)
 
 
-@pytest.mark.parametrize("rounds,m,G,gcd,lean", [(0, 16, 64, 1, 0), (1, 4, 7, 0, 0), (3, 32, 64, 1, 0), (6, 16, 16, 1, 0),
-                                                 (4, 32, 16, 1, 1), (2, 5, 3, 0, 1), (3, 8, 16, 1, 2)])
-def test_batched_affine_rounds(rounds, m, G, gcd, lean):
+@pytest.mark.parametrize("rounds,m,G,gcd", [(0, 16, 64, 1), (1, 4, 7, 0), (3, 32, 64, 1), (6, 16, 16, 1), (4, 32, 16, 1),
+                                            (2, 5, 3, 0), (3, 8, 16, 1)])
+def test_batched_affine_rounds(rounds, m, G, gcd):
     """The batched-affine pre-reduction (csrc/msm_ba.cuh; default: 4 rounds on G1 MSMs; g16_set_option "msm_ba" /
     "msm_ba_g2") must not change a single bit whatever the number of rounds (0 = plain XYZZ accumulation), the additions
-    per thread, the products per inversion, the inversion routine or the kernel build (lean = 1: the register-lean round
-    kernels, "ba_occ_g1" / "ba_occ_g2"; lean = 2: capped grids pulling tiles from a counter, "ba_cap_*"): skewed G1 MSM with repeated bases, a 2^14-point G2
+    per thread, the products per inversion or the inversion routine: skewed G1 MSM with repeated bases, a 2^14-point G2
     MSM, and full proofs (synthetic 2^14, and the degenerate DummyCircuit where every scalar is equal) against the CPU
     oracle."""
     import orc
@@ -337,9 +335,7 @@ def test_batched_affine_rounds(rounds, m, G, gcd, lean):
     from groth16_b200.workload import dummy_r1cs, synthetic_r1cs
     saved = {name: {k: engine(name).get_option(k) for k in _BA_OPTIONS} for name in ALL_CURVES}   # whatever the engines hold now
     try:
-        cap = 1 if lean == 2 else 0
-        _set_ba(rounds, rounds, ba_m=m, ba_g=G, ba_inv_gcd=gcd, ba_occ_g1=int(lean == 1), ba_occ_g2=int(lean == 1),
-                ba_cap_fwd_g1=cap, ba_cap_bwd_g1=cap, ba_cap_fwd_g2=cap, ba_cap_bwd_g2=cap)
+        _set_ba(rounds, rounds, ba_m=m, ba_g=G, ba_inv_gcd=gcd)
         _ba_body(orc, GENERATORS, dummy_r1cs, synthetic_r1cs)
     finally:
         for name, opts in saved.items():

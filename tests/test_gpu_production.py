@@ -73,38 +73,16 @@ def test_ntt_three_pass_plan(curve, log_n):
 
 @pytest.mark.parametrize("curve,log_n", [("bn254", 14), ("bls12_381", 15), ("bls12_377", 16), ("bn254", 17), ("bls12_381", 19),
                                          ("bn254", 21), ("bls12_381", 22)])
-def test_ntt_tma_plans(curve, log_n):
-    """Every shape of the TMA-tiled plan (csrc/ntt_tma.cuh): one strided pass with 2^4 .. 2^10 rows (log n = 14 .. 20), two
-    strided passes (21, 22), forward + coset-inverse; and the generic passes (g16_set_option ntt_tma 0) give the same bits."""
+def test_ntt_plans(curve, log_n):
+    """The plans around test_ntt_three_pass_plan's sizes: one strided pass + the bit-reversing pass (log n = 14 .. 17), two
+    strided passes with uneven (19, 21) and even (22) splits; forward + coset-inverse, all four modes at 16 and 21."""
     g = engine(curve)
     cid = P.CURVES[curve].cid
     vals = rand_fr_mont(np.random.RandomState(2000 + log_n), 1 << log_n)
     modes = ((False, False), (True, True)) + (((False, True), (True, False)) if log_n in (16, 21) else ())
     for inverse, coset in modes:
         want = orc.ntt(cid, log_n, vals, inverse=inverse, coset=coset, threads=THREADS)
-        try:
-            g.set_option("ntt_tma", 1)
-            assert np.array_equal(g.ntt_log(log_n, vals, inverse=inverse, coset=coset), want), (curve, log_n, inverse, coset, "tma")
-            g.set_option("ntt_tma", 0)
-            assert np.array_equal(g.ntt_log(log_n, vals, inverse=inverse, coset=coset), want), (curve, log_n, inverse, coset, "generic")
-        finally:
-            g.set_option("ntt_tma", -1)
-
-
-def test_witness_map_with_tma_passes():
-    """r1cs_to_qap.rs:172-235 with every transform on the TMA-tiled passes (fused n^-1 g^i load table, (a*b - c) * Z^-1 load,
-    n^-1 g^-i store table) at 2^14 and 2^16, against the oracle."""
-    curve = "bls12_381"
-    g = engine(curve)
-    for log_n in (14, 16):
-        m, z, _ = synthetic_r1cs(curve, log_n, seed=8)
-        g.load_matrices(m)
-        try:
-            g.set_option("ntt_tma", 1)
-            h = g.witness_map_from_matrices(None, m.num_instance_variables, m.num_constraints, z)
-        finally:
-            g.set_option("ntt_tma", -1)
-        assert np.array_equal(h, orc.witness_map(P.CURVES[curve].cid, m, z, threads=THREADS))
+        assert np.array_equal(g.ntt_log(log_n, vals, inverse=inverse, coset=coset), want), (curve, log_n, inverse, coset)
 
 
 def _setup(curve, m):

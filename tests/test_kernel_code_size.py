@@ -1,7 +1,7 @@
 """CPU test of the compiled BLS12-381 MSM kernels: every hot kernel calls one out-of-line Fq product body instead of
 inlining each product (fp.cuh, Fp::mont_mul_call).  Inlined, the G2 kernels spill and the proof is slower (DESIGN.md
-section 3).  Guards against a change that quietly inlines the products again, and against register spills in the default
-batched-affine round kernels."""
+section 3).  Guards against a change that quietly inlines the products again, against register spills in the batched-affine
+round kernels, and against hot kernels appearing or disappearing: each object holds exactly the seven listed in HOT."""
 import os
 import re
 import shutil
@@ -25,8 +25,8 @@ pytestmark = pytest.mark.skipif(CUOBJDUMP is None, reason="cuobjdump (CUDA toolk
 
 # Hot kernels (mangled-name fragments) and the SASS size each must stay under.  A kernel's text includes its copy of the
 # out-of-line product and point-operation bodies.  Inlined, these kernels were 60..200 KB (G1) and 140..560 KB (G2).
-HOT = ("ba_forward_kernel", "ba_backward_kernel", "ba_combine_kernel", "ba_forward_tiles_kernel", "ba_backward_tiles_kernel",
-       "msm_accum_l0", "msm_accum_ln", "msm_accum_tail", "msm_sum_strided")
+HOT = ("ba_forward_kernel", "ba_backward_kernel", "ba_combine_kernel", "msm_accum_l0", "msm_accum_ln", "msm_accum_tail",
+       "msm_sum_strided")
 MAX_KB = {"g1": 64, "g2": 176}
 # An inlined 12-limb Montgomery product is ~290 IMAD.WIDE / IMAD.HI; more than two products' worth means inlined copies.
 MAX_WIDE_MULS = 2 * 330
@@ -73,20 +73,20 @@ def objects():
 
 
 @pytest.mark.parametrize("group", ["g1", "g2"])
-def test_hot_kernels_small(objects, group):
+def test_hot_kernel_set_and_size(objects, group):
     sass = _sass(objects[group])
     hot = {fn: v for fn, v in sass.items() if any(re.search(rf"\d{h}I", fn) for h in HOT)}
-    assert len(hot) >= 11, sorted(sass)   # plain, lean and tiles round kernels + the four accumulation kernels
+    # exactly one instance of each: the three round kernels and the four accumulation kernels
+    assert sorted(next(h for h in HOT if re.search(rf"\d{h}I", fn)) for fn in hot) == sorted(HOT), sorted(sass)
     for fn, (size, wide) in hot.items():
         assert size <= MAX_KB[group] * 1024, f"{fn}: {size / 1024:.1f} KB of SASS (limit {MAX_KB[group]} KB)"
         assert wide <= MAX_WIDE_MULS, f"{fn}: {wide} wide multiplies: Fq products are inlined again"
 
 
 @pytest.mark.parametrize("group", ["g1", "g2"])
-def test_default_round_kernels_do_not_spill(objects, group):
+def test_round_kernels_do_not_spill(objects, group):
     use = _res_usage(objects[group])
-    # default (OCC = 0) forward and backward round kernels: ..._kernelI<field>Li0EEEvNS_7BaRound...
-    default = {fn: u for fn, u in use.items() if re.search(r"\d(ba_forward_kernel|ba_backward_kernel)I.*Li0EEEv", fn)}
-    assert len(default) == 2, sorted(use)
-    for fn, u in default.items():
+    rounds = {fn: u for fn, u in use.items() if re.search(r"\d(ba_forward_kernel|ba_backward_kernel)I", fn)}
+    assert len(rounds) == 2, sorted(use)
+    for fn, u in rounds.items():
         assert u["STACK"] == 0 and u["LOCAL"] == 0, f"{fn}: {u}"

@@ -3,7 +3,7 @@
 per-MSM accumulation-stage times for each, every proof compared bit for bit with the first.  Writes JSON lines to
 gpurun_out/sweep_<tag>.jsonl.  Development tool (not part of the product or the tests).
 
-  python tools/sweep.py --curve bls12_381 --log-n 20 --tag r02a [--set name=spec ...]
+  python tools/sweep.py --curve bls12_381 --log-n 20 --tag r02a [--grid '[{"msm_ba": 4, "ba_m": 16}, ...]']
 """
 import argparse
 import json
@@ -38,8 +38,7 @@ DEFAULT_GRID = [
     {"msm_ba": 4, "msm_ba_g2": 0, "acc_k0_g2": 64},
 ]
 BASE = {"msm_ba": 4, "msm_ba_g2": 4, "ba_m": 32, "ba_g": 16, "ba_inv_gcd": 1, "acc_k0_g1": 0, "acc_k0_g2": 0, "acc_block": 128,
-        "share_b_sort": 1, "ba_occ_g1": 0, "ba_occ_g2": 0, "ntt_tma": -1,
-        "ba_cap_fwd_g1": 0, "ba_cap_bwd_g1": 0, "ba_cap_fwd_g2": 0, "ba_cap_bwd_g2": 0}
+        "share_b_sort": 1}
 
 
 def main():
