@@ -61,6 +61,7 @@ SIGNATURES = [
     ("g16_prove_assemble_prepare", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     ("g16_prove_submit", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
     ("g16_prove_wait", C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    ("g16_prove_batch", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     ("g16_prove_partial_submit", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_uint32]),
     ("g16_prove_partial_wait", C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     ("g16_witness_map", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),

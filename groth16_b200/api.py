@@ -340,6 +340,37 @@ class Groth16:
     def prove_wait_raw(self, slot: int, out: np.ndarray):
         _check(self._lib.g16_prove_wait(self._ctx, slot, _ptr(out)))
 
+    # ---- batch proving: many proofs of the resident circuit in one call (g16_prove_batch) ----
+    def create_proofs_batch(self, r, s, full_assignments: np.ndarray, group: int = 0, flags: int = 0) -> List[Proof]:
+        """Proof i equals create_proof_with_reduction_and_matrices(None, r[i], s[i], None, ..., full_assignments[i]).
+        r, s: sequences of ints or (K, 4) Montgomery limbs; full_assignments: (K, nv, 4) Montgomery limbs.  `group` caps the
+        proofs that share one pass of the kernels (0 = as many as fit); results never depend on it."""
+        m = self._matrices
+        if m is None or not self._pk_resident:
+            raise ValueError("matrices and proving key must be loaded")
+        nv = m.num_instance_variables + m.num_witness_variables
+        z = np.ascontiguousarray(full_assignments, dtype=np.uint64)
+        if z.ndim != 3 or z.shape[1:] != (nv, 4):
+            raise ValueError(f"full_assignments must have shape (K, {nv}, 4)")
+        k = z.shape[0]
+        rr, ss = self._fr_args(r), self._fr_args(s)
+        if rr.shape[0] != k or ss.shape[0] != k:
+            raise ValueError("r, s and full_assignments must hold the same number of proofs")
+        if not 0 <= group < 1 << 32:
+            raise ValueError("group must be a non-negative 32-bit count")
+        nq = self.nq
+        out = np.zeros((k, 8 * nq), dtype=np.uint64)
+        if k:
+            self.prove_batch_raw(k, rr, ss, z.ctypes.data, group, flags, out)
+        return [Proof(p[:2 * nq].copy(), p[2 * nq:6 * nq].copy(), p[6 * nq:].copy()) for p in out]
+
+    def prove_batch_raw(self, count: int, r_limbs: np.ndarray, s_limbs: np.ndarray, z_ptr, group: int, flags: int,
+                        out: np.ndarray):
+        """g16_prove_batch with everything in ABI form; z_ptr is a host or (G16_ASSIGNMENT_ON_DEVICE) device address of
+        count * nv Montgomery Fr; out holds count * 8 * N64 limbs."""
+        _check(self._lib.g16_prove_batch(self._ctx, count, _ptr(r_limbs), _ptr(s_limbs), C.c_void_p(z_ptr), group, flags,
+                                         _ptr(out)))
+
     def prove_partial_submit_raw(self, slot: int, r_limbs: np.ndarray, z_ptr, flags: int):
         _check(self._lib.g16_prove_partial_submit(self._ctx, slot, _ptr(r_limbs), C.c_void_p(z_ptr), flags))
 
@@ -444,3 +475,15 @@ class Groth16:
         if isinstance(x, (int, np.integer)):
             return np.ascontiguousarray(self.codec.fr.enc1(int(x)))
         return np.ascontiguousarray(x, dtype=np.uint64).reshape(4)
+
+    def _fr_args(self, xs) -> np.ndarray:
+        """a sequence of ints, or a (K, 4) array of Montgomery limbs -> (K, 4) contiguous limbs"""
+        if isinstance(xs, np.ndarray):
+            a = np.ascontiguousarray(xs, dtype=np.uint64)
+            if a.ndim != 2 or a.shape[1] != 4:
+                raise ValueError("scalar limbs must have shape (K, 4)")
+            return a
+        xs = list(xs)
+        if not xs:
+            return np.zeros((0, 4), dtype=np.uint64)
+        return np.ascontiguousarray(np.stack([self._fr_arg(x) for x in xs]), dtype=np.uint64)

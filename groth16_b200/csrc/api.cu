@@ -160,6 +160,11 @@ int g16_prove_wait(g16_ctx* ctx, int slot, uint64_t* proof_out) {
   CTX_OR_FAIL(ctx);
   return ctx->eng->prove_wait(slot, proof_out);
 }
+int g16_prove_batch(g16_ctx* ctx, uint32_t count, const uint64_t* r, const uint64_t* s, const uint64_t* full_assignments,
+                    uint32_t group, uint32_t flags, uint64_t* proofs_out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->prove_batch(count, r, s, full_assignments, group, flags, proofs_out);
+}
 int g16_prove_partial_submit(g16_ctx* ctx, int slot, const uint64_t* r, const uint64_t* full_assignment, uint32_t flags) {
   CTX_OR_FAIL(ctx);
   return ctx->eng->partial_submit(slot, r, full_assignment, flags);

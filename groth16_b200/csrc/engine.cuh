@@ -23,6 +23,7 @@
 #include <thread>
 #include <vector>
 #include "../../include/g16b200.h"
+#include "batch.cuh"
 #include "ec.cuh"
 #include "msm.cuh"
 #include "ntt.cuh"
@@ -143,6 +144,8 @@ struct IEngine {
   virtual int assemble_prepare(const uint64_t* r, const uint64_t* s) = 0;
   virtual int prove_submit(int slot, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags) = 0;
   virtual int prove_wait(int slot, uint64_t* proof) = 0;
+  virtual int prove_batch(uint32_t count, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t group, uint32_t flags,
+                          uint64_t* proofs) = 0;
   virtual int partial_submit(int slot, const uint64_t* r, const uint64_t* z, uint32_t flags) = 0;
   virtual int partial_wait(int slot, uint64_t* partial) = 0;
   virtual int witness_map(const uint64_t* z, uint32_t flags, uint64_t* h) = 0;
@@ -207,6 +210,11 @@ struct Engine : IEngine {
     FixedMuls fx;
     std::shared_ptr<HostPool::Ticket> helper, helper2;   // (r, s)-only scalar multiplications in flight on the pool
     unsigned long long launches0 = 0;
+    // batch proving (g16_prove_batch): the group this slot holds, and its fixed-base products
+    uint32_t batch_first = 0, batch_count = 0;
+    DevBuf d_tail;          // per proof: r, s, r s (Fr), then r d1, (r s) d1, s P_a, r P_b (G1 affine), s d2 (G2 affine)
+    uint64_t* h_tail = nullptr;   // pinned copy of d_tail
+    size_t h_tail_cap = 0;
   };
   static constexpr int NSLOTS = 2;
   Slot slots[NSLOTS];
@@ -466,6 +474,13 @@ struct Engine : IEngine {
   }
   A1 a0, b1_0, alpha_g1, beta_g1, delta_g1;
   A2 b2_0, beta_g2, delta_g2;
+  // batch proving: fixed-base tables of d1, P_a = a0 + alpha_g1, P_b = b1_0 + beta_g1 (G1) and d2 (G2), built by the first
+  // g16_prove_batch under a key and dropped whenever the circuit or key changes
+  enum { TAB_D1 = 0, TAB_PA = 1, TAB_PB = 2, TAB_D2 = 3 };
+  DevBuf tail_tab[4];
+  bool tail_ready = false;
+  A1 p_a;
+  A2 p_2;
   // setup-only extras for pk_export
   A2 gamma_g2;
   DevBuf d_gamma_abc;
@@ -535,6 +550,8 @@ struct Engine : IEngine {
     dom_api.release();
     for (Slot& sl : slots) {
       sl.d_z.release(); sl.d_a.release(); sl.d_b.release(); sl.d_c.release(); sl.d_t.release(); sl.d_h.release();
+      sl.d_tail.release();
+      if (sl.h_tail) cudaFreeHost(sl.h_tail);
       for (auto& w : sl.ws1) w.release();
       sl.ws2.release();
       if (sl.st_main) cudaStreamDestroy(sl.st_main);
@@ -545,6 +562,8 @@ struct Engine : IEngine {
     }
     for (int m = 0; m < 3; m++) { csr_rp[m].release(); csr_col[m].release(); csr_val[m].release(); }
     for (auto& x : q) { x.bases.release(); x.mask.release(); }
+    for (auto& t : tail_tab) t.release();
+    if (ev_batch) cudaEventDestroy(ev_batch);
     d_gamma_abc.release(); full_a.release(); full_b1.release(); full_b2.release();
   }
   int fq_limbs() const override { return NQ64; }
@@ -589,8 +608,8 @@ struct Engine : IEngine {
   }
 
   // ---- domain + buffers ----
-  int ensure_slot_buffers(Slot& sl, int Ln) {
-    const size_t bytes = (size_t)sizeof(Fr) << Ln;
+  int ensure_slot_buffers(Slot& sl, int Ln, uint32_t count = 1) {
+    const size_t bytes = ((size_t)sizeof(Fr) << Ln) * count;
     G16_CUDA(sl.d_a.reserve(bytes)); G16_CUDA(sl.d_b.reserve(bytes)); G16_CUDA(sl.d_c.reserve(bytes));
     G16_CUDA(sl.d_t.reserve(bytes)); G16_CUDA(sl.d_h.reserve(bytes));
     return G16_OK;
@@ -614,8 +633,9 @@ struct Engine : IEngine {
 
   // one transform (ntt.cuh), counted in ntt_launches
   void ntt_any(cudaStream_t st, const NttDomain<Fr>& d, bool inverse, const Fr* src, Fr* work, Fr* dst, int load_mode, const Fr* ltab,
-               const Fr* in_b, const Fr* in_c, const Fr& load_cst, int store_mode, const Fr* stab, const Fr& store_cst) {
-    ntt_run<Fr>(st, d, inverse, src, work, dst, load_mode, ltab, in_b, in_c, load_cst, store_mode, stab, store_cst, &ntt_launches);
+               const Fr* in_b, const Fr* in_c, const Fr& load_cst, int store_mode, const Fr* stab, const Fr& store_cst,
+               uint32_t nvec = 1) {
+    ntt_run<Fr>(st, d, inverse, src, work, dst, load_mode, ltab, in_b, in_c, load_cst, store_mode, stab, store_cst, &ntt_launches, nvec);
   }
 
   // ---- NTT API ----
@@ -645,18 +665,19 @@ struct Engine : IEngine {
   }
 
   // a, b, c (device, evaluations over the domain) -> S0.d_h (coefficients of h).  r1cs_to_qap.rs:201-232
-  void witness_map_device(Slot& sl, const NttDomain<Fr>& dom) {
+  // count > 1: the witness maps of `count` proofs, vectors n apart in every buffer, one launch per pass for all of them
+  void witness_map_device(Slot& sl, const NttDomain<Fr>& dom, uint32_t count = 1) {
     cudaStream_t st = sl.st_main;
     Fr* A = sl.d_a.template as<Fr>(); Fr* B = sl.d_b.template as<Fr>(); Fr* C = sl.d_c.template as<Fr>(); Fr* T = sl.d_t.template as<Fr>(); Fr* H = sl.d_h.template as<Fr>();
     const Fr zero = Fr::zero();
     for (Fr* X : {A, B, C}) {
       // domain.ifft_in_place (r1cs_to_qap.rs:201-202,220) followed by coset_domain.fft_in_place (:204-207,221): the inverse
       // transform's n^-1 and the coset pre-scaling g^i are one multiplication by the table n^-1 g^i at the second load
-      ntt_any(st, dom, true, X, X, T, NTT_LOAD_PLAIN, nullptr, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero);
-      ntt_any(st, dom, false, T, T, X, NTT_LOAD_MUL_TABLE, dom.coset_fwd_ninv, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero);
+      ntt_any(st, dom, true, X, X, T, NTT_LOAD_PLAIN, nullptr, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero, count);
+      ntt_any(st, dom, false, T, T, X, NTT_LOAD_MUL_TABLE, dom.coset_fwd_ninv, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero, count);
     }
     // (a*b - c) * Z^-1 fused into the load of coset_domain.ifft_in_place (r1cs_to_qap.rs:209,223-232)
-    ntt_any(st, dom, true, A, T, H, NTT_LOAD_AB_MINUS_C, nullptr, B, C, dom.z_inv, NTT_STORE_MUL_TABLE, dom.coset_inv, zero);
+    ntt_any(st, dom, true, A, T, H, NTT_LOAD_AB_MINUS_C, nullptr, B, C, dom.z_inv, NTT_STORE_MUL_TABLE, dom.coset_inv, zero, count);
   }
 
   // The witness map of a SHARDED proof (SURVEY.md section 8e: the chains a, b, c are independent, r1cs_to_qap.rs:201-207,
@@ -730,7 +751,7 @@ struct Engine : IEngine {
       G16_CUDA(cudaMemcpyAsync(ds.p, scalars, n * 32, cudaMemcpyHostToDevice, S0.st_main));
       G16_CUDA(msm_prepare_query<F>(S0.st_main, db.template as<Affine<F>>(), (uint32_t)n, 1, 0, dm.template as<uint8_t>()));
       const MsmGeom g = with_k0(msm_geom(n, FR_BITS, (int)tune.c, 0), sizeof(F) > 48);   // caller-supplied bases: no precomputed copies
-      cudaError_t e = msm_enqueue<F, Fr>(S0.st_main, ws, g, db.template as<Affine<F>>(), dm.template as<uint8_t>(), ds.template as<uint32_t>(), 1, false, &ctr, nullptr, nullptr, nullptr, nullptr, nullptr);
+      cudaError_t e = msm_enqueue<F, Fr>(S0.st_main, ws, g, db.template as<Affine<F>>(), dm.template as<uint8_t>(), ds.template as<uint32_t>(), 1, false, &ctr, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
       if (e != cudaSuccess) { db.release(); ds.release(); dm.release(); return fail(G16_ERR_CUDA, std::string("msm_enqueue: ") + cudaGetErrorString(e)); }
       e = cudaStreamSynchronize(S0.st_main);
       db.release(); ds.release(); dm.release();
@@ -782,6 +803,7 @@ struct Engine : IEngine {
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
     have_circuit = true;
     have_pk = false;
+    tail_ready = false;
     return G16_OK;
   }
 
@@ -822,6 +844,7 @@ struct Engine : IEngine {
     if (pk->a_len < 1 || pk->b_g1_len < 1 || pk->b_g2_len < 1) return fail(G16_ERR_MALFORMED_KEY, "a/b queries must hold at least the constant-one base");
     if ((pk->h_len && !pk->h_query) || (pk->l_len && !pk->l_query)) return fail(G16_ERR_BAD_ARGUMENT, "null h/l query");
     G16_CUDA(cudaSetDevice(device));
+    tail_ready = false;
     rank = rk; world = wd;
     const uint64_t n = 1ull << L;
     const uint64_t nz1 = nvars() - 1;  // |input_assignment ++ aux_assignment|, prover.rs:85
@@ -912,6 +935,7 @@ struct Engine : IEngine {
       for (uint64_t i = 0; i + 1 < n; i++) { hs[i] = p; p = Fr::mul(p, tau); }
     }
     // --- fixed-base batch multiplications on the GPU (generator.rs:129-183) ---
+    tail_ready = false;
     rank = 0; world = 1;
     DevBuf d_s, tab1, tab2;
     const uint64_t maxs = std::max<uint64_t>(nv, n);
@@ -988,31 +1012,32 @@ struct Engine : IEngine {
 
   // ---- proving ----
   // enqueue on sl.st_main: upload z, row evaluation, witness map
-  int enqueue_witness_map(Slot& sl, const uint64_t* z, uint32_t flags) {
+  // count > 1 (batch proving): `count` assignments, nv elements apart, and as many witness maps
+  int enqueue_witness_map(Slot& sl, const uint64_t* z, uint32_t flags, uint32_t count = 1) {
     const uint64_t nv = nvars();
     int rc = ensure_circuit_domain();   // no-op unless something rebuilt `dom` for another size
     if (rc) return rc;
-    if ((rc = ensure_slot_buffers(sl, L))) return rc;
-    G16_CUDA(sl.d_z.reserve((size_t)nv * 32));
+    if ((rc = ensure_slot_buffers(sl, L, count))) return rc;
+    G16_CUDA(sl.d_z.reserve((size_t)nv * 32 * count));
     sl.tm.h2d_bytes = 0;
     G16_CUDA(cudaEventRecord(sl.ev_start, sl.st_main));
     if (flags & G16_ASSIGNMENT_ON_DEVICE) {
-      G16_CUDA(cudaMemcpyAsync(sl.d_z.p, z, nv * 32, cudaMemcpyDeviceToDevice, sl.st_main));
+      G16_CUDA(cudaMemcpyAsync(sl.d_z.p, z, nv * 32 * count, cudaMemcpyDeviceToDevice, sl.st_main));
     } else {
-      G16_CUDA(cudaMemcpyAsync(sl.d_z.p, z, nv * 32, cudaMemcpyHostToDevice, sl.st_main));
-      sl.tm.h2d_bytes = nv * 32;
+      G16_CUDA(cudaMemcpyAsync(sl.d_z.p, z, nv * 32 * count, cudaMemcpyHostToDevice, sl.st_main));
+      sl.tm.h2d_bytes = nv * 32 * count;
     }
     G16_CUDA(cudaEventRecord(sl.ev_z, sl.st_main));
     const uint32_t n = 1u << L;
     CsrDev cs[3];
     for (int m = 0; m < 3; m++) cs[m] = CsrDev{csr_rp[m].template as<uint32_t>(), csr_col[m].template as<uint32_t>(), csr_val[m].p};
     r1cs_matvec<Fr>(sl.st_main, cs, sl.d_z.template as<Fr>(), num_constraints, num_inputs, n, sl.d_a.template as<Fr>(),
-                    sl.d_b.template as<Fr>(), sl.d_c.template as<Fr>());
+                    sl.d_b.template as<Fr>(), sl.d_c.template as<Fr>(), count, (uint32_t)nv);
     ntt_launches++;
     if (sl.split_wm && nccl_comm_wm) {
       if ((rc = witness_map_split(sl))) return rc;
     } else {
-      witness_map_device(sl, dom);
+      witness_map_device(sl, dom, count);
     }
     G16_CUDA(cudaGetLastError());
     G16_CUDA(cudaEventRecord(sl.ev_h, sl.st_main));
@@ -1085,8 +1110,8 @@ struct Engine : IEngine {
         const bool wm_first = !sl.serial && (tune.wm_first > 0 || (tune.wm_first < 0 && world > 1));
         cudaEvent_t gate = (wm_first && m != M_H) ? sl.ev_h : nullptr;
         if (m == M_B2 && share) { sl.b_sorted = MsmSorted{}; sl.b_sorted.ready = sl.ev_bsort; }
-        if (m == M_B2) e = msm_enqueue<Fq2, Fr>(st, sl.ws2, sl.geom[m], q[m].bases.template as<A2>(), q[m].mask.template as<uint8_t>(), sc, world, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], share ? &sl.b_sorted : nullptr, nullptr, gate);
-        else e = msm_enqueue<Fq, Fr>(st, sl.ws1[m], sl.geom[m], q[m].bases.template as<A1>(), q[m].mask.template as<uint8_t>(), sc, world, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], nullptr, (m == M_B1 && share) ? &sl.b_sorted : nullptr, gate);
+        if (m == M_B2) e = msm_enqueue<Fq2, Fr>(st, sl.ws2, sl.geom[m], q[m].bases.template as<A2>(), q[m].mask.template as<uint8_t>(), sc, world, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], share ? &sl.b_sorted : nullptr, nullptr, gate, 0);
+        else e = msm_enqueue<Fq, Fr>(st, sl.ws1[m], sl.geom[m], q[m].bases.template as<A1>(), q[m].mask.template as<uint8_t>(), sc, world, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], nullptr, (m == M_B1 && share) ? &sl.b_sorted : nullptr, gate, 0);
         if (e != cudaSuccess) return fail(G16_ERR_CUDA, std::string("msm_enqueue: ") + cudaGetErrorString(e));
       }
       G16_CUDA(cudaEventRecord(sl.ev_m1[m], st));
@@ -1279,6 +1304,246 @@ struct Engine : IEngine {
     int rc = prove_submit(0, r, s, z, flags);
     if (rc) return rc;
     return prove_wait(0, proof);
+  }
+
+  // ---- batch proving (g16_prove_batch) ----
+  // The proofs of a group share every launch: proof k owns bucket sets k*ne .. k*ne+ne-1 of each MSM over the same resident
+  // bases (msm_digits, blockIdx.y = k), so one sort, one set of batched-affine rounds and one bucket reduction per MSM
+  // serve the group, and the group's 7 transforms are one launch per NTT pass.  Groups alternate between the two proof
+  // slots (proof_slots = 2): the host tail of group g overlaps the GPU work of group g + 1.
+  cudaEvent_t ev_batch = nullptr;   // start of the current g16_prove_batch call (timings)
+  // padded sorted entries of the largest MSM of one proof, at the largest bucket padding the rounds can ask for
+  uint64_t batch_entries_per_proof() const {
+    uint64_t e = 0;
+    for (const Query& x : q)
+      if (x.hi > x.lo) e = std::max<uint64_t>(e, x.geom.max_entries + (uint64_t)x.geom.nkeys * ((1u << MSM_BA_MAX_ROUNDS) - 1));
+    return e;
+  }
+  // device workspace of one proof of a group (upper bound): work vectors, sorted lists, partial lists, buckets and
+  // reduction scratch of every MSM, the rounds' work lists, the fixed-base scalars and products
+  uint64_t batch_bytes_per_proof() const {
+    const uint64_t n = 1ull << L;
+    uint64_t b = nvars() * 32 + 5 * n * 32 + 3 * 32 + 4 * sizeof(A1) + sizeof(A2);
+    for (int m = 0; m < 5; m++) {
+      if (q[m].hi <= q[m].lo) continue;
+      const uint64_t pt = m == M_B2 ? sizeof(P2) : sizeof(P1);
+      MsmGeom g = q[m].geom;
+      g.k0 = 8;
+      g.ba = g.ba_pad = 0;
+      MsmBaPlan bp;
+      bp.make(g);
+      b += bp.len[0] * 8 + 3 * bp.l0_threads(g) * (4 + pt) + 2 * (uint64_t)g.nkeys * pt;
+      g.ba = g.ba_pad = MSM_BA_MAX_ROUNDS;
+      bp.make(g);
+      b += (m == M_B2 ? bp.template extra_bytes<Fq2>() : bp.template extra_bytes<Fq>()) + (bp.len[0] - g.max_entries) * 8;
+    }
+    return b;
+  }
+  // geometry of `count` proofs' MSMs in one pass: the single proof's windows, k0 and rounds re-derived from the entry count
+  void batch_geoms(uint32_t count, bool share, MsmGeom* gb) const {
+    for (int m = 0; m < 5; m++) {
+      gb[m] = with_k0(msm_geom_batch(q[m].geom, count), m == M_B2, m);
+      gb[m].ba_pad = gb[m].ba;
+    }
+    if (share) gb[M_B1].ba_pad = gb[M_B2].ba_pad = std::max(gb[M_B1].ba, gb[M_B2].ba);   // one padding for the shared list
+  }
+  int ensure_tail_tables() {
+    if (tail_ready) return G16_OK;
+    P1 pa = P1::from_affine(a0), pb = P1::from_affine(b1_0);
+    P2 p2 = P2::from_affine(b2_0);
+    pa.madd(alpha_g1);
+    pb.madd(beta_g1);
+    p2.madd(beta_g2);
+    p_a = pa.to_affine();
+    p_2 = p2.to_affine();
+    const A1 gens[3] = {delta_g1, p_a, pb.to_affine()};   // TAB_D1, TAB_PA, TAB_PB
+    for (int t = 0; t < 3; t++) {
+      G16_CUDA(tail_tab[t].reserve((size_t)FB_WINDOWS * 255 * sizeof(P1)));
+      G16_CUDA((fb_batch_mul<Fq, Fr>(S0.st_main, gens[t], nullptr, 0, nullptr, tail_tab[t].template as<P1>())));
+    }
+    G16_CUDA(tail_tab[TAB_D2].reserve((size_t)FB_WINDOWS * 255 * sizeof(P2)));
+    G16_CUDA((fb_batch_mul<Fq2, Fr>(S0.st_main, delta_g2, nullptr, 0, nullptr, tail_tab[TAB_D2].template as<P2>())));
+    ctr.launches += 4;
+    G16_CUDA(cudaStreamSynchronize(S0.st_main));
+    tail_ready = true;
+    return G16_OK;
+  }
+  static size_t tail_scalar_bytes(uint32_t count) { return (size_t)3 * count * sizeof(Fr); }
+  static size_t tail_point_bytes(uint32_t count) { return (size_t)count * (4 * sizeof(A1) + sizeof(A2)); }
+  // enqueue proofs first .. first + count - 1 on the slot's streams
+  int batch_submit(Slot& sl, uint32_t first, uint32_t count, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags) {
+    const uint64_t nv = nvars(), n = 1ull << L;
+    sl.serial = (flags & G16_SERIAL_MSMS) != 0;
+    sl.batch_first = first;
+    sl.batch_count = count;
+    const size_t sc_bytes = tail_scalar_bytes(count), pt_bytes = tail_point_bytes(count);
+    G16_CUDA(sl.d_tail.reserve(sc_bytes + pt_bytes));
+    if (sl.h_tail_cap < sc_bytes + pt_bytes) {
+      if (sl.h_tail) cudaFreeHost(sl.h_tail);
+      sl.h_tail = nullptr;
+      sl.h_tail_cap = 0;
+      G16_CUDA(cudaMallocHost(&sl.h_tail, sc_bytes + pt_bytes));
+      sl.h_tail_cap = sc_bytes + pt_bytes;
+    }
+    Fr* hsc = reinterpret_cast<Fr*>(sl.h_tail);   // r[count], s[count], (r s)[count]
+    for (uint32_t k = 0; k < count; k++) {
+      hsc[k] = load_fr(r + 4 * (size_t)(first + k));
+      hsc[count + k] = load_fr(s + 4 * (size_t)(first + k));
+      hsc[2 * count + k] = Fr::mul(hsc[k], hsc[count + k]);
+    }
+    int rc;
+    {
+      NvtxSpan span_wm(SPAN_WITNESS_MAP);
+      rc = enqueue_witness_map(sl, z + (size_t)first * nv * 4, flags, count);
+    }
+    if (rc) return rc;
+    // the five fixed-base products of every proof, after the witness map on its stream (the H MSM waits for ev_h only)
+    cudaStream_t st = sl.st_main;
+    G16_CUDA(cudaMemcpyAsync(sl.d_tail.p, sl.h_tail, sc_bytes, cudaMemcpyHostToDevice, st));
+    const Fr* d_r = sl.d_tail.template as<Fr>();
+    const Fr* d_s = d_r + count;
+    const Fr* d_rs = d_r + 2 * count;
+    A1* o1 = reinterpret_cast<A1*>(sl.d_tail.template as<char>() + sc_bytes);   // r d1, (r s) d1, s P_a, r P_b
+    A2* o2 = reinterpret_cast<A2*>(o1 + 4 * (size_t)count);                       // s d2
+    G16_CUDA((fb_mul<Fq, Fr>(st, tail_tab[TAB_D1].template as<P1>(), d_r, count, o1)));
+    G16_CUDA((fb_mul<Fq, Fr>(st, tail_tab[TAB_D1].template as<P1>(), d_rs, count, o1 + count)));
+    G16_CUDA((fb_mul<Fq, Fr>(st, tail_tab[TAB_PA].template as<P1>(), d_s, count, o1 + 2 * (size_t)count)));
+    G16_CUDA((fb_mul<Fq, Fr>(st, tail_tab[TAB_PB].template as<P1>(), d_r, count, o1 + 3 * (size_t)count)));
+    G16_CUDA((fb_mul<Fq2, Fr>(st, tail_tab[TAB_D2].template as<P2>(), d_s, count, o2)));
+    ctr.launches += 5;
+    G16_CUDA(cudaMemcpyAsync(sl.h_tail + sc_bytes / 8, o1, pt_bytes, cudaMemcpyDeviceToHost, st));
+    // the five MSMs of the group, with the stream layout of submit()
+    const uint32_t* zs = sl.d_z.template as<uint32_t>();
+    const uint32_t* hs = sl.d_h.template as<uint32_t>();
+    const uint32_t* src[5] = {hs, zs + (size_t)num_inputs * 8, zs + 8, zs + 8, zs + 8};
+    const uint64_t stride[5] = {n * 8, nv * 8, nv * 8, nv * 8, nv * 8};   // 32-bit words between two proofs' scalars
+    for (int m = 0; m < 5; m++) {
+      sl.run[m] = q[m].hi > q[m].lo;
+      sl.tm.msm_pairs[m] = sl.run[m] ? (q[m].hi - q[m].lo) * count : 0;
+    }
+    const bool share = share_b_sort && sl.run[M_B1] && sl.run[M_B2];
+    batch_geoms(count, share, sl.geom);
+    const int order[5] = {M_L, M_A, M_B2, M_B1, M_H};
+    for (int oi = 0; oi < 5; oi++) {
+      const int m = order[oi];
+      NvtxSpan span_msm(span_of(m));
+      cudaStream_t sm = sl.serial ? sl.st_main : sl.st_msm[m];
+      if (!sl.serial) G16_CUDA(cudaStreamWaitEvent(sm, m == M_H ? sl.ev_h : sl.ev_z, 0));
+      G16_CUDA(cudaEventRecord(sl.ev_m0[m], sm));
+      if (sl.run[m]) {
+        const bool wm_first = !sl.serial && tune.wm_first > 0;
+        cudaEvent_t gate = (wm_first && m != M_H) ? sl.ev_h : nullptr;
+        cudaError_t e;
+        if (m == M_B2 && share) { sl.b_sorted = MsmSorted{}; sl.b_sorted.ready = sl.ev_bsort; }
+        if (m == M_B2) e = msm_enqueue<Fq2, Fr>(sm, sl.ws2, sl.geom[m], q[m].bases.template as<A2>(), q[m].mask.template as<uint8_t>(), src[m], 1, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], share ? &sl.b_sorted : nullptr, nullptr, gate, stride[m]);
+        else e = msm_enqueue<Fq, Fr>(sm, sl.ws1[m], sl.geom[m], q[m].bases.template as<A1>(), q[m].mask.template as<uint8_t>(), src[m], 1, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], nullptr, (m == M_B1 && share) ? &sl.b_sorted : nullptr, gate, stride[m]);
+        if (e != cudaSuccess) return fail(G16_ERR_CUDA, std::string("msm_enqueue: ") + cudaGetErrorString(e));
+      }
+      G16_CUDA(cudaEventRecord(sl.ev_m1[m], sm));
+    }
+    return G16_OK;
+  }
+  // wait for the slot's group, then finish its proofs on the pool (one proof per task); adds the group to `acc`
+  int batch_finish(Slot& sl, const uint64_t* r, const uint64_t* s, uint64_t* proofs, g16_timings& acc, float* host_ms) {
+    const uint32_t count = sl.batch_count, first = sl.batch_first;
+    sl.batch_count = 0;
+    for (int m = 0; m < 5 && !sl.serial; m++) G16_CUDA(cudaStreamSynchronize(sl.st_msm[m]));
+    G16_CUDA(cudaStreamSynchronize(sl.st_main));
+    const auto t0 = std::chrono::steady_clock::now();
+    const A1* o1 = reinterpret_cast<const A1*>(sl.h_tail + tail_scalar_bytes(count) / 8);
+    const A2* o2 = reinterpret_cast<const A2*>(o1 + 4 * (size_t)count);
+    std::vector<std::shared_ptr<HostPool::Ticket>> tk(count);
+    for (uint32_t k = 0; k < count; k++) {
+      tk[k] = pool->submit([&, k]() {
+        BatchTailIn<Fq, Fq2> x;
+        x.r_d1 = o1[k];
+        x.rs_d1 = o1[count + k];
+        x.s_pa = o1[2 * (size_t)count + k];
+        x.r_pb = o1[3 * (size_t)count + k];
+        x.s_d2 = o2[k];
+        P1* outs[4] = {&x.h, &x.l, &x.a, &x.b1};
+        for (int m = 0; m < 4; m++) *outs[m] = sl.run[m] ? msm_finish<Fq>(sl.ws1[m], sl.geom[m], k) : P1::inf();
+        x.b2 = sl.run[M_B2] ? msm_finish<Fq2>(sl.ws2, sl.geom[M_B2], k) : P2::inf();
+        const Fr rk = load_fr(r + 4 * (size_t)(first + k)), sk = load_fr(s + 4 * (size_t)(first + k));
+        uint32_t rc[8], sc[8];
+        fr_to_canon(rk, rc);
+        fr_to_canon(sk, sc);
+        P1 g_a, g_c;
+        P2 g2_b;
+        batch_tail(x, p_a, p_2, rc, sc, rk.is_zero(), g_a, g2_b, g_c);
+        uint64_t* pf = proofs + (size_t)(first + k) * 8 * NQ64;
+        store_a1(pf, g_a.to_affine());
+        store_a2(pf + 2 * NQ64, g2_b.to_affine());
+        store_a1(pf + 6 * NQ64, g_c.to_affine());
+      });
+    }
+    for (auto& t : tk) t->wait();
+    *host_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    float ms = 0;
+    cudaEventElapsedTime(&ms, sl.ev_start, sl.ev_z); acc.h2d_ms += ms;
+    cudaEventElapsedTime(&ms, sl.ev_z, sl.ev_h); acc.witness_map_ms += ms;
+    cudaEventElapsedTime(&ms, ev_batch, sl.ev_h);
+    acc.total_ms = std::max(acc.total_ms, ms);
+    acc.h2d_bytes += sl.tm.h2d_bytes;
+    acc.d2h_bytes += tail_point_bytes(count);
+    for (int m = 0; m < 5; m++) {
+      acc.msm_pairs[m] += sl.tm.msm_pairs[m];
+      cudaEventElapsedTime(&ms, sl.ev_m0[m], sl.ev_m1[m]); acc.msm_ms[m] += ms;
+      cudaEventElapsedTime(&ms, ev_batch, sl.ev_m0[m]);
+      acc.msm_begin_ms[m] = first == 0 ? ms : std::min(acc.msm_begin_ms[m], ms);
+      cudaEventElapsedTime(&ms, ev_batch, sl.ev_m1[m]);
+      acc.msm_end_ms[m] = std::max(acc.msm_end_ms[m], ms);
+      acc.total_ms = std::max(acc.total_ms, ms);
+      if (!sl.run[m]) continue;
+      cudaEventElapsedTime(&ms, sl.ev_a0[m], sl.ev_a1[m]); acc.msm_accum_ms[m] += ms;
+      acc.msm_entries[m] += m == M_B2 ? *sl.ws2.h_total : *sl.ws1[m].h_total;
+      acc.d2h_bytes += (m == M_B2 ? sl.ws2.plan.leaf_pts * sizeof(P2) : sl.ws1[m].plan.leaf_pts * sizeof(P1)) * sl.geom[m].sets();
+    }
+    return G16_OK;
+  }
+  int prove_batch(uint32_t count, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t group, uint32_t flags,
+                  uint64_t* proofs) override {
+    if (count == 0) return G16_OK;
+    if (!r || !s || !z || !proofs) return fail(G16_ERR_BAD_ARGUMENT, "null buffer");
+    if (!have_circuit || !have_pk) return fail(G16_ERR_BAD_ARGUMENT, "circuit and proving key must be resident");
+    if (world != 1) return fail(G16_ERR_BAD_ARGUMENT, "key is sharded: batch proving needs the whole key (world 1)");
+    G16_NOT_BUSY();
+    G16_CUDA(cudaSetDevice(device));
+    NvtxSpan span(SPAN_PROVER);
+    int rc = ensure_tail_tables();
+    if (rc) return rc;
+    size_t free_b = 0, total_b = 0;
+    G16_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const uint32_t nslots = (uint32_t)tune.proof_slots;
+    const uint32_t G = batch_group_size(count, group, batch_entries_per_proof(), batch_bytes_per_proof(), free_b, nslots);
+    const unsigned long long launches0 = ctr.launches + ntt_launches;
+    if (!ev_batch) G16_CUDA(cudaEventCreate(&ev_batch));
+    G16_CUDA(cudaEventRecord(ev_batch, slots[0].st_main));
+    g16_timings acc{};
+    float host_ms = 0;
+    int order[NSLOTS] = {-1, -1};   // slots holding a group, oldest first
+    auto finish_oldest = [&]() -> int {
+      const int si = order[0];
+      order[0] = order[1];
+      order[1] = -1;
+      return batch_finish(slots[si], r, s, proofs, acc, &host_ms);
+    };
+    for (uint32_t first = 0, gi = 0; first < count && !rc; first += G, gi++) {
+      const int si = nslots > 1 ? (int)(gi & 1) : 0;
+      if (slots[si].batch_count) rc = finish_oldest();   // the slot's previous group (with one slot: the only one)
+      if (!rc) rc = batch_submit(slots[si], first, std::min(G, count - first), r, s, z, flags);
+      if (!rc) order[order[0] < 0 ? 0 : 1] = si;
+    }
+    while (!rc && order[0] >= 0) rc = finish_oldest();
+    if (rc) {   // leave no group half-finished behind
+      cudaDeviceSynchronize();
+      for (Slot& sl : slots) sl.batch_count = 0;
+      return rc;
+    }
+    acc.host_finish_ms = host_ms;   // host work after the last group's GPU work
+    acc.launches = ctr.launches + ntt_launches - launches0;
+    tm = acc;
+    return G16_OK;
   }
   // ---- sharded proof with the exchange inside the library (g16_comm_init + g16_prove_sharded*) ----
   // Every rank holds pair i of every MSM with i mod world == rank.  Per proof a rank contributes THREE points:

@@ -45,6 +45,9 @@ struct MsmGeom {
   int ba_G;          // batched-affine: thread products per field inversion
   int ba_gcd;        // batched-affine: 1 = safegcd inversion, 0 = Fermat
   int acc_block;     // threads per block of the level-0 accumulation (32 / 64 / 128)
+  uint32_t batch;    // MSMs over the same bases in one pass (proof k owns bucket sets k*ne .. k*ne+ne-1); 0 and 1 = one
+  // bucket sets of the whole pass (a zero-initialised MsmGeom is one MSM)
+  __host__ __device__ uint32_t sets() const { return (uint32_t)ne * (batch > 1 ? batch : 1u); }
 };
 
 static constexpr int MSM_K0_MAX = 64;
@@ -73,7 +76,8 @@ inline MsmGeom msm_geom(uint64_t n, int scalar_bits, int c_override = 0, int ne_
   g.ne = (ne_req <= 0 || ne_req > g.W) ? g.W : ne_req;
   g.copies = (g.W + g.ne - 1) / g.ne;
   g.B = 1u << (g.c - 1);
-  g.nkeys = (uint32_t)g.ne * g.B;
+  g.batch = 1;
+  g.nkeys = g.sets() * g.B;
   g.max_entries = (uint64_t)n * g.W;
   g.k0 = MSM_K0_MAX;
   g.ba = 0;
@@ -84,18 +88,30 @@ inline MsmGeom msm_geom(uint64_t n, int scalar_bits, int c_override = 0, int ne_
   g.acc_block = 128;
   return g;
 }
+// `batch` MSMs of one geometry over the same bases, sorted and reduced together (k0 / rounds are re-derived by the caller)
+inline MsmGeom msm_geom_batch(MsmGeom g, uint32_t batch) {
+  g.batch = batch;
+  g.nkeys = g.sets() * g.B;
+  g.max_entries = (uint64_t)g.n * g.W * (batch > 1 ? batch : 1u);
+  return g;
+}
 
 // ------------------------------------------------------------------------------------------------
 // 1/3. digit extraction + histogram / scatter
 // ------------------------------------------------------------------------------------------------
 // Signed-digit recoding of a canonical scalar k < 2^bits:  k = sum_w d_w 2^(c w), d_w in [-2^(c-1), 2^(c-1)].
+// blockIdx.y = MSM k of a batch: its scalars start batch_stride 32-bit words after those of MSM k-1, its keys lie in bucket
+// sets k*ne .. k*ne+ne-1; the sorted index is the same (copy * n + i | sign) for every k, since the bases are shared.
 template <class FrF, bool SCATTER>
 __global__ void __launch_bounds__(256) msm_digits(const uint32_t* __restrict__ scalars, uint32_t scalar_stride, int scalars_mont,
                                                   const uint8_t* __restrict__ skip, MsmGeom g,
                                                   uint32_t* __restrict__ counters,  // COUNT: histogram; SCATTER: cursors
-                                                  uint32_t* __restrict__ sidx, uint32_t* __restrict__ skey) {
+                                                  uint32_t* __restrict__ sidx, uint32_t* __restrict__ skey,
+                                                  uint64_t batch_stride) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t lane = threadIdx.x & 31;
+  const uint32_t set0 = blockIdx.y * (uint32_t)g.ne;
+  scalars += blockIdx.y * batch_stride;
   bool live = i < g.n;
   FrF s = FrF::zero();
   if (live) {
@@ -123,7 +139,7 @@ __global__ void __launch_bounds__(256) msm_digits(const uint32_t* __restrict__ s
     if (raw > g.B) { raw = (1u << g.c) - raw; neg = 1; carry = 1; }
     const bool emit = live && raw != 0;
     const int e = w % g.ne, j = w / g.ne;
-    const uint32_t key = emit ? (uint32_t)e * g.B + (raw - 1) : MSM_INVALID;
+    const uint32_t key = emit ? (set0 + (uint32_t)e) * g.B + (raw - 1) : MSM_INVALID;
     // warp-aggregated atomic: one atomicAdd per distinct key in the warp
     const uint32_t peers = __match_any_sync(0xffffffffu, key);
     if (emit) {
@@ -650,10 +666,10 @@ struct MsmWorkspace {
       plan_m = g.c - 1;
       plan_ne = g.ne;
     }
-    G16_TRY(red_inner.reserve((plan.inner_pts * g.ne + 1) * sizeof(XYZZ<F>)));
-    G16_TRY(red_leaf.reserve((plan.leaf_pts * g.ne + 1) * sizeof(XYZZ<F>)));
+    G16_TRY(red_inner.reserve((plan.inner_pts * g.sets() + 1) * sizeof(XYZZ<F>)));
+    G16_TRY(red_leaf.reserve((plan.leaf_pts * g.sets() + 1) * sizeof(XYZZ<F>)));
     if (!h_total) G16_TRY(cudaMallocHost(&h_total, 16));
-    const size_t need = plan.leaf_pts * g.ne;
+    const size_t need = plan.leaf_pts * g.sets();
     if (h_cap < need) {
       if (h_leaf) cudaFreeHost(h_leaf);
       h_leaf = nullptr;
@@ -691,11 +707,13 @@ struct MsmSorted {
   const uint32_t* total0 = nullptr;
   cudaEvent_t ready = nullptr;   // recorded on the lender's stream once the list is complete
 };
+// A batched geometry (g.batch > 1) runs g.batch MSMs over the same bases in one pass: MSM k reads its scalars at
+// d_scalars + k * batch_stride (32-bit words) and its result is msm_finish(ws, g, k).
 template <class F, class FrF>
 cudaError_t msm_enqueue(cudaStream_t st, MsmWorkspace<F>& ws, const MsmGeom& g, const Affine<F>* d_bases,
                         const uint8_t* d_skip, const uint32_t* d_scalars, uint32_t scalar_stride, bool scalars_mont,
                         MsmCounters* ctr, cudaEvent_t ev_acc0, cudaEvent_t ev_acc1, MsmSorted* lend, const MsmSorted* borrow,
-                        cudaEvent_t gate_accum) {
+                        cudaEvent_t gate_accum, uint64_t batch_stride) {
   cudaError_t e;
   if (g.n == 0) return cudaSuccess;
   if ((e = ws.prepare(g)) != cudaSuccess) return e;
@@ -719,14 +737,14 @@ cudaError_t msm_enqueue(cudaStream_t st, MsmWorkspace<F>& ws, const MsmGeom& g, 
     total0 = borrow->total0;
   } else {
     cudaMemsetAsync(counters, 0, (size_t)(g.nkeys + 1) * 4, st);
-    const uint32_t nb = (g.n + 255) / 256;
-    msm_digits<FrF, false><<<nb, 256, 0, st>>>(d_scalars, scalar_stride, scalars_mont ? 1 : 0, d_skip, g, counters, nullptr, nullptr);
+    const dim3 nb((g.n + 255) / 256, g.batch > 1 ? g.batch : 1u);
+    msm_digits<FrF, false><<<nb, 256, 0, st>>>(d_scalars, scalar_stride, scalars_mont ? 1 : 0, d_skip, g, counters, nullptr, nullptr, batch_stride);
     const uint32_t pad_mask = bp.pad > 0 ? (1u << bp.pad) - 1 : 0;
     const uint32_t sb = (g.nkeys + SCAN_BLOCK - 1) / SCAN_BLOCK;
     msm_scan_blocks<<<sb, 1024, 0, st>>>(counters, g.nkeys, offsets, blocktot, pad_mask);
     msm_scan_tops<<<1, 1024, 0, st>>>(blocktot, sb, offsets + g.nkeys);
     msm_scan_fix<<<sb, 1024, 0, st>>>(offsets, g.nkeys, blocktot, counters);
-    msm_digits<FrF, true><<<nb, 256, 0, st>>>(d_scalars, scalar_stride, scalars_mont ? 1 : 0, d_skip, g, counters, sidx, skey);
+    msm_digits<FrF, true><<<nb, 256, 0, st>>>(d_scalars, scalar_stride, scalars_mont ? 1 : 0, d_skip, g, counters, sidx, skey, batch_stride);
     nl += 5;
     if (pad_mask) {
       msm_pad_fill<<<(g.nkeys + 255) / 256, 256, 0, st>>>(counters, offsets, g.nkeys, sidx, skey);
@@ -802,7 +820,7 @@ cudaError_t msm_enqueue(cudaStream_t st, MsmWorkspace<F>& ws, const MsmGeom& g, 
   auto arr = [&](int id) -> XYZZ<F>* {
     if (id == 0) return buckets;
     const MsmRedNode& nd = pl.nodes[id];
-    return (nd.leaf ? leaf : inner) + nd.off * g.ne;
+    return (nd.leaf ? leaf : inner) + nd.off * g.sets();
   };
   // one launch per depth of the plan: the row and column sums of every non-leaf node at that depth are independent jobs
   {
@@ -840,7 +858,7 @@ cudaError_t msm_enqueue(cudaStream_t st, MsmWorkspace<F>& ws, const MsmGeom& g, 
           jb.len = rows ? (1u << nd.a0) : (1u << nd.a1);
           jb.stride = rows ? 1u : (1u << nd.a0);
           jb.base_mul = rows ? (1u << nd.a0) : 1u;
-          jb.n_out = jb.per_win_out * (uint32_t)g.ne;
+          jb.n_out = jb.per_win_out * g.sets();
           uint32_t tpo = TPB;
           while (tpo > jb.len) tpo >>= 1;
           jb.tpo = tpo;
@@ -855,7 +873,7 @@ cudaError_t msm_enqueue(cudaStream_t st, MsmWorkspace<F>& ws, const MsmGeom& g, 
   if (ctr) ctr->launches += nl;
   const XYZZ<F>* leaf_src = pl.nodes[0].leaf ? buckets : leaf;
   cudaMemcpyAsync(ws.h_total, total0, 4, cudaMemcpyDeviceToHost, st);
-  e = cudaMemcpyAsync(ws.h_leaf, leaf_src, pl.leaf_pts * g.ne * sizeof(XYZZ<F>), cudaMemcpyDeviceToHost, st);
+  e = cudaMemcpyAsync(ws.h_leaf, leaf_src, pl.leaf_pts * g.sets() * sizeof(XYZZ<F>), cudaMemcpyDeviceToHost, st);
   if (e != cudaSuccess) return e;
   return cudaGetLastError();
 }
@@ -866,13 +884,13 @@ template <class F>
 struct MsmHostRed {
   const MsmWorkspace<F>& ws;
   const MsmGeom& g;
-  int w;
+  int w;   // bucket set (of all g.sets() in the pass)
   // returns T(node) = sum_i (i + 1) X_i and sets total = sum_i X_i
   XYZZ<F> T(int id, XYZZ<F>& total) const {
     const MsmRedNode& nd = ws.plan.nodes[id];
     if (nd.leaf) {
       const size_t len = (size_t)1 << nd.log_len;
-      const XYZZ<F>* x = ws.h_leaf + nd.off * g.ne + (size_t)w * len;
+      const XYZZ<F>* x = ws.h_leaf + nd.off * g.sets() + (size_t)w * len;
       XYZZ<F> running = XYZZ<F>::inf(), acc = XYZZ<F>::inf();
       for (size_t i = len; i-- > 0;) {
         running.add(x[i]);
@@ -892,13 +910,14 @@ struct MsmHostRed {
     return tr;
   }
 };
+// `k`: which MSM of a batched pass (its bucket sets are k*ne .. k*ne+ne-1)
 template <class F>
-XYZZ<F> msm_finish(const MsmWorkspace<F>& ws, const MsmGeom& g) {
+XYZZ<F> msm_finish(const MsmWorkspace<F>& ws, const MsmGeom& g, uint32_t k = 0) {
   XYZZ<F> acc = XYZZ<F>::inf();
   if (g.n == 0) return acc;
   for (int w = g.ne - 1; w >= 0; w--) {
-    for (int k = 0; k < g.c; k++) acc.dbl_inplace();
-    MsmHostRed<F> hr{ws, g, w};
+    for (int i = 0; i < g.c; i++) acc.dbl_inplace();
+    MsmHostRed<F> hr{ws, g, (int)(k * g.ne) + w};
     XYZZ<F> tot;
     acc.add(hr.T(0, tot));
   }
@@ -958,14 +977,21 @@ cudaError_t fb_batch_mul(cudaStream_t st, const Affine<F>& gen, const FrF* d_sca
   if (cnt) fb_mul_kernel<F, FrF><<<(unsigned)((cnt + 127) / 128), 128, 0, st>>>(d_table, d_scalars, (uint32_t)cnt, d_out);
   return cudaGetLastError();
 }
+// d_out[i] = d_scalars[i] * gen for a table fb_batch_mul already built (batch proving: one table per key point)
+template <class F, class FrF>
+cudaError_t fb_mul(cudaStream_t st, const XYZZ<F>* d_table, const FrF* d_scalars, uint64_t cnt, Affine<F>* d_out) {
+  if (cnt) fb_mul_kernel<F, FrF><<<(unsigned)((cnt + 127) / 128), 128, 0, st>>>(d_table, d_scalars, (uint32_t)cnt, d_out);
+  return cudaGetLastError();
+}
 
 // Explicit-instantiation lists: kernels are compiled in their own translation units (k_msm_*.cu), the engine TU only
 // declares them `extern template` (keeps ptxas work parallel across make jobs).
 #define G16_MSM_TEMPLATES(X, F, FrF)                                                                                     \
   X cudaError_t msm_enqueue<F, FrF>(cudaStream_t, MsmWorkspace<F>&, const MsmGeom&, const Affine<F>*, const uint8_t*,    \
                                     const uint32_t*, uint32_t, bool, MsmCounters*, cudaEvent_t, cudaEvent_t, MsmSorted*, \
-                                    const MsmSorted*, cudaEvent_t);                                                      \
+                                    const MsmSorted*, cudaEvent_t, uint64_t);                                            \
   X cudaError_t msm_prepare_query<F>(cudaStream_t, Affine<F>*, uint32_t, int, int, uint8_t*);                            \
-  X cudaError_t fb_batch_mul<F, FrF>(cudaStream_t, const Affine<F>&, const FrF*, uint64_t, Affine<F>*, XYZZ<F>*);
+  X cudaError_t fb_batch_mul<F, FrF>(cudaStream_t, const Affine<F>&, const FrF*, uint64_t, Affine<F>*, XYZZ<F>*);       \
+  X cudaError_t fb_mul<F, FrF>(cudaStream_t, const XYZZ<F>*, const FrF*, uint64_t, Affine<F>*);
 
 }  // namespace g16

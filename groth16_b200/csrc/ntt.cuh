@@ -37,6 +37,7 @@ struct NttPass {
   int L, s0, k, logC;
   int load_mode, store_mode;
   int bitrev_store;  // 1 on the last pass
+  uint64_t vstride;  // elements between the vectors of a batch: blockIdx.y selects in / in_b / in_c / out; tables are shared
 };
 
 template <class Fr>
@@ -72,16 +73,17 @@ __global__ void __launch_bounds__(256) ntt_pass_kernel(NttPass<Fr> a) {
   const uint32_t top = blockIdx.x / lowblks, lowblk = blockIdx.x % lowblks;
   const uint64_t gbase = ((uint64_t)top << (a.L - a.s0)) + ((uint64_t)lowblk << logC);
   const uint32_t T = blockDim.x;
+  const uint64_t voff = blockIdx.y * a.vstride;
 
   // ---- load ----
   for (uint32_t e = threadIdx.x; e < tile; e += T) {
     const uint32_t mid = e >> logC, cl = e & (C - 1);
     const uint64_t gi = gbase + ((uint64_t)mid << low_bits) + cl;
-    Fr x = ntt_ldg(a.in + gi);
+    Fr x = ntt_ldg(a.in + voff + gi);
     if (a.load_mode == NTT_LOAD_MUL_TABLE) {
       x = Fr::mul(x, ntt_ldg(a.ltab + gi));
     } else if (a.load_mode == NTT_LOAD_AB_MINUS_C) {
-      Fr y = ntt_ldg(a.in_b + gi), z = ntt_ldg(a.in_c + gi);
+      Fr y = ntt_ldg(a.in_b + voff + gi), z = ntt_ldg(a.in_c + voff + gi);
       x = Fr::mul(Fr::sub(Fr::mul(x, y), z), a.lcst);
     }
 #pragma unroll
@@ -124,7 +126,7 @@ __global__ void __launch_bounds__(256) ntt_pass_kernel(NttPass<Fr> a) {
     if (a.bitrev_store && a.L > 0) gi = __brevll(gi) >> (64 - a.L);
     if (a.store_mode == NTT_STORE_MUL_CONST) x = Fr::mul(x, a.scst);
     else if (a.store_mode == NTT_STORE_MUL_TABLE) x = Fr::mul(x, ntt_ldg(a.stab + gi));
-    ntt_stg(a.out + gi, x);
+    ntt_stg(a.out + voff + gi, x);
   }
 }
 
@@ -144,6 +146,7 @@ __global__ void ntt_powers_kernel(Fr* out, uint64_t n, Fr base, Fr c0) {
 
 // Sparse rows times the assignment (evaluate_constraint, r1cs_to_qap.rs:28-67) for the three matrices at once,
 // plus the instance copy a[nc + i] = z[i] (r1cs_to_qap.rs:195-199) and the zero tail up to the domain size.
+// blockIdx.y = proof k of a batch: it reads z + k * nv and writes a, b, c + k * n.
 struct CsrDev {
   const uint32_t* row_ptr;  // nc + 1
   const uint32_t* col;
@@ -152,9 +155,13 @@ struct CsrDev {
 template <class Fr>
 __global__ void __launch_bounds__(256) r1cs_matvec_kernel(CsrDev A, CsrDev B, CsrDev Cm, const Fr* __restrict__ z,
                                                           uint32_t nc, uint32_t num_inputs, uint32_t n, Fr* a, Fr* b,
-                                                          Fr* c) {
+                                                          Fr* c, uint32_t nv) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  z += (size_t)blockIdx.y * nv;
+  a += (size_t)blockIdx.y * n;
+  b += (size_t)blockIdx.y * n;
+  c += (size_t)blockIdx.y * n;
   Fr ra = Fr::zero(), rb = Fr::zero(), rc = Fr::zero();
   if (i < nc) {
     const CsrDev* ms[3] = {&A, &B, &Cm};
@@ -287,10 +294,11 @@ inline NttPlan ntt_plan(int L) {
 // Full transform, natural order in -> natural order out.  `src` is read by the first pass only; `work` (n
 // elements) carries the intermediate passes in place; the last pass scatters into `dst` (dst != work; dst may
 // equal src when there is more than one pass).  For a single-pass transform src -> dst directly (dst != src).
+// nvec > 1: the same transform of nvec vectors stored n elements apart in every buffer, one launch per pass.
 template <class Fr>
 void ntt_run(cudaStream_t st, const NttDomain<Fr>& d, bool inverse, const Fr* src, Fr* work, Fr* dst, int load_mode,
              const Fr* ltab, const Fr* in_b, const Fr* in_c, const Fr& load_cst, int store_mode, const Fr* stab,
-             const Fr& store_cst, unsigned long long* launches) {
+             const Fr& store_cst, unsigned long long* launches, uint32_t nvec) {
   const NttPlan p = ntt_plan(d.L);
   int s0 = 0;
   for (int i = 0; i < p.npass; i++) {
@@ -312,28 +320,30 @@ void ntt_run(cudaStream_t st, const NttDomain<Fr>& d, bool inverse, const Fr* sr
     a.load_mode = first ? load_mode : NTT_LOAD_PLAIN;
     a.store_mode = last ? store_mode : NTT_STORE_PLAIN;
     a.bitrev_store = last ? 1 : 0;
+    a.vstride = nvec > 1 ? d.n : 0;
     const int tile_log = a.k + a.logC;
     const uint64_t blocks = d.n >> tile_log;
     uint32_t threads = (1u << tile_log) / 2;
     if (threads > 256) threads = 256;
     if (threads < 32) threads = 32;
-    ntt_pass_kernel<Fr><<<(unsigned)blocks, threads, 0, st>>>(a);
+    ntt_pass_kernel<Fr><<<dim3((unsigned)blocks, nvec > 1 ? nvec : 1u), threads, 0, st>>>(a);
     if (launches) (*launches)++;
     s0 += a.k;
   }
 }
 
 
+// `count` assignments of nv elements each (z, contiguous) -> count row evaluations of n elements each (a, b, c)
 template <class Fr>
 void r1cs_matvec(cudaStream_t st, const CsrDev* cs, const Fr* z, uint32_t nc, uint32_t num_inputs, uint32_t n, Fr* a, Fr* b,
-                 Fr* c) {
-  r1cs_matvec_kernel<Fr><<<(n + 255) / 256, 256, 0, st>>>(cs[0], cs[1], cs[2], z, nc, num_inputs, n, a, b, c);
+                 Fr* c, uint32_t count, uint32_t nv) {
+  r1cs_matvec_kernel<Fr><<<dim3((n + 255) / 256, count > 1 ? count : 1u), 256, 0, st>>>(cs[0], cs[1], cs[2], z, nc, num_inputs, n, a, b, c, nv);
 }
 
 #define G16_NTT_TEMPLATES(X, Fr)                                                                                       \
   X void ntt_run<Fr>(cudaStream_t, const NttDomain<Fr>&, bool, const Fr*, Fr*, Fr*, int, const Fr*, const Fr*, const Fr*, \
-                     const Fr&, int, const Fr*, const Fr&, unsigned long long*);                                       \
+                     const Fr&, int, const Fr*, const Fr&, unsigned long long*, uint32_t);                             \
   X cudaError_t ntt_domain_build<Fr>(NttDomain<Fr>&, int, cudaStream_t, unsigned long long*);                          \
-  X void r1cs_matvec<Fr>(cudaStream_t, const CsrDev*, const Fr*, uint32_t, uint32_t, uint32_t, Fr*, Fr*, Fr*);
+  X void r1cs_matvec<Fr>(cudaStream_t, const CsrDev*, const Fr*, uint32_t, uint32_t, uint32_t, Fr*, Fr*, Fr*, uint32_t, uint32_t);
 
 }  // namespace g16

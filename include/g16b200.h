@@ -152,6 +152,18 @@ int g16_prove_partial_wait(g16_ctx* ctx, int slot, uint64_t* partial_out);
 /* limbs per partial record: 4*2*N64 + 4*N64 */
 int g16_partial_limbs(const g16_ctx* ctx);
 
+/* Batch proving (no reference counterpart: ark-groth16 proves one proof per call): `count` proofs of the resident circuit
+ * under the resident key, one call.  Proof i is bit-identical to
+ * g16_prove(ctx, r + 4 i, s + 4 i, full_assignments + 4 i nv, flags, proofs_out + 8 N64 i), nv = num_inputs + num_witness.
+ * r, s: count Montgomery Fr each.  full_assignments: count * nv Montgomery Fr (host, or device with
+ * G16_ASSIGNMENT_ON_DEVICE).  proofs_out: count * 8 * N64 limbs.  group: at most this many proofs share one pass of the
+ * kernels (0 = automatic: as many as fit); results never depend on it.  Sharded keys (world > 1) are refused, and so is a
+ * call while a proof is in flight in either slot.  count == 0 returns G16_OK and touches nothing.  Afterwards
+ * g16_get_timings describes the whole call: total_ms is its device span, msm_pairs / msm_entries are summed over the batch,
+ * launches counts its kernels, host_finish_ms is the host time after the last group's GPU work. */
+int g16_prove_batch(g16_ctx* ctx, uint32_t count, const uint64_t* r, const uint64_t* s, const uint64_t* full_assignments,
+                    uint32_t group, uint32_t flags, uint64_t* proofs_out);
+
 /* Sharded proving with the exchange INSIDE the library: one NCCL all-gather (over NVLink / NVSwitch) of three partial points
  * per rank, issued by the library on its own stream (SURVEY.md section 8e; no reference counterpart -- ark-groth16 is a
  * single-process CPU prover).  One process per GPU:

@@ -325,6 +325,40 @@ impl<E: SwPairing> B200Prover<E> {
         self.create_proof_with_reduction(circuit, pk, r, s)
     }
 
+    /// Many proofs of the resident circuit in one call (g16_prove_batch; no reference counterpart).  Proof i equals
+    /// `create_proof_with_reduction_and_matrices` with (rs[i], ss[i], assignments[i]).
+    pub fn create_proofs_batch(
+        &self,
+        rs: &[E::ScalarField],
+        ss: &[E::ScalarField],
+        assignments: &[Vec<E::ScalarField>],
+    ) -> R1CSResult<Vec<Proof<E>>> {
+        let count = assignments.len();
+        if rs.len() != count || ss.len() != count || assignments.iter().any(|z| z.len() != self.num_variables) {
+            return Err(SynthesisError::MalformedVerifyingKey);
+        }
+        if count == 0 {
+            return Ok(Vec::new());
+        }
+        let z: Vec<E::ScalarField> = assignments.concat();
+        let w = 8 * self.fq_limbs;
+        let mut out = ark_std::vec![0u64; count * w];
+        status(unsafe {
+            sys::g16_prove_batch(self.ctx, count as u32, scalars_ptr(rs), scalars_ptr(ss), scalars_ptr(&z), 0, 0, out.as_mut_ptr())
+        })?;
+        Ok(out.chunks(w).map(|p| self.proof_from_limbs(p)).collect())
+    }
+    /// `create_proofs_batch` with fresh randomness: for each proof `r` is sampled before `s`, as src/prover.rs:146-147.
+    pub fn create_random_proofs_batch(&self, assignments: &[Vec<E::ScalarField>], rng: &mut impl Rng) -> R1CSResult<Vec<Proof<E>>> {
+        let mut rs = Vec::with_capacity(assignments.len());
+        let mut ss = Vec::with_capacity(assignments.len());
+        for _ in assignments {
+            rs.push(E::ScalarField::rand(rng));
+            ss.push(E::ScalarField::rand(rng));
+        }
+        self.create_proofs_batch(&rs, &ss, assignments)
+    }
+
     /// Multi-GPU, first half: this rank's five partial MSM sums ([h, l, a, b_g1] G1 affine, then b_g2 G2 affine).
     pub fn prove_partial(&self, r: E::ScalarField, full_assignment: &[E::ScalarField]) -> R1CSResult<Vec<u64>> {
         let mut out = ark_std::vec![0u64; unsafe { sys::g16_partial_limbs(self.ctx) } as usize];

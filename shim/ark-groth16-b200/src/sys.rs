@@ -122,6 +122,7 @@ extern "C" {
     pub fn g16_prove_assemble_prepare(ctx: *mut g16_ctx, r: *const u64, s: *const u64) -> c_int;
     pub fn g16_prove_submit(ctx: *mut g16_ctx, slot: c_int, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32) -> c_int;
     pub fn g16_prove_wait(ctx: *mut g16_ctx, slot: c_int, proof_out: *mut u64) -> c_int;
+    pub fn g16_prove_batch(ctx: *mut g16_ctx, count: u32, r: *const u64, s: *const u64, full_assignments: *const u64, group: u32, flags: u32, proofs_out: *mut u64) -> c_int;
     pub fn g16_prove_partial_submit(ctx: *mut g16_ctx, slot: c_int, r: *const u64, full_assignment: *const u64, flags: u32) -> c_int;
     pub fn g16_prove_partial_wait(ctx: *mut g16_ctx, slot: c_int, partial_out: *mut u64) -> c_int;
     pub fn g16_comm_unique_id(out128: *mut u8) -> c_int;
