@@ -1,5 +1,5 @@
-// batch.cuh -- host rules of batch proving (g16_prove_batch): how many proofs share one pass of the kernels, and the
-// per-proof tail that turns the five MSM results and the five fixed-base products of one proof into its group elements.
+// batch.cuh -- host rules of proving: how many proofs of a batch (g16_prove_batch) share one pass of the kernels, and the
+// tail every prover path shares, which turns a proof's MSM results and its five key products into its group elements.
 // Pure host code over the field / curve templates, so tests/host/batch_plan_check.cu checks it without a GPU.
 #pragma once
 #include <algorithm>
@@ -32,41 +32,38 @@ inline uint32_t batch_group_size(uint32_t count, uint32_t group, uint64_t entrie
   return (uint32_t)std::max<uint64_t>(1, g);
 }
 
-// The (r, s)-only terms of a proof, regrouped so that every scalar multiplication by r or s of a KEY point is one
-// fixed-base product computed on the GPU for the whole batch (prover.rs:76-131, with P_a = a_query[0] + alpha_g1,
-// P_b = b_g1_query[0] + beta_g1, P_2 = b_g2_query[0] + beta_g2):
+// The tail of every proof (prover.rs:76-131), regrouped so that each scalar multiplication of a KEY point by r, s or r s
+// is one of five key products, with P_a = a_query[0] + alpha_g1, P_b = b_g1_query[0] + beta_g1 and
+// P_2 = b_g2_query[0] + beta_g2:
 //   g_a  = r d1 + P_a + A
 //   g2_b = s d2 + P_2 + B2
-//   g_c  = (r s) d1 + s P_a + r P_b + s A + r B1 + L + H
+//   g_c  = (r s) d1 + s P_a + r P_b + C,      C = s A + r B1 + L + H
 // prover.rs forms g_c = s g_a + r g1_b - (r s) d1 + L + H with g1_b = s d1 + P_b + B1; expanding gives the line above
-// (when r == 0, prover.rs skips g1_b: every r term is the identity here too).  The affine result is unique, so the bytes
-// equal g16_prove's.
+// (when r == 0, prover.rs skips g1_b: r P_b and r B1 are the identity here too).  A, B2 and C are sums over the ranks
+// when the key is sharded.  The affine result is unique, so the bytes equal the prover.rs order's.
 template <class Fq, class Fq2>
-struct BatchTailIn {
-  Affine<Fq> r_d1, rs_d1, s_pa, r_pb;   // fixed-base products of this proof
-  Affine<Fq2> s_d2;
-  XYZZ<Fq> a, b1, l, h;                 // MSM results of this proof
-  XYZZ<Fq2> b2;
+struct KeyProducts {
+  XYZZ<Fq> r_d1, rs_d1, s_pa, r_pb;
+  XYZZ<Fq2> s_d2;
 };
-// r, s: canonical (not Montgomery) 32-bit limbs
 template <class Fq, class Fq2>
-void batch_tail(const BatchTailIn<Fq, Fq2>& x, const Affine<Fq>& p_a, const Affine<Fq2>& p_2, const uint32_t r[8],
-                const uint32_t s[8], bool r_zero, XYZZ<Fq>& g_a, XYZZ<Fq2>& g2_b, XYZZ<Fq>& g_c) {
-  g_a = XYZZ<Fq>::from_affine(x.r_d1);
-  g_a.madd(p_a);
-  g_a.add(x.a);
-  g2_b = XYZZ<Fq2>::from_affine(x.s_d2);
-  g2_b.madd(p_2);
-  g2_b.add(x.b2);
-  g_c = x.a.mul_u32(s, 8);
-  g_c.madd(x.rs_d1);
-  g_c.madd(x.s_pa);
-  if (!r_zero) {
-    g_c.madd(x.r_pb);
-    g_c.add(x.b1.mul_u32(r, 8));
-  }
-  g_c.add(x.l);
-  g_c.add(x.h);
+struct ProofPoints {
+  XYZZ<Fq> g_a;
+  XYZZ<Fq2> g2_b;
+  XYZZ<Fq> g_c;
+};
+template <class Fq, class Fq2>
+ProofPoints<Fq, Fq2> proof_tail(const KeyProducts<Fq, Fq2>& k, const Affine<Fq>& p_a, const Affine<Fq2>& p_2,
+                                const XYZZ<Fq>& a, const XYZZ<Fq2>& b2, const XYZZ<Fq>& c) {
+  ProofPoints<Fq, Fq2> p{k.r_d1, k.s_d2, k.rs_d1};
+  p.g_a.madd(p_a);
+  p.g_a.add(a);
+  p.g2_b.madd(p_2);
+  p.g2_b.add(b2);
+  p.g_c.add(k.s_pa);
+  p.g_c.add(k.r_pb);
+  p.g_c.add(c);
+  return p;
 }
 
 }  // namespace g16

@@ -2,7 +2,8 @@
 //
 // Mirrors, function by function, what /root/reference does between `create_proof_with_reduction_and_matrices`
 // (prover.rs:26-51) and `Proof{a,b,c}` (prover.rs:127-131); the heavy steps are the CUDA kernels of ntt.cuh and
-// msm.cuh, the O(1) tail (six scalar multiplications, sums, into_affine) runs on the host with the same field code.
+// msm.cuh, the O(1) tail (scalar multiplications by r and s, sums, into_affine; batch.cuh) runs on the host with the
+// same field code.
 #pragma once
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>       // header-only NVTX v3: no-ops unless a profiler injects itself
@@ -185,10 +186,7 @@ struct Engine : IEngine {
   int device = 0;
   // Everything one in-flight proof owns: streams, events, work vectors, MSM workspaces, timings.  Two slots allow a
   // software pipeline (g16_prove_submit / g16_prove_wait): the latency-bound tail of proof i overlaps the bulk of proof i+1.
-  // (r, s, key)-only parts of the proof, computed on pool threads while the GPU works (prover.rs:76,90-92,100-101,112-113):
-  //   ga0 = r*delta_g1 + a_query[0] + alpha_g1        s_ga0 = s * ga0            neg_rs_d1 = -(r*s) * delta_g1
-  //   r_gb0 = r * (s*delta_g1 + b_g1_query[0] + beta_g1)   (identity when r == 0)   gb2_0 = s*delta_g2 + b_g2_query[0] + beta_g2
-  struct FixedMuls { P1 ga0, s_ga0, r_gb0, neg_rs_d1; P2 gb2_0; };
+  using Products = KeyProducts<Fq, Fq2>;
   // MSM results of this rank; sa = s * a and rb1 = r * b1 are formed by the finisher threads of the A / B-in-G1 MSMs as soon
   // as those MSMs are done (scaled == true), i.e. while the H MSM is still running, instead of after everything.
   struct Partials { P1 h, l, a, b1; P2 b2; P1 sa, rb1; bool scaled = false; };
@@ -207,8 +205,8 @@ struct Engine : IEngine {
     bool run[5] = {};
     MsmGeom geom[5] = {};
     Fr r, s;
-    FixedMuls fx;
-    std::shared_ptr<HostPool::Ticket> helper, helper2;   // (r, s)-only scalar multiplications in flight on the pool
+    Products kp;
+    std::shared_ptr<HostPool::Ticket> helper, helper2;   // key products in flight on the pool
     unsigned long long launches0 = 0;
     // batch proving (g16_prove_batch): the group this slot holds, and its fixed-base products
     uint32_t batch_first = 0, batch_count = 0;
@@ -472,15 +470,16 @@ struct Engine : IEngine {
                                   x.mask.template as<uint8_t>()));
     return G16_OK;
   }
-  A1 a0, b1_0, alpha_g1, beta_g1, delta_g1;
-  A2 b2_0, beta_g2, delta_g2;
-  // batch proving: fixed-base tables of d1, P_a = a0 + alpha_g1, P_b = b1_0 + beta_g1 (G1) and d2 (G2), built by the first
-  // g16_prove_batch under a key and dropped whenever the circuit or key changes
+  A1 alpha_g1, beta_g1, delta_g1;
+  A2 beta_g2, delta_g2;
+  // the key points of the proof tail (batch.cuh): a_query[0] + alpha_g1, b_g1_query[0] + beta_g1, b_g2_query[0] + beta_g2
+  A1 p_a, p_b;
+  A2 p_2;
+  // batch proving: fixed-base tables of d1, P_a, P_b (G1) and d2 (G2), built by the first g16_prove_batch under a key and
+  // dropped whenever the circuit or key changes
   enum { TAB_D1 = 0, TAB_PA = 1, TAB_PB = 2, TAB_D2 = 3 };
   DevBuf tail_tab[4];
   bool tail_ready = false;
-  A1 p_a;
-  A2 p_2;
   // setup-only extras for pk_export
   A2 gamma_g2;
   DevBuf d_gamma_abc;
@@ -835,6 +834,17 @@ struct Engine : IEngine {
     return finish_query<F>(x);
   }
   uint64_t nvars() const { return (uint64_t)num_inputs + num_witness; }
+  // a_q0, b1_q0, b2_q0: element 0 of a_query, b_g1_query, b_g2_query; alpha_g1, beta_g1, beta_g2 already set
+  void set_tail_points(const A1& a_q0, const A1& b1_q0, const A2& b2_q0) {
+    P1 pa = P1::from_affine(a_q0), pb = P1::from_affine(b1_q0);
+    P2 p2 = P2::from_affine(b2_q0);
+    pa.madd(alpha_g1);
+    pb.madd(beta_g1);
+    p2.madd(beta_g2);
+    p_a = pa.to_affine();
+    p_b = pb.to_affine();
+    p_2 = p2.to_affine();
+  }
   int pk_load(const g16_pk_desc* pk, uint32_t rk, uint32_t wd) override {
     if (!have_circuit) return fail(G16_ERR_BAD_ARGUMENT, "g16_circuit_load must precede g16_pk_load");
     if (!pk || wd == 0 || rk >= wd) return fail(G16_ERR_BAD_ARGUMENT, "bad pk / rank / world");
@@ -862,9 +872,9 @@ struct Engine : IEngine {
     if ((rc = upload_query<Fq>(q[M_A], pk->a_query, 1))) return rc;
     if ((rc = upload_query<Fq>(q[M_B1], pk->b_g1_query, 1))) return rc;
     if ((rc = upload_query<Fq2>(q[M_B2], pk->b_g2_query, 1))) return rc;
-    a0 = load_a1(pk->a_query); b1_0 = load_a1(pk->b_g1_query); b2_0 = load_a2(pk->b_g2_query);
     alpha_g1 = load_a1(pk->alpha_g1); beta_g1 = load_a1(pk->beta_g1); delta_g1 = load_a1(pk->delta_g1);
     beta_g2 = load_a2(pk->beta_g2); delta_g2 = load_a2(pk->delta_g2);
+    set_tail_points(load_a1(pk->a_query), load_a1(pk->b_g1_query), load_a2(pk->b_g2_query));
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
     have_pk = true;
     from_setup = false;
@@ -973,9 +983,11 @@ struct Engine : IEngine {
     for (int m = 0; m < 5; m++) {
       if ((rc = (m == M_B2) ? finish_query<Fq2>(q[m]) : finish_query<Fq>(q[m]))) return rc;
     }
-    G16_CUDA(cudaMemcpyAsync(&a0, full_a.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
-    G16_CUDA(cudaMemcpyAsync(&b1_0, full_b1.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
-    G16_CUDA(cudaMemcpyAsync(&b2_0, full_b2.p, sizeof(A2), cudaMemcpyDeviceToHost, S0.st_main));
+    A1 a_q0, b1_q0;
+    A2 b2_q0;
+    G16_CUDA(cudaMemcpyAsync(&a_q0, full_a.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
+    G16_CUDA(cudaMemcpyAsync(&b1_q0, full_b1.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
+    G16_CUDA(cudaMemcpyAsync(&b2_q0, full_b2.p, sizeof(A2), cudaMemcpyDeviceToHost, S0.st_main));
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
     // single points on the host (generator.rs:147-151,182)
     uint32_t k[8];
@@ -983,6 +995,7 @@ struct Engine : IEngine {
     auto mul2 = [&](const Fr& s) { fr_to_canon(s, k); return P2::from_affine(g2).mul_u32(k, 8).to_affine(); };
     alpha_g1 = mul1(alpha); beta_g1 = mul1(beta); delta_g1 = mul1(delta);
     beta_g2 = mul2(beta); gamma_g2 = mul2(gamma); delta_g2 = mul2(delta);
+    set_tail_points(a_q0, b1_q0, b2_q0);
     d_s.release(); tab1.release(); tab2.release();
     have_pk = true;
     from_setup = true;
@@ -1055,8 +1068,41 @@ struct Engine : IEngine {
     return G16_OK;
   }
 
+  // The five MSMs of the slot's proof or group on its streams, with the geometry sl.geom[] and the flags sl.run[] the
+  // caller set.  Proof k of a batched geometry reads its scalars k times one proof's vector length further on.
+  int enqueue_msms(Slot& sl) {
+    const uint64_t nv = nvars(), n = 1ull << L;
+    const uint32_t* zs = sl.d_z.template as<uint32_t>();
+    const uint32_t* hs = sl.d_h.template as<uint32_t>();
+    // scalar sources (prover.rs:63-85): H <- h ; L <- aux ; A, B1, B2 <- input[1..] ++ aux
+    const uint32_t* src[5] = {hs, zs + (size_t)num_inputs * 8, zs + 8, zs + 8, zs + 8};
+    const uint64_t stride[5] = {n * 8, nv * 8, nv * 8, nv * 8, nv * 8};   // 32-bit words between two proofs' scalars
+    // B in G1 and B in G2 run over the same scalars and identity pattern: one counting sort serves both.  B2 sorts
+    // (its stream has the higher priority and its tail is the longest), B1 borrows the list.
+    const bool share = share_b_sort && sl.run[M_B1] && sl.run[M_B2];
+    // "witness map first" (option, off by default): the MSMs that do not need h sort their entries at once but start
+    // accumulating only when the witness map is done, so that their register-heavy blocks do not slow the NTT kernels.
+    const bool wm_first = !sl.serial && (tune.wm_first > 0 || (tune.wm_first < 0 && world > 1));
+    for (int m : {M_L, M_A, M_B2, M_B1, M_H}) {   // H last: it waits for the witness map; B1 borrows B2's sorted list
+      NvtxSpan span_msm(span_of(m));
+      cudaStream_t st = sl.serial ? sl.st_main : sl.st_msm[m];
+      if (!sl.serial) G16_CUDA(cudaStreamWaitEvent(st, m == M_H ? sl.ev_h : sl.ev_z, 0));
+      G16_CUDA(cudaEventRecord(sl.ev_m0[m], st));
+      if (sl.run[m]) {
+        const uint32_t* sc = src[m] + q[m].lo * 8;   // first owned scalar; the digit kernel strides by `world`
+        cudaEvent_t gate = (wm_first && m != M_H) ? sl.ev_h : nullptr;
+        cudaError_t e;
+        if (m == M_B2 && share) { sl.b_sorted = MsmSorted{}; sl.b_sorted.ready = sl.ev_bsort; }
+        if (m == M_B2) e = msm_enqueue<Fq2, Fr>(st, sl.ws2, sl.geom[m], q[m].bases.template as<A2>(), q[m].mask.template as<uint8_t>(), sc, world, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], share ? &sl.b_sorted : nullptr, nullptr, gate, stride[m]);
+        else e = msm_enqueue<Fq, Fr>(st, sl.ws1[m], sl.geom[m], q[m].bases.template as<A1>(), q[m].mask.template as<uint8_t>(), sc, world, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], nullptr, (m == M_B1 && share) ? &sl.b_sorted : nullptr, gate, stride[m]);
+        if (e != cudaSuccess) return fail(G16_ERR_CUDA, std::string("msm_enqueue: ") + cudaGetErrorString(e));
+      }
+      G16_CUDA(cudaEventRecord(sl.ev_m1[m], st));
+    }
+    return G16_OK;
+  }
   // Asynchronous half of a proof: everything is enqueued on the slot's streams, nothing is waited for.
-  // s may be null (partial proof: the (r, s)-only scalar multiplications are skipped).
+  // s may be null (partial proof: the key products are skipped).
   int submit(Slot& sl, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags) {
     if (!have_circuit || !have_pk) return fail(G16_ERR_BAD_ARGUMENT, "circuit and proving key must be resident");
     if (!r || !z) return fail(G16_ERR_BAD_ARGUMENT, "null buffer");
@@ -1068,12 +1114,11 @@ struct Engine : IEngine {
     sl.r = load_fr(r);
     sl.have_s = s != nullptr;
     if (s) sl.s = load_fr(s);
-    const bool r_zero = sl.r.is_zero();
     if (sl.have_s) {
       if (sl.helper) sl.helper->wait();
       if (sl.helper2) sl.helper2->wait();
-      sl.helper = pool->submit([this, &sl]() { fixed_muls_a(sl.r, sl.s, sl.fx); });
-      sl.helper2 = pool->submit([this, &sl]() { fixed_muls_b(sl.r, sl.s, sl.fx); });
+      sl.helper = pool->submit([this, &sl]() { key_products_a(sl.r, sl.s, sl.kp); });
+      sl.helper2 = pool->submit([this, &sl]() { key_products_b(sl.r, sl.s, sl.kp); });
     }
     int rc;
     {
@@ -1081,44 +1126,39 @@ struct Engine : IEngine {
       rc = enqueue_witness_map(sl, z, flags);
     }
     if (rc) return rc;
-    const uint32_t* zs = sl.d_z.template as<uint32_t>();
-    const uint32_t* hs = sl.d_h.template as<uint32_t>();
-    // scalar sources (prover.rs:63-85): H <- h ; L <- aux ; A, B1, B2 <- input[1..] ++ aux
-    const uint32_t* src[5] = {hs, zs + (size_t)num_inputs * 8, zs + 8, zs + 8, zs + 8};
     for (int m = 0; m < 5; m++) {
       const uint64_t cnt = q[m].hi - q[m].lo;
       sl.geom[m] = q[m].geom;
-      sl.run[m] = cnt > 0 && !(m == M_B1 && r_zero);                     // prover.rs:98: B in G1 skipped when r == 0
+      sl.run[m] = cnt > 0 && !(m == M_B1 && sl.r.is_zero());             // prover.rs:98: B in G1 skipped when r == 0
       sl.tm.msm_pairs[m] = sl.run[m] ? cnt : 0;
     }
-    const int order[5] = {M_L, M_A, M_B2, M_B1, M_H};                    // H last: it waits for the witness map; B2 (higher
-                                                                         // stream priority) sorts, B1 borrows its sorted list
-    for (int oi = 0; oi < 5; oi++) {
-      const int m = order[oi];
-      NvtxSpan span_msm(span_of(m));
-      cudaStream_t st = sl.serial ? sl.st_main : sl.st_msm[m];
-      if (!sl.serial) G16_CUDA(cudaStreamWaitEvent(st, m == M_H ? sl.ev_h : sl.ev_z, 0));
-      G16_CUDA(cudaEventRecord(sl.ev_m0[m], st));
-      if (sl.run[m]) {
-        const uint32_t* sc = src[m] + q[m].lo * 8;   // first owned scalar; the digit kernel strides by `world`
-        cudaError_t e;
-        // B in G1 and B in G2 run over the same scalars and identity pattern: one counting sort serves both.  B2 sorts
-        // (its stream has the higher priority and its tail is the longest), B1 borrows the list.
-        const bool share = share_b_sort && sl.run[M_B1] && sl.run[M_B2];
-        // "witness map first" (option, off by default): the MSMs that do not need h sort their entries at once but start
-        // accumulating only when the witness map is done, so that their register-heavy blocks do not slow the NTT kernels.
-        const bool wm_first = !sl.serial && (tune.wm_first > 0 || (tune.wm_first < 0 && world > 1));
-        cudaEvent_t gate = (wm_first && m != M_H) ? sl.ev_h : nullptr;
-        if (m == M_B2 && share) { sl.b_sorted = MsmSorted{}; sl.b_sorted.ready = sl.ev_bsort; }
-        if (m == M_B2) e = msm_enqueue<Fq2, Fr>(st, sl.ws2, sl.geom[m], q[m].bases.template as<A2>(), q[m].mask.template as<uint8_t>(), sc, world, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], share ? &sl.b_sorted : nullptr, nullptr, gate, 0);
-        else e = msm_enqueue<Fq, Fr>(st, sl.ws1[m], sl.geom[m], q[m].bases.template as<A1>(), q[m].mask.template as<uint8_t>(), sc, world, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], nullptr, (m == M_B1 && share) ? &sl.b_sorted : nullptr, gate, 0);
-        if (e != cudaSuccess) return fail(G16_ERR_CUDA, std::string("msm_enqueue: ") + cudaGetErrorString(e));
-      }
-      G16_CUDA(cudaEventRecord(sl.ev_m1[m], st));
-    }
+    if ((rc = enqueue_msms(sl))) return rc;
     sl.launches0 = ctr.launches + ntt_launches - sl.launches0;   // kernels launched for this proof
     sl.busy = true;
     return G16_OK;
+  }
+  // Adds the slot's CUDA events and counts to `t`: spans, their timeline measured from `origin`, entries, pairs and bytes.
+  // The first group of a call sets the MSMs' begin times, later groups can only lower them.
+  void add_timings(const Slot& sl, cudaEvent_t origin, bool first_group, g16_timings& t) const {
+    float ms = 0;
+    cudaEventElapsedTime(&ms, sl.ev_start, sl.ev_z); t.h2d_ms += ms;
+    cudaEventElapsedTime(&ms, sl.ev_z, sl.ev_h); t.witness_map_ms += ms;
+    cudaEventElapsedTime(&ms, origin, sl.ev_h);
+    t.total_ms = std::max(t.total_ms, ms);
+    t.h2d_bytes += sl.tm.h2d_bytes;
+    for (int m = 0; m < 5; m++) {
+      t.msm_pairs[m] += sl.tm.msm_pairs[m];
+      cudaEventElapsedTime(&ms, sl.ev_m0[m], sl.ev_m1[m]); t.msm_ms[m] += ms;
+      cudaEventElapsedTime(&ms, origin, sl.ev_m0[m]);
+      t.msm_begin_ms[m] = first_group ? ms : std::min(t.msm_begin_ms[m], ms);
+      cudaEventElapsedTime(&ms, origin, sl.ev_m1[m]);
+      t.msm_end_ms[m] = std::max(t.msm_end_ms[m], ms);
+      t.total_ms = std::max(t.total_ms, ms);
+      if (!sl.run[m]) continue;
+      cudaEventElapsedTime(&ms, sl.ev_a0[m], sl.ev_a1[m]); t.msm_accum_ms[m] += ms;
+      t.msm_entries[m] += m == M_B2 ? *sl.ws2.h_total : *sl.ws1[m].h_total;
+      t.d2h_bytes += (m == M_B2 ? sl.ws2.plan.leaf_pts * sizeof(P2) : sl.ws1[m].plan.leaf_pts * sizeof(P1)) * sl.geom[m].sets();
+    }
   }
   // Synchronous half: wait for the slot's streams, finish every MSM on the host (leaf sums of the bucket reduction,
   // Horner) as soon as its stream drains, one host thread per MSM.
@@ -1153,31 +1193,11 @@ struct Engine : IEngine {
         if (errs[m] != cudaSuccess) return fail(G16_ERR_CUDA, std::string("msm stream sync: ") + cudaGetErrorString(errs[m]));
       G16_CUDA(cudaStreamSynchronize(sl.st_main));
     }
-    sl.tm.host_finish_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    // timings
-    float ms = 0, tot = 0;
-    cudaEventElapsedTime(&sl.tm.h2d_ms, sl.ev_start, sl.ev_z);
-    cudaEventElapsedTime(&sl.tm.witness_map_ms, sl.ev_z, sl.ev_h);
-    cudaEventElapsedTime(&tot, sl.ev_start, sl.ev_h);
-    for (int m = 0; m < 5; m++) {
-      cudaEventElapsedTime(&sl.tm.msm_ms[m], sl.ev_m0[m], sl.ev_m1[m]);
-      sl.tm.msm_accum_ms[m] = 0;
-      sl.tm.msm_entries[m] = 0;
-      if (sl.run[m]) {
-        cudaEventElapsedTime(&sl.tm.msm_accum_ms[m], sl.ev_a0[m], sl.ev_a1[m]);
-        sl.tm.msm_entries[m] = m == M_B2 ? *sl.ws2.h_total : *sl.ws1[m].h_total;
-      }
-      cudaEventElapsedTime(&sl.tm.msm_begin_ms[m], sl.ev_start, sl.ev_m0[m]);
-      cudaEventElapsedTime(&ms, sl.ev_start, sl.ev_m1[m]);
-      sl.tm.msm_end_ms[m] = ms;
-      if (ms > tot) tot = ms;
-    }
-    sl.tm.total_ms = tot;
-    sl.tm.launches = sl.launches0;
-    sl.tm.d2h_bytes = 0;
-    for (int m = 0; m < 5; m++)
-      if (sl.run[m]) sl.tm.d2h_bytes += (m == M_B2 ? sl.ws2.plan.leaf_pts * sizeof(P2) : sl.ws1[m].plan.leaf_pts * sizeof(P1)) * sl.geom[m].ne;
-    tm = sl.tm;
+    g16_timings t{};
+    t.host_finish_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    add_timings(sl, sl.ev_start, true, t);
+    t.launches = sl.launches0;
+    sl.tm = tm = t;
     return G16_OK;
   }
   void store_partials(uint64_t* p, const Partials& x) {
@@ -1208,62 +1228,30 @@ struct Engine : IEngine {
     store_partials(partial, x);
     return G16_OK;
   }
-  // prover.rs:76-131 on the host, regrouped so that nothing heavy is left once the last MSM is done: with
-  //   A, B1, B2, L, H the five MSM results,
-  //   g_a  = (r d1 + a0 + alpha1) + A                                   = ga0 + A
-  //   g2_b = (s d2 + b2_0 + beta2) + B2                                 = gb2_0 + B2
-  //   g_c  = s g_a + r g1_b - rs d1 + L + H                             = s_ga0 + s A + r_gb0 + r B1 + neg_rs_d1 + L + H
-  // (scalar multiplication distributes over the group law, so the affine proof is the reference's bit for bit).
-  // fixed_muls_a / _b: six scalar multiplications that need only (r, s, key), on two pool threads during the GPU work.
-  void fixed_muls_a(const Fr& r, const Fr& s, FixedMuls& f) const {
+  // The five key products of the proof tail (batch.cuh), for the single-proof paths: computed on the host by two pool
+  // threads while the GPU works, split into halves of similar cost (a G2 product costs about three G1 products).
+  void key_products_a(const Fr& r, const Fr& s, Products& p) const {
     uint32_t rk[8], sk[8], rsk[8];
     fr_to_canon(r, rk);
     fr_to_canon(s, sk);
     fr_to_canon(Fr::mul(r, s), rsk);
     const P1 d1 = P1::from_affine(delta_g1);
-    f.neg_rs_d1 = d1.mul_u32(rsk, 8);                      // prover.rs:76
-    f.neg_rs_d1.negate();
-    f.ga0 = d1.mul_u32(rk, 8);                             // prover.rs:90
-    f.ga0.madd(a0);
-    f.ga0.madd(alpha_g1);
-    f.s_ga0 = f.ga0.mul_u32(sk, 8);                        // prover.rs:94 (its key-only part)
+    p.r_d1 = d1.mul_u32(rk, 8);
+    p.rs_d1 = d1.mul_u32(rsk, 8);
+    p.s_pa = P1::from_affine(p_a).mul_u32(sk, 8);
   }
-  void fixed_muls_b(const Fr& r, const Fr& s, FixedMuls& f) const {
+  void key_products_b(const Fr& r, const Fr& s, Products& p) const {
     uint32_t rk[8], sk[8];
     fr_to_canon(r, rk);
     fr_to_canon(s, sk);
-    f.r_gb0 = P1::inf();
-    if (!r.is_zero()) {                                    // prover.rs:98-108
-      P1 gb0 = P1::from_affine(delta_g1).mul_u32(sk, 8);   // prover.rs:100
-      gb0.madd(b1_0);
-      gb0.madd(beta_g1);
-      f.r_gb0 = gb0.mul_u32(rk, 8);                        // prover.rs:114 (its key-only part)
-    }
-    f.gb2_0 = P2::from_affine(delta_g2).mul_u32(sk, 8);    // prover.rs:112
-    f.gb2_0.madd(b2_0);
-    f.gb2_0.madd(beta_g2);
+    p.r_pb = P1::from_affine(p_b).mul_u32(rk, 8);   // the identity when r == 0
+    p.s_d2 = P2::from_affine(delta_g2).mul_u32(sk, 8);
   }
-  FixedMuls fixed_muls(const Fr& r, const Fr& s) const {
-    FixedMuls f;
-    fixed_muls_a(r, s, f);
-    fixed_muls_b(r, s, f);
-    return f;
-  }
-  // a_sum, b2_sum: A and B2 MSM results (summed over the ranks); c_sum = s A + r B1 + L + H (summed over the ranks)
-  int assemble_sums(const P1& a_sum, const P2& b2_sum, const P1& c_sum, const FixedMuls& f, uint64_t* proof) {
-    NvtxSpan span_finish(SPAN_FINISH_C);
-    P1 g_a = f.ga0;                                       // prover.rs:90-92,252-270
-    g_a.add(a_sum);
-    P2 g2_b = f.gb2_0;                                    // prover.rs:112-113
-    g2_b.add(b2_sum);
-    P1 g_c = f.s_ga0;                                     // prover.rs:119-124
-    g_c.add(f.r_gb0);
-    g_c.add(f.neg_rs_d1);
-    g_c.add(c_sum);
-    store_a1(proof, g_a.to_affine());                     // prover.rs:127-131
-    store_a2(proof + 2 * NQ64, g2_b.to_affine());
-    store_a1(proof + 6 * NQ64, g_c.to_affine());
-    return G16_OK;
+  Products key_products(const Fr& r, const Fr& s) const {
+    Products p;
+    key_products_a(r, s, p);
+    key_products_b(r, s, p);
+    return p;
   }
   // this rank's contribution to g_c that depends on its MSM results: s A + r B1 + L + H
   P1 c_part(const Fr& r, const Fr& s, const Partials& x) const {
@@ -1274,8 +1262,13 @@ struct Engine : IEngine {
     c.add(x.h);
     return c;
   }
-  int assemble(const Fr& r, const Fr& s, const Partials& x, const FixedMuls& f, uint64_t* proof) {
-    return assemble_sums(x.a, x.b2, c_part(r, s, x), f, proof);
+  // a, b2: the A and B-in-G2 MSM results; c = c_part (each summed over the ranks when the key is sharded)
+  void store_proof(uint64_t* proof, const Products& kp, const P1& a, const P2& b2, const P1& c) const {
+    NvtxSpan span_finish(SPAN_FINISH_C);
+    const ProofPoints<Fq, Fq2> pf = proof_tail(kp, p_a, p_2, a, b2, c);
+    store_a1(proof, pf.g_a.to_affine());   // prover.rs:127-131
+    store_a2(proof + 2 * NQ64, pf.g2_b.to_affine());
+    store_a1(proof + 6 * NQ64, pf.g_c.to_affine());
   }
   int prove_submit(int slot, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags) override {
     if (slot < 0 || slot >= NSLOTS) return fail(G16_ERR_BAD_ARGUMENT, "bad slot");
@@ -1283,21 +1276,27 @@ struct Engine : IEngine {
     if (world != 1) return fail(G16_ERR_BAD_ARGUMENT, "key is sharded: use g16_prove_partial + g16_prove_assemble");
     return submit(slots[slot], r, s, z, flags);
   }
-  int prove_wait(int slot, uint64_t* proof) override {
-    if (slot < 0 || slot >= NSLOTS || !proof) return fail(G16_ERR_BAD_ARGUMENT, "bad slot / null buffer");
-    Slot& sl = slots[slot];
-    Partials x;
+  // the MSM results and key products of a whole proof (not a partial one) in the slot
+  int wait_proof(Slot& sl, Partials& x) {
     int rc = wait_partials(sl, x);
     if (sl.helper) { sl.helper->wait(); sl.helper.reset(); }
     if (sl.helper2) { sl.helper2->wait(); sl.helper2.reset(); }
     if (rc) return rc;
     if (!sl.have_s) return fail(G16_ERR_BAD_ARGUMENT, "slot holds a partial proof (use g16_prove_partial_wait)");
+    return G16_OK;
+  }
+  int prove_wait(int slot, uint64_t* proof) override {
+    if (slot < 0 || slot >= NSLOTS || !proof) return fail(G16_ERR_BAD_ARGUMENT, "bad slot / null buffer");
+    Slot& sl = slots[slot];
+    Partials x;
+    int rc = wait_proof(sl, x);
+    if (rc) return rc;
     auto t0 = std::chrono::steady_clock::now();
-    rc = assemble(sl.r, sl.s, x, sl.fx, proof);
+    store_proof(proof, sl.kp, x.a, x.b2, c_part(sl.r, sl.s, x));
     sl.tm.host_finish_ms += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
     sl.tm.d2h_bytes += 8 * NQ64 * 8;
     tm = sl.tm;
-    return rc;
+    return G16_OK;
   }
   int prove(const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags, uint64_t* proof) override {
     if (!proof) return fail(G16_ERR_BAD_ARGUMENT, "null buffer");
@@ -1349,14 +1348,7 @@ struct Engine : IEngine {
   }
   int ensure_tail_tables() {
     if (tail_ready) return G16_OK;
-    P1 pa = P1::from_affine(a0), pb = P1::from_affine(b1_0);
-    P2 p2 = P2::from_affine(b2_0);
-    pa.madd(alpha_g1);
-    pb.madd(beta_g1);
-    p2.madd(beta_g2);
-    p_a = pa.to_affine();
-    p_2 = p2.to_affine();
-    const A1 gens[3] = {delta_g1, p_a, pb.to_affine()};   // TAB_D1, TAB_PA, TAB_PB
+    const A1 gens[3] = {delta_g1, p_a, p_b};   // TAB_D1, TAB_PA, TAB_PB
     for (int t = 0; t < 3; t++) {
       G16_CUDA(tail_tab[t].reserve((size_t)FB_WINDOWS * 255 * sizeof(P1)));
       G16_CUDA((fb_batch_mul<Fq, Fr>(S0.st_main, gens[t], nullptr, 0, nullptr, tail_tab[t].template as<P1>())));
@@ -1372,7 +1364,7 @@ struct Engine : IEngine {
   static size_t tail_point_bytes(uint32_t count) { return (size_t)count * (4 * sizeof(A1) + sizeof(A2)); }
   // enqueue proofs first .. first + count - 1 on the slot's streams
   int batch_submit(Slot& sl, uint32_t first, uint32_t count, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags) {
-    const uint64_t nv = nvars(), n = 1ull << L;
+    const uint64_t nv = nvars();
     sl.serial = (flags & G16_SERIAL_MSMS) != 0;
     sl.batch_first = first;
     sl.batch_count = count;
@@ -1412,36 +1404,12 @@ struct Engine : IEngine {
     G16_CUDA((fb_mul<Fq2, Fr>(st, tail_tab[TAB_D2].template as<P2>(), d_s, count, o2)));
     ctr.launches += 5;
     G16_CUDA(cudaMemcpyAsync(sl.h_tail + sc_bytes / 8, o1, pt_bytes, cudaMemcpyDeviceToHost, st));
-    // the five MSMs of the group, with the stream layout of submit()
-    const uint32_t* zs = sl.d_z.template as<uint32_t>();
-    const uint32_t* hs = sl.d_h.template as<uint32_t>();
-    const uint32_t* src[5] = {hs, zs + (size_t)num_inputs * 8, zs + 8, zs + 8, zs + 8};
-    const uint64_t stride[5] = {n * 8, nv * 8, nv * 8, nv * 8, nv * 8};   // 32-bit words between two proofs' scalars
     for (int m = 0; m < 5; m++) {
       sl.run[m] = q[m].hi > q[m].lo;
       sl.tm.msm_pairs[m] = sl.run[m] ? (q[m].hi - q[m].lo) * count : 0;
     }
-    const bool share = share_b_sort && sl.run[M_B1] && sl.run[M_B2];
-    batch_geoms(count, share, sl.geom);
-    const int order[5] = {M_L, M_A, M_B2, M_B1, M_H};
-    for (int oi = 0; oi < 5; oi++) {
-      const int m = order[oi];
-      NvtxSpan span_msm(span_of(m));
-      cudaStream_t sm = sl.serial ? sl.st_main : sl.st_msm[m];
-      if (!sl.serial) G16_CUDA(cudaStreamWaitEvent(sm, m == M_H ? sl.ev_h : sl.ev_z, 0));
-      G16_CUDA(cudaEventRecord(sl.ev_m0[m], sm));
-      if (sl.run[m]) {
-        const bool wm_first = !sl.serial && tune.wm_first > 0;
-        cudaEvent_t gate = (wm_first && m != M_H) ? sl.ev_h : nullptr;
-        cudaError_t e;
-        if (m == M_B2 && share) { sl.b_sorted = MsmSorted{}; sl.b_sorted.ready = sl.ev_bsort; }
-        if (m == M_B2) e = msm_enqueue<Fq2, Fr>(sm, sl.ws2, sl.geom[m], q[m].bases.template as<A2>(), q[m].mask.template as<uint8_t>(), src[m], 1, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], share ? &sl.b_sorted : nullptr, nullptr, gate, stride[m]);
-        else e = msm_enqueue<Fq, Fr>(sm, sl.ws1[m], sl.geom[m], q[m].bases.template as<A1>(), q[m].mask.template as<uint8_t>(), src[m], 1, true, &ctr, sl.ev_a0[m], sl.ev_a1[m], nullptr, (m == M_B1 && share) ? &sl.b_sorted : nullptr, gate, stride[m]);
-        if (e != cudaSuccess) return fail(G16_ERR_CUDA, std::string("msm_enqueue: ") + cudaGetErrorString(e));
-      }
-      G16_CUDA(cudaEventRecord(sl.ev_m1[m], sm));
-    }
-    return G16_OK;
+    batch_geoms(count, share_b_sort && sl.run[M_B1] && sl.run[M_B2], sl.geom);
+    return enqueue_msms(sl);
   }
   // wait for the slot's group, then finish its proofs on the pool (one proof per task); adds the group to `acc`
   int batch_finish(Slot& sl, const uint64_t* r, const uint64_t* s, uint64_t* proofs, g16_timings& acc, float* host_ms) {
@@ -1455,50 +1423,20 @@ struct Engine : IEngine {
     std::vector<std::shared_ptr<HostPool::Ticket>> tk(count);
     for (uint32_t k = 0; k < count; k++) {
       tk[k] = pool->submit([&, k]() {
-        BatchTailIn<Fq, Fq2> x;
-        x.r_d1 = o1[k];
-        x.rs_d1 = o1[count + k];
-        x.s_pa = o1[2 * (size_t)count + k];
-        x.r_pb = o1[3 * (size_t)count + k];
-        x.s_d2 = o2[k];
+        const Products kp{P1::from_affine(o1[k]), P1::from_affine(o1[count + k]), P1::from_affine(o1[2 * (size_t)count + k]),
+                          P1::from_affine(o1[3 * (size_t)count + k]), P2::from_affine(o2[k])};
+        Partials x;
         P1* outs[4] = {&x.h, &x.l, &x.a, &x.b1};
         for (int m = 0; m < 4; m++) *outs[m] = sl.run[m] ? msm_finish<Fq>(sl.ws1[m], sl.geom[m], k) : P1::inf();
         x.b2 = sl.run[M_B2] ? msm_finish<Fq2>(sl.ws2, sl.geom[M_B2], k) : P2::inf();
         const Fr rk = load_fr(r + 4 * (size_t)(first + k)), sk = load_fr(s + 4 * (size_t)(first + k));
-        uint32_t rc[8], sc[8];
-        fr_to_canon(rk, rc);
-        fr_to_canon(sk, sc);
-        P1 g_a, g_c;
-        P2 g2_b;
-        batch_tail(x, p_a, p_2, rc, sc, rk.is_zero(), g_a, g2_b, g_c);
-        uint64_t* pf = proofs + (size_t)(first + k) * 8 * NQ64;
-        store_a1(pf, g_a.to_affine());
-        store_a2(pf + 2 * NQ64, g2_b.to_affine());
-        store_a1(pf + 6 * NQ64, g_c.to_affine());
+        store_proof(proofs + (size_t)(first + k) * 8 * NQ64, kp, x.a, x.b2, c_part(rk, sk, x));
       });
     }
     for (auto& t : tk) t->wait();
     *host_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    float ms = 0;
-    cudaEventElapsedTime(&ms, sl.ev_start, sl.ev_z); acc.h2d_ms += ms;
-    cudaEventElapsedTime(&ms, sl.ev_z, sl.ev_h); acc.witness_map_ms += ms;
-    cudaEventElapsedTime(&ms, ev_batch, sl.ev_h);
-    acc.total_ms = std::max(acc.total_ms, ms);
-    acc.h2d_bytes += sl.tm.h2d_bytes;
+    add_timings(sl, ev_batch, first == 0, acc);
     acc.d2h_bytes += tail_point_bytes(count);
-    for (int m = 0; m < 5; m++) {
-      acc.msm_pairs[m] += sl.tm.msm_pairs[m];
-      cudaEventElapsedTime(&ms, sl.ev_m0[m], sl.ev_m1[m]); acc.msm_ms[m] += ms;
-      cudaEventElapsedTime(&ms, ev_batch, sl.ev_m0[m]);
-      acc.msm_begin_ms[m] = first == 0 ? ms : std::min(acc.msm_begin_ms[m], ms);
-      cudaEventElapsedTime(&ms, ev_batch, sl.ev_m1[m]);
-      acc.msm_end_ms[m] = std::max(acc.msm_end_ms[m], ms);
-      acc.total_ms = std::max(acc.total_ms, ms);
-      if (!sl.run[m]) continue;
-      cudaEventElapsedTime(&ms, sl.ev_a0[m], sl.ev_a1[m]); acc.msm_accum_ms[m] += ms;
-      acc.msm_entries[m] += m == M_B2 ? *sl.ws2.h_total : *sl.ws1[m].h_total;
-      acc.d2h_bytes += (m == M_B2 ? sl.ws2.plan.leaf_pts * sizeof(P2) : sl.ws1[m].plan.leaf_pts * sizeof(P1)) * sl.geom[m].sets();
-    }
     return G16_OK;
   }
   int prove_batch(uint32_t count, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t group, uint32_t flags,
@@ -1621,11 +1559,8 @@ struct Engine : IEngine {
     if (!nccl_comm) return fail(G16_ERR_BAD_ARGUMENT, "g16_comm_init must precede g16_prove_sharded");
     Slot& sl = slots[slot];
     Partials x;
-    int rc = wait_partials(sl, x);
-    if (sl.helper) { sl.helper->wait(); sl.helper.reset(); }
-    if (sl.helper2) { sl.helper2->wait(); sl.helper2.reset(); }
+    int rc = wait_proof(sl, x);
     if (rc) return rc;
-    if (!sl.have_s) return fail(G16_ERR_BAD_ARGUMENT, "slot holds a partial proof");
     auto t0 = std::chrono::steady_clock::now();
     static_assert(sizeof(P1) == 4 * sizeof(Fq) && sizeof(P2) == 4 * sizeof(Fq2), "XYZZ records are packed");
     uint64_t* w = h_comm_send;
@@ -1651,17 +1586,17 @@ struct Engine : IEngine {
       c_sum.add(c);
       b2_sum.add(b2);
     }
-    rc = assemble_sums(a_sum, b2_sum, c_sum, sl.fx, proof);
+    store_proof(proof, sl.kp, a_sum, b2_sum, c_sum);
     sl.tm.host_finish_ms += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
     sl.tm.d2h_bytes += REC_LIMBS * 8 * comm_world;
     tm = sl.tm;
-    return rc;
+    return G16_OK;
   }
 
-  // Sharded path: the (r, s)-only scalar multiplications can be started before the partial sums exist
+  // Sharded path: the key products can be started before the partial sums exist
   // (g16_prove_assemble_prepare), so that they overlap the GPU work and the gather; prove_assemble picks them up.
   Fr asm_r, asm_s;
-  FixedMuls asm_fx;
+  Products asm_kp;
   bool asm_valid = false;
   std::shared_ptr<HostPool::Ticket> asm_helper;
   int assemble_prepare(const uint64_t* r, const uint64_t* s) override {
@@ -1671,7 +1606,7 @@ struct Engine : IEngine {
     asm_r = load_fr(r);
     asm_s = load_fr(s);
     asm_valid = true;
-    asm_helper = pool->submit([this]() { asm_fx = fixed_muls(asm_r, asm_s); });
+    asm_helper = pool->submit([this]() { asm_kp = key_products(asm_r, asm_s); });
     return G16_OK;
   }
   int prove_assemble(const uint64_t* r, const uint64_t* s, const uint64_t* partials, uint32_t nparts, uint64_t* proof) override {
@@ -1689,11 +1624,10 @@ struct Engine : IEngine {
       x.b2.madd(load_a2(p + 8 * NQ64));
     }
     const Fr rr = load_fr(r), ss = load_fr(s);
-    if (asm_valid && rr == asm_r && ss == asm_s) {
-      asm_valid = false;
-      return assemble(rr, ss, x, asm_fx, proof);
-    }
-    return assemble(rr, ss, x, fixed_muls(rr, ss), proof);
+    const bool prepared = asm_valid && rr == asm_r && ss == asm_s;
+    if (prepared) asm_valid = false;
+    store_proof(proof, prepared ? asm_kp : key_products(rr, ss), x.a, x.b2, c_part(rr, ss, x));
+    return G16_OK;
   }
 };
 

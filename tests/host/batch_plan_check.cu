@@ -1,10 +1,10 @@
-// Host-only check (built by nvcc, runs without a GPU) of the batch-proving rules of groth16_b200/csrc:
+// Host-only check (built by nvcc, runs without a GPU) of the batch-proving rules and the proof tail of groth16_b200/csrc:
 //   1. the bucket-reduction layout of a batched MSM pass (msm.cuh): K proofs x ne bucket sets, msm_sum_strided replaced by
 //      literal host sums as in msm_plan_check.cu; msm_finish(ws, g, k) must equal the Horner definition for proof k alone;
 //   2. a zero-initialised MsmGeom (batch 0) and batch 1 give the same layout and result;
 //   3. batch_group_size (batch.cuh): each of its three caps binds, the result stays in [1, count], an explicit group is kept;
-//   4. batch_tail (batch.cuh) against the prover.rs-order tail of Engine::fixed_muls_a / fixed_muls_b / assemble_sums, on the
-//      host EC back-end, for BN254 and BLS12-381.
+//   4. proof_tail (batch.cuh), which every prover path uses, against a tail in prover.rs's own order kept here as the
+//      reference, with the key products in projective and in affine form, on the host EC back-end, for BN254 and BLS12-381.
 // stdin: the G1 and G2 generators of BN254 then BLS12-381 as Montgomery u64 limbs in hex (affine x || y).
 #include <cstdio>
 #include <cstring>
@@ -154,7 +154,7 @@ struct TailCheck {
       canon(r, rk);
       canon(s, sk);
       canon(Fr::mul(r, s), rsk);
-      // prover.rs order (Engine::fixed_muls_a / fixed_muls_b, c_part, assemble_sums)
+      // the reference: prover.rs's own order, g_c = s g_a + r g1_b - (r s) d1 + L + H
       P1 neg_rs_d1 = P1::from_affine(d1).mul_u32(rsk, 8);
       neg_rs_d1.negate();
       P1 ga0 = P1::from_affine(d1).mul_u32(rk, 8);
@@ -183,24 +183,25 @@ struct TailCheck {
       want_c.add(r_gb0);
       want_c.add(neg_rs_d1);
       want_c.add(c);
-      // regrouped: the five fixed-base products as the GPU returns them (affine), the rest on the host
+      // proof_tail: the five key products as the host helpers compute them (projective) and as the GPU returns them
+      // (affine), with C = s A + r B1 + L + H from above
       P1 pa = P1::from_affine(a0), pb = P1::from_affine(b1_0);
       pa.madd(alpha);
       pb.madd(beta);
       P2 p2 = P2::from_affine(b2_0);
       p2.madd(beta2);
       const A1 p_a = pa.to_affine(), p_b = pb.to_affine();
-      BatchTailIn<Fq, Fq2> x;
-      x.r_d1 = P1::from_affine(d1).mul_u32(rk, 8).to_affine();
-      x.rs_d1 = P1::from_affine(d1).mul_u32(rsk, 8).to_affine();
-      x.s_pa = P1::from_affine(p_a).mul_u32(sk, 8).to_affine();
-      x.r_pb = P1::from_affine(p_b).mul_u32(rk, 8).to_affine();
-      x.s_d2 = P2::from_affine(d2).mul_u32(sk, 8).to_affine();
-      x.a = A; x.b1 = B1; x.l = L; x.h = H; x.b2 = B2;
-      P1 g_a, g_c;
-      P2 g2_b;
-      batch_tail(x, p_a, p2.to_affine(), rk, sk, r.is_zero(), g_a, g2_b, g_c);
-      CHECK(same(g_a, want_a) && same(g2_b, want_b) && same(g_c, want_c), "%s tail case %d: regrouped proof differs", name, it);
+      const KeyProducts<Fq, Fq2> host{P1::from_affine(d1).mul_u32(rk, 8), P1::from_affine(d1).mul_u32(rsk, 8),
+                                      P1::from_affine(p_a).mul_u32(sk, 8), P1::from_affine(p_b).mul_u32(rk, 8),
+                                      P2::from_affine(d2).mul_u32(sk, 8)};
+      const KeyProducts<Fq, Fq2> gpu{P1::from_affine(host.r_d1.to_affine()), P1::from_affine(host.rs_d1.to_affine()),
+                                     P1::from_affine(host.s_pa.to_affine()), P1::from_affine(host.r_pb.to_affine()),
+                                     P2::from_affine(host.s_d2.to_affine())};
+      for (const KeyProducts<Fq, Fq2>* k : {&host, &gpu}) {
+        const ProofPoints<Fq, Fq2> got = proof_tail(*k, p_a, p2.to_affine(), A, B2, c);
+        CHECK(same(got.g_a, want_a) && same(got.g2_b, want_b) && same(got.g_c, want_c),
+              "%s tail case %d (%s products): regrouped proof differs", name, it, k == &host ? "projective" : "affine");
+      }
       n++;
     }
     return n;

@@ -1,6 +1,7 @@
 """CPU tier of batch proving (g16_prove_batch): tests/host/batch_plan_check.cu, built by nvcc and run without a GPU, checks the
 bucket-reduction layout of K proofs x ne bucket sets (msm_finish(ws, g, k) is proof k's Horner sum and nothing else), that a
-zero-initialised MsmGeom is one MSM, the group-size rule, and the regrouped per-proof tail against the prover.rs order."""
+zero-initialised MsmGeom is one MSM, the group-size rule, and the proof tail every prover path shares against the prover.rs
+order."""
 import os
 import shutil
 import subprocess
@@ -24,7 +25,7 @@ def _generator_limbs():
     return " ".join(out) + "\n"
 
 
-def test_batch_plan_host(tmp_path):
+def test_batch_plan_and_proof_tail_host(tmp_path):
     if shutil.which("nvcc") is None:
         pytest.skip("nvcc not available")
     exe = str(tmp_path / "batch_plan_check")

@@ -235,6 +235,32 @@ def test_sharded_prove_equals_single():
     assert (pf.a, pf.b, pf.c) == (want.a, want.b, want.c)
 
 
+@pytest.mark.parametrize("r_zero", [False, True])
+def test_assemble_prepare_equals_unprepared(r_zero):
+    """g16_prove_assemble_prepare computes the key products of (r, s) before the partial points exist; the proof
+    g16_prove_assemble then builds from them equals the one it builds without the preparation, and g16_prove's."""
+    curve = "bn254"
+    c = P.CURVES[curve]
+    cx = P.ctx(c)
+    g = engine(curve)
+    cd = g.codec
+    cs = P.synthetic_circuit(c, 50, seed=5, num_inputs=2)
+    g.generate_parameters_with_qap(matrices_from_r1cs(cs), *toxic(c, 25), cx.g1_gen(), cx.g2_gen())
+    rng = P.Rng(13)
+    r_, s_ = rng.fr(c.r), rng.fr(c.r)
+    if r_zero:
+        r_ = 0
+    z = np.ascontiguousarray(cd.fr.enc(cs.assignment))
+    single = g.create_proof_with_reduction_and_matrices(None, r_, s_, None, cs.num_instance, cs.num_constraints, z)
+    part = np.zeros(g.partial_limbs(), dtype=np.uint64)
+    g.prove_partial_raw(np.ascontiguousarray(cd.fr.enc1(r_)), z.ctypes.data, 0, part)
+    plain = g.prove_assemble(r_, s_, part[None])
+    g.prove_assemble_prepare(r_, s_)
+    prepared = g.prove_assemble(r_, s_, part[None])
+    for pf in (plain, prepared):
+        assert np.array_equal(single.a, pf.a) and np.array_equal(single.b, pf.b) and np.array_equal(single.c, pf.c)
+
+
 def _oracle_vs_gpu(curve, m, z, flags=0):
     """full prove through the C ABI vs the C++ CPU oracle on the same (pk, matrices, assignment, r, s)"""
     import orc
