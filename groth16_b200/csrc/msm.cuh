@@ -9,7 +9,8 @@
 // Pipeline (all on one stream, no host synchronisation until the leaf sums of the bucket reduction are read back):
 //   1. msm_digits<COUNT>   scalar -> W signed c-bit digits; histogram of (bucket set, |digit|) keys (warp-aggregated atomics)
 //   2. msm_scan_*          exclusive prefix sum of the histogram -> bucket offsets (three small launches)
-//   3. msm_digits<SCATTER> counting-sort scatter: sorted (copy * n + base index | sign) and key per entry
+//   3. msm_digits<SCATTER> counting-sort scatter: sorted (copy * n + base index | sign) per entry; msm_pad_fill then writes
+//                          the key of every sorted slot bucket by bucket and marks the bucket padding empty
 //   4. msm_accum_l0        load-balanced segmented reduction: every thread owns K0 consecutive sorted entries,
 //                          mixed-adds them (XYZZ += affine, gathered from the resident base array), writes buckets
 //                          that are complete inside its chunk and emits <= 2 boundary partials
@@ -106,8 +107,7 @@ template <class FrF, bool SCATTER>
 __global__ void __launch_bounds__(256) msm_digits(const uint32_t* __restrict__ scalars, uint32_t scalar_stride, int scalars_mont,
                                                   const uint8_t* __restrict__ skip, MsmGeom g,
                                                   uint32_t* __restrict__ counters,  // COUNT: histogram; SCATTER: cursors
-                                                  uint32_t* __restrict__ sidx, uint32_t* __restrict__ skey,
-                                                  uint64_t batch_stride) {
+                                                  uint32_t* __restrict__ sidx, uint64_t batch_stride) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t set0 = blockIdx.y * (uint32_t)g.ne;
@@ -148,11 +148,7 @@ __global__ void __launch_bounds__(256) msm_digits(const uint32_t* __restrict__ s
       uint32_t base = 0;
       if ((int)lane == leader) base = atomicAdd(&counters[key], (uint32_t)__popc(peers));
       base = __shfl_sync(peers, base, leader);
-      if (SCATTER) {
-        const uint32_t pos = base + rank;
-        sidx[pos] = ((uint32_t)j * g.n + i) | (neg << 31);
-        skey[pos] = key;
-      }
+      if (SCATTER) sidx[base + rank] = ((uint32_t)j * g.n + i) | (neg << 31);   // its key: msm_pad_fill
     }
   }
 }
@@ -230,14 +226,22 @@ static __global__ void __launch_bounds__(1024) msm_scan_fix(uint32_t* offsets, u
     }
 }
 
-// After the scatter the cursor of bucket b stands at the end of its real entries; the slots from there to the start of
-// the next bucket are padding: marked empty (index) and given the bucket's key.  One thread per bucket, < 2^R writes.
-static __global__ void __launch_bounds__(256) msm_pad_fill(const uint32_t* __restrict__ cursors, const uint32_t* __restrict__ offsets,
-                                                           uint32_t nkeys, uint32_t* __restrict__ sidx, uint32_t* __restrict__ skey) {
-  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+// Every sorted slot of bucket b, [offsets[b], offsets[b + 1]), gets its key b here, one warp per bucket, in unit-stride
+// stores.  The scatter does not write keys: there every entry is a random 4-byte store, and the sorted list is larger
+// than L2, so each such store costs DRAM traffic.  After the scatter the cursor of bucket b stands at the end of its
+// real entries; the slots from there to the start of the next bucket are padding and are marked empty.
+static constexpr uint32_t MSM_FILL_BLOCK = 256;
+static __global__ void __launch_bounds__(MSM_FILL_BLOCK) msm_pad_fill(const uint32_t* __restrict__ cursors,
+                                                                      const uint32_t* __restrict__ offsets, uint32_t nkeys,
+                                                                      uint32_t* __restrict__ sidx, uint32_t* __restrict__ skey) {
+  const uint64_t b = ((uint64_t)blockIdx.x * MSM_FILL_BLOCK + threadIdx.x) >> 5;
+  const uint32_t lane = threadIdx.x & 31;
   if (b >= nkeys) return;
-  const uint32_t end = offsets[b + 1];
-  for (uint32_t p = cursors[b]; p < end; p++) { sidx[p] = MSM_INVALID; skey[p] = b; }
+  const uint32_t real_end = cursors[b], end = offsets[b + 1];
+  for (uint32_t p = offsets[b] + lane; p < end; p += 32) {
+    skey[p] = (uint32_t)b;
+    if (p >= real_end) sidx[p] = MSM_INVALID;
+  }
 }
 
 }  // namespace g16
@@ -738,18 +742,16 @@ cudaError_t msm_enqueue(cudaStream_t st, MsmWorkspace<F>& ws, const MsmGeom& g, 
   } else {
     cudaMemsetAsync(counters, 0, (size_t)(g.nkeys + 1) * 4, st);
     const dim3 nb((g.n + 255) / 256, g.batch > 1 ? g.batch : 1u);
-    msm_digits<FrF, false><<<nb, 256, 0, st>>>(d_scalars, scalar_stride, scalars_mont ? 1 : 0, d_skip, g, counters, nullptr, nullptr, batch_stride);
+    msm_digits<FrF, false><<<nb, 256, 0, st>>>(d_scalars, scalar_stride, scalars_mont ? 1 : 0, d_skip, g, counters, nullptr, batch_stride);
     const uint32_t pad_mask = bp.pad > 0 ? (1u << bp.pad) - 1 : 0;
     const uint32_t sb = (g.nkeys + SCAN_BLOCK - 1) / SCAN_BLOCK;
     msm_scan_blocks<<<sb, 1024, 0, st>>>(counters, g.nkeys, offsets, blocktot, pad_mask);
     msm_scan_tops<<<1, 1024, 0, st>>>(blocktot, sb, offsets + g.nkeys);
     msm_scan_fix<<<sb, 1024, 0, st>>>(offsets, g.nkeys, blocktot, counters);
-    msm_digits<FrF, true><<<nb, 256, 0, st>>>(d_scalars, scalar_stride, scalars_mont ? 1 : 0, d_skip, g, counters, sidx, skey, batch_stride);
-    nl += 5;
-    if (pad_mask) {
-      msm_pad_fill<<<(g.nkeys + 255) / 256, 256, 0, st>>>(counters, offsets, g.nkeys, sidx, skey);
-      nl += 1;
-    }
+    msm_digits<FrF, true><<<nb, 256, 0, st>>>(d_scalars, scalar_stride, scalars_mont ? 1 : 0, d_skip, g, counters, sidx, batch_stride);
+    const uint64_t fill_warps_per_block = MSM_FILL_BLOCK / 32;
+    msm_pad_fill<<<(unsigned)((g.nkeys + fill_warps_per_block - 1) / fill_warps_per_block), MSM_FILL_BLOCK, 0, st>>>(counters, offsets, g.nkeys, sidx, skey);
+    nl += 6;
     if (lend) {
       lend->sidx = sidx;
       lend->skey = skey;
