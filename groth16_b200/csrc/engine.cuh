@@ -342,7 +342,7 @@ struct Engine : IEngine {
   bool ba_allowed = true;   // cleared by pk_load / setup when the rounds' work lists would not fit in device memory
   uint32_t ba_allowed_mask = 0x1f;   // per MSM (bit m): the work lists of MSM m fit next to the key and the other MSMs' lists
   MsmGeom with_k0(MsmGeom g, bool g2, int m = -1) const {
-    g.k0 = msm_pick_k0(g.max_entries, (uint64_t)sm_count * 128 * (g2 ? 2 : 3), g2 ? 16 : 8);
+    g.k0 = msm_pick_k0(g.max_entries, (uint64_t)sm_count * 128 * (g2 ? 2 : 3), g2 ? MSM_K0_AUTO_MIN_G2 : MSM_K0_AUTO_MIN_G1);
     // G2 additions are ~3x longer: 32 entries per thread (twice the thread count) shortens the last partial wave (-13 %)
     if (g2 && g.k0 > 32) g.k0 = 32;
     const int k = (int)(g2 ? tune.k0_g2 : tune.k0_g1);
@@ -1318,23 +1318,18 @@ struct Engine : IEngine {
       if (x.hi > x.lo) e = std::max<uint64_t>(e, x.geom.max_entries + (uint64_t)x.geom.nkeys * ((1u << MSM_BA_MAX_ROUNDS) - 1));
     return e;
   }
-  // device workspace of one proof of a group (upper bound): work vectors, sorted lists, partial lists, buckets and
-  // reduction scratch of every MSM, the rounds' work lists, the fixed-base scalars and products
+  // device workspace of one proof of a group (upper bound): work vectors, the fixed-base scalars and products, and every
+  // MSM's workspace (msm_batch_bytes_per_proof) at the smallest k0 with_k0 can pick under the current knobs (acc_k0 4 .. 7
+  // goes below the automatic floor), any round count and, for the B MSMs sharing one sorted list, any padding
   uint64_t batch_bytes_per_proof() const {
     const uint64_t n = 1ull << L;
     uint64_t b = nvars() * 32 + 5 * n * 32 + 3 * 32 + 4 * sizeof(A1) + sizeof(A2);
     for (int m = 0; m < 5; m++) {
       if (q[m].hi <= q[m].lo) continue;
-      const uint64_t pt = m == M_B2 ? sizeof(P2) : sizeof(P1);
-      MsmGeom g = q[m].geom;
-      g.k0 = 8;
-      g.ba = g.ba_pad = 0;
-      MsmBaPlan bp;
-      bp.make(g);
-      b += bp.len[0] * 8 + 3 * bp.l0_threads(g) * (4 + pt) + 2 * (uint64_t)g.nkeys * pt;
-      g.ba = g.ba_pad = MSM_BA_MAX_ROUNDS;
-      bp.make(g);
-      b += (m == M_B2 ? bp.template extra_bytes<Fq2>() : bp.template extra_bytes<Fq>()) + (bp.len[0] - g.max_entries) * 8;
+      const bool g2 = m == M_B2;
+      const int k0_min = msm_k0_floor(g2, g2 ? tune.k0_g2 : tune.k0_g1);
+      const bool shared = share_b_sort && (m == M_B1 || m == M_B2);
+      b += g2 ? msm_batch_bytes_per_proof<Fq2>(q[m].geom, k0_min, shared) : msm_batch_bytes_per_proof<Fq>(q[m].geom, k0_min, shared);
     }
     return b;
   }

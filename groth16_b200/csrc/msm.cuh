@@ -59,6 +59,11 @@ inline int msm_pick_k0(uint64_t max_entries, uint64_t resident_threads, int k0_m
   while (k0 > k0_min && max_entries / k0 < resident_threads * 2) k0 >>= 1;
   return k0;
 }
+static constexpr int MSM_K0_AUTO_MIN_G1 = 8, MSM_K0_AUTO_MIN_G2 = 16;   // k0_min of the automatic rule (Engine::with_k0)
+// the smallest k0 an MSM can run with under acc_k0 = k0_knob (0: automatic; 4 .. 1024: exactly that many)
+inline int msm_k0_floor(bool g2, long long k0_knob) {
+  return (k0_knob >= 4 && k0_knob <= 1024) ? (int)k0_knob : (g2 ? MSM_K0_AUTO_MIN_G2 : MSM_K0_AUTO_MIN_G1);
+}
 inline int msm_pick_c(uint64_t n) {
   int lg = 0;
   while ((1ull << lg) < n) lg++;
@@ -629,6 +634,71 @@ struct MsmBaPlan {
   }
 };
 
+// Device bytes of every buffer MsmWorkspace::prepare reserves for geometry g, with bap = the rounds' plan of g and plan =
+// the reduction plan of 2^(c-1) buckets.  prepare reserves exactly these sizes and the batch prover's group bound is taken
+// from them (msm_batch_bytes_per_proof), so the bound cannot drift from the allocation.
+struct MsmWsBytes {
+  uint64_t ba_pre, ba_prod, ba_pre2, ba_l0, ba_l1;          // batched-affine rounds (0 without rounds)
+  uint64_t counters, offsets, blocktot, sidx, skey, buckets;
+  uint64_t pk0, pp0, pk1, pp1, pending;                     // partial lists of the accumulation levels
+  uint64_t red_inner, red_leaf;                             // bucket reduction
+  uint64_t total() const {
+    return ba_pre + ba_prod + ba_pre2 + ba_l0 + ba_l1 + counters + offsets + blocktot + sidx + skey + buckets + pk0 + pp0 +
+           pk1 + pp1 + pending + red_inner + red_leaf;
+  }
+};
+template <class F>
+MsmWsBytes msm_ws_bytes(const MsmGeom& g, const MsmBaPlan& bap, const MsmRedPlan& plan) {
+  MsmWsBytes b{};
+  const uint64_t T0 = bap.l0_threads(g);
+  const uint64_t S1 = 2 * T0;
+  const uint64_t S2 = 2 * msm_level_threads(S1, MSM_KF);
+  if (bap.R > 0) {
+    b.ba_pre = bap.len[1] * sizeof(F) + 16;
+    b.ba_prod = b.ba_pre2 = bap.threads_max * sizeof(F) + 16;
+    b.ba_l0 = bap.len[1] * sizeof(Affine<F>) + 16;
+    if (bap.R > 1) b.ba_l1 = bap.len[2] * sizeof(Affine<F>) + 16;
+  }
+  b.counters = b.offsets = ((uint64_t)g.nkeys + 1) * 4;
+  b.blocktot = (((uint64_t)g.nkeys + SCAN_BLOCK - 1) / SCAN_BLOCK + 1) * 4;
+  b.sidx = b.skey = bap.len[0] * 4 + 16;
+  b.buckets = (uint64_t)g.nkeys * sizeof(XYZZ<F>);
+  b.pk0 = S1 * 4 + 16;
+  b.pp0 = S1 * sizeof(XYZZ<F>);
+  b.pk1 = S2 * 4 + 16;
+  b.pp1 = S2 * sizeof(XYZZ<F>);
+  b.pending = 64 * 4;   // one partial-list counter per accumulation level
+  b.red_inner = (plan.inner_pts * g.sets() + 1) * sizeof(XYZZ<F>);
+  b.red_leaf = (plan.leaf_pts * g.sets() + 1) * sizeof(XYZZ<F>);
+  return b;
+}
+// Device workspace per proof of a batched pass of MSM g (g16_prove_batch): an upper bound of msm_ws_bytes / G for the pass
+// of any group of G proofs (msm_geom_batch(g, G)) with at least k0_min sorted entries per level-0 thread, at every round
+// count 0 .. MSM_BA_MAX_ROUNDS and, when the MSM's sorted list is shared with another MSM (`shared_pad`), at every larger
+// bucket padding too: a list padded for the other MSM's rounds is walked at its padded length, with or without rounds.
+// Each term of msm_ws_bytes grows at most G-fold from one proof to G at the same k0, rounds and padding, and falls with k0,
+// but for the padded length MsmBaPlan::make rounds down to a multiple of 2^pad: G proofs' sum can round to up to 2^pad - 1
+// slots more than G times one proof's, so one proof is counted with that many entries more.
+template <class F>
+uint64_t msm_batch_bytes_per_proof(MsmGeom g, int k0_min, bool shared_pad) {
+  g = msm_geom_batch(g, 1);
+  g.k0 = k0_min;
+  const uint64_t entries = g.max_entries;
+  MsmRedPlan plan;
+  plan.make(g.c - 1);
+  uint64_t worst = 0;
+  for (int R = 0; R <= MSM_BA_MAX_ROUNDS; R++)
+    for (int pad = R; pad <= (shared_pad ? MSM_BA_MAX_ROUNDS : R); pad++) {
+      g.ba = R;
+      g.ba_pad = pad;
+      g.max_entries = entries + (1u << pad) - 1;
+      MsmBaPlan bap;
+      bap.make(g);
+      worst = std::max(worst, msm_ws_bytes<F>(g, bap, plan).total());
+    }
+  return worst;
+}
+
 template <class F>
 struct MsmWorkspace {
   DevBuf counters, offsets, blocktot, sidx, skey, buckets, pk0, pp0, pk1, pp1, pending, red_inner, red_leaf;
@@ -642,36 +712,31 @@ struct MsmWorkspace {
   cudaError_t prepare(const MsmGeom& g) {
     cudaError_t e;
     bap.make(g);
-    const uint64_t T0 = bap.l0_threads(g);
-    const uint64_t S1 = 2 * T0;
-    const uint64_t T1 = msm_level_threads(S1, MSM_KF);
-    const uint64_t S2 = 2 * T1;
-#define G16_TRY(x) if ((e = (x)) != cudaSuccess) return e
-    if (bap.R > 0) {
-      G16_TRY(ba_pre.reserve(bap.len[1] * sizeof(F) + 16));
-      G16_TRY(ba_prod.reserve(bap.threads_max * sizeof(F) + 16));
-      G16_TRY(ba_pre2.reserve(bap.threads_max * sizeof(F) + 16));
-      G16_TRY(ba_l0.reserve(bap.len[1] * sizeof(Affine<F>) + 16));
-      if (bap.R > 1) G16_TRY(ba_l1.reserve(bap.len[2] * sizeof(Affine<F>) + 16));
-    }
-    G16_TRY(counters.reserve((size_t)(g.nkeys + 1) * 4));
-    G16_TRY(offsets.reserve((size_t)(g.nkeys + 1) * 4));
-    G16_TRY(blocktot.reserve((size_t)((g.nkeys + SCAN_BLOCK - 1) / SCAN_BLOCK + 1) * 4));
-    G16_TRY(sidx.reserve(bap.len[0] * 4 + 16));
-    G16_TRY(skey.reserve(bap.len[0] * 4 + 16));
-    G16_TRY(buckets.reserve((size_t)g.nkeys * sizeof(XYZZ<F>)));
-    G16_TRY(pk0.reserve(S1 * 4 + 16));
-    G16_TRY(pp0.reserve(S1 * sizeof(XYZZ<F>)));
-    G16_TRY(pk1.reserve(S2 * 4 + 16));
-    G16_TRY(pp1.reserve(S2 * sizeof(XYZZ<F>)));
-    G16_TRY(pending.reserve(64 * 4));   // one partial-list counter per accumulation level
     if (plan_m != g.c - 1 || plan_ne != g.ne) {
       plan.make(g.c - 1);
       plan_m = g.c - 1;
       plan_ne = g.ne;
     }
-    G16_TRY(red_inner.reserve((plan.inner_pts * g.sets() + 1) * sizeof(XYZZ<F>)));
-    G16_TRY(red_leaf.reserve((plan.leaf_pts * g.sets() + 1) * sizeof(XYZZ<F>)));
+    const MsmWsBytes b = msm_ws_bytes<F>(g, bap, plan);   // 0 bytes (no rounds): reserve keeps what the buffer has
+#define G16_TRY(x) if ((e = (x)) != cudaSuccess) return e
+    G16_TRY(ba_pre.reserve(b.ba_pre));
+    G16_TRY(ba_prod.reserve(b.ba_prod));
+    G16_TRY(ba_pre2.reserve(b.ba_pre2));
+    G16_TRY(ba_l0.reserve(b.ba_l0));
+    G16_TRY(ba_l1.reserve(b.ba_l1));
+    G16_TRY(counters.reserve(b.counters));
+    G16_TRY(offsets.reserve(b.offsets));
+    G16_TRY(blocktot.reserve(b.blocktot));
+    G16_TRY(sidx.reserve(b.sidx));
+    G16_TRY(skey.reserve(b.skey));
+    G16_TRY(buckets.reserve(b.buckets));
+    G16_TRY(pk0.reserve(b.pk0));
+    G16_TRY(pp0.reserve(b.pp0));
+    G16_TRY(pk1.reserve(b.pk1));
+    G16_TRY(pp1.reserve(b.pp1));
+    G16_TRY(pending.reserve(b.pending));
+    G16_TRY(red_inner.reserve(b.red_inner));
+    G16_TRY(red_leaf.reserve(b.red_leaf));
     if (!h_total) G16_TRY(cudaMallocHost(&h_total, 16));
     const size_t need = plan.leaf_pts * g.sets();
     if (h_cap < need) {

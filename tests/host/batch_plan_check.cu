@@ -4,7 +4,10 @@
 //   2. a zero-initialised MsmGeom (batch 0) and batch 1 give the same layout and result;
 //   3. batch_group_size (batch.cuh): each of its three caps binds, the result stays in [1, count], an explicit group is kept;
 //   4. proof_tail (batch.cuh), which every prover path uses, against a tail in prover.rs's own order kept here as the
-//      reference, with the key products in projective and in affine form, on the host EC back-end, for BN254 and BLS12-381.
+//      reference, with the key products in projective and in affine form, on the host EC back-end, for BN254 and BLS12-381;
+//   5. the batch prover's per-proof workspace bound (msm_batch_bytes_per_proof, which Engine::batch_bytes_per_proof sums):
+//      G times it covers what MsmWorkspace::prepare reserves (msm_ws_bytes) for a group of G = 1, 2, 64 at every acc_k0
+//      (4 .. 7 included), 0 .. 6 rounds, uneven rounds on a shared B sorted list, msm_ne 0 / 1 / 8, msm_c 12 .. 16.
 // stdin: the G1 and G2 generators of BN254 then BLS12-381 as Montgomery u64 limbs in hex (affine x || y).
 #include <cstdio>
 #include <cstring>
@@ -208,6 +211,65 @@ struct TailCheck {
   }
 };
 
+// ---- 5: the batch prover's workspace bound against what the workspaces of a group reserve ---------------------------------
+// Engine::with_k0 at the geometry of a group: the automatic k0 on 132 SMs, or the explicit acc_k0
+static int group_k0(const MsmGeom& g, bool g2, long long knob) {
+  int k0 = msm_pick_k0(g.max_entries, 132ull * 128 * (g2 ? 2 : 3), g2 ? MSM_K0_AUTO_MIN_G2 : MSM_K0_AUTO_MIN_G1);
+  if (g2 && k0 > 32) k0 = 32;
+  return (knob >= 4 && knob <= 1024) ? (int)knob : k0;
+}
+// Engine::pick_geom
+static MsmGeom resident_geom(uint64_t n, int bits, int c_knob, int ne_knob) {
+  if (ne_knob <= 0) return msm_geom(n, bits, c_knob, 0);
+  const int c = c_knob > 0 ? c_knob : (n >= (1u << 16) ? 16 : 0);
+  int ne = ne_knob;
+  MsmGeom g = msm_geom(n, bits, c, ne);
+  while (g.copies > MSM_MAX_COPIES) g = msm_geom(n, bits, c, ++ne);
+  return g;
+}
+// For a group of G proofs at every acc_k0, round count and (for a shared sorted list) every uneven pairing of round counts,
+// msm_ws_bytes of the group's pass must stay within G times msm_batch_bytes_per_proof of the resident geometry.
+template <class F>
+static int bound_cases(const char* name, bool g2) {
+  std::vector<long long> knobs = {0};
+  for (long long k = 4; k <= 64; k++) knobs.push_back(k);
+  for (long long k : {96, 100, 127, 128, 255, 256, 511, 512, 1000, 1023, 1024}) knobs.push_back(k);
+  int n_bad = 0;
+  for (uint64_t n : {(1ull << 12) - 1, (1ull << 17) - 1})
+    for (int c_knob : {0, 12, 13, 14, 15, 16})
+      for (int ne_knob : {0, 1, 8})
+        for (int ba_m : {1, 32}) {
+          MsmGeom g1 = resident_geom(n, 255, c_knob, ne_knob);
+          g1.ba_m = ba_m;
+          MsmRedPlan plan;
+          plan.make(g1.c - 1);
+          for (long long knob : knobs)
+            for (bool shared : {false, true}) {
+              const uint64_t per = msm_batch_bytes_per_proof<F>(g1, msm_k0_floor(g2, knob), shared);
+              for (uint32_t G : {1u, 2u, 64u}) {
+                MsmGeom gG = msm_geom_batch(g1, G);
+                gG.k0 = group_k0(gG, g2, knob);
+                for (int R = 0; R <= MSM_BA_MAX_ROUNDS; R++)
+                  for (int other = 0; other <= (shared ? MSM_BA_MAX_ROUNDS : 0); other++) {
+                    gG.ba = R;
+                    gG.ba_pad = std::max(R, other);   // Engine::batch_geoms: one padding for the shared list
+                    MsmBaPlan bap;
+                    bap.make(gG);
+                    const uint64_t need = msm_ws_bytes<F>(gG, bap, plan).total();
+                    const bool ok = need <= per * G;
+                    if (!ok && n_bad++ < 8)
+                      fprintf(stderr, "%s n=%llu c=%d ne=%d ba_m=%d acc_k0=%lld shared=%d G=%u rounds=%d pad=%d: workspace %llu B > "
+                              "%u x %llu B\n", name, (unsigned long long)n, g1.c, g1.ne, ba_m, knob, (int)shared, G, R, gG.ba_pad,
+                              (unsigned long long)need, G, (unsigned long long)per);
+                  }
+              }
+            }
+        }
+  cases++;
+  if (n_bad) bad++;
+  return n_bad;
+}
+
 static uint64_t read_hex() {
   unsigned long long x = 0;
   if (scanf("%llx", &x) != 1) { fprintf(stderr, "missing generator limbs on stdin\n"); exit(2); }
@@ -258,11 +320,16 @@ int main() {
   CHECK(batch_group_size(100, 4, 1024, 1, huge, 2) == 4, "explicit group below the automatic size is kept");
   CHECK(batch_group_size(100, 500, 1024, 1, huge, 2) == 100, "explicit group capped by count");
   CHECK(batch_group_size(1000, 900, 1ull << 24, 1, huge, 2) == 255, "explicit group capped by the 32-bit offsets");
+  // 5: workspace bound, G1 and G2 points of both curves
+  const int nb = bound_cases<F1>("bn254 g1", false) + bound_cases<Fp<BLS381_FqP>>("bls12_381 g1", false) +
+                 bound_cases<Fp2<BN254_FqP, BN254_Params::FQ2_NONRESIDUE_NEG>>("bn254 g2", true) +
+                 bound_cases<Fp2<BLS381_FqP, BLS381_Params::FQ2_NONRESIDUE_NEG>>("bls12_381 g2", true);
   // 4: tail formula
   TailCheck<BN254_FrP, BN254_FqP, BN254_Params::FQ2_NONRESIDUE_NEG> bn;
   TailCheck<BLS381_FrP, BLS381_FqP, BLS381_Params::FQ2_NONRESIDUE_NEG> bls;
   read_point(bn.g1); read_point(bn.g2); read_point(bls.g1); read_point(bls.g2);
   const int nt = bn.run("bn254") + bls.run("bls12_381");
   printf("%d checks (%d tail cases), %d mismatches\n", cases, nt, bad);
+  printf("workspace bound: %d group passes over it\n", nb);
   return bad ? 1 : 0;
 }

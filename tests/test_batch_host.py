@@ -1,7 +1,7 @@
 """CPU tier of batch proving (g16_prove_batch): tests/host/batch_plan_check.cu, built by nvcc and run without a GPU, checks the
 bucket-reduction layout of K proofs x ne bucket sets (msm_finish(ws, g, k) is proof k's Horner sum and nothing else), that a
-zero-initialised MsmGeom is one MSM, the group-size rule, and the proof tail every prover path shares against the prover.rs
-order."""
+zero-initialised MsmGeom is one MSM, the group-size rule, the proof tail every prover path shares against the prover.rs
+order, and that the per-proof workspace bound which sizes an automatic group covers what a group's MSM workspaces reserve."""
 import os
 import shutil
 import subprocess
@@ -37,3 +37,4 @@ def test_batch_plan_and_proof_tail_host(tmp_path):
     checks = int(res.stdout.split()[0])
     assert checks >= 60, res.stdout          # layout, geometry and group-size checks plus 96 tail cases
     assert "(96 tail cases)" in res.stdout, res.stdout
+    assert "workspace bound: 0 group passes over it" in res.stdout, res.stdout

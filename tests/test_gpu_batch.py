@@ -3,7 +3,10 @@
 Every proof of a batch must equal, bit for bit as raw limbs, g16_prove of the same (r, s, assignment): per curve on a 2^12
 synthetic circuit (some proofs also against the CPU oracle, one pairing-verified), across group boundaries, slot counts and
 G16_SERIAL_MSMS, with edge rows (r = 0, s = 0, r = s, an all-zero assignment, repeated rows, a constant witness), on the
-c = 16 / batched-affine path of a 2^17 circuit, from a device buffer, and on every error path.  The assignments need not
+c = 16 / batched-affine path of a 2^17 circuit, from a device buffer, and on every error path.  Against the CPU oracle, the
+geometries only a batch reaches: rounds a group switches on, the three-pass NTT with several vectors per launch, a group
+of 65535 proofs on grid y, device assignments over several groups, and residency plans changed between batch calls
+(geometries the matrix of test_gpu_geometry.py runs in batches are there).  The assignments need not
 satisfy the circuit: the library and the oracle compute the same deterministic function of them either way."""
 import random
 
@@ -217,3 +220,134 @@ def test_errors_and_state_after_a_batch():
     finally:
         g.load_proving_key(c.pk)
     assert np.array_equal(c.batch(r, s, z), got)   # the tail tables are rebuilt for the re-loaded key
+
+
+# ---- geometries only a batch reaches -------------------------------------------------------------------------------------
+def alone_entries(c, r, s, z):
+    """rows' msm_entries summed over single proofs; a row with r = 0 is counted with r = 1 (a single proof skips B in G1,
+    and with it the shared B sort, when r = 0; its entries do not depend on r)"""
+    one = c.fr([1])[0]
+    total = {}
+    for k in range(len(r)):
+        c.single(r[k] if r[k].any() else one, s[k], z[k])
+        for n, v in c.g.timings()["msm_entries"].items():
+            total[n] = total.get(n, 0) + v
+    return total
+
+
+def options(g, **opts):
+    saved = {k: g.get_option(k) for k in opts}
+    for k, v in opts.items():
+        g.set_option(k, v)
+    return saved
+
+
+ROUNDS = [dict(ba_adaptive=1), dict(ba_adaptive=0)] + [dict(ba_adaptive=0, msm_ba=r, msm_ba_g2=r) for r in range(1, 7)]
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("log_n,count", [(8, 20), (10, 8), (14, 3)])
+def test_rounds_switched_on_by_the_group(curve, log_n, count):
+    """at 2^8 and 2^10 one proof has fewer than 2^18 MSM entries and runs no batched-affine rounds; `count` of them in one
+    group cross 2^18 (ba_min_entries 0) and do, with bucket padding per proof's bucket sets (at 2^14 one proof already runs
+    them, and the group the same count).  Adaptive and forced 1 .. 6 rounds, one group and groups of 2: every proof against
+    the oracle, and the sorted slots against the rows' single-proof sum"""
+    c = ctx(curve, log_n)
+    r, s, z = c.rows(count)
+    r[1] = c.fr([0])[0]
+    z[count // 2, 1:] = c.fr([0x9e3779b])[0]       # constant witness: one giant bucket per window
+    want = np.stack([c.oracle(r[k], s[k], z[k]) for k in range(count)])
+    for opts in ROUNDS:
+        saved = options(c.g, ba_min_entries_g1=0, ba_min_entries_g2=0, **opts)
+        try:
+            alone = alone_entries(c, r, s, z)
+            for group in (0, 2):
+                out = np.zeros((count, 8 * c.g.nq), dtype=np.uint64)
+                c.g.prove_batch_raw(count, r, s, z.ctypes.data, group, 0, out)
+                for k in range(count):
+                    assert np.array_equal(out[k], want[k]), (curve, log_n, opts, group, k)
+                entries = c.g.timings()["msm_entries"]
+                if log_n < 14 and group == 0:   # the group pads its buckets for rounds a single proof never runs
+                    assert entries["h"] > alone["h"], (curve, log_n, opts, entries, alone)
+                else:   # groups of 2 stay under 2^18 entries; at 2^14 one proof runs the group's rounds itself
+                    assert entries == alone, (curve, log_n, opts, group, entries, alone)
+        finally:
+            options(c.g, **saved)
+
+
+@pytest.mark.parametrize("curve", ["bls12_381", "bn254"])
+def test_three_pass_ntt_with_vstride(curve):
+    """a 2^18 domain takes the three-pass NTT plan; with 3 proofs per group every pass selects the proof's vector by
+    blockIdx.y (NttPass::vstride).  One group of 3, and groups of 2 and 1"""
+    c = ctx(curve, 18)
+    r, s, z = c.rows(3)
+    want = [c.oracle(r[k], s[k], z[k]) for k in range(3)]
+    for group in (0, 2):
+        got = c.batch(r, s, z, group=group)
+        for k in range(3):
+            assert np.array_equal(got[k], want[k]), (curve, group, k)
+
+
+def test_grid_y_cap():
+    """65541 proofs with group 100000: the library clamps the group to 65535 (grid y), so one group of 65535 and one of 6.
+    Rows repeat with period 7 (coprime to 65535 and to powers of two): a proof index that wraps at 2^15, 2^16 or 65535
+    lands on a row with other contents.  Proof k must equal proof k mod 7, and the 7 distinct proofs g16_prove's and the
+    oracle's"""
+    import resource
+    import time
+    c = ctx("bn254", 3)
+    period, count = 7, 65541
+    assert count % period == 0
+    r7, s7, z7 = c.rows(period)
+    r7[3] = c.fr([0])[0]
+    t0 = time.perf_counter()
+    reps = count // period
+    r, s = np.ascontiguousarray(np.tile(r7, (reps, 1))), np.ascontiguousarray(np.tile(s7, (reps, 1)))
+    z = np.ascontiguousarray(np.tile(z7, (reps, 1, 1)))
+    out = np.zeros((count, 8 * c.g.nq), dtype=np.uint64)
+    c.g.prove_batch_raw(count, r, s, z.ctypes.data, 100000, 0, out)
+    wall = time.perf_counter() - t0
+    pairs = c.g.timings()["msm_pairs"]
+    assert (out.reshape(reps, period, -1) == out[None, :period]).all()
+    for k in range(period):
+        one = c.single(r7[k], s7[k], z7[k])
+        if k == 0:   # every MSM of every proof ran (B in G1 too: a batch runs it whatever r is)
+            assert pairs == {n: count * v for n, v in c.g.timings()["msm_pairs"].items()}
+        assert np.array_equal(out[k], one), k
+        assert np.array_equal(one, c.oracle(r7[k], s7[k], z7[k])), k
+    print(f"grid-y cap: {count} proofs in {wall:.1f} s, peak host RSS {resource.getrusage(resource.RUSAGE_SELF).ru_maxrss / 2**20:.2f} GiB")
+
+
+def test_assignments_on_device_over_groups():
+    import torch
+    c = ctx("bls12_381")
+    r, s, z = c.rows(7)
+    want = c.batch(r, s, z)
+    dz = torch.from_numpy(z.view(np.int64).reshape(-1)).to("cuda:0")
+    torch.cuda.synchronize()
+    for group in (3, 1):
+        out = np.zeros((7, 8 * c.g.nq), dtype=np.uint64)
+        c.g.prove_batch_raw(7, r, s, dz.data_ptr(), group, _lib.ASSIGNMENT_ON_DEVICE, out)
+        assert np.array_equal(out, want), group
+
+
+@pytest.mark.parametrize("curve", ["bn254", "bls12_377"])
+def test_plan_change_between_batches(curve):
+    """batch under msm_ne 1, re-load the key under msm_ne 8, then 0, and batch again on the same context: the slots keep
+    their grown workspaces and tail buffers across the plans (other bucket-set counts per proof, other copies)"""
+    c = ctx(curve)
+    r, s, z = c.rows(5)
+    want = np.stack([c.oracle(r[k], s[k], z[k]) for k in range(5)])
+    ne0 = c.g.get_option("msm_ne")
+    seen = []
+    try:
+        for ne in (1, 8, 0):
+            c.g.set_option("msm_ne", ne)
+            c.g.load_proving_key(c.pk)
+            seen.append((c.g.config()["ne"], c.g.config()["copies"]))
+            for group in (0, 2):
+                assert np.array_equal(c.batch(r, s, z, group=group), want), (curve, ne, group)
+    finally:
+        c.g.set_option("msm_ne", ne0)
+        c.g.load_proving_key(c.pk)
+    assert len(set(seen)) == 3, seen

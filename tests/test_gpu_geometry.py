@@ -5,6 +5,8 @@ single-GPU plan only (c = 16, one bucket set, 16 precomputed multiples, equal ba
 2^17-constraint key per curve (every query >= 2^16 pairs, so c = 16 is chosen) and ONE oracle proof per curve serve a matrix
 of residency plans, uneven rounds, accumulation knobs, schedules and sharded keys: every configuration re-loads the key,
 asserts through g16_get_config that the geometry it asked for was reached, proves, and must match the oracle bit for bit.
+Each matrix test has a `_batch` twin that proves K = 3 rows per curve in one g16_prove_batch instead (one group, then
+groups of 2 and 1), each against its own oracle proof, with the batch's sorted slots equal to the rows' single-proof sum.
 Further: adversarial bases (duplicates, opposite pairs, identity runs) and signed-digit edge scalars at the resident
 geometry, partial MSMs against the oracle's msm_bigint; the stand-alone g16_msm_g1 / g2 at c = 12 .. 16 and c = 17 / 20."""
 import contextlib
@@ -89,6 +91,8 @@ class Case:
     want: np.ndarray
     defaults: dict
     config0: dict
+    rows: tuple = None       # (r, s, z) of the K batch rows, row 0 = (r, s, z) above
+    wants: np.ndarray = None  # their oracle proofs
 
     @property
     def bits(self):
@@ -127,8 +131,36 @@ def case(curve) -> Case:
         g.load_proving_key(pk)
         r, s = np.ascontiguousarray(cd.fr.enc1(0x1234567 + cd.c.cid)), np.ascontiguousarray(cd.fr.enc1(0x7654321))
         want, _ = orc.prove(cd.c.cid, cd.nq, pk, m, z, r, s, threads=THREADS)
-        _CASES[curve] = Case(curve, g, m, z, pk, r, s, want, defaults, g.config())
+        cs = Case(curve, g, m, z, pk, r, s, want, defaults, g.config())
+        cs.rows = batch_rows(cs)
+        R, S, Z = cs.rows
+        cs.wants = np.stack([want] + [orc.prove(cd.c.cid, cd.nq, pk, m, Z[k], R[k], S[k], threads=THREADS)[0]
+                                      for k in range(1, K)])
+        _CASES[curve] = cs
     return _CASES[curve]
+
+
+K = 3   # batch rows per curve
+
+
+def batch_rows(cs):
+    """K rows that stress the bucket-set layout of a batch: row 0 is the module's (r, s, z); row 1 has a constant witness
+    below 2^32 (one giant bucket per window, and with ne > 1 empty high bucket sets between its neighbours' sets); row 2 has
+    r = 0 and runs of zero witness entries.  Rows 1 and 2 come from a fixed seed."""
+    cd = cs.g.codec
+    rr = np.random.RandomState(41)
+    rnd = lambda: int.from_bytes(rr.bytes(32), "little") % cd.c.r
+    z0 = cs.z
+    nv = z0.shape[0]
+    R = np.stack([cs.r, cd.fr.enc1(rnd()), cd.fr.enc1(0)]).astype(np.uint64)
+    S = np.stack([cs.s, cd.fr.enc1(rnd()), cd.fr.enc1(rnd())]).astype(np.uint64)
+    z1 = np.ascontiguousarray(np.broadcast_to(cd.fr.enc1(0x9e3779b), (nv, 4)))
+    z1[0] = cd.fr.enc1(1)
+    z2 = np.ascontiguousarray(np.roll(z0, 17, axis=0))
+    z2[0] = cd.fr.enc1(1)
+    for lo in range(1000, nv - 4000, 9000):
+        z2[lo:lo + 4000] = 0
+    return np.ascontiguousarray(R), np.ascontiguousarray(S), np.ascontiguousarray(np.stack([z0, z1, z2]))
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -169,13 +201,47 @@ def prove(cs, flags=0):
     return np.concatenate([pf.a, pf.b, pf.c])
 
 
-def run_config(curve, opts, check=None, flags=0):
+MSMS = ("h", "l", "a", "b_g1", "b_g2")
+
+
+def single_entries(cs, R, S, Z, flags=0):
+    """msm_entries (sorted slots, bucket padding included) of each row proved alone.  Entries do not depend on r, but with
+    r = 0 a single proof skips B in G1 and with it the shared B sort: such a row is counted with r = 1."""
+    one = cs.g.codec.fr.enc1(1)
+    out = np.zeros(8 * cs.g.nq, dtype=np.uint64)
+    total = dict.fromkeys(MSMS, 0)
+    for k in range(len(R)):
+        r = R[k] if R[k].any() else one
+        cs.g.prove_raw(np.ascontiguousarray(r), np.ascontiguousarray(S[k]), Z[k].ctypes.data, flags, out)
+        for n, v in cs.g.timings()["msm_entries"].items():
+            total[n] += v
+    return total
+
+
+def prove_batch(cs, rows, wants, flags=0, tag=()):
+    """all rows in one g16_prove_batch, as one group and in groups of 2 (a group of 2 and a group of 1): every proof equals
+    its oracle proof, and the batch's msm_entries equal the rows' single-proof sum, so each proof's bucket sets were sorted
+    at the single proof's padding, disjoint from the other proofs' sets"""
+    R, S, Z = rows
+    alone = single_entries(cs, R, S, Z, flags)
+    for group in (0, 2):
+        out = np.zeros((len(R), 8 * cs.g.nq), dtype=np.uint64)
+        cs.g.prove_batch_raw(len(R), R, S, Z.ctypes.data, group, flags, out)
+        for k in range(len(R)):
+            assert np.array_equal(out[k], wants[k]), (cs.curve, tag, group, k)
+        assert cs.g.timings()["msm_entries"] == alone, (cs.curve, tag, group)
+
+
+def run_config(curve, opts, check=None, flags=0, batch=False):
     cs = case(curve)
     with knobs(cs, **opts):
         cfg = load(cs, opts)
         if check:
             check(cfg)
-        assert np.array_equal(prove(cs, flags), cs.want), (curve, opts)
+        if batch:
+            prove_batch(cs, cs.rows, cs.wants, flags, tag=tuple(opts.items()))
+        else:
+            assert np.array_equal(prove(cs, flags), cs.want), (curve, opts)
 
 
 # ---- residency plans ------------------------------------------------------------------------------------------------------
@@ -184,11 +250,7 @@ RESIDENCY = ([dict(msm_ne=ne) for ne in (0, 1, 2, 3, 5, 8, 16)] +
              [dict(msm_ne=1, msm_c=c) for c in (12, 13, 14)])
 
 
-@pytest.mark.parametrize("curve", ALL_CURVES)
-@pytest.mark.parametrize("opts", RESIDENCY, ids=lambda o: "-".join(f"{k}{v}" for k, v in o.items()))
-def test_residency_plan(curve, opts):
-    """msm_ne 0 (no copies, c from n), 1 .. 16 effective windows (3 and 5 leave a ragged last copy), a copies cap that forces
-    ne up, and c = 12 / 13 / 14 (22 windows: above the 20-copy cap, so ne = 2; 20 windows: exactly on the cap; 19)."""
+def _residency_check(opts):
     def check(cfg):
         if opts.get("msm_ne") == 0:
             assert cfg["copies"] == 1 and cfg["c"] == 13
@@ -198,7 +260,23 @@ def test_residency_plan(curve, opts):
             assert (cfg["c"], cfg["ne"], cfg["copies"]) == {12: (12, 2, 11), 13: (13, 1, 20), 14: (14, 1, 19)}[opts["msm_c"]]
         else:
             assert cfg["ne"] == opts["msm_ne"] and cfg["copies"] == -(-16 // opts["msm_ne"])
-    run_config(curve, opts, check)
+    return check
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("opts", RESIDENCY, ids=lambda o: "-".join(f"{k}{v}" for k, v in o.items()))
+def test_residency_plan(curve, opts):
+    """msm_ne 0 (no copies, c from n), 1 .. 16 effective windows (3 and 5 leave a ragged last copy), a copies cap that forces
+    ne up, and c = 12 / 13 / 14 (22 windows: above the 20-copy cap, so ne = 2; 20 windows: exactly on the cap; 19)."""
+    run_config(curve, opts, _residency_check(opts))
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("opts", RESIDENCY, ids=lambda o: "-".join(f"{k}{v}" for k, v in o.items()))
+def test_residency_plan_batch(curve, opts):
+    """the same plans with K rows per g16_prove_batch: ne > 1 gives every proof several bucket sets, ragged copies and
+    c = 12 .. 14 other set sizes"""
+    run_config(curve, opts, _residency_check(opts), batch=True)
 
 
 @pytest.mark.parametrize("curve", ALL_CURVES)
@@ -242,20 +320,40 @@ UNEVEN = [dict(msm_ba=b1, msm_ba_g2=b2, ba_adaptive=0, share_b_sort=sh)
          [dict(msm_ba=4, msm_ba_g2=0, ba_adaptive=0, share_b_sort=1, msm_ne=8)]
 
 
+def _uneven_check(opts):
+    def check(cfg):
+        assert (cfg["ba_rounds_g1"], cfg["ba_rounds_g2"]) == (opts["msm_ba"], opts["msm_ba_g2"])
+        assert cfg["ba_rounds_g1"] != cfg["ba_rounds_g2"]
+    return check
+
+
 @pytest.mark.parametrize("curve", ALL_CURVES)
 @pytest.mark.parametrize("opts", UNEVEN, ids=lambda o: "-".join(f"{k}{v}" for k, v in o.items()))
 def test_uneven_rounds(curve, opts):
     """B in G1 and B in G2 with different round counts: with share_b_sort 1 they still share one sorted list, padded for the
     larger count (ba_pad = max), so the MSM with fewer rounds (or none) walks a list longer than its own entries."""
-    def check(cfg):
-        assert (cfg["ba_rounds_g1"], cfg["ba_rounds_g2"]) == (opts["msm_ba"], opts["msm_ba_g2"])
-        assert cfg["ba_rounds_g1"] != cfg["ba_rounds_g2"]
-    run_config(curve, opts, check)
+    run_config(curve, opts, _uneven_check(opts))
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("opts", UNEVEN, ids=lambda o: "-".join(f"{k}{v}" for k, v in o.items()))
+def test_uneven_rounds_batch(curve, opts):
+    """the same uneven rounds under the batch's own padding (Engine::batch_geoms): one shared list for a whole group"""
+    run_config(curve, opts, _uneven_check(opts), batch=True)
 
 
 # ---- accumulation knobs ---------------------------------------------------------------------------------------------------
 ACCUM = [("acc_k0_g1", v) for v in (4, 24, 128, 1024)] + [("acc_k0_g2", v) for v in (4, 48, 256)] + \
         [("acc_block", v) for v in (32, 64)]
+
+
+def _accumulation_config(curve, rounds, knob, value, batch=False):
+    opts = {knob: value} if rounds else {knob: value, "msm_ba": 0, "msm_ba_g2": 0}
+
+    def check(cfg):
+        assert cfg[{"acc_k0_g1": "k0_g1", "acc_k0_g2": "k0_g2", "acc_block": "acc_block"}[knob]] == value
+        assert (cfg["ba_rounds_g1"] > 0 and cfg["ba_rounds_g2"] > 0) if rounds else (cfg["ba_rounds_g1"] == cfg["ba_rounds_g2"] == 0)
+    run_config(curve, opts, check, batch=batch)
 
 
 @pytest.mark.parametrize("curve", ALL_CURVES)
@@ -264,12 +362,15 @@ ACCUM = [("acc_k0_g1", v) for v in (4, 24, 128, 1024)] + [("acc_k0_g2", v) for v
 def test_accumulation_knobs(curve, rounds, knob, value):
     """sorted entries per level-0 thread (any value in 4 .. 1024, powers of two or not, above MSM_K0_MAX too; with rounds the
     last list runs k0 >> R) and the level-0 block size, with and without the batched-affine rounds"""
-    opts = {knob: value} if rounds else {knob: value, "msm_ba": 0, "msm_ba_g2": 0}
+    _accumulation_config(curve, rounds, knob, value)
 
-    def check(cfg):
-        assert cfg[{"acc_k0_g1": "k0_g1", "acc_k0_g2": "k0_g2", "acc_block": "acc_block"}[knob]] == value
-        assert (cfg["ba_rounds_g1"] > 0 and cfg["ba_rounds_g2"] > 0) if rounds else (cfg["ba_rounds_g1"] == cfg["ba_rounds_g2"] == 0)
-    run_config(curve, opts, check)
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("rounds", [1, 0], ids=["rounds", "no_rounds"])
+@pytest.mark.parametrize("knob,value", ACCUM)
+def test_accumulation_knobs_batch(curve, rounds, knob, value):
+    """the same knobs over a group's sorted list (k0 1024 and 4 at the group's length)"""
+    _accumulation_config(curve, rounds, knob, value, batch=True)
 
 
 INT64_MAX = (1 << 63) - 1
@@ -347,6 +448,14 @@ def test_schedules(curve):
             cs.g.prove_wait_raw(slot, outs[slot])
         for o in outs:
             assert np.array_equal(o, cs.want)
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+def test_schedules_batch(curve):
+    """witness map first, one proof slot (the groups then share slot 0) and serialised MSMs under ne = 8, in batches"""
+    run_config(curve, dict(wm_first=1), batch=True)
+    run_config(curve, dict(proof_slots=1), batch=True)
+    run_config(curve, dict(msm_ne=8), flags=_lib.SERIAL_MSMS, batch=True)
 
 
 # ---- sharded keys ---------------------------------------------------------------------------------------------------------
@@ -447,6 +556,50 @@ def adversarial(curve):
     return _ADV[curve]
 
 
+_ADV_ROWS = {}
+
+
+def adversarial_rows(curve):
+    """batch rows on the adversarial key: its edge-scalar assignment, the same negated (every scalar but the constant One
+    becomes r - z_i, so every signed digit and carry flips) and a random row; with their oracle proofs"""
+    if curve not in _ADV_ROWS:
+        cs = case(curve)
+        cd = cs.g.codec
+        pk, z, _ = adversarial(curve)
+        vals = cd.fr.dec(z)
+        zn = cd.fr.enc([vals[0]] + [(-v) % cd.c.r for v in vals[1:]]).reshape(z.shape)
+        rr = np.random.RandomState(43)
+        R, S = (np.ascontiguousarray(cd.fr.enc([int.from_bytes(rr.bytes(32), "little") % cd.c.r for _ in range(K)]))
+                for _ in range(2))
+        rows = (R, S, np.ascontiguousarray(np.stack([z, zn, np.roll(cs.z, 5, axis=0)])))
+        wants = np.stack([orc.prove(cd.c.cid, cd.nq, pk, cs.m, rows[2][k], rows[0][k], rows[1][k], threads=THREADS)[0]
+                          for k in range(K)])
+        _ADV_ROWS[curve] = (rows, wants)
+    return _ADV_ROWS[curve]
+
+
+def _adversarial_opts(ne, rounds):
+    return dict(msm_ne=ne, ba_adaptive=0, msm_ba=4 if rounds else 0, msm_ba_g2=4 if rounds else 0)
+
+
+@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("ne", [0, 1, 8])
+@pytest.mark.parametrize("rounds", [1, 0], ids=["rounds", "no_rounds"])
+def test_adversarial_batch(curve, ne, rounds):
+    """the adversarial key in batches: there is no batch partial API, so full proofs of the edge-scalar row, its negation
+    and a random row, against the oracle's proofs on that key"""
+    cs = case(curve)
+    pk = adversarial(curve)[0]
+    rows, wants = adversarial_rows(curve)
+    opts = _adversarial_opts(ne, rounds)
+    try:
+        with knobs(cs, **opts):
+            assert load(cs, opts, pk=pk)["c"] == (13 if ne == 0 else 16)
+            prove_batch(cs, rows, wants, tag=("adversarial", ne, rounds))
+    finally:
+        cs.g.load_proving_key(cs.pk)
+
+
 @pytest.mark.parametrize("curve", ALL_CURVES)
 @pytest.mark.parametrize("ne", [0, 1, 8])
 @pytest.mark.parametrize("rounds", [1, 0], ids=["rounds", "no_rounds"])
@@ -456,7 +609,7 @@ def test_adversarial_partials(curve, ne, rounds):
     cs = case(curve)
     pk, z, want = adversarial(curve)
     nq = cs.g.nq
-    opts = dict(msm_ne=ne, ba_adaptive=0, msm_ba=4 if rounds else 0, msm_ba_g2=4 if rounds else 0)
+    opts = _adversarial_opts(ne, rounds)
     try:
         with knobs(cs, **opts):
             cfg = load(cs, opts, pk=pk)
