@@ -52,6 +52,8 @@ SIGNATURES = [
     ("g16_msm_g1", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     ("g16_msm_g2", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     ("g16_circuit_load", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(Csr), C.POINTER(Csr), C.POINTER(Csr)]),
+    ("g16_circuit_load_qap", C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(Csr), C.POINTER(Csr),
+                                       C.POINTER(Csr)]),
     ("g16_pk_load", C.c_int, [C.c_void_p, C.POINTER(PkDesc), C.c_uint32, C.c_uint32]),
     ("g16_setup", C.c_int, [C.c_void_p] + [C.c_void_p] * 7),
     ("g16_pk_export", C.c_int, [C.c_void_p, C.POINTER(PkExportDesc)]),
@@ -84,6 +86,9 @@ ERR_CUDA = 3
 ERR_MALFORMED_KEY = 4
 ASSIGNMENT_ON_DEVICE = 1
 SERIAL_MSMS = 2
+QAP_LIBSNARK = 0
+QAP_CIRCOM = 1
+QAPS = {"libsnark": QAP_LIBSNARK, "circom": QAP_CIRCOM}
 
 _lib = None
 

@@ -130,9 +130,17 @@ class Proof:
 
 class Groth16:
     """One instance = one curve on one GPU (a g16_ctx).  The circuit (matrices) and the proving key are made
-    resident once and reused by every proof, like a long-lived prover process would."""
+    resident once and reused by every proof, like a long-lived prover process would.
 
-    def __init__(self, curve, device: int = 0):
+    `qap` is the R1CS-to-QAP reduction, the second type parameter of ark-groth16's Groth16<E, QAP>: "libsnark"
+    (LibsnarkReduction, ark-groth16's default) or "circom" (ark-circom's CircomReduction, for circom circuits with
+    snarkjs-compatible keys).  It decides the witness map (circom: n evaluations at the odd powers of omega_2n) and the
+    H query of generate_parameters_with_qap / export_proving_key (circom: n points instead of n - 1)."""
+
+    def __init__(self, curve, device: int = 0, qap: str = "libsnark"):
+        if qap not in _lib.QAPS:
+            raise ValueError(f"qap must be one of {sorted(_lib.QAPS)}, not {qap!r}")
+        self.qap = qap
         self.curve: CurveParams = get_curve(curve)
         self.codec = CurveCodec(self.curve)
         self._lib = _lib.load()
@@ -241,9 +249,9 @@ class Groth16:
             s, k = csr(t)
             structs.append(s)
             keep.append(k)
-        _check(self._lib.g16_circuit_load(self._ctx, m.num_instance_variables, m.num_constraints,
-                                          m.num_witness_variables, C.byref(structs[0]), C.byref(structs[1]),
-                                          C.byref(structs[2])))
+        _check(self._lib.g16_circuit_load_qap(self._ctx, _lib.QAPS[self.qap], m.num_instance_variables, m.num_constraints,
+                                              m.num_witness_variables, C.byref(structs[0]), C.byref(structs[1]),
+                                              C.byref(structs[2])))
         self._matrices = m
         self._pk_resident = False
         self._pk_obj = None
@@ -288,8 +296,9 @@ class Groth16:
         nq = self.nq
         nv = m.num_instance_variables + m.num_witness_variables
         n = 1 << self._lib.g16_domain_log(self._ctx)
+        hn = n if self.qap == "circom" else n - 1   # CircomReduction::h_query_scalars gives n scalars, libsnark n - 1
         z = lambda rows, w: np.zeros((rows, w), dtype=np.uint64)
-        out = dict(a_query=z(nv, 2 * nq), b_g1_query=z(nv, 2 * nq), b_g2_query=z(nv, 4 * nq), h_query=z(n - 1, 2 * nq),
+        out = dict(a_query=z(nv, 2 * nq), b_g1_query=z(nv, 2 * nq), b_g2_query=z(nv, 4 * nq), h_query=z(hn, 2 * nq),
                    l_query=z(m.num_witness_variables, 2 * nq), alpha_g1=z(1, 2 * nq), beta_g1=z(1, 2 * nq),
                    delta_g1=z(1, 2 * nq), beta_g2=z(1, 4 * nq), gamma_g2=z(1, 4 * nq), delta_g2=z(1, 4 * nq),
                    gamma_abc_g1=z(m.num_instance_variables, 2 * nq))
@@ -419,7 +428,8 @@ class Groth16:
 
     def witness_map_from_matrices(self, matrices: Optional[ConstraintMatrices], num_inputs: int, num_constraints: int,
                                   full_assignment: np.ndarray) -> np.ndarray:
-        """R1CSToQAP::witness_map_from_matrices (r1cs_to_qap.rs:172-235) -> domain_size Montgomery Fr coefficients."""
+        """R1CSToQAP::witness_map_from_matrices (r1cs_to_qap.rs:172-235) -> domain_size Montgomery Fr coefficients; with
+        qap="circom", CircomReduction's domain_size evaluations at the odd powers of omega_2n."""
         if matrices is not None and matrices is not self._matrices:
             self.load_matrices(matrices)
         m = self._matrices

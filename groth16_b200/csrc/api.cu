@@ -121,7 +121,12 @@ int g16_msm_g2(g16_ctx* ctx, const uint64_t* bases, const uint64_t* scalars, uin
 int g16_circuit_load(g16_ctx* ctx, uint32_t num_inputs, uint32_t num_constraints, uint32_t num_witness, const g16_csr* a,
                      const g16_csr* b, const g16_csr* c) {
   CTX_OR_FAIL(ctx);
-  return ctx->eng->circuit_load(num_inputs, num_constraints, num_witness, a, b, c);
+  return ctx->eng->circuit_load(G16_QAP_LIBSNARK, num_inputs, num_constraints, num_witness, a, b, c);
+}
+int g16_circuit_load_qap(g16_ctx* ctx, int qap, uint32_t num_inputs, uint32_t num_constraints, uint32_t num_witness,
+                         const g16_csr* a, const g16_csr* b, const g16_csr* c) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->circuit_load(qap, num_inputs, num_constraints, num_witness, a, b, c);
 }
 int g16_pk_load(g16_ctx* ctx, const g16_pk_desc* pk, uint32_t rank, uint32_t world) {
   CTX_OR_FAIL(ctx);

@@ -134,7 +134,7 @@ struct IEngine {
   virtual int witness_map_evals(uint32_t log_n, const uint64_t* a, const uint64_t* b, const uint64_t* c, uint64_t* h) = 0;
   virtual int msm_g1(const uint64_t* bases, const uint64_t* scalars, uint64_t n, uint64_t* out) = 0;
   virtual int msm_g2(const uint64_t* bases, const uint64_t* scalars, uint64_t n, uint64_t* out) = 0;
-  virtual int circuit_load(uint32_t ni, uint32_t nc, uint32_t nw, const g16_csr* a, const g16_csr* b, const g16_csr* c) = 0;
+  virtual int circuit_load(int qap, uint32_t ni, uint32_t nc, uint32_t nw, const g16_csr* a, const g16_csr* b, const g16_csr* c) = 0;
   virtual int pk_load(const g16_pk_desc* pk, uint32_t rank, uint32_t world) = 0;
   virtual int setup(const uint64_t* alpha, const uint64_t* beta, const uint64_t* gamma, const uint64_t* delta,
                     const uint64_t* tau, const uint64_t* g1, const uint64_t* g2) = 0;
@@ -227,6 +227,7 @@ struct Engine : IEngine {
 
   // resident circuit
   bool have_circuit = false;
+  int qap = G16_QAP_LIBSNARK;   // its R1CS-to-QAP reduction: the witness map and the H query follow it
   uint32_t num_inputs = 0, num_constraints = 0, num_witness = 0;
   int L = 0;
   DevBuf csr_rp[3], csr_col[3], csr_val[3];
@@ -621,8 +622,14 @@ struct Engine : IEngine {
     }
     return ensure_slot_buffers(S0, Ln);
   }
-  // the resident circuit's domain must be the one the prover / setup run with
-  int ensure_circuit_domain() { return ensure_domain(dom, L); }
+  // the resident circuit's domain must be the one the prover / setup run with (plus, for CircomReduction, its table)
+  int ensure_circuit_domain() {
+    int rc = ensure_domain(dom, L);
+    if (rc || qap != G16_QAP_CIRCOM || dom.odd_fwd_ninv) return rc;
+    G16_CUDA(ntt_domain_build_odd(dom, S0.st_main, &ntt_launches));
+    G16_CUDA(cudaStreamSynchronize(S0.st_main));
+    return G16_OK;
+  }
   // stand-alone transforms: the circuit's tables when the size matches, a separate domain otherwise
   NttDomain<Fr>* api_domain(int Ln, int* rc) {
     NttDomain<Fr>* d = (have_circuit && Ln == L) ? &dom : &dom_api;
@@ -633,8 +640,9 @@ struct Engine : IEngine {
   // one transform (ntt.cuh), counted in ntt_launches
   void ntt_any(cudaStream_t st, const NttDomain<Fr>& d, bool inverse, const Fr* src, Fr* work, Fr* dst, int load_mode, const Fr* ltab,
                const Fr* in_b, const Fr* in_c, const Fr& load_cst, int store_mode, const Fr* stab, const Fr& store_cst,
-               uint32_t nvec = 1) {
-    ntt_run<Fr>(st, d, inverse, src, work, dst, load_mode, ltab, in_b, in_c, load_cst, store_mode, stab, store_cst, &ntt_launches, nvec);
+               uint32_t nvec = 1, const Fr* st_a = nullptr, const Fr* st_b = nullptr) {
+    ntt_run<Fr>(st, d, inverse, src, work, dst, load_mode, ltab, in_b, in_c, load_cst, store_mode, stab, store_cst, &ntt_launches, nvec,
+                st_a, st_b);
   }
 
   // ---- NTT API ----
@@ -679,6 +687,24 @@ struct Engine : IEngine {
     ntt_any(st, dom, true, A, T, H, NTT_LOAD_AB_MINUS_C, nullptr, B, C, dom.z_inv, NTT_STORE_MUL_TABLE, dom.coset_inv, zero, count);
   }
 
+  // ark-circom's CircomReduction::witness_map_from_matrices on a, b (device row evaluations; c is not read) -> S0.d_h: the n
+  // evaluations h[j] = A[j] B[j] - C[j] at the odd powers omega_2n^(2j+1), where X[j] is x's interpolant there and c = a o b.
+  // Per vector: ifft, then the pre-scaling by omega_2n^i (one multiplication by n^-1 omega_2n^i at the forward load), then
+  // fft.  6 transforms, no elementwise launch: c = a o b is formed by the load of c's iFFT -- first, while A and B still
+  // hold the row evaluations -- and A*B - C by the last-pass store of c's forward transform.
+  void witness_map_device_circom(Slot& sl, const NttDomain<Fr>& dom, uint32_t count = 1) {
+    cudaStream_t st = sl.st_main;
+    Fr* A = sl.d_a.template as<Fr>(); Fr* B = sl.d_b.template as<Fr>(); Fr* C = sl.d_c.template as<Fr>(); Fr* T = sl.d_t.template as<Fr>(); Fr* H = sl.d_h.template as<Fr>();
+    const Fr zero = Fr::zero();
+    ntt_any(st, dom, true, A, H, C, NTT_LOAD_AB, nullptr, B, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero, count);
+    for (Fr* X : {A, B}) {
+      ntt_any(st, dom, true, X, X, T, NTT_LOAD_PLAIN, nullptr, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero, count);
+      ntt_any(st, dom, false, T, T, X, NTT_LOAD_MUL_TABLE, dom.odd_fwd_ninv, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero, count);
+    }
+    ntt_any(st, dom, false, C, C, H, NTT_LOAD_MUL_TABLE, dom.odd_fwd_ninv, nullptr, nullptr, zero, NTT_STORE_AB_MINUS, nullptr, zero,
+            count, A, B);
+  }
+
   // The witness map of a SHARDED proof (SURVEY.md section 8e: the chains a, b, c are independent, r1cs_to_qap.rs:201-207,
   // 220-221): chain v (iFFT then coset FFT of one vector) runs on rank v mod world, the three results meet on rank
   // 3 mod world (ncclSend / ncclRecv of 32 B * n each over NVLink), which forms (a*b - c)/Z and the last coset iFFT
@@ -693,10 +719,17 @@ struct Engine : IEngine {
     const Fr zero = Fr::zero();
     const int w = (int)comm_world, me = (int)comm_rank, fin = 3 % w;
     const size_t bytes = (size_t)sizeof(Fr) << L;
+    const bool circom = qap == G16_QAP_CIRCOM;
+    const Fr* fwd_tab = circom ? dom.odd_fwd_ninv : dom.coset_fwd_ninv;
+    // CircomReduction: chain c starts from a o b of this rank's own row evaluations, before chains a / b overwrite them
+    if (circom && 2 % w == me) {
+      ntt_any(st, dom, true, V[0], V[2], T, NTT_LOAD_AB, nullptr, V[1], nullptr, zero, NTT_STORE_PLAIN, nullptr, zero);
+      ntt_any(st, dom, false, T, T, V[2], NTT_LOAD_MUL_TABLE, fwd_tab, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero);
+    }
     for (int v = 0; v < 3; v++) {
-      if (v % w != me) continue;
+      if (v % w != me || (circom && v == 2)) continue;
       ntt_any(st, dom, true, V[v], V[v], T, NTT_LOAD_PLAIN, nullptr, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero);
-      ntt_any(st, dom, false, T, T, V[v], NTT_LOAD_MUL_TABLE, dom.coset_fwd_ninv, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero);
+      ntt_any(st, dom, false, T, T, V[v], NTT_LOAD_MUL_TABLE, fwd_tab, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero);
     }
     int rc = api.GroupStart();
     for (int v = 0; v < 3 && rc == 0; v++) {
@@ -707,8 +740,12 @@ struct Engine : IEngine {
     }
     if (rc == 0) rc = api.GroupEnd(); else api.GroupEnd();
     if (rc != 0) return fail(G16_ERR_CUDA, std::string("witness-map exchange (ncclSend/Recv): ") + api.GetErrorString(rc));
-    if (me == fin)
+    if (me == fin && circom) {
+      ntt_ab_minus_c<Fr>(st, V[0], V[1], V[2], H, 1ull << L);
+      ntt_launches++;
+    } else if (me == fin) {
       ntt_any(st, dom, true, V[0], T, H, NTT_LOAD_AB_MINUS_C, nullptr, V[1], V[2], dom.z_inv, NTT_STORE_MUL_TABLE, dom.coset_inv, zero);
+    }
     rc = api.Broadcast(H, H, bytes, 1, fin, nccl_comm_wm, st);
     if (rc != 0) return fail(G16_ERR_CUDA, std::string("witness-map broadcast (ncclBroadcast): ") + api.GetErrorString(rc));
     return G16_OK;
@@ -764,7 +801,8 @@ struct Engine : IEngine {
   int msm_g2(const uint64_t* bases, const uint64_t* scalars, uint64_t n, uint64_t* out) override { return msm_host<Fq2>(S0.ws2, bases, scalars, n, out); }
 
   // ---- circuit ----
-  int circuit_load(uint32_t ni, uint32_t nc, uint32_t nw, const g16_csr* a, const g16_csr* b, const g16_csr* c) override {
+  int circuit_load(int qp, uint32_t ni, uint32_t nc, uint32_t nw, const g16_csr* a, const g16_csr* b, const g16_csr* c) override {
+    if (qp != G16_QAP_LIBSNARK && qp != G16_QAP_CIRCOM) return fail(G16_ERR_BAD_ARGUMENT, "unknown R1CS-to-QAP reduction");
     if (!a || !b || !c || ni == 0) return fail(G16_ERR_BAD_ARGUMENT, "bad circuit description");
     G16_NOT_BUSY();
     uint64_t need = (uint64_t)nc + ni;
@@ -772,6 +810,9 @@ struct Engine : IEngine {
     while ((1ull << Ln) < need) Ln++;
     int rc = check_log((uint32_t)Ln);
     if (rc) return rc;
+    // CircomReduction evaluates at the odd powers of omega_2n: the domain of size 2n must exist
+    if (qp == G16_QAP_CIRCOM && Ln + 1 > CP::FrP::TWO_ADICITY)
+      return fail(G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "CircomReduction needs a domain of twice the size, which exceeds the field's two-adicity (PolynomialDegreeTooLarge)");
     G16_CUDA(cudaSetDevice(device));
     const g16_csr* ms[3] = {a, b, c};
     const uint32_t nvars = ni + nw;
@@ -796,7 +837,7 @@ struct Engine : IEngine {
         G16_CUDA(cudaMemcpy(csr_val[m].p, ms[m]->val, (size_t)nnz * 32, cudaMemcpyHostToDevice));
       }
     }
-    num_inputs = ni; num_constraints = nc; num_witness = nw; L = Ln;
+    num_inputs = ni; num_constraints = nc; num_witness = nw; L = Ln; qap = qp;
     G16_CUDA(S0.d_z.reserve((size_t)nvars * 32));
     if ((rc = ensure_circuit_domain())) return rc;
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
@@ -909,6 +950,8 @@ struct Engine : IEngine {
     for (int i = 0; i < L; i++) tn = Fr::sqr(tn);
     const Fr zt = Fr::sub(tn, Fr::one());                      // evaluate_vanishing_polynomial(t)
     if (zt.is_zero()) return fail(G16_ERR_BAD_ARGUMENT, "tau lies in the evaluation domain");
+    const bool circom = qap == G16_QAP_CIRCOM;
+    if (circom && Fr::sqr(tn) == Fr::one()) return fail(G16_ERR_BAD_ARGUMENT, "tau lies in the domain of size 2n (CircomReduction)");
     // Lagrange coefficients u_i = zt * w^i / (n (tau - w^i))   (evaluate_all_lagrange_coefficients)
     std::vector<Fr> u(n), den(n);
     {
@@ -934,15 +977,18 @@ struct Engine : IEngine {
           dst = Fr::add(dst, Fr::mul(u[i], h_val[m][e]));                          // r1cs_to_qap.rs:157-167
         }
     const Fr gi = Fr::inv(gamma), di = Fr::inv(delta);
-    std::vector<Fr> gabc(ni), lq(num_witness), hs(n - 1);
+    const uint64_t hn = circom ? n : n - 1;   // H query length
+    std::vector<Fr> gabc(ni), lq(num_witness), hs(hn);
     for (uint64_t i = 0; i < nv; i++) {
       const Fr t = Fr::add(Fr::add(Fr::mul(beta, qa[i]), Fr::mul(alpha, qb[i])), qc[i]);
       if (i < ni) gabc[i] = Fr::mul(t, gi);                                        // generator.rs:113-117
       else lq[i - ni] = Fr::mul(t, di);                                            // generator.rs:119-123
     }
-    {
+    if (!circom) {
       Fr p = Fr::mul(zt, di);                                                      // h_query_scalars, r1cs_to_qap.rs:237-247
       for (uint64_t i = 0; i + 1 < n; i++) { hs[i] = p; p = Fr::mul(p, tau); }
+    } else {
+      circom_h_scalars(tau, tn, di, hs);
     }
     // --- fixed-base batch multiplications on the GPU (generator.rs:129-183) ---
     tail_ready = false;
@@ -956,8 +1002,8 @@ struct Engine : IEngine {
     };
     G16_CUDA(full_a.reserve(nv * sizeof(A1))); G16_CUDA(full_b1.reserve(nv * sizeof(A1))); G16_CUDA(full_b2.reserve(nv * sizeof(A2)));
     G16_CUDA(d_gamma_abc.reserve((size_t)ni * sizeof(A1)));
-    shard(q[M_H], n - 1); shard(q[M_L], num_witness); shard(q[M_A], nv - 1); shard(q[M_B1], nv - 1); shard(q[M_B2], nv - 1);
-    G16_CUDA(q[M_H].bases.reserve((size_t)q[M_H].geom.copies * (n - 1) * sizeof(A1) + 16));
+    shard(q[M_H], hn); shard(q[M_L], num_witness); shard(q[M_A], nv - 1); shard(q[M_B1], nv - 1); shard(q[M_B2], nv - 1);
+    G16_CUDA(q[M_H].bases.reserve((size_t)q[M_H].geom.copies * hn * sizeof(A1) + 16));
     G16_CUDA(q[M_L].bases.reserve((size_t)q[M_L].geom.copies * num_witness * sizeof(A1) + 16));
     // a_query / b_g1_query / b_g2_query
     G16_CUDA(up(qa)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), nv, full_a.template as<A1>(), tab1))) return rc;
@@ -965,7 +1011,7 @@ struct Engine : IEngine {
     G16_CUDA(up(qb)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), nv, full_b1.template as<A1>(), tab1))) return rc;
     if ((rc = batch_mul<Fq2>(g2, d_s.template as<Fr>(), nv, full_b2.template as<A2>(), tab2))) return rc;
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
-    G16_CUDA(up(hs)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), n - 1, q[M_H].bases.template as<A1>(), tab1))) return rc;
+    G16_CUDA(up(hs)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), hn, q[M_H].bases.template as<A1>(), tab1))) return rc;
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
     G16_CUDA(up(lq)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), num_witness, q[M_L].bases.template as<A1>(), tab1))) return rc;
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
@@ -1003,6 +1049,32 @@ struct Engine : IEngine {
     decide_ba_memory();
     return G16_OK;
   }
+  // CircomReduction::h_query_scalars(n - 1, tau, _, delta^-1): the odd entries 1, 3, .., 2n - 1 of the size-2n ifft of
+  // v[i] = delta^-1 tau^i (i < 2n - 1), v[2n - 1] = 0.  With w = omega_2n, k = 2j + 1 and the geometric sum in closed form:
+  //   out[j] = delta^-1 / (2n) * [ (tau^2n - 1) / (tau w^-k - 1) - tau^(2n-1) w^k ]
+  // O(n), one batch inversion.  tn = tau^n; tau^2n != 1 is checked by the caller.
+  void circom_h_scalars(const Fr& tau, const Fr& tn, const Fr& di, std::vector<Fr>& hs) const {
+    const uint64_t n = hs.size();
+    const Fr w = fr_domain_root<Fr>(L + 1), w_inv = Fr::inv(w);
+    const Fr w2 = Fr::sqr(w), w2_inv = Fr::sqr(w_inv);
+    const Fr t2n = Fr::sqr(tn), t2n_m1 = Fr::sub(t2n, Fr::one());
+    Fr tn1 = Fr::one();                                                           // tau^(n-1): n - 1 = L one bits
+    for (int i = 0; i < L; i++) tn1 = Fr::mul(Fr::sqr(tn1), tau);
+    const Fr t2n1 = Fr::mul(tn, tn1);                                             // tau^(2n-1)
+    const Fr c = Fr::mul(di, Fr::inv(fr_from_u64<Fr>(2 * n)));
+    std::vector<Fr> den(n), pref(n);
+    Fr wk_inv = w_inv;
+    for (uint64_t j = 0; j < n; j++) { den[j] = Fr::sub(Fr::mul(tau, wk_inv), Fr::one()); wk_inv = Fr::mul(wk_inv, w2_inv); }
+    Fr acc = Fr::one();
+    for (uint64_t j = 0; j < n; j++) { pref[j] = acc; acc = Fr::mul(acc, den[j]); }
+    Fr ai = Fr::inv(acc);
+    for (uint64_t j = n; j-- > 0;) { const Fr t = Fr::mul(ai, pref[j]); ai = Fr::mul(ai, den[j]); den[j] = t; }
+    Fr wk = w;
+    for (uint64_t j = 0; j < n; j++) {
+      hs[j] = Fr::mul(c, Fr::sub(Fr::mul(t2n_m1, den[j]), Fr::mul(t2n1, wk)));
+      wk = Fr::mul(wk, w2);
+    }
+  }
   int pk_export(const g16_pk_export_desc* o) override {
     if (!have_pk || !from_setup) return fail(G16_ERR_BAD_ARGUMENT, "g16_pk_export needs a key produced by g16_setup");
     if (!o) return fail(G16_ERR_BAD_ARGUMENT, "null");
@@ -1011,7 +1083,8 @@ struct Engine : IEngine {
     if (o->a_query) G16_CUDA(cudaMemcpy(o->a_query, full_a.p, nv * sizeof(A1), cudaMemcpyDeviceToHost));
     if (o->b_g1_query) G16_CUDA(cudaMemcpy(o->b_g1_query, full_b1.p, nv * sizeof(A1), cudaMemcpyDeviceToHost));
     if (o->b_g2_query) G16_CUDA(cudaMemcpy(o->b_g2_query, full_b2.p, nv * sizeof(A2), cudaMemcpyDeviceToHost));
-    if (o->h_query && n > 1) G16_CUDA(cudaMemcpy(o->h_query, q[M_H].bases.p, (n - 1) * sizeof(A1), cudaMemcpyDeviceToHost));
+    const uint64_t hn = qap == G16_QAP_CIRCOM ? n : n - 1;
+    if (o->h_query && hn) G16_CUDA(cudaMemcpy(o->h_query, q[M_H].bases.p, hn * sizeof(A1), cudaMemcpyDeviceToHost));
     if (o->l_query && num_witness) G16_CUDA(cudaMemcpy(o->l_query, q[M_L].bases.p, (size_t)num_witness * sizeof(A1), cudaMemcpyDeviceToHost));
     if (o->gamma_abc_g1) G16_CUDA(cudaMemcpy(o->gamma_abc_g1, d_gamma_abc.p, (size_t)num_inputs * sizeof(A1), cudaMemcpyDeviceToHost));
     if (o->alpha_g1) store_a1(o->alpha_g1, alpha_g1);
@@ -1045,10 +1118,12 @@ struct Engine : IEngine {
     CsrDev cs[3];
     for (int m = 0; m < 3; m++) cs[m] = CsrDev{csr_rp[m].template as<uint32_t>(), csr_col[m].template as<uint32_t>(), csr_val[m].p};
     r1cs_matvec<Fr>(sl.st_main, cs, sl.d_z.template as<Fr>(), num_constraints, num_inputs, n, sl.d_a.template as<Fr>(),
-                    sl.d_b.template as<Fr>(), sl.d_c.template as<Fr>(), count, (uint32_t)nv);
+                    sl.d_b.template as<Fr>(), sl.d_c.template as<Fr>(), count, (uint32_t)nv, qap == G16_QAP_LIBSNARK);
     ntt_launches++;
     if (sl.split_wm && nccl_comm_wm) {
       if ((rc = witness_map_split(sl))) return rc;
+    } else if (qap == G16_QAP_CIRCOM) {
+      witness_map_device_circom(sl, dom, count);
     } else {
       witness_map_device(sl, dom, count);
     }

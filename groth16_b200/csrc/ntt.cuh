@@ -14,21 +14,31 @@
 //                    in natural order, with the n^-1 / coset scalings fused into that store
 // The element-wise work of the witness map -- coset pre-scaling by g^i (r1cs_to_qap.rs:204-207), (a*b - c)/Z
 // (r1cs_to_qap.rs:209,223-230), n^-1 g^-i (r1cs_to_qap.rs:232) -- is fused into the first-pass load / last-pass store.
+// The same holds for ark-circom's CircomReduction: c = a o b is formed by the load of c's iFFT (NTT_LOAD_AB), the
+// n^-1 omega_2n^i pre-scaling by the load of each forward transform, and h = A*B - C by the last-pass store of c's forward
+// transform (NTT_STORE_AB_MINUS).  Those two modes live in a separate instantiation of the pass kernel (CIRCOM = true), so
+// the kernel the libsnark reduction runs is compiled exactly as before.
 #pragma once
 #include <cuda_runtime.h>
 #include "fp.cuh"
 
 namespace g16 {
 
-enum NttLoad { NTT_LOAD_PLAIN = 0, NTT_LOAD_MUL_TABLE = 1, NTT_LOAD_AB_MINUS_C = 2 };
-enum NttStore { NTT_STORE_PLAIN = 0, NTT_STORE_MUL_CONST = 1, NTT_STORE_MUL_TABLE = 2 };
+enum NttLoad { NTT_LOAD_PLAIN = 0, NTT_LOAD_MUL_TABLE = 1, NTT_LOAD_AB_MINUS_C = 2, NTT_LOAD_AB = 3 };
+enum NttStore { NTT_STORE_PLAIN = 0, NTT_STORE_MUL_CONST = 1, NTT_STORE_MUL_TABLE = 2, NTT_STORE_AB_MINUS = 3 };
+// NTT_LOAD_AB: x = in[i] * in_b[i] (natural index).  NTT_STORE_AB_MINUS: out[i] = st_a[i] * st_b[i] - x (natural index).
+static inline bool ntt_circom_mode(int load_mode, int store_mode) {
+  return load_mode == NTT_LOAD_AB || store_mode == NTT_STORE_AB_MINUS;
+}
 
 template <class Fr>
 struct NttPass {
   const Fr* in;      // input (NTT_LOAD_AB_MINUS_C: the `a` vector)
-  const Fr* in_b;    // AB_MINUS_C only
+  const Fr* in_b;    // AB_MINUS_C and AB only
   const Fr* in_c;    // AB_MINUS_C only
   Fr* out;
+  const Fr* st_a;    // STORE_AB_MINUS only
+  const Fr* st_b;
   const Fr* tw;      // tw[i] = root^i, i < n/2
   const Fr* ltab;    // load table, natural index
   const Fr* stab;    // store table, natural (bit-reversed-address) index
@@ -37,7 +47,8 @@ struct NttPass {
   int L, s0, k, logC;
   int load_mode, store_mode;
   int bitrev_store;  // 1 on the last pass
-  uint64_t vstride;  // elements between the vectors of a batch: blockIdx.y selects in / in_b / in_c / out; tables are shared
+  uint64_t vstride;  // elements between the vectors of a batch: blockIdx.y selects in / in_b / in_c / out / st_a / st_b;
+                     // tables are shared
 };
 
 template <class Fr>
@@ -60,7 +71,8 @@ static constexpr int NTT_TILE_LOG = 10;
 static constexpr int NTT_TILE = 1 << NTT_TILE_LOG;
 
 // One pass: stages s0 .. s0+k-1 of an L-stage DIF transform.  blockDim.x = min(256, tile/2).
-template <class Fr>
+// CIRCOM = false: the libsnark load / store modes; CIRCOM = true: NTT_LOAD_AB / NTT_STORE_AB_MINUS (plus plain / table loads)
+template <class Fr, bool CIRCOM>
 __global__ void __launch_bounds__(256) ntt_pass_kernel(NttPass<Fr> a) {
   static_assert(Fr::N == 8, "Fr must be 8 x 32-bit limbs");
   __shared__ uint32_t sm[8][NTT_TILE];
@@ -82,6 +94,8 @@ __global__ void __launch_bounds__(256) ntt_pass_kernel(NttPass<Fr> a) {
     Fr x = ntt_ldg(a.in + voff + gi);
     if (a.load_mode == NTT_LOAD_MUL_TABLE) {
       x = Fr::mul(x, ntt_ldg(a.ltab + gi));
+    } else if constexpr (CIRCOM) {
+      if (a.load_mode == NTT_LOAD_AB) x = Fr::mul(x, ntt_ldg(a.in_b + voff + gi));
     } else if (a.load_mode == NTT_LOAD_AB_MINUS_C) {
       Fr y = ntt_ldg(a.in_b + voff + gi), z = ntt_ldg(a.in_c + voff + gi);
       x = Fr::mul(Fr::sub(Fr::mul(x, y), z), a.lcst);
@@ -124,8 +138,12 @@ __global__ void __launch_bounds__(256) ntt_pass_kernel(NttPass<Fr> a) {
 #pragma unroll
     for (int w = 0; w < 8; w++) x.v[w] = sm[w][e];
     if (a.bitrev_store && a.L > 0) gi = __brevll(gi) >> (64 - a.L);
-    if (a.store_mode == NTT_STORE_MUL_CONST) x = Fr::mul(x, a.scst);
-    else if (a.store_mode == NTT_STORE_MUL_TABLE) x = Fr::mul(x, ntt_ldg(a.stab + gi));
+    if constexpr (CIRCOM) {
+      if (a.store_mode == NTT_STORE_AB_MINUS) x = Fr::sub(Fr::mul(ntt_ldg(a.st_a + voff + gi), ntt_ldg(a.st_b + voff + gi)), x);
+    } else {
+      if (a.store_mode == NTT_STORE_MUL_CONST) x = Fr::mul(x, a.scst);
+      else if (a.store_mode == NTT_STORE_MUL_TABLE) x = Fr::mul(x, ntt_ldg(a.stab + gi));
+    }
     ntt_stg(a.out + voff + gi, x);
   }
 }
@@ -147,12 +165,13 @@ __global__ void ntt_powers_kernel(Fr* out, uint64_t n, Fr base, Fr c0) {
 // Sparse rows times the assignment (evaluate_constraint, r1cs_to_qap.rs:28-67) for the three matrices at once,
 // plus the instance copy a[nc + i] = z[i] (r1cs_to_qap.rs:195-199) and the zero tail up to the domain size.
 // blockIdx.y = proof k of a batch: it reads z + k * nv and writes a, b, c + k * n.
+// WITH_C = false (CircomReduction, which never reads matrix C): only a and b; c is neither read nor written.
 struct CsrDev {
   const uint32_t* row_ptr;  // nc + 1
   const uint32_t* col;
   const void* val;          // Fr, Montgomery
 };
-template <class Fr>
+template <class Fr, bool WITH_C>
 __global__ void __launch_bounds__(256) r1cs_matvec_kernel(CsrDev A, CsrDev B, CsrDev Cm, const Fr* __restrict__ z,
                                                           uint32_t nc, uint32_t num_inputs, uint32_t n, Fr* a, Fr* b,
                                                           Fr* c, uint32_t nv) {
@@ -167,7 +186,7 @@ __global__ void __launch_bounds__(256) r1cs_matvec_kernel(CsrDev A, CsrDev B, Cs
     const CsrDev* ms[3] = {&A, &B, &Cm};
     Fr* outs[3] = {&ra, &rb, &rc};
 #pragma unroll
-    for (int m = 0; m < 3; m++) {
+    for (int m = 0; m < (WITH_C ? 3 : 2); m++) {
       const uint32_t lo = ms[m]->row_ptr[i], hi = ms[m]->row_ptr[i + 1];
       const Fr* vals = reinterpret_cast<const Fr*>(ms[m]->val);
       Fr acc = Fr::zero();
@@ -179,7 +198,14 @@ __global__ void __launch_bounds__(256) r1cs_matvec_kernel(CsrDev A, CsrDev B, Cs
   }
   ntt_stg(a + i, ra);
   ntt_stg(b + i, rb);
-  ntt_stg(c + i, rc);
+  if (WITH_C) ntt_stg(c + i, rc);
+}
+
+// h[i] = a[i] * b[i] - c[i], i < n: the pointwise step of CircomReduction when a, b, c were transformed on different GPUs
+template <class Fr>
+__global__ void ntt_ab_minus_c_kernel(const Fr* a, const Fr* b, const Fr* c, Fr* h, uint64_t n) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) ntt_stg(h + i, Fr::sub(Fr::mul(ntt_ldg(a + i), ntt_ldg(b + i)), ntt_ldg(c + i)));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -194,6 +220,8 @@ struct NttDomain {
   Fr* coset_fwd = nullptr;  // g^i          i < n
   Fr* coset_inv = nullptr;  // n^-1 g^-i    i < n
   Fr* coset_fwd_ninv = nullptr;  // n^-1 g^i  i < n: iFFT's n^-1 and the following coset pre-scaling in one multiplication
+  Fr* odd_fwd_ninv = nullptr;    // n^-1 omega_2n^i  i < n: the same for CircomReduction's odd-point evaluation (built on
+                                 // demand by ntt_domain_build_odd, for a CircomReduction circuit only)
   Fr n_inv, z_inv;          // n^-1 ; (g^n - 1)^-1   (Montgomery form, host copies)
   Fr omega;
   void release() {
@@ -202,7 +230,8 @@ struct NttDomain {
     if (coset_fwd) cudaFree(coset_fwd);
     if (coset_inv) cudaFree(coset_inv);
     if (coset_fwd_ninv) cudaFree(coset_fwd_ninv);
-    tw_fwd = tw_inv = coset_fwd = coset_inv = coset_fwd_ninv = nullptr;
+    if (odd_fwd_ninv) cudaFree(odd_fwd_ninv);
+    tw_fwd = tw_inv = coset_fwd = coset_inv = coset_fwd_ninv = odd_fwd_ninv = nullptr;
     L = -1;
   }
 };
@@ -266,6 +295,18 @@ cudaError_t ntt_domain_build(NttDomain<Fr>& d, int L, cudaStream_t st, unsigned 
   return cudaGetLastError();
 }
 
+// The table n^-1 omega_2n^i of a built domain (CircomReduction); the caller has checked that L + 1 <= the two-adicity
+template <class Fr>
+cudaError_t ntt_domain_build_odd(NttDomain<Fr>& d, cudaStream_t st, unsigned long long* launches) {
+  if (d.odd_fwd_ninv) return cudaSuccess;
+  cudaError_t e;
+  if ((e = cudaMalloc(&d.odd_fwd_ninv, d.n * sizeof(Fr))) != cudaSuccess) return e;
+  const uint64_t threads = (d.n + 31) / 32;
+  ntt_powers_kernel<Fr><<<(unsigned)((threads + 127) / 128), 128, 0, st>>>(d.odd_fwd_ninv, d.n, fr_domain_root<Fr>(d.L + 1), d.n_inv);
+  if (launches) (*launches)++;
+  return cudaGetLastError();
+}
+
 struct NttPlan {
   int npass;
   int k[8];
@@ -298,7 +339,7 @@ inline NttPlan ntt_plan(int L) {
 template <class Fr>
 void ntt_run(cudaStream_t st, const NttDomain<Fr>& d, bool inverse, const Fr* src, Fr* work, Fr* dst, int load_mode,
              const Fr* ltab, const Fr* in_b, const Fr* in_c, const Fr& load_cst, int store_mode, const Fr* stab,
-             const Fr& store_cst, unsigned long long* launches, uint32_t nvec) {
+             const Fr& store_cst, unsigned long long* launches, uint32_t nvec, const Fr* st_a, const Fr* st_b) {
   const NttPlan p = ntt_plan(d.L);
   int s0 = 0;
   for (int i = 0; i < p.npass; i++) {
@@ -308,6 +349,8 @@ void ntt_run(cudaStream_t st, const NttDomain<Fr>& d, bool inverse, const Fr* sr
     a.in_b = in_b;
     a.in_c = in_c;
     a.out = last ? dst : work;
+    a.st_a = st_a;
+    a.st_b = st_b;
     a.tw = inverse ? d.tw_inv : d.tw_fwd;
     a.ltab = ltab;
     a.stab = stab;
@@ -326,24 +369,38 @@ void ntt_run(cudaStream_t st, const NttDomain<Fr>& d, bool inverse, const Fr* sr
     uint32_t threads = (1u << tile_log) / 2;
     if (threads > 256) threads = 256;
     if (threads < 32) threads = 32;
-    ntt_pass_kernel<Fr><<<dim3((unsigned)blocks, nvec > 1 ? nvec : 1u), threads, 0, st>>>(a);
+    const dim3 grid((unsigned)blocks, nvec > 1 ? nvec : 1u);
+    if (ntt_circom_mode(a.load_mode, a.store_mode)) ntt_pass_kernel<Fr, true><<<grid, threads, 0, st>>>(a);
+    else ntt_pass_kernel<Fr, false><<<grid, threads, 0, st>>>(a);
     if (launches) (*launches)++;
     s0 += a.k;
   }
 }
 
 
-// `count` assignments of nv elements each (z, contiguous) -> count row evaluations of n elements each (a, b, c)
+// `count` assignments of nv elements each (z, contiguous) -> count row evaluations of n elements each (a, b and, with
+// with_c, c)
 template <class Fr>
 void r1cs_matvec(cudaStream_t st, const CsrDev* cs, const Fr* z, uint32_t nc, uint32_t num_inputs, uint32_t n, Fr* a, Fr* b,
-                 Fr* c, uint32_t count, uint32_t nv) {
-  r1cs_matvec_kernel<Fr><<<dim3((n + 255) / 256, count > 1 ? count : 1u), 256, 0, st>>>(cs[0], cs[1], cs[2], z, nc, num_inputs, n, a, b, c, nv);
+                 Fr* c, uint32_t count, uint32_t nv, bool with_c) {
+  const dim3 grid((n + 255) / 256, count > 1 ? count : 1u);
+  if (with_c) r1cs_matvec_kernel<Fr, true><<<grid, 256, 0, st>>>(cs[0], cs[1], cs[2], z, nc, num_inputs, n, a, b, c, nv);
+  else r1cs_matvec_kernel<Fr, false><<<grid, 256, 0, st>>>(cs[0], cs[1], cs[2], z, nc, num_inputs, n, a, b, c, nv);
+}
+
+// h = a o b - c over `count` vectors of n elements (one launch)
+template <class Fr>
+void ntt_ab_minus_c(cudaStream_t st, const Fr* a, const Fr* b, const Fr* c, Fr* h, uint64_t n) {
+  ntt_ab_minus_c_kernel<Fr><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, b, c, h, n);
 }
 
 #define G16_NTT_TEMPLATES(X, Fr)                                                                                       \
   X void ntt_run<Fr>(cudaStream_t, const NttDomain<Fr>&, bool, const Fr*, Fr*, Fr*, int, const Fr*, const Fr*, const Fr*, \
-                     const Fr&, int, const Fr*, const Fr&, unsigned long long*, uint32_t);                             \
+                     const Fr&, int, const Fr*, const Fr&, unsigned long long*, uint32_t, const Fr*, const Fr*);       \
   X cudaError_t ntt_domain_build<Fr>(NttDomain<Fr>&, int, cudaStream_t, unsigned long long*);                          \
-  X void r1cs_matvec<Fr>(cudaStream_t, const CsrDev*, const Fr*, uint32_t, uint32_t, uint32_t, Fr*, Fr*, Fr*, uint32_t, uint32_t);
+  X cudaError_t ntt_domain_build_odd<Fr>(NttDomain<Fr>&, cudaStream_t, unsigned long long*);                           \
+  X void r1cs_matvec<Fr>(cudaStream_t, const CsrDev*, const Fr*, uint32_t, uint32_t, uint32_t, Fr*, Fr*, Fr*, uint32_t, uint32_t, \
+                         bool);                                                                                         \
+  X void ntt_ab_minus_c<Fr>(cudaStream_t, const Fr*, const Fr*, const Fr*, Fr*, uint64_t);
 
 }  // namespace g16

@@ -86,6 +86,27 @@ int g16_circuit_load(g16_ctx* ctx, uint32_t num_inputs /* instance variables inc
                      uint32_t num_constraints, uint32_t num_witness, const g16_csr* a, const g16_csr* b,
                      const g16_csr* c);
 
+/* ---- R1CS-to-QAP reduction of the resident circuit: the second type parameter of ark-groth16's
+ * Groth16<E, QAP: R1CSToQAP = LibsnarkReduction> (lib.rs:55, r1cs_to_qap.rs:71-120).
+ *   G16_QAP_LIBSNARK : LibsnarkReduction (r1cs_to_qap.rs:122-248); what g16_circuit_load loads.
+ *   G16_QAP_CIRCOM   : ark-circom's CircomReduction (circom circuits with snarkjs-compatible keys).  Its witness map never
+ *                      reads matrix C: c = a o b; a, b, c are interpolated on the domain of size n and evaluated at the odd
+ *                      powers omega_2n^(2j+1); h[j] = A[j] B[j] - C[j] (n evaluations, no division by Z).  Its H query
+ *                      holds n points: the odd entries of the size-2n ifft of delta^-1 tau^i (i < 2n - 1; entry 2n - 1 = 0).
+ * Everything that uses the circuit follows its reduction: g16_witness_map (n evaluations), g16_setup / g16_pk_export (H
+ * query of n points), g16_prove, submit / wait, g16_prove_batch, g16_prove_partial / g16_prove_assemble and
+ * g16_prove_sharded (with "wm_split").  g16_witness_map_evals has no circuit and stays LibsnarkReduction.  C must still
+ * be passed: g16_setup needs it.
+ * g16_circuit_load_qap(ctx, qap, ...) is g16_circuit_load with the reduction named; an unknown qap is G16_ERR_BAD_ARGUMENT,
+ * and for G16_QAP_CIRCOM a domain of size 2n above the field's two-adicity is G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE (BN254
+ * at n = 2^28).  Both are decided from the sizes alone, before any array is read or any resident state is released. */
+enum {
+  G16_QAP_LIBSNARK = 0,
+  G16_QAP_CIRCOM = 1
+};
+int g16_circuit_load_qap(g16_ctx* ctx, int qap, uint32_t num_inputs, uint32_t num_constraints, uint32_t num_witness,
+                         const g16_csr* a, const g16_csr* b, const g16_csr* c);
+
 /* ---- proving key: data_structures.rs:126-143.  Query arrays are the FULL ark vectors (a_query[0] included).
  * With world > 1 the context keeps only the index range of every query owned by `rank` (SURVEY.md section 8e):
  * round-robin split of each MSM's (base, scalar) pairs: pair i belongs to rank i mod world. */
@@ -93,7 +114,8 @@ typedef struct {
   const uint64_t* a_query;    uint64_t a_len;     /* G1, num_inputs + num_witness      (generator.rs:155) */
   const uint64_t* b_g1_query; uint64_t b_g1_len;  /* G1, same length                   (generator.rs:161) */
   const uint64_t* b_g2_query; uint64_t b_g2_len;  /* G2, same length                   (generator.rs:134) */
-  const uint64_t* h_query;    uint64_t h_len;     /* G1, domain_size - 1               (generator.rs:168) */
+  const uint64_t* h_query;    uint64_t h_len;     /* G1, domain_size - 1               (generator.rs:168);
+                                                     G16_QAP_CIRCOM: domain_size */
   const uint64_t* l_query;    uint64_t l_len;     /* G1, num_witness                   (generator.rs:174) */
   const uint64_t* alpha_g1;   /* vk.alpha_g1 */
   const uint64_t* beta_g1;
@@ -113,7 +135,7 @@ typedef struct {
   uint64_t* a_query;    /* capacity (num_inputs + num_witness) G1 */
   uint64_t* b_g1_query;
   uint64_t* b_g2_query;
-  uint64_t* h_query;    /* capacity domain_size - 1 */
+  uint64_t* h_query;    /* capacity domain_size - 1 (G16_QAP_CIRCOM: domain_size) */
   uint64_t* l_query;    /* capacity num_witness */
   uint64_t* alpha_g1; uint64_t* beta_g1; uint64_t* delta_g1;
   uint64_t* beta_g2; uint64_t* gamma_g2; uint64_t* delta_g2;
@@ -185,14 +207,14 @@ int g16_prove_sharded_submit(g16_ctx* ctx, int slot, const uint64_t* r, const ui
 int g16_prove_sharded_wait(g16_ctx* ctx, int slot, uint64_t* proof_out);
 
 /* ---- witness map alone on the resident circuit (R1CSToQAP::witness_map_from_matrices, r1cs_to_qap.rs:172-235):
- * h_out receives domain_size Montgomery Fr coefficients. */
+ * h_out receives domain_size Montgomery Fr coefficients (G16_QAP_CIRCOM: domain_size evaluations, see above). */
 int g16_witness_map(g16_ctx* ctx, const uint64_t* full_assignment, uint32_t flags, uint64_t* h_out);
 
 /* ---- measurement hooks (bench.py) ---------------------------------------------------------------------------- */
 typedef struct {
   float total_ms;        /* CUDA-event time of the last g16_prove / g16_prove_partial, first enqueue to last kernel */
   float h2d_ms;          /* assignment upload                                                                    */
-  float witness_map_ms;  /* row evaluation + 7 NTTs                                                              */
+  float witness_map_ms;  /* row evaluation + 7 NTTs (G16_QAP_CIRCOM: 6)                                             */
   float msm_ms[5];       /* h, l, a, b_g1, b_g2: whole MSM pipeline on its stream                                 */
   float msm_accum_ms[5]; /* the bucket-accumulation kernel (msm_accum_l0) of each MSM                             */
   float host_finish_ms;  /* host Horner + final assembly (prover.rs:76-131)                                       */

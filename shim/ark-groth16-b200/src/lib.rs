@@ -7,6 +7,9 @@
 //!   * `impl SNARK for Groth16<E, QAP>`                             src/lib.rs:59-97      -> [`Groth16B200`] (setup / verify forwarded)
 //!   * `R1CSToQAP::witness_map_from_matrices`                       src/r1cs_to_qap.rs:172-235 -> [`GpuReduction`] (NTT path only,
 //!     selectable as `ark_groth16::Groth16<E, GpuReduction>` without touching the MSMs)
+//!   * ark-circom's `CircomReduction` (circom circuits, snarkjs-compatible keys)  -> [`GpuCircomReduction`] for
+//!     `ark_groth16::Groth16<E, GpuCircomReduction>` (setup and witness map), and [`B200Prover::new_with_qap`] with
+//!     `sys::G16_QAP_CIRCOM` for the whole proof
 //! The MSMs have no hook inside ark-groth16 (src/prover.rs:66,74,262 call `msm_bigint` on `E::G1` / `E::G2` directly),
 //! hence the sibling prover type instead of a trait implementation.
 //!
@@ -195,7 +198,22 @@ impl<E: SwPairing> Drop for B200Prover<E> {
 impl<E: SwPairing> B200Prover<E> {
     /// Once per circuit: `ConstraintMatrices` -> CSR, `ProvingKey` -> packed queries; both stay resident on the GPU.
     /// `rank` / `world`: this process's share of a multi-GPU proof (pair i of every MSM lives on rank i mod world).
+    /// The circuit is proved under `LibsnarkReduction`, ark-groth16's default (`new_with_qap` names another).
     pub fn new(device: i32, matrices: &ConstraintMatrices<E::ScalarField>, pk: &ProvingKey<E>, rank: u32, world: u32) -> R1CSResult<Self> {
+        Self::new_with_qap(device, sys::G16_QAP_LIBSNARK, matrices, pk, rank, world)
+    }
+
+    /// `new` under the R1CS-to-QAP reduction `qap` (`sys::G16_QAP_LIBSNARK` or `sys::G16_QAP_CIRCOM`), the counterpart of
+    /// the second type parameter of `Groth16<E, QAP>`: a key made by `Groth16<E, CircomReduction>` (or
+    /// `Groth16<E, GpuCircomReduction>`) is proved with `sys::G16_QAP_CIRCOM`.
+    pub fn new_with_qap(
+        device: i32,
+        qap: i32,
+        matrices: &ConstraintMatrices<E::ScalarField>,
+        pk: &ProvingKey<E>,
+        rank: u32,
+        world: u32,
+    ) -> R1CSResult<Self> {
         let curve = curve_id::<E::ScalarField>().ok_or(SynthesisError::Unsatisfiable)?;
         let mut ctx = core::ptr::null_mut();
         status(unsafe { sys::g16_ctx_create(curve, device, &mut ctx) })?;
@@ -209,8 +227,9 @@ impl<E: SwPairing> B200Prover<E> {
         };
         let (a, b, c) = (Csr::new(&matrices.a), Csr::new(&matrices.b), Csr::new(&matrices.c));
         status(unsafe {
-            sys::g16_circuit_load(
+            sys::g16_circuit_load_qap(
                 ctx,
+                qap,
                 matrices.num_instance_variables as u32,
                 matrices.num_constraints as u32,
                 matrices.num_witness_variables as u32,
@@ -402,7 +421,9 @@ pub struct GpuReduction;
 
 struct ThreadCtx {
     ctx: *mut sys::g16_ctx,
-    loaded: Option<(usize, usize, usize, usize)>, // (instance vars, witness vars, constraints, nnz(a)) of the resident circuit
+    // (reduction, instance vars, witness vars, constraints, nnz(a)) of the resident circuit: a circuit loaded under one
+    // reduction is never reused for the other
+    loaded: Option<(i32, usize, usize, usize, usize)>,
 }
 thread_local! {
     static CTXS: RefCell<BTreeMap<i32, ThreadCtx>> = RefCell::new(BTreeMap::new());
@@ -421,15 +442,17 @@ fn with_thread_ctx<F: PrimeField, T>(f: impl FnOnce(&mut ThreadCtx) -> R1CSResul
         f(m.get_mut(&curve).unwrap())
     })
 }
-fn load_matrices_once<F: PrimeField>(t: &mut ThreadCtx, m: &ConstraintMatrices<F>) -> R1CSResult<()> {
-    let key = (m.num_instance_variables, m.num_witness_variables, m.num_constraints, m.a_num_non_zero);
+fn load_matrices_once<F: PrimeField>(t: &mut ThreadCtx, m: &ConstraintMatrices<F>, qap: i32) -> R1CSResult<()> {
+    let key = (qap, m.num_instance_variables, m.num_witness_variables, m.num_constraints, m.a_num_non_zero);
     if t.loaded == Some(key) {
         return Ok(());
     }
+    t.loaded = None; // a failed load below may have replaced part of the resident circuit
     let (a, b, c) = (Csr::new(&m.a), Csr::new(&m.b), Csr::new(&m.c));
     status(unsafe {
-        sys::g16_circuit_load(
+        sys::g16_circuit_load_qap(
             t.ctx,
+            qap,
             m.num_instance_variables as u32,
             m.num_constraints as u32,
             m.num_witness_variables as u32,
@@ -440,6 +463,24 @@ fn load_matrices_once<F: PrimeField>(t: &mut ThreadCtx, m: &ConstraintMatrices<F
     })?;
     t.loaded = Some(key);
     Ok(())
+}
+
+/// g16_witness_map on this thread's context with `matrices` resident under the reduction `qap`: n values (LibsnarkReduction:
+/// coefficients of h; CircomReduction: evaluations at the odd powers of omega_2n)
+fn gpu_witness_map<F: PrimeField>(
+    matrices: &ConstraintMatrices<F>,
+    num_inputs: usize,
+    num_constraints: usize,
+    full_assignment: &[F],
+    qap: i32,
+) -> R1CSResult<Vec<F>> {
+    with_thread_ctx::<F, _>(|t| {
+        load_matrices_once(t, matrices, qap)?;
+        let n = (num_constraints + num_inputs).next_power_of_two();
+        let mut h = ark_std::vec![F::zero(); n];
+        status(unsafe { sys::g16_witness_map(t.ctx, scalars_ptr(full_assignment), 0, h.as_mut_ptr() as *mut u64) })?;
+        Ok(h)
+    })
 }
 
 impl R1CSToQAP for GpuReduction {
@@ -456,13 +497,7 @@ impl R1CSToQAP for GpuReduction {
         num_constraints: usize,
         full_assignment: &[F],
     ) -> R1CSResult<Vec<F>> {
-        with_thread_ctx::<F, _>(|t| {
-            load_matrices_once(t, matrices)?;
-            let n = (num_constraints + num_inputs).next_power_of_two();
-            let mut h = ark_std::vec![F::zero(); n];
-            status(unsafe { sys::g16_witness_map(t.ctx, scalars_ptr(full_assignment), 0, h.as_mut_ptr() as *mut u64) })?;
-            Ok(h)
-        })
+        gpu_witness_map(matrices, num_inputs, num_constraints, full_assignment, sys::G16_QAP_LIBSNARK)
     }
 
     fn h_query_scalars<F: PrimeField, D: EvaluationDomain<F>>(
@@ -472,6 +507,54 @@ impl R1CSToQAP for GpuReduction {
         delta_inverse: F,
     ) -> Result<Vec<F>, SynthesisError> {
         LibsnarkReduction::h_query_scalars::<F, D>(max_power, t, zt, delta_inverse) // src/r1cs_to_qap.rs:237-247
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// ark-circom's CircomReduction with its witness map on the GPU: `ark_groth16::Groth16<E, GpuCircomReduction>` makes and
+// uses the same keys and proofs as `Groth16<E, ark_circom::CircomReduction>`.  ark-circom is not a dependency of this
+// crate; the reduction is restated from its definition:
+//   witness map: c = a o b (matrix C is not read); a, b, c interpolated on the domain of size n and evaluated at the odd
+//                powers omega_2n^(2j+1); h[j] = A[j] B[j] - C[j] (n evaluations)
+//   H query:     the odd entries of the size-2n ifft of delta^-1 t^i (i < 2n - 1; entry 2n - 1 is zero): n scalars
+// ---------------------------------------------------------------------------------------------------------------------
+pub struct GpuCircomReduction;
+
+impl R1CSToQAP for GpuCircomReduction {
+    fn instance_map_with_evaluation<F: PrimeField, D: EvaluationDomain<F>>(
+        cs: ConstraintSystemRef<F>,
+        t: &F,
+    ) -> Result<(Vec<F>, Vec<F>, Vec<F>, F, usize, usize), SynthesisError> {
+        LibsnarkReduction::instance_map_with_evaluation::<F, D>(cs, t) // CircomReduction's is LibsnarkReduction's
+    }
+
+    fn witness_map_from_matrices<F: PrimeField, D: EvaluationDomain<F>>(
+        matrices: &ConstraintMatrices<F>,
+        num_inputs: usize,
+        num_constraints: usize,
+        full_assignment: &[F],
+    ) -> R1CSResult<Vec<F>> {
+        gpu_witness_map(matrices, num_inputs, num_constraints, full_assignment, sys::G16_QAP_CIRCOM)
+    }
+
+    /// max_power = n - 1 (generator.rs passes the domain size minus one); zt is not used
+    fn h_query_scalars<F: PrimeField, D: EvaluationDomain<F>>(
+        max_power: usize,
+        t: F,
+        _zt: F,
+        delta_inverse: F,
+    ) -> Result<Vec<F>, SynthesisError> {
+        let n2 = 2 * (max_power + 1);
+        let domain = D::new(n2).ok_or(SynthesisError::PolynomialDegreeTooLarge)?;
+        let mut v = Vec::with_capacity(n2);
+        let mut p = delta_inverse;
+        for _ in 0..n2 - 1 {
+            v.push(p);
+            p *= t;
+        }
+        v.push(F::zero());
+        domain.ifft_in_place(&mut v);
+        Ok(v.into_iter().skip(1).step_by(2).collect())
     }
 }
 

@@ -18,6 +18,9 @@ pub const G16_ERR_BAD_ARGUMENT: c_int = 2;
 pub const G16_ERR_CUDA: c_int = 3;
 pub const G16_ERR_MALFORMED_KEY: c_int = 4;
 
+pub const G16_QAP_LIBSNARK: c_int = 0;
+pub const G16_QAP_CIRCOM: c_int = 1;
+
 pub const G16_ASSIGNMENT_ON_DEVICE: u32 = 1;
 pub const G16_SERIAL_MSMS: u32 = 2;
 
@@ -113,6 +116,7 @@ extern "C" {
     pub fn g16_msm_g1(ctx: *mut g16_ctx, bases: *const u64, scalars: *const u64, n: u64, out_xyz: *mut u64) -> c_int;
     pub fn g16_msm_g2(ctx: *mut g16_ctx, bases: *const u64, scalars: *const u64, n: u64, out_xyz: *mut u64) -> c_int;
     pub fn g16_circuit_load(ctx: *mut g16_ctx, num_inputs: u32, num_constraints: u32, num_witness: u32, a: *const g16_csr, b: *const g16_csr, c: *const g16_csr) -> c_int;
+    pub fn g16_circuit_load_qap(ctx: *mut g16_ctx, qap: c_int, num_inputs: u32, num_constraints: u32, num_witness: u32, a: *const g16_csr, b: *const g16_csr, c: *const g16_csr) -> c_int;
     pub fn g16_pk_load(ctx: *mut g16_ctx, pk: *const g16_pk_desc, rank: u32, world: u32) -> c_int;
     pub fn g16_setup(ctx: *mut g16_ctx, alpha: *const u64, beta: *const u64, gamma: *const u64, delta: *const u64, tau: *const u64, g1: *const u64, g2: *const u64) -> c_int;
     pub fn g16_pk_export(ctx: *mut g16_ctx, out: *const g16_pk_export_desc) -> c_int;
