@@ -57,6 +57,9 @@ SIGNATURES = [
     ("g16_pk_load", C.c_int, [C.c_void_p, C.POINTER(PkDesc), C.c_uint32, C.c_uint32]),
     ("g16_setup", C.c_int, [C.c_void_p] + [C.c_void_p] * 7),
     ("g16_pk_export", C.c_int, [C.c_void_p, C.POINTER(PkExportDesc)]),
+    ("g16_pk_load_serialized", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
+                                         C.POINTER(PkExportDesc)]),
+    ("g16_pk_export_serialized", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("g16_prove", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     ("g16_prove_partial", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     ("g16_prove_assemble", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -84,6 +87,9 @@ ERR_POLYNOMIAL_DEGREE_TOO_LARGE = 1
 ERR_BAD_ARGUMENT = 2
 ERR_CUDA = 3
 ERR_MALFORMED_KEY = 4
+ERR_INVALID_DATA = 5
+SER_COMPRESSED = 1
+SER_VALIDATE = 2
 ASSIGNMENT_ON_DEVICE = 1
 SERIAL_MSMS = 2
 QAP_LIBSNARK = 0

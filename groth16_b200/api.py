@@ -20,6 +20,7 @@ import numpy as np
 from . import _lib
 from .codec import CurveCodec
 from .params import CurveParams, get_curve
+from .serialize import DeserializeError
 
 
 class SynthesisError(Exception):
@@ -48,6 +49,8 @@ def _check(rc: int):
         raise MalformedKey(msg)
     if rc == _lib.ERR_CUDA:
         raise CudaError(msg)
+    if rc == _lib.ERR_INVALID_DATA:
+        raise DeserializeError(msg)
     raise ValueError(msg)
 
 
@@ -309,6 +312,45 @@ class Groth16:
         vk = VerifyingKey(out["alpha_g1"][0], out["beta_g2"][0], out["gamma_g2"][0], out["delta_g2"][0], out["gamma_abc_g1"])
         return ProvingKey(vk, out["beta_g1"][0], out["delta_g1"][0], out["a_query"], out["b_g1_query"], out["b_g2_query"],
                           out["h_query"], out["l_query"])
+
+    # ---- ark-serialized proving keys (ProvingKey::serialize_* / deserialize_with_mode), decoded and encoded on the GPU ----
+    def load_proving_key_bytes(self, data: bytes, compress: bool = True, validate: bool = True, rank: int = 0,
+                               world: int = 1) -> VerifyingKey:
+        """g16_pk_load_serialized: make the key in `data` (a whole ark-serialized ProvingKey of this curve) resident, exactly as
+        load_proving_key would the same key in limbs, and return its verifying key (with beta_g1 / delta_g1 on the side as
+        attributes).  A rejected key raises serialize.DeserializeError naming the first bad item; a gamma_abc_g1 that does not
+        match the circuit raises MalformedKey.  Afterwards no key is resident until a load succeeds."""
+        m = self._matrices
+        if m is None:
+            raise ValueError("load_matrices must come first")
+        buf = np.frombuffer(data, dtype=np.uint8)
+        nq, ni = self.nq, m.num_instance_variables
+        z = lambda rows, w: np.zeros((rows, w), dtype=np.uint64)
+        out = dict(alpha_g1=z(1, 2 * nq), beta_g1=z(1, 2 * nq), delta_g1=z(1, 2 * nq), beta_g2=z(1, 4 * nq),
+                   gamma_g2=z(1, 4 * nq), delta_g2=z(1, 4 * nq), gamma_abc_g1=z(ni, 2 * nq))
+        d = _lib.PkExportDesc()
+        for k, v in out.items():
+            setattr(d, k, _u64p(v) if v.size else None)
+        flags = (_lib.SER_COMPRESSED if compress else 0) | (_lib.SER_VALIDATE if validate else 0)
+        self._pk_resident = False
+        self._pk_obj = None
+        _check(self._lib.g16_pk_load_serialized(self._ctx, buf.ctypes.data_as(C.c_void_p) if buf.size else None, buf.size, flags,
+                                                rank, world, C.byref(d)))
+        self._pk_resident = True
+        self.world = world
+        vk = VerifyingKey(out["alpha_g1"][0], out["beta_g2"][0], out["gamma_g2"][0], out["delta_g2"][0], out["gamma_abc_g1"])
+        vk.beta_g1, vk.delta_g1 = out["beta_g1"][0], out["delta_g1"][0]
+        return vk
+
+    def export_proving_key_bytes(self, compress: bool = True) -> bytes:
+        """g16_pk_export_serialized: the resident key (made by generate_parameters_with_qap) as ark-serialize writes it,
+        byte for byte ArkCodec.proving_key of the exported limbs."""
+        flags = _lib.SER_COMPRESSED if compress else 0
+        n = C.c_uint64()
+        _check(self._lib.g16_pk_export_serialized(self._ctx, flags, None, 0, C.byref(n)))
+        out = np.zeros(n.value, dtype=np.uint8)
+        _check(self._lib.g16_pk_export_serialized(self._ctx, flags, out.ctypes.data_as(C.c_void_p), out.size, C.byref(n)))
+        return out.tobytes()
 
     # ---- prover.rs:26-51 ----
     def create_proof_with_reduction_and_matrices(self, pk: Optional[ProvingKey], r, s,

@@ -141,6 +141,15 @@ int g16_pk_export(g16_ctx* ctx, const g16_pk_export_desc* out) {
   CTX_OR_FAIL(ctx);
   return ctx->eng->pk_export(out);
 }
+int g16_pk_load_serialized(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
+                           const g16_pk_export_desc* vk_out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->pk_load_serialized(bytes, len, flags, rank, world, vk_out);
+}
+int g16_pk_export_serialized(g16_ctx* ctx, uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->pk_export_serialized(flags, out, cap, len_out);
+}
 int g16_prove(g16_ctx* ctx, const uint64_t* r, const uint64_t* s, const uint64_t* full_assignment, uint32_t flags, uint64_t* proof_out) {
   CTX_OR_FAIL(ctx);
   return ctx->eng->prove(r, s, full_assignment, flags, proof_out);

@@ -28,6 +28,7 @@
 #include "ec.cuh"
 #include "msm.cuh"
 #include "ntt.cuh"
+#include "ser.cuh"
 
 namespace g16 {
 
@@ -139,6 +140,9 @@ struct IEngine {
   virtual int setup(const uint64_t* alpha, const uint64_t* beta, const uint64_t* gamma, const uint64_t* delta,
                     const uint64_t* tau, const uint64_t* g1, const uint64_t* g2) = 0;
   virtual int pk_export(const g16_pk_export_desc* out) = 0;
+  virtual int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
+                                 const g16_pk_export_desc* vk_out) = 0;
+  virtual int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) = 0;
   virtual int prove(const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags, uint64_t* proof) = 0;
   virtual int prove_partial(const uint64_t* r, const uint64_t* z, uint32_t flags, uint64_t* partial) = 0;
   virtual int prove_assemble(const uint64_t* r, const uint64_t* s, const uint64_t* partials, uint32_t nparts, uint64_t* proof) = 0;
@@ -1096,6 +1100,208 @@ struct Engine : IEngine {
     return G16_OK;
   }
 
+  // ---- ark-serialized proving keys (ser.cuh) ----
+  // Points are decoded in chunks of at most SER_CHUNK (every query of a 2^20 key spans several), staged through two pinned
+  // buffers so that the copy of chunk i + 1 overlaps the decode of chunk i; extra device memory does not grow with the key.
+  static constexpr uint32_t SER_CHUNK = 1u << 17;
+  struct SerStaging {   // released on every return path
+    cudaStream_t st_copy = nullptr, st_dec = nullptr;
+    cudaEvent_t ev_h2d[2] = {}, ev_dec[2] = {};
+    uint8_t* host[2] = {};
+    DevBuf dev[2], aux, err;
+    ~SerStaging() {
+      if (st_dec) cudaStreamSynchronize(st_dec);
+      if (st_copy) cudaStreamSynchronize(st_copy);
+      for (int k = 0; k < 2; k++) {
+        if (ev_h2d[k]) cudaEventDestroy(ev_h2d[k]);
+        if (ev_dec[k]) cudaEventDestroy(ev_dec[k]);
+        if (host[k]) cudaFreeHost(host[k]);
+        dev[k].release();
+      }
+      if (st_dec) cudaStreamDestroy(st_dec);
+      if (st_copy) cudaStreamDestroy(st_copy);
+      aux.release();
+      err.release();
+    }
+  };
+  int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rk, uint32_t wd,
+                         const g16_pk_export_desc* vk) override {
+    using Fmt = SerFormat<CP>;
+    if (!have_circuit) return fail(G16_ERR_BAD_ARGUMENT, "g16_circuit_load must precede g16_pk_load_serialized");
+    if ((!bytes && len) || wd == 0 || rk >= wd) return fail(G16_ERR_BAD_ARGUMENT, "bad bytes / rank / world");
+    if (flags & ~(uint32_t)(G16_SER_COMPRESSED | G16_SER_VALIDATE)) return fail(G16_ERR_BAD_ARGUMENT, "unknown serialization flags");
+    if (vk && (vk->a_query || vk->b_g1_query || vk->b_g2_query || vk->h_query || vk->l_query))
+      return fail(G16_ERR_BAD_ARGUMENT, "vk_out receives the verifying key only: its query members must be NULL");
+    G16_NOT_BUSY();
+    G16_CUDA(cudaSetDevice(device));
+    // from here on a rejected key leaves no key resident
+    have_pk = false;
+    from_setup = false;
+    tail_ready = false;
+    SerItem it[SER_ITEMS];
+    const std::string why = ser_walk(bytes, len, Fmt::NB, flags & G16_SER_COMPRESSED, it);
+    if (!why.empty()) return fail(G16_ERR_INVALID_DATA, why);
+    if (it[SER_A].len < 1 || it[SER_B_G1].len < 1 || it[SER_B_G2].len < 1)
+      return fail(G16_ERR_MALFORMED_KEY, "a/b queries must hold at least the constant-one base");
+    if (it[SER_GAMMA_ABC].len != num_inputs)
+      return fail(G16_ERR_MALFORMED_KEY, "vk.gamma_abc_g1 holds " + std::to_string(it[SER_GAMMA_ABC].len) +
+                                             " points, the circuit has " + std::to_string(num_inputs) + " instance variables");
+    rank = rk; world = wd;
+    const uint64_t n = 1ull << L;
+    const uint64_t nz1 = nvars() - 1;
+    // the same truncation and shards as g16_pk_load
+    shard(q[M_H], std::min<uint64_t>(it[SER_H].len, n));
+    shard(q[M_L], std::min<uint64_t>(it[SER_L].len, num_witness));
+    shard(q[M_A], std::min<uint64_t>(it[SER_A].len - 1, nz1));
+    shard(q[M_B1], std::min<uint64_t>(it[SER_B_G1].len - 1, nz1));
+    shard(q[M_B2], std::min<uint64_t>(it[SER_B_G2].len - 1, nz1));
+    for (int m = 0; m < 5; m++) {
+      if (!geom_fits(q[m])) return fail(G16_ERR_BAD_ARGUMENT, "query too large for one GPU: shard it (world > 1) or raise G16_MSM_NE");
+      const size_t esz = m == M_B2 ? sizeof(A2) : sizeof(A1);
+      G16_CUDA(q[m].bases.reserve((size_t)q[m].geom.copies * (q[m].hi - q[m].lo) * esz + 16));
+    }
+    // host-bound points: the seven single points, element 0 of a / b_g1 / b_g2, gamma_abc_g1
+    enum { AUX_A0 = 7, AUX_B10 = 8, AUX_B20 = 9, AUX_ABC = 10 };
+    const size_t aux_bytes = AUX_ABC * sizeof(A2) + (size_t)num_inputs * sizeof(A1);
+    SerStaging sg;
+    G16_CUDA(cudaStreamCreateWithFlags(&sg.st_copy, cudaStreamNonBlocking));
+    G16_CUDA(cudaStreamCreateWithFlags(&sg.st_dec, cudaStreamNonBlocking));
+    // reset on the decode stream itself: st_dec does not wait for the legacy default stream, so a plain cudaMemset there
+    // could land after the first decodes and wipe their points or their error
+    G16_CUDA(sg.aux.reserve(aux_bytes));
+    G16_CUDA(cudaMemsetAsync(sg.aux.p, 0, aux_bytes, sg.st_dec));
+    G16_CUDA(sg.err.reserve(8));
+    G16_CUDA(cudaMemsetAsync(sg.err.p, 0xff, 8, sg.st_dec));
+    auto aux_at = [&](int slot) { return (char*)sg.aux.p + (size_t)slot * sizeof(A2); };
+    const std::vector<SerChunk> plan = ser_plan(it, SER_CHUNK);
+    size_t stage = 0;
+    for (const SerChunk& c : plan) stage = std::max<size_t>(stage, (size_t)c.count * it[c.member].psize);
+    for (int k = 0; k < 2; k++) {
+      G16_CUDA(cudaEventCreateWithFlags(&sg.ev_h2d[k], cudaEventDisableTiming));
+      G16_CUDA(cudaEventCreateWithFlags(&sg.ev_dec[k], cudaEventDisableTiming));
+      G16_CUDA(cudaHostAlloc((void**)&sg.host[k], stage + 1, cudaHostAllocDefault));
+      G16_CUDA(sg.dev[k].reserve(stage + 1));
+    }
+    for (size_t ci = 0; ci < plan.size(); ci++) {
+      const SerChunk& c = plan[ci];
+      const SerItem& x = it[c.member];
+      const int k = (int)(ci & 1);
+      const size_t nbytes = (size_t)c.count * x.psize;
+      if (ci >= 2) G16_CUDA(cudaEventSynchronize(sg.ev_h2d[k]));   // staging buffer k is free again
+      memcpy(sg.host[k], bytes + c.off, nbytes);
+      if (ci >= 2) G16_CUDA(cudaStreamWaitEvent(sg.st_copy, sg.ev_dec[k], 0));   // the decode that read dev[k] is done
+      G16_CUDA(cudaMemcpyAsync(sg.dev[k].p, sg.host[k], nbytes, cudaMemcpyHostToDevice, sg.st_copy));
+      G16_CUDA(cudaEventRecord(sg.ev_h2d[k], sg.st_copy));
+      G16_CUDA(cudaStreamWaitEvent(sg.st_dec, sg.ev_h2d[k], 0));
+      SerDest d;
+      d.rank = rank;
+      d.world = world;
+      d.aux_n = 1;
+      switch (c.member) {
+        case SER_GAMMA_ABC: d.aux = aux_at(AUX_ABC); d.aux_n = x.len; break;
+        case SER_A: d.aux = aux_at(AUX_A0); d.bases = q[M_A].bases.p; d.skip = 1; d.pairs = q[M_A].pairs; break;
+        case SER_B_G1: d.aux = aux_at(AUX_B10); d.bases = q[M_B1].bases.p; d.skip = 1; d.pairs = q[M_B1].pairs; break;
+        case SER_B_G2: d.aux = aux_at(AUX_B20); d.bases = q[M_B2].bases.p; d.skip = 1; d.pairs = q[M_B2].pairs; break;
+        case SER_H: d.aux_n = 0; d.bases = q[M_H].bases.p; d.pairs = q[M_H].pairs; break;
+        case SER_L: d.aux_n = 0; d.bases = q[M_L].bases.p; d.pairs = q[M_L].pairs; break;
+        default: d.aux = aux_at(c.member); break;   // single points: slots 0 .. 6 in stream order
+      }
+      const uint8_t* src = sg.dev[k].template as<uint8_t>();
+      unsigned long long* err = sg.err.template as<unsigned long long>();
+      const cudaError_t e = x.g2 ? ser_decode_enqueue<CP, true>(sg.st_dec, src, c.first, c.count, flags, c.off, d, err)
+                                 : ser_decode_enqueue<CP, false>(sg.st_dec, src, c.first, c.count, flags, c.off, d, err);
+      G16_CUDA(e);
+      G16_CUDA(cudaEventRecord(sg.ev_dec[k], sg.st_dec));
+    }
+    G16_CUDA(cudaStreamSynchronize(sg.st_dec));
+    unsigned long long first_err = 0;
+    G16_CUDA(cudaMemcpy(&first_err, sg.err.p, 8, cudaMemcpyDeviceToHost));
+    if (first_err != ~0ull) {
+      const uint64_t off = first_err >> 8;
+      return fail(G16_ERR_INVALID_DATA, ser_locate(it, off) + " (byte " + std::to_string(off) + "): " + ser_reason(first_err & 0xff));
+    }
+    std::vector<char> aux(aux_bytes);
+    G16_CUDA(cudaMemcpy(aux.data(), sg.aux.p, aux_bytes, cudaMemcpyDeviceToHost));
+    auto a1 = [&](int slot) { A1 r; memcpy(&r, aux.data() + (size_t)slot * sizeof(A2), sizeof(A1)); return r; };
+    auto a2 = [&](int slot) { A2 r; memcpy(&r, aux.data() + (size_t)slot * sizeof(A2), sizeof(A2)); return r; };
+    alpha_g1 = a1(SER_ALPHA_G1); beta_g1 = a1(SER_BETA_G1); delta_g1 = a1(SER_DELTA_G1);
+    beta_g2 = a2(SER_BETA_G2); delta_g2 = a2(SER_DELTA_G2);
+    int rc;
+    for (int m = 0; m < 5; m++)
+      if ((rc = (m == M_B2) ? finish_query<Fq2>(q[m]) : finish_query<Fq>(q[m]))) return rc;
+    set_tail_points(a1(AUX_A0), a1(AUX_B10), a2(AUX_B20));
+    G16_CUDA(cudaStreamSynchronize(S0.st_main));
+    have_pk = true;
+    if ((rc = decide_b_sort_sharing())) return rc;
+    decide_ba_memory();
+    if (vk) {
+      if (vk->alpha_g1) store_a1(vk->alpha_g1, alpha_g1);
+      if (vk->beta_g1) store_a1(vk->beta_g1, beta_g1);
+      if (vk->delta_g1) store_a1(vk->delta_g1, delta_g1);
+      if (vk->beta_g2) store_a2(vk->beta_g2, beta_g2);
+      if (vk->gamma_g2) store_a2(vk->gamma_g2, a2(SER_GAMMA_G2));
+      if (vk->delta_g2) store_a2(vk->delta_g2, delta_g2);
+      if (vk->gamma_abc_g1)
+        for (uint32_t i = 0; i < num_inputs; i++) {
+          A1 p;
+          memcpy(&p, aux.data() + AUX_ABC * sizeof(A2) + (size_t)i * sizeof(A1), sizeof(A1));
+          store_a1(vk->gamma_abc_g1 + (size_t)i * 2 * NQ64, p);
+        }
+    }
+    return G16_OK;
+  }
+  int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) override {
+    using Fmt = SerFormat<CP>;
+    if (!have_pk || !from_setup) return fail(G16_ERR_BAD_ARGUMENT, "g16_pk_export_serialized needs a key produced by g16_setup");
+    if (!len_out) return fail(G16_ERR_BAD_ARGUMENT, "null len_out");
+    if (flags & ~(uint32_t)G16_SER_COMPRESSED) return fail(G16_ERR_BAD_ARGUMENT, "export takes G16_SER_COMPRESSED only");
+    G16_NOT_BUSY();
+    const uint64_t nv = nvars(), n = 1ull << L;
+    SerItem it[SER_ITEMS];
+    ser_items(it);
+    it[SER_GAMMA_ABC].len = num_inputs;
+    it[SER_A].len = it[SER_B_G1].len = it[SER_B_G2].len = nv;
+    it[SER_H].len = qap == G16_QAP_CIRCOM ? n : n - 1;
+    it[SER_L].len = num_witness;
+    const uint64_t size = ser_size(it, Fmt::NB, flags & G16_SER_COMPRESSED);
+    *len_out = size;
+    if (!out) return G16_OK;
+    if (cap < size)
+      return fail(G16_ERR_BAD_ARGUMENT, "output buffer holds " + std::to_string(cap) + " bytes, the key needs " + std::to_string(size));
+    G16_CUDA(cudaSetDevice(device));
+    const A1 g1s[SER_ITEMS] = {alpha_g1, {}, {}, {}, {}, beta_g1, delta_g1};
+    const A2 g2s[SER_ITEMS] = {{}, beta_g2, gamma_g2, delta_g2};
+    const void* src[SER_ITEMS] = {};
+    src[SER_GAMMA_ABC] = d_gamma_abc.p; src[SER_A] = full_a.p; src[SER_B_G1] = full_b1.p; src[SER_B_G2] = full_b2.p;
+    src[SER_H] = q[M_H].bases.p; src[SER_L] = q[M_L].bases.p;
+    DevBuf stage;
+    int rc = G16_OK;
+    for (int m = 0; m < SER_ITEMS && rc == G16_OK; m++) {
+      const SerItem& x = it[m];
+      if (!x.vec) {   // a single point: encoded here, with the kernel's own function
+        if (x.g2) ser_encode<CP, true>(g2s[m], flags, out + x.off);
+        else ser_encode<CP, false>(g1s[m], flags, out + x.off);
+        continue;
+      }
+      for (int k = 0; k < 8; k++) out[x.off - 8 + k] = (uint8_t)(x.len >> (8 * k));
+      const size_t esz = x.g2 ? sizeof(A2) : sizeof(A1);
+      for (uint64_t f = 0; f < x.len && rc == G16_OK; f += SER_CHUNK) {
+        const uint32_t cnt = (uint32_t)std::min<uint64_t>(SER_CHUNK, x.len - f);
+        cudaError_t e = stage.reserve((size_t)SER_CHUNK * 4 * Fmt::NB);
+        const void* s = (const char*)src[m] + f * esz;
+        if (e == cudaSuccess)
+          e = x.g2 ? ser_encode_enqueue<CP, true>(S0.st_main, s, cnt, flags, stage.template as<uint8_t>())
+                   : ser_encode_enqueue<CP, false>(S0.st_main, s, cnt, flags, stage.template as<uint8_t>());
+        if (e == cudaSuccess)
+          e = cudaMemcpyAsync(out + x.off + f * x.psize, stage.p, (size_t)cnt * x.psize, cudaMemcpyDeviceToHost, S0.st_main);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(S0.st_main);
+        if (e != cudaSuccess) rc = fail(G16_ERR_CUDA, std::string("pk_export_serialized: ") + cudaGetErrorString(e));
+      }
+    }
+    stage.release();
+    return rc;
+  }
+
   // ---- proving ----
   // enqueue on sl.st_main: upload z, row evaluation, witness map
   // count > 1 (batch proving): `count` assignments, nv elements apart, and as many witness maps
@@ -1705,7 +1911,8 @@ struct Engine : IEngine {
 #define G16_CURVE_KERNELS(X, CP)                                                                  \
   G16_NTT_TEMPLATES(X, Fp<CP::FrP>)                                                               \
   G16_MSM_TEMPLATES(X, Fp<CP::FqP>, Fp<CP::FrP>)                                                  \
-  G16_MSM_TEMPLATES(X, G16_FQ2(CP), Fp<CP::FrP>)
+  G16_MSM_TEMPLATES(X, G16_FQ2(CP), Fp<CP::FrP>)                                                  \
+  G16_SER_TEMPLATES(X, CP)
 #define G16_FQ2(CP) Fp2<CP::FqP, CP::FQ2_NONRESIDUE_NEG>
 
 template <class CP>

@@ -35,7 +35,9 @@ enum {
   G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE = 1, /* SynthesisError::PolynomialDegreeTooLarge, r1cs_to_qap.rs:134,179 */
   G16_ERR_BAD_ARGUMENT = 2,                /* null pointer / inconsistent length / unknown curve               */
   G16_ERR_CUDA = 3,                        /* CUDA failure or no usable sm_90 device; see g16_last_error()     */
-  G16_ERR_MALFORMED_KEY = 4                /* SynthesisError::MalformedVerifyingKey-class length mismatch      */
+  G16_ERR_MALFORMED_KEY = 4,               /* SynthesisError::MalformedVerifyingKey-class length mismatch      */
+  G16_ERR_INVALID_DATA = 5                 /* ark_serialize::SerializationError::{InvalidData, UnexpectedFlags,
+                                              NotEnoughSpace}: a rejected serialized key                         */
 };
 
 typedef struct g16_ctx g16_ctx;
@@ -142,6 +144,30 @@ typedef struct {
   uint64_t* gamma_abc_g1; /* capacity num_inputs G1 */
 } g16_pk_export_desc;
 int g16_pk_export(g16_ctx* ctx, const g16_pk_export_desc* out);
+
+/* ---- ark-serialized proving keys: `ProvingKey::serialize_{compressed,uncompressed}` / `deserialize_with_mode`
+ * (data_structures.rs:125 derives them).  The bytes are a whole ProvingKey<E> as ark-serialize 0.5 writes it: vk {alpha_g1,
+ * beta_g2, gamma_g2, delta_g2, gamma_abc_g1}, beta_g1, delta_g1, a_query, b_g1_query, b_g2_query, h_query, l_query; vectors
+ * are u64-LE length-prefixed.  Points: BLS12-381 zcash / IETF (big-endian, three flag bits, Fq2 as c1 || c0); BN254 and
+ * BLS12-377 generic short Weierstrass (little-endian, SWFlags in the top bits of the last byte).  The VerifyingKey bytes are
+ * the prefix of the ProvingKey bytes.
+ *   G16_SER_COMPRESSED selects the encoding (x and a sign bit); G16_SER_VALIDATE adds the prime-order-subgroup check
+ *   [r]P = O of every point (not needed, and skipped, for BN254 G1, whose cofactor is 1).  Always checked: truncation,
+ *   trailing bytes, length prefixes above 2^28, the flag bits, zero bytes under the infinity flag, canonical coordinates
+ *   (< q), that a compressed x has a curve point and that an uncompressed point is on the curve.
+ * g16_pk_load_serialized decodes, validates and places the key on the GPU and makes it resident with exactly the rules of
+ * g16_pk_load: truncation to the circuit, rank / world shares; every rank decodes and validates all points.  A rejected key
+ * returns G16_ERR_INVALID_DATA, g16_last_error() naming the first bad item in stream order (member, index, reason); a
+ * gamma_abc_g1 that does not hold num_inputs points, or an empty a/b query, returns G16_ERR_MALFORMED_KEY.  After either no
+ * key is resident.  A non-null vk_out receives alpha_g1, beta_g1, delta_g1, beta_g2, gamma_g2, delta_g2 and gamma_abc_g1
+ * (capacity num_inputs); its five query members must be NULL.
+ * g16_pk_export_serialized writes the resident key (made by g16_setup; any other is G16_ERR_BAD_ARGUMENT) in the same
+ * format; flags is 0 or G16_SER_COMPRESSED.  out == NULL: *len_out receives the size only; cap below it is
+ * G16_ERR_BAD_ARGUMENT with the size in *len_out. */
+enum { G16_SER_COMPRESSED = 1, G16_SER_VALIDATE = 2 };
+int g16_pk_load_serialized(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
+                           const g16_pk_export_desc* vk_out);
+int g16_pk_export_serialized(g16_ctx* ctx, uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out);
 
 /* ---- proving: Groth16::create_proof_with_reduction_and_matrices, prover.rs:26-51
  *      = witness_map_from_matrices (r1cs_to_qap.rs:172-235) + create_proof_with_assignment (prover.rs:54-132).

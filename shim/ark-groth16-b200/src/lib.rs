@@ -36,6 +36,7 @@ use ark_groth16::{
     Groth16, PreparedVerifyingKey, Proof, ProvingKey, VerifyingKey,
 };
 use ark_poly::EvaluationDomain;
+use ark_serialize::{Compress, SerializationError, Validate};
 use ark_relations::r1cs::{
     ConstraintMatrices, ConstraintSynthesizer, ConstraintSystem, ConstraintSystemRef, Matrix, OptimizationGoal,
     Result as R1CSResult, SynthesisError,
@@ -63,6 +64,24 @@ fn status(rc: i32) -> R1CSResult<()> {
             eprintln!("libg16b200: {msg}");
             Err(SynthesisError::Unsatisfiable)
         },
+    }
+}
+
+/// status codes of the serialized-key calls -> SerializationError.  A rejected key (G16_ERR_INVALID_DATA, and a
+/// gamma_abc_g1 / query length that does not fit the circuit, G16_ERR_MALFORMED_KEY) is `InvalidData`, whose message naming
+/// the member, index and reason goes to stderr; a CUDA failure or a bad argument is an `IoError` carrying the library's
+/// message, so that callers can tell a missing GPU from bad key data.
+fn ser_status(rc: i32) -> Result<(), SerializationError> {
+    if rc == sys::G16_OK {
+        return Ok(());
+    }
+    let msg = unsafe { CStr::from_ptr(sys::g16_last_error()) }.to_string_lossy().into_owned();
+    match rc {
+        sys::G16_ERR_INVALID_DATA | sys::G16_ERR_MALFORMED_KEY => {
+            eprintln!("libg16b200: {msg}");
+            Err(SerializationError::InvalidData)
+        },
+        _ => Err(SerializationError::IoError(ark_std::io::Error::new(ark_std::io::ErrorKind::Other, msg))),
     }
 }
 
@@ -272,6 +291,104 @@ impl<E: SwPairing> B200Prover<E> {
             delta_g2: delta_g2.as_ptr(),
         };
         status(unsafe { sys::g16_pk_load(self.ctx, &desc, rank, world) })
+    }
+
+    /// `ProvingKey::<E>::deserialize_with_mode(bytes, compress, validate)` and `new` in one step, decoded and validated on the
+    /// GPU (g16_pk_load_serialized): `bytes` is a whole ark-serialized ProvingKey<E>.  Returns the prover and the key's
+    /// VerifyingKey (whose bytes are the prefix of `bytes`).  Every rank decodes and validates all points.
+    #[allow(clippy::too_many_arguments)]
+    pub fn new_from_bytes(
+        device: i32,
+        qap: i32,
+        matrices: &ConstraintMatrices<E::ScalarField>,
+        bytes: &[u8],
+        compress: Compress,
+        validate: Validate,
+        rank: u32,
+        world: u32,
+    ) -> Result<(Self, VerifyingKey<E>), SerializationError> {
+        let curve = curve_id::<E::ScalarField>().ok_or_else(|| {
+            SerializationError::IoError(ark_std::io::Error::new(ark_std::io::ErrorKind::Other, "libg16b200 does not support this curve"))
+        })?;
+        let mut ctx = core::ptr::null_mut();
+        ser_status(unsafe { sys::g16_ctx_create(curve, device, &mut ctx) })?;
+        let me = Self {
+            ctx,
+            num_inputs: matrices.num_instance_variables,
+            num_constraints: matrices.num_constraints,
+            num_variables: matrices.num_instance_variables + matrices.num_witness_variables,
+            fq_limbs: unsafe { sys::g16_fq_limbs(ctx) } as usize,
+            _e: PhantomData,
+        };
+        let (a, b, c) = (Csr::new(&matrices.a), Csr::new(&matrices.b), Csr::new(&matrices.c));
+        ser_status(unsafe {
+            sys::g16_circuit_load_qap(
+                ctx,
+                qap,
+                matrices.num_instance_variables as u32,
+                matrices.num_constraints as u32,
+                matrices.num_witness_variables as u32,
+                &a.desc(),
+                &b.desc(),
+                &c.desc(),
+            )
+        })?;
+        let vk = me.load_proving_key_bytes(bytes, compress, validate, rank, world)?;
+        Ok((me, vk))
+    }
+
+    /// Replace the resident key by the ark-serialized ProvingKey in `bytes` (g16_pk_load_serialized).  A rejected key
+    /// leaves no key resident.
+    pub fn load_proving_key_bytes(
+        &self,
+        bytes: &[u8],
+        compress: Compress,
+        validate: Validate,
+        rank: u32,
+        world: u32,
+    ) -> Result<VerifyingKey<E>, SerializationError> {
+        let (w1, w2) = (point_limbs::<E::G1Config>(), point_limbs::<E::G2Config>());
+        let (mut alpha_g1, mut beta_g1, mut delta_g1) = (ark_std::vec![0u64; w1], ark_std::vec![0u64; w1], ark_std::vec![0u64; w1]);
+        let (mut beta_g2, mut gamma_g2, mut delta_g2) = (ark_std::vec![0u64; w2], ark_std::vec![0u64; w2], ark_std::vec![0u64; w2]);
+        let mut abc = ark_std::vec![0u64; w1 * self.num_inputs];
+        let null = core::ptr::null_mut();
+        let desc = sys::g16_pk_export_desc {
+            a_query: null,
+            b_g1_query: null,
+            b_g2_query: null,
+            h_query: null,
+            l_query: null,
+            alpha_g1: alpha_g1.as_mut_ptr(),
+            beta_g1: beta_g1.as_mut_ptr(),
+            delta_g1: delta_g1.as_mut_ptr(),
+            beta_g2: beta_g2.as_mut_ptr(),
+            gamma_g2: gamma_g2.as_mut_ptr(),
+            delta_g2: delta_g2.as_mut_ptr(),
+            gamma_abc_g1: abc.as_mut_ptr(),
+        };
+        let mut flags = if matches!(compress, Compress::Yes) { sys::G16_SER_COMPRESSED } else { 0 };
+        if matches!(validate, Validate::Yes) {
+            flags |= sys::G16_SER_VALIDATE;
+        }
+        ser_status(unsafe { sys::g16_pk_load_serialized(self.ctx, bytes.as_ptr(), bytes.len() as u64, flags, rank, world, &desc) })?;
+        Ok(VerifyingKey {
+            alpha_g1: unpack_point(&alpha_g1),
+            beta_g2: unpack_point(&beta_g2),
+            gamma_g2: unpack_point(&gamma_g2),
+            delta_g2: unpack_point(&delta_g2),
+            gamma_abc_g1: abc.chunks(w1).map(|l| unpack_point(l)).collect(),
+        })
+    }
+
+    /// `ProvingKey::serialize_with_mode(compress)` of the resident key, encoded on the GPU (g16_pk_export_serialized).  Only
+    /// a key made by the library's own setup can be exported.
+    pub fn export_proving_key_bytes(&self, compress: Compress) -> Result<Vec<u8>, SerializationError> {
+        let flags = if matches!(compress, Compress::Yes) { sys::G16_SER_COMPRESSED } else { 0 };
+        let mut n = 0u64;
+        ser_status(unsafe { sys::g16_pk_export_serialized(self.ctx, flags, core::ptr::null_mut(), 0, &mut n) })?;
+        let mut out = ark_std::vec![0u8; n as usize];
+        ser_status(unsafe { sys::g16_pk_export_serialized(self.ctx, flags, out.as_mut_ptr(), n, &mut n) })?;
+        Ok(out)
     }
 
     fn proof_from_limbs(&self, out: &[u64]) -> Proof<E> {

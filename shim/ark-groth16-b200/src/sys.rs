@@ -17,6 +17,10 @@ pub const G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE: c_int = 1;
 pub const G16_ERR_BAD_ARGUMENT: c_int = 2;
 pub const G16_ERR_CUDA: c_int = 3;
 pub const G16_ERR_MALFORMED_KEY: c_int = 4;
+pub const G16_ERR_INVALID_DATA: c_int = 5;
+
+pub const G16_SER_COMPRESSED: u32 = 1;
+pub const G16_SER_VALIDATE: u32 = 2;
 
 pub const G16_QAP_LIBSNARK: c_int = 0;
 pub const G16_QAP_CIRCOM: c_int = 1;
@@ -120,6 +124,8 @@ extern "C" {
     pub fn g16_pk_load(ctx: *mut g16_ctx, pk: *const g16_pk_desc, rank: u32, world: u32) -> c_int;
     pub fn g16_setup(ctx: *mut g16_ctx, alpha: *const u64, beta: *const u64, gamma: *const u64, delta: *const u64, tau: *const u64, g1: *const u64, g2: *const u64) -> c_int;
     pub fn g16_pk_export(ctx: *mut g16_ctx, out: *const g16_pk_export_desc) -> c_int;
+    pub fn g16_pk_load_serialized(ctx: *mut g16_ctx, bytes: *const u8, len: u64, flags: u32, rank: u32, world: u32, vk_out: *const g16_pk_export_desc) -> c_int;
+    pub fn g16_pk_export_serialized(ctx: *mut g16_ctx, flags: u32, out: *mut u8, cap: u64, len_out: *mut u64) -> c_int;
     pub fn g16_prove(ctx: *mut g16_ctx, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32, proof_out: *mut u64) -> c_int;
     pub fn g16_prove_partial(ctx: *mut g16_ctx, r: *const u64, full_assignment: *const u64, flags: u32, partial_out: *mut u64) -> c_int;
     pub fn g16_prove_assemble(ctx: *mut g16_ctx, r: *const u64, s: *const u64, partials: *const u64, nparts: u32, proof_out: *mut u64) -> c_int;
