@@ -10,8 +10,8 @@ _os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 from .api import (ConstraintMatrices, CudaError, Groth16, MalformedKey, PolynomialDegreeTooLarge, Proof, ProvingKey,
                   SynthesisError, VerifyingKey)
 from .codec import CurveCodec, FieldCodec
-from .params import BLS12_377, BLS12_381, BN254, CURVES, get_curve
+from .params import BLS12_377, BLS12_381, BN254, BW6_761, CURVES, get_curve
 
 __all__ = ["Groth16", "ConstraintMatrices", "ProvingKey", "VerifyingKey", "Proof", "SynthesisError",
-           "PolynomialDegreeTooLarge", "MalformedKey", "CudaError", "CurveCodec", "FieldCodec", "CURVES", "BLS12_381",
+           "PolynomialDegreeTooLarge", "MalformedKey", "CudaError", "CurveCodec", "FieldCodec", "CURVES", "BW6_761", "BLS12_381",
            "BN254", "BLS12_377", "get_curve"]

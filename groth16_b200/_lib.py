@@ -45,6 +45,8 @@ SIGNATURES = [
     ("g16_ctx_destroy", None, [C.c_void_p]),
     ("g16_last_error", C.c_char_p, []),
     ("g16_fq_limbs", C.c_int, [C.c_void_p]),
+    ("g16_fr_limbs", C.c_int, [C.c_void_p]),
+    ("g16_g2_limbs", C.c_int, [C.c_void_p]),
     ("g16_partial_limbs", C.c_int, [C.c_void_p]),
     ("g16_domain_log", C.c_uint32, [C.c_void_p]),
     ("g16_ntt", C.c_int, [C.c_void_p, C.c_uint32, C.c_int, C.c_int, C.c_void_p]),

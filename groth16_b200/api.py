@@ -97,7 +97,7 @@ class ConstraintMatrices:
                     vals.append(cf)
                 rp[i + 1] = len(cols)
             col = np.asarray(cols, dtype=np.uint32)
-            val = cd.fr.enc(vals) if vals else np.zeros((0, 4), dtype=np.uint64)
+            val = cd.fr.enc(vals) if vals else np.zeros((0, cd.fr.nl), dtype=np.uint64)
             return rp, col, np.ascontiguousarray(val)
 
         return ConstraintMatrices(num_instance, num_witness, len(a_rows), csr(a_rows), csr(b_rows), csr(c_rows))
@@ -156,6 +156,16 @@ class Groth16:
         self._pk_obj: Optional[ProvingKey] = None   # identity of the resident key (None: minted by g16_setup and not exported)
         self.world = 1
 
+    @property
+    def nr(self) -> int:
+        """u64 limbs per Fr element / BigInt scalar (g16_fr_limbs)"""
+        return self.curve.fr_limbs
+
+    @property
+    def ng2(self) -> int:
+        """u64 limbs per G2 affine point (g16_g2_limbs)"""
+        return self.curve.g2_limbs
+
     def close(self):
         if getattr(self, "_ctx", None):
             self._lib.g16_ctx_destroy(self._ctx)
@@ -170,7 +180,7 @@ class Groth16:
     # ---- the two dependency-level operations (ark-poly / ark-ec) ----
     def ntt(self, values: np.ndarray, inverse: bool = False, coset: bool = False) -> np.ndarray:
         """Radix2EvaluationDomain::{fft,ifft}_in_place / coset variants on 2^k Montgomery Fr elements."""
-        v = np.ascontiguousarray(values, dtype=np.uint64).reshape(-1, 4).copy()
+        v = np.ascontiguousarray(values, dtype=np.uint64).reshape(-1, self.nr).copy()
         n = v.shape[0]
         log_n = max(n - 1, 0).bit_length()
         if (1 << log_n) != n:
@@ -180,8 +190,8 @@ class Groth16:
 
     def ntt_log(self, log_n: int, values: np.ndarray, inverse=False, coset=False) -> np.ndarray:
         """Same transform with the domain size given explicitly (error-path tests: log_n above the two-adicity).  The C side
-        copies 32 << log_n bytes in and out of `values`, so the length is checked here."""
-        v = np.ascontiguousarray(values, dtype=np.uint64).reshape(-1, 4).copy()
+        copies 8 * nr << log_n bytes in and out of `values`, so the length is checked here."""
+        v = np.ascontiguousarray(values, dtype=np.uint64).reshape(-1, self.nr).copy()
         if log_n < 0 or (log_n <= self.curve.two_adicity and v.shape[0] != (1 << log_n)):
             raise ValueError(f"values must hold exactly 2^{log_n} field elements")
         # log_n above the two-adicity: the C side returns PolynomialDegreeTooLarge before it touches the buffer
@@ -189,9 +199,9 @@ class Groth16:
         return v
 
     def witness_map_from_evals(self, a: np.ndarray, b: np.ndarray, c: np.ndarray) -> np.ndarray:
-        a = np.ascontiguousarray(a, dtype=np.uint64).reshape(-1, 4)
-        b = np.ascontiguousarray(b, dtype=np.uint64).reshape(-1, 4)
-        c = np.ascontiguousarray(c, dtype=np.uint64).reshape(-1, 4)
+        a = np.ascontiguousarray(a, dtype=np.uint64).reshape(-1, self.nr)
+        b = np.ascontiguousarray(b, dtype=np.uint64).reshape(-1, self.nr)
+        c = np.ascontiguousarray(c, dtype=np.uint64).reshape(-1, self.nr)
         n = a.shape[0]
         log_n = max(n - 1, 0).bit_length()
         if (1 << log_n) != n or b.shape != a.shape or c.shape != a.shape:
@@ -203,17 +213,17 @@ class Groth16:
     def msm_g1(self, bases: np.ndarray, scalars: np.ndarray) -> np.ndarray:
         """VariableBaseMSM::msm_bigint on G1: truncates to the shorter operand like ark (prover.rs:66 relies on it)."""
         bases = np.ascontiguousarray(bases, dtype=np.uint64).reshape(-1, 2 * self.nq)
-        scalars = np.ascontiguousarray(scalars, dtype=np.uint64).reshape(-1, 4)
+        scalars = np.ascontiguousarray(scalars, dtype=np.uint64).reshape(-1, self.nr)
         n = min(bases.shape[0], scalars.shape[0])
         out = np.zeros(3 * self.nq, dtype=np.uint64)
         _check(self._lib.g16_msm_g1(self._ctx, _ptr(bases), _ptr(scalars), n, _ptr(out)))
         return out
 
     def msm_g2(self, bases: np.ndarray, scalars: np.ndarray) -> np.ndarray:
-        bases = np.ascontiguousarray(bases, dtype=np.uint64).reshape(-1, 4 * self.nq)
-        scalars = np.ascontiguousarray(scalars, dtype=np.uint64).reshape(-1, 4)
+        bases = np.ascontiguousarray(bases, dtype=np.uint64).reshape(-1, self.ng2)
+        scalars = np.ascontiguousarray(scalars, dtype=np.uint64).reshape(-1, self.nr)
         n = min(bases.shape[0], scalars.shape[0])
-        out = np.zeros(6 * self.nq, dtype=np.uint64)
+        out = np.zeros(3 * self.ng2 // 2, dtype=np.uint64)
         _check(self._lib.g16_msm_g2(self._ctx, _ptr(bases), _ptr(scalars), n, _ptr(out)))
         return out
 
@@ -226,7 +236,7 @@ class Groth16:
             raise MalformedKey("verifying key has no gamma_abc_g1")
         abc = np.ascontiguousarray(vk.gamma_abc_g1, dtype=np.uint64).reshape(-1, 2 * self.nq)
         if isinstance(public_inputs, np.ndarray):
-            xs = self.codec.fr.dec(np.ascontiguousarray(public_inputs, dtype=np.uint64).reshape(-1, 4))
+            xs = self.codec.fr.dec(np.ascontiguousarray(public_inputs, dtype=np.uint64).reshape(-1, self.nr))
         else:
             xs = [int(x) % self.curve.r for x in public_inputs]
         if len(xs) + 1 != abc.shape[0]:
@@ -265,7 +275,7 @@ class Groth16:
         for name in ("a_query", "b_g1_query", "b_g2_query", "h_query", "l_query"):
             arr = np.ascontiguousarray(getattr(pk, name), dtype=np.uint64)
             arrs[name] = arr
-            width = 4 * self.nq if name == "b_g2_query" else 2 * self.nq
+            width = self.ng2 if name == "b_g2_query" else 2 * self.nq
             arr2 = arr.reshape(-1, width)
             setattr(d, name, _u64p(arr) if arr.size else None)
             setattr(d, name.replace("_query", "_len"), arr2.shape[0])
@@ -296,14 +306,14 @@ class Groth16:
 
     def export_proving_key(self) -> ProvingKey:
         m = self._matrices
-        nq = self.nq
+        nq, ng2 = self.nq, self.ng2
         nv = m.num_instance_variables + m.num_witness_variables
         n = 1 << self._lib.g16_domain_log(self._ctx)
         hn = n if self.qap == "circom" else n - 1   # CircomReduction::h_query_scalars gives n scalars, libsnark n - 1
         z = lambda rows, w: np.zeros((rows, w), dtype=np.uint64)
-        out = dict(a_query=z(nv, 2 * nq), b_g1_query=z(nv, 2 * nq), b_g2_query=z(nv, 4 * nq), h_query=z(hn, 2 * nq),
+        out = dict(a_query=z(nv, 2 * nq), b_g1_query=z(nv, 2 * nq), b_g2_query=z(nv, ng2), h_query=z(hn, 2 * nq),
                    l_query=z(m.num_witness_variables, 2 * nq), alpha_g1=z(1, 2 * nq), beta_g1=z(1, 2 * nq),
-                   delta_g1=z(1, 2 * nq), beta_g2=z(1, 4 * nq), gamma_g2=z(1, 4 * nq), delta_g2=z(1, 4 * nq),
+                   delta_g1=z(1, 2 * nq), beta_g2=z(1, ng2), gamma_g2=z(1, ng2), delta_g2=z(1, ng2),
                    gamma_abc_g1=z(m.num_instance_variables, 2 * nq))
         d = _lib.PkExportDesc()
         for k, v in out.items():
@@ -324,10 +334,10 @@ class Groth16:
         if m is None:
             raise ValueError("load_matrices must come first")
         buf = np.frombuffer(data, dtype=np.uint8)
-        nq, ni = self.nq, m.num_instance_variables
+        nq, ng2, ni = self.nq, self.ng2, m.num_instance_variables
         z = lambda rows, w: np.zeros((rows, w), dtype=np.uint64)
-        out = dict(alpha_g1=z(1, 2 * nq), beta_g1=z(1, 2 * nq), delta_g1=z(1, 2 * nq), beta_g2=z(1, 4 * nq),
-                   gamma_g2=z(1, 4 * nq), delta_g2=z(1, 4 * nq), gamma_abc_g1=z(ni, 2 * nq))
+        out = dict(alpha_g1=z(1, 2 * nq), beta_g1=z(1, 2 * nq), delta_g1=z(1, 2 * nq), beta_g2=z(1, ng2),
+                   gamma_g2=z(1, ng2), delta_g2=z(1, ng2), gamma_abc_g1=z(ni, 2 * nq))
         d = _lib.PkExportDesc()
         for k, v in out.items():
             setattr(d, k, _u64p(v) if v.size else None)
@@ -371,13 +381,13 @@ class Groth16:
             raise ValueError("num_inputs / num_constraints do not match the matrices")
         rr = self._fr_arg(r)
         ss = self._fr_arg(s)
-        z = np.ascontiguousarray(full_assignment, dtype=np.uint64).reshape(-1, 4)
+        z = np.ascontiguousarray(full_assignment, dtype=np.uint64).reshape(-1, self.nr)
         if z.shape[0] != m.num_instance_variables + m.num_witness_variables:
             raise ValueError("full_assignment has the wrong length")
-        nq = self.nq
-        out = np.zeros(8 * nq, dtype=np.uint64)
+        nq, ng2 = self.nq, self.ng2
+        out = np.zeros(4 * nq + ng2, dtype=np.uint64)
         _check(self._lib.g16_prove(self._ctx, _ptr(rr), _ptr(ss), _ptr(z), flags, _ptr(out)))
-        return Proof(out[:2 * nq].copy(), out[2 * nq:6 * nq].copy(), out[6 * nq:].copy())
+        return Proof(out[:2 * nq].copy(), out[2 * nq:2 * nq + ng2].copy(), out[2 * nq + ng2:].copy())
 
     def prove_raw(self, r_limbs: np.ndarray, s_limbs: np.ndarray, z_ptr, flags: int, out: np.ndarray):
         """Thin call used by bench.py: everything already in ABI form; z_ptr is a host or device address."""
@@ -401,19 +411,19 @@ class Groth16:
             raise ValueError("matrices and proving key must be loaded")
         nv = m.num_instance_variables + m.num_witness_variables
         z = np.ascontiguousarray(full_assignments, dtype=np.uint64)
-        if z.ndim != 3 or z.shape[1:] != (nv, 4):
-            raise ValueError(f"full_assignments must have shape (K, {nv}, 4)")
+        if z.ndim != 3 or z.shape[1:] != (nv, self.nr):
+            raise ValueError(f"full_assignments must have shape (K, {nv}, {self.nr})")
         k = z.shape[0]
         rr, ss = self._fr_args(r), self._fr_args(s)
         if rr.shape[0] != k or ss.shape[0] != k:
             raise ValueError("r, s and full_assignments must hold the same number of proofs")
         if not 0 <= group < 1 << 32:
             raise ValueError("group must be a non-negative 32-bit count")
-        nq = self.nq
-        out = np.zeros((k, 8 * nq), dtype=np.uint64)
+        nq, ng2 = self.nq, self.ng2
+        out = np.zeros((k, 4 * nq + ng2), dtype=np.uint64)
         if k:
             self.prove_batch_raw(k, rr, ss, z.ctypes.data, group, flags, out)
-        return [Proof(p[:2 * nq].copy(), p[2 * nq:6 * nq].copy(), p[6 * nq:].copy()) for p in out]
+        return [Proof(p[:2 * nq].copy(), p[2 * nq:2 * nq + ng2].copy(), p[2 * nq + ng2:].copy()) for p in out]
 
     def prove_batch_raw(self, count: int, r_limbs: np.ndarray, s_limbs: np.ndarray, z_ptr, group: int, flags: int,
                         out: np.ndarray):
@@ -460,10 +470,10 @@ class Groth16:
         rr, ss = self._fr_arg(r), self._fr_arg(s)
         pl = self._lib.g16_partial_limbs(self._ctx)
         p = np.ascontiguousarray(partials, dtype=np.uint64).reshape(-1, pl)
-        nq = self.nq
-        out = np.zeros(8 * nq, dtype=np.uint64)
+        nq, ng2 = self.nq, self.ng2
+        out = np.zeros(4 * nq + ng2, dtype=np.uint64)
         _check(self._lib.g16_prove_assemble(self._ctx, _ptr(rr), _ptr(ss), _ptr(p), p.shape[0], _ptr(out)))
-        return Proof(out[:2 * nq].copy(), out[2 * nq:6 * nq].copy(), out[6 * nq:].copy())
+        return Proof(out[:2 * nq].copy(), out[2 * nq:2 * nq + ng2].copy(), out[2 * nq + ng2:].copy())
 
     def partial_limbs(self) -> int:
         return self._lib.g16_partial_limbs(self._ctx)
@@ -475,11 +485,11 @@ class Groth16:
         if matrices is not None and matrices is not self._matrices:
             self.load_matrices(matrices)
         m = self._matrices
-        z = np.ascontiguousarray(full_assignment, dtype=np.uint64).reshape(-1, 4)
+        z = np.ascontiguousarray(full_assignment, dtype=np.uint64).reshape(-1, self.nr)
         if z.shape[0] != m.num_instance_variables + m.num_witness_variables:
             raise ValueError("full_assignment has the wrong length")
         n = 1 << self._lib.g16_domain_log(self._ctx)
-        h = np.zeros((n, 4), dtype=np.uint64)
+        h = np.zeros((n, self.nr), dtype=np.uint64)
         _check(self._lib.g16_witness_map(self._ctx, _ptr(z), 0, _ptr(h)))
         return h
 
@@ -526,16 +536,16 @@ class Groth16:
     def _fr_arg(self, x) -> np.ndarray:
         if isinstance(x, (int, np.integer)):
             return np.ascontiguousarray(self.codec.fr.enc1(int(x)))
-        return np.ascontiguousarray(x, dtype=np.uint64).reshape(4)
+        return np.ascontiguousarray(x, dtype=np.uint64).reshape(self.nr)
 
     def _fr_args(self, xs) -> np.ndarray:
-        """a sequence of ints, or a (K, 4) array of Montgomery limbs -> (K, 4) contiguous limbs"""
+        """a sequence of ints, or a (K, nr) array of Montgomery limbs -> (K, nr) contiguous limbs"""
         if isinstance(xs, np.ndarray):
             a = np.ascontiguousarray(xs, dtype=np.uint64)
-            if a.ndim != 2 or a.shape[1] != 4:
-                raise ValueError("scalar limbs must have shape (K, 4)")
+            if a.ndim != 2 or a.shape[1] != self.nr:
+                raise ValueError(f"scalar limbs must have shape (K, {self.nr})")
             return a
         xs = list(xs)
         if not xs:
-            return np.zeros((0, 4), dtype=np.uint64)
+            return np.zeros((0, self.nr), dtype=np.uint64)
         return np.ascontiguousarray(np.stack([self._fr_arg(x) for x in xs]), dtype=np.uint64)

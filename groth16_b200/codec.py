@@ -52,7 +52,8 @@ class FieldCodec:
 
 
 class CurveCodec:
-    """G1 points are (x, y) int tuples or None; G2 points are ((x0, x1), (y0, y1)) or None."""
+    """G1 points are (x, y) int tuples or None; G2 points are ((x0, x1), (y0, y1)) or None, or (x, y) when G2 is over Fq
+    (BW6-761)."""
 
     def __init__(self, c: CurveParams):
         self.c = c
@@ -71,6 +72,8 @@ class CurveCodec:
         return arr
 
     def enc_g2(self, pts) -> np.ndarray:
+        if self.c.g2_over_fq:
+            return self.enc_g1(pts)
         flat = []
         for P in pts:
             flat.extend((0, 0, 0, 0) if P is None else (P[0][0], P[0][1], P[1][0], P[1][1]))
@@ -89,6 +92,8 @@ class CurveCodec:
         return out
 
     def dec_g2(self, arr) -> list:
+        if self.c.g2_over_fq:
+            return self.dec_g1(arr)
         a = np.ascontiguousarray(arr, dtype="<u8").reshape(-1, 4 * self.nq)
         vals = self.fq.dec(a.reshape(-1, self.nq))
         out = []
@@ -102,5 +107,7 @@ class CurveCodec:
         return None if v[2] == 0 else (v[0], v[1])
 
     def dec_proj_g2(self, arr):
+        if self.c.g2_over_fq:
+            return self.dec_proj_g1(arr)
         v = self.fq.dec(np.asarray(arr).reshape(6, self.nq))
         return None if (v[4] == 0 and v[5] == 0) else ((v[0], v[1]), (v[2], v[3]))

@@ -52,6 +52,7 @@ int fail(int code, const std::string& msg) {
 IEngine* make_engine_bls381(int device, int* rc);
 IEngine* make_engine_bn254(int device, int* rc);
 IEngine* make_engine_bls377(int device, int* rc);
+IEngine* make_engine_bw6(int device, int* rc);
 }  // namespace g16
 
 struct g16_ctx {
@@ -82,6 +83,7 @@ int g16_ctx_create(int curve, int device, g16_ctx** out) {
     case G16_CURVE_BLS12_381: e = make_engine_bls381(device, &rc); break;
     case G16_CURVE_BN254: e = make_engine_bn254(device, &rc); break;
     case G16_CURVE_BLS12_377: e = make_engine_bls377(device, &rc); break;
+    case G16_CURVE_BW6_761: e = make_engine_bw6(device, &rc); break;
     default: return fail(G16_ERR_BAD_ARGUMENT, "unknown curve id");
   }
   if (!e) return rc ? rc : G16_ERR_CUDA;
@@ -99,6 +101,8 @@ const char* g16_last_error(void) { return last_error_ref().c_str(); }
   if (!(ctx) || !(ctx)->eng) return fail(G16_ERR_BAD_ARGUMENT, "null context")
 
 int g16_fq_limbs(const g16_ctx* ctx) { return (ctx && ctx->eng) ? ctx->eng->fq_limbs() : 0; }
+int g16_fr_limbs(const g16_ctx* ctx) { return (ctx && ctx->eng) ? ctx->eng->fr_limbs() : 0; }
+int g16_g2_limbs(const g16_ctx* ctx) { return (ctx && ctx->eng) ? ctx->eng->g2_limbs() : 0; }
 int g16_partial_limbs(const g16_ctx* ctx) { return (ctx && ctx->eng) ? ctx->eng->partial_limbs() : 0; }
 uint32_t g16_domain_log(const g16_ctx* ctx) { return (ctx && ctx->eng) ? ctx->eng->domain_log() : 0; }
 

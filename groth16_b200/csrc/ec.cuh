@@ -65,6 +65,16 @@ struct alignas(16) Fp2 {
   }
 };
 
+// Wide points: coordinates of 96 bytes, Fq2 over a 384-bit Fq (every G2) or BW6-761's 761-bit Fq (its G1 and G2 alike).
+// They set the register budget and the load pattern of the MSM accumulation and batched-affine kernels (msm.cuh,
+// msm_ba.cuh).
+template <class F>
+struct MsmWide { static constexpr bool value = false; };
+template <class P, int NR>
+struct MsmWide<Fp2<P, NR>> { static constexpr bool value = true; };
+template <>
+struct MsmWide<Fp<BW6_FqP>> { static constexpr bool value = true; };
+
 // ------------------------------------------------------------------------------------------------
 // Points
 // ------------------------------------------------------------------------------------------------

@@ -130,6 +130,8 @@ NcclApi& nccl_api();
 struct IEngine {
   virtual ~IEngine() {}
   virtual int fq_limbs() const = 0;
+  virtual int fr_limbs() const = 0;
+  virtual int g2_limbs() const = 0;
   virtual int partial_limbs() const = 0;
   virtual int ntt(uint32_t log_n, int inverse, int coset, uint64_t* inout) = 0;
   virtual int witness_map_evals(uint32_t log_n, const uint64_t* a, const uint64_t* b, const uint64_t* c, uint64_t* h) = 0;
@@ -169,12 +171,15 @@ template <class CP>
 struct Engine : IEngine {
   using Fr = Fp<typename CP::FrP>;
   using Fq = Fp<typename CP::FqP>;
-  using Fq2 = Fp2<typename CP::FqP, CP::FQ2_NONRESIDUE_NEG>;
+  using Fq2 = typename CP::G2F;   // G2's coordinate field: Fq2, or Fq itself (BW6-761)
   using A1 = Affine<Fq>;
   using A2 = Affine<Fq2>;
   using P1 = XYZZ<Fq>;
   using P2 = XYZZ<Fq2>;
   static constexpr int NQ64 = Fq::N / 2;
+  static constexpr int FR64 = Fr::N / 2;                  // u64 limbs of one ABI scalar
+  static constexpr int G2_64 = (int)(sizeof(A2) / 8);     // u64 limbs of one ABI G2 affine point
+  static constexpr int PROOF64 = 4 * NQ64 + G2_64;        // A (G1) || B (G2) || C (G1)
   static constexpr int FR_BITS = CP::FrP::BITS;
   enum { M_H = 0, M_L = 1, M_A = 2, M_B1 = 3, M_B2 = 4 };
   static const char* span_of(int m) {
@@ -571,7 +576,9 @@ struct Engine : IEngine {
     d_gamma_abc.release(); full_a.release(); full_b1.release(); full_b2.release();
   }
   int fq_limbs() const override { return NQ64; }
-  int partial_limbs() const override { return 4 * 2 * NQ64 + 4 * NQ64; }
+  int fr_limbs() const override { return FR64; }
+  int g2_limbs() const override { return G2_64; }
+  int partial_limbs() const override { return 4 * 2 * NQ64 + G2_64; }
   uint32_t domain_log() const override { return (uint32_t)L; }
 
   bool any_busy() const { return slots[0].busy || slots[1].busy; }
@@ -581,17 +588,10 @@ struct Engine : IEngine {
   // ---- small host helpers ----
   static Fr load_fr(const uint64_t* p) { Fr r; memcpy(r.v, p, sizeof(r.v)); return r; }
   static A1 load_a1(const uint64_t* p) { A1 r; memcpy(&r.x, p, sizeof(Fq)); memcpy(&r.y, p + NQ64, sizeof(Fq)); return r; }
-  static A2 load_a2(const uint64_t* p) {
-    A2 r;
-    memcpy(&r.x.c0, p, sizeof(Fq)); memcpy(&r.x.c1, p + NQ64, sizeof(Fq));
-    memcpy(&r.y.c0, p + 2 * NQ64, sizeof(Fq)); memcpy(&r.y.c1, p + 3 * NQ64, sizeof(Fq));
-    return r;
-  }
+  // x || y, each coordinate c0 || c1 over Fq2: exactly the packed image of A2
+  static A2 load_a2(const uint64_t* p) { A2 r; memcpy(&r, p, sizeof(A2)); return r; }
   static void store_a1(uint64_t* p, const A1& a) { memcpy(p, &a.x, sizeof(Fq)); memcpy(p + NQ64, &a.y, sizeof(Fq)); }
-  static void store_a2(uint64_t* p, const A2& a) {
-    memcpy(p, &a.x.c0, sizeof(Fq)); memcpy(p + NQ64, &a.x.c1, sizeof(Fq));
-    memcpy(p + 2 * NQ64, &a.y.c0, sizeof(Fq)); memcpy(p + 3 * NQ64, &a.y.c1, sizeof(Fq));
-  }
+  static void store_a2(uint64_t* p, const A2& a) { memcpy(p, &a, sizeof(A2)); }
   // Jacobian normalised to Z = 1 (identity: (1,1,0) like ark)
   template <class F, class PT>
   static void store_proj(uint64_t* p, const PT& pt) {
@@ -601,9 +601,9 @@ struct Engine : IEngine {
     if (pt.is_inf()) { memcpy(p, &one, sizeof(F)); memcpy(p + w, &one, sizeof(F)); memcpy(p + 2 * w, &zero, sizeof(F)); }
     else { memcpy(p, &a.x, sizeof(F)); memcpy(p + w, &a.y, sizeof(F)); memcpy(p + 2 * w, &one, sizeof(F)); }
   }
-  static void fr_to_canon(const Fr& m, uint32_t out[8]) {
+  static void fr_to_canon(const Fr& m, uint32_t out[Fr::N]) {
     Fr c = Fr::from_mont(m);
-    memcpy(out, c.v, 32);
+    memcpy(out, c.v, sizeof(Fr));
   }
   static int check_log(uint32_t log_n) {
     if ((int)log_n > CP::FrP::TWO_ADICITY) return fail(G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "domain size exceeds the field's two-adicity (PolynomialDegreeTooLarge)");
@@ -776,7 +776,7 @@ struct Engine : IEngine {
 
   // ---- stand-alone MSM API (msm_bigint) ----
   template <class F, class WS>
-  int msm_host(WS& ws, const uint64_t* bases, const uint64_t* scalars, uint64_t n, uint64_t* out) {
+  int msm_host(WS& ws, bool g2, const uint64_t* bases, const uint64_t* scalars, uint64_t n, uint64_t* out) {
     if (!out || (n && (!bases || !scalars))) return fail(G16_ERR_BAD_ARGUMENT, "null buffer");
     if (n >= (1ull << 27)) return fail(G16_ERR_BAD_ARGUMENT, "n too large");
     G16_NOT_BUSY();
@@ -785,12 +785,12 @@ struct Engine : IEngine {
     if (n) {
       DevBuf db, ds, dm;
       G16_CUDA(db.reserve(n * sizeof(Affine<F>)));
-      G16_CUDA(ds.reserve(n * 32));
+      G16_CUDA(ds.reserve(n * sizeof(Fr)));
       G16_CUDA(dm.reserve(n));
       G16_CUDA(cudaMemcpyAsync(db.p, bases, n * sizeof(Affine<F>), cudaMemcpyHostToDevice, S0.st_main));
-      G16_CUDA(cudaMemcpyAsync(ds.p, scalars, n * 32, cudaMemcpyHostToDevice, S0.st_main));
+      G16_CUDA(cudaMemcpyAsync(ds.p, scalars, n * sizeof(Fr), cudaMemcpyHostToDevice, S0.st_main));
       G16_CUDA(msm_prepare_query<F>(S0.st_main, db.template as<Affine<F>>(), (uint32_t)n, 1, 0, dm.template as<uint8_t>()));
-      const MsmGeom g = with_k0(msm_geom(n, FR_BITS, (int)tune.c, 0), sizeof(F) > 48);   // caller-supplied bases: no precomputed copies
+      const MsmGeom g = with_k0(msm_geom(n, FR_BITS, (int)tune.c, 0), g2);   // caller-supplied bases: no precomputed copies
       cudaError_t e = msm_enqueue<F, Fr>(S0.st_main, ws, g, db.template as<Affine<F>>(), dm.template as<uint8_t>(), ds.template as<uint32_t>(), 1, false, &ctr, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
       if (e != cudaSuccess) { db.release(); ds.release(); dm.release(); return fail(G16_ERR_CUDA, std::string("msm_enqueue: ") + cudaGetErrorString(e)); }
       e = cudaStreamSynchronize(S0.st_main);
@@ -801,8 +801,8 @@ struct Engine : IEngine {
     store_proj<F>(out, res);
     return G16_OK;
   }
-  int msm_g1(const uint64_t* bases, const uint64_t* scalars, uint64_t n, uint64_t* out) override { return msm_host<Fq>(S0.ws1[0], bases, scalars, n, out); }
-  int msm_g2(const uint64_t* bases, const uint64_t* scalars, uint64_t n, uint64_t* out) override { return msm_host<Fq2>(S0.ws2, bases, scalars, n, out); }
+  int msm_g1(const uint64_t* bases, const uint64_t* scalars, uint64_t n, uint64_t* out) override { return msm_host<Fq>(S0.ws1[0], false, bases, scalars, n, out); }
+  int msm_g2(const uint64_t* bases, const uint64_t* scalars, uint64_t n, uint64_t* out) override { return msm_host<Fq2>(S0.ws2, true, bases, scalars, n, out); }
 
   // ---- circuit ----
   int circuit_load(int qp, uint32_t ni, uint32_t nc, uint32_t nw, const g16_csr* a, const g16_csr* b, const g16_csr* c) override {
@@ -831,18 +831,18 @@ struct Engine : IEngine {
       h_rp[m].assign(ms[m]->row_ptr, ms[m]->row_ptr + nc + 1);
       h_col[m].assign(ms[m]->col, ms[m]->col + nnz);
       h_val[m].resize(nnz);
-      if (nnz) memcpy(h_val[m].data(), ms[m]->val, (size_t)nnz * 32);
+      if (nnz) memcpy(h_val[m].data(), ms[m]->val, (size_t)nnz * sizeof(Fr));
       G16_CUDA(csr_rp[m].reserve((size_t)(nc + 1) * 4));
       G16_CUDA(csr_col[m].reserve((size_t)nnz * 4 + 4));
-      G16_CUDA(csr_val[m].reserve((size_t)nnz * 32 + 32));
+      G16_CUDA(csr_val[m].reserve((size_t)nnz * sizeof(Fr) + sizeof(Fr)));
       G16_CUDA(cudaMemcpy(csr_rp[m].p, ms[m]->row_ptr, (size_t)(nc + 1) * 4, cudaMemcpyHostToDevice));
       if (nnz) {
         G16_CUDA(cudaMemcpy(csr_col[m].p, ms[m]->col, (size_t)nnz * 4, cudaMemcpyHostToDevice));
-        G16_CUDA(cudaMemcpy(csr_val[m].p, ms[m]->val, (size_t)nnz * 32, cudaMemcpyHostToDevice));
+        G16_CUDA(cudaMemcpy(csr_val[m].p, ms[m]->val, (size_t)nnz * sizeof(Fr), cudaMemcpyHostToDevice));
       }
     }
     num_inputs = ni; num_constraints = nc; num_witness = nw; L = Ln; qap = qp;
-    G16_CUDA(S0.d_z.reserve((size_t)nvars * 32));
+    G16_CUDA(S0.d_z.reserve((size_t)nvars * sizeof(Fr)));
     if ((rc = ensure_circuit_domain())) return rc;
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
     have_circuit = true;
@@ -931,7 +931,7 @@ struct Engine : IEngine {
   // ---- setup (generator.rs:47-208) ----
   template <class F>
   int batch_mul(const Affine<F>& gen, const Fr* d_scalars, uint64_t cnt, Affine<F>* d_out, DevBuf& table) {
-    G16_CUDA(table.reserve((size_t)FB_WINDOWS * 255 * sizeof(XYZZ<F>)));
+    G16_CUDA(table.reserve((size_t)fb_windows<Fr>() * 255 * sizeof(XYZZ<F>)));
     G16_CUDA((fb_batch_mul<F, Fr>(S0.st_main, gen, d_scalars, cnt, d_out, table.template as<XYZZ<F>>())));
     return G16_OK;
   }
@@ -999,10 +999,10 @@ struct Engine : IEngine {
     rank = 0; world = 1;
     DevBuf d_s, tab1, tab2;
     const uint64_t maxs = std::max<uint64_t>(nv, n);
-    G16_CUDA(d_s.reserve(maxs * 32));
+    G16_CUDA(d_s.reserve(maxs * sizeof(Fr)));
     int rc;
     auto up = [&](const std::vector<Fr>& v) -> cudaError_t {
-      return v.empty() ? cudaSuccess : cudaMemcpyAsync(d_s.p, v.data(), v.size() * 32, cudaMemcpyHostToDevice, S0.st_main);
+      return v.empty() ? cudaSuccess : cudaMemcpyAsync(d_s.p, v.data(), v.size() * sizeof(Fr), cudaMemcpyHostToDevice, S0.st_main);
     };
     G16_CUDA(full_a.reserve(nv * sizeof(A1))); G16_CUDA(full_b1.reserve(nv * sizeof(A1))); G16_CUDA(full_b2.reserve(nv * sizeof(A2)));
     G16_CUDA(d_gamma_abc.reserve((size_t)ni * sizeof(A1)));
@@ -1040,9 +1040,9 @@ struct Engine : IEngine {
     G16_CUDA(cudaMemcpyAsync(&b2_q0, full_b2.p, sizeof(A2), cudaMemcpyDeviceToHost, S0.st_main));
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
     // single points on the host (generator.rs:147-151,182)
-    uint32_t k[8];
-    auto mul1 = [&](const Fr& s) { fr_to_canon(s, k); return P1::from_affine(g1).mul_u32(k, 8).to_affine(); };
-    auto mul2 = [&](const Fr& s) { fr_to_canon(s, k); return P2::from_affine(g2).mul_u32(k, 8).to_affine(); };
+    uint32_t k[Fr::N];
+    auto mul1 = [&](const Fr& s) { fr_to_canon(s, k); return P1::from_affine(g1).mul_u32(k, Fr::N).to_affine(); };
+    auto mul2 = [&](const Fr& s) { fr_to_canon(s, k); return P2::from_affine(g2).mul_u32(k, Fr::N).to_affine(); };
     alpha_g1 = mul1(alpha); beta_g1 = mul1(beta); delta_g1 = mul1(delta);
     beta_g2 = mul2(beta); gamma_g2 = mul2(gamma); delta_g2 = mul2(delta);
     set_tail_points(a_q0, b1_q0, b2_q0);
@@ -1139,7 +1139,7 @@ struct Engine : IEngine {
     from_setup = false;
     tail_ready = false;
     SerItem it[SER_ITEMS];
-    const std::string why = ser_walk(bytes, len, Fmt::NB, flags & G16_SER_COMPRESSED, it);
+    const std::string why = ser_walk(bytes, len, Fmt::NB, flags & G16_SER_COMPRESSED, it, Fmt::G2_NC);
     if (!why.empty()) return fail(G16_ERR_INVALID_DATA, why);
     if (it[SER_A].len < 1 || it[SER_B_G1].len < 1 || it[SER_B_G2].len < 1)
       return fail(G16_ERR_MALFORMED_KEY, "a/b queries must hold at least the constant-one base");
@@ -1263,7 +1263,7 @@ struct Engine : IEngine {
     it[SER_A].len = it[SER_B_G1].len = it[SER_B_G2].len = nv;
     it[SER_H].len = qap == G16_QAP_CIRCOM ? n : n - 1;
     it[SER_L].len = num_witness;
-    const uint64_t size = ser_size(it, Fmt::NB, flags & G16_SER_COMPRESSED);
+    const uint64_t size = ser_size(it, Fmt::NB, flags & G16_SER_COMPRESSED, Fmt::G2_NC);
     *len_out = size;
     if (!out) return G16_OK;
     if (cap < size)
@@ -1310,14 +1310,14 @@ struct Engine : IEngine {
     int rc = ensure_circuit_domain();   // no-op unless something rebuilt `dom` for another size
     if (rc) return rc;
     if ((rc = ensure_slot_buffers(sl, L, count))) return rc;
-    G16_CUDA(sl.d_z.reserve((size_t)nv * 32 * count));
+    G16_CUDA(sl.d_z.reserve((size_t)nv * sizeof(Fr) * count));
     sl.tm.h2d_bytes = 0;
     G16_CUDA(cudaEventRecord(sl.ev_start, sl.st_main));
     if (flags & G16_ASSIGNMENT_ON_DEVICE) {
-      G16_CUDA(cudaMemcpyAsync(sl.d_z.p, z, nv * 32 * count, cudaMemcpyDeviceToDevice, sl.st_main));
+      G16_CUDA(cudaMemcpyAsync(sl.d_z.p, z, nv * sizeof(Fr) * count, cudaMemcpyDeviceToDevice, sl.st_main));
     } else {
-      G16_CUDA(cudaMemcpyAsync(sl.d_z.p, z, nv * 32 * count, cudaMemcpyHostToDevice, sl.st_main));
-      sl.tm.h2d_bytes = nv * 32 * count;
+      G16_CUDA(cudaMemcpyAsync(sl.d_z.p, z, nv * sizeof(Fr) * count, cudaMemcpyHostToDevice, sl.st_main));
+      sl.tm.h2d_bytes = nv * sizeof(Fr) * count;
     }
     G16_CUDA(cudaEventRecord(sl.ev_z, sl.st_main));
     const uint32_t n = 1u << L;
@@ -1344,7 +1344,7 @@ struct Engine : IEngine {
     G16_CUDA(cudaSetDevice(device));
     int rc = enqueue_witness_map(S0, z, flags);
     if (rc) return rc;
-    G16_CUDA(cudaMemcpyAsync(h, S0.d_h.p, (size_t)32 << L, cudaMemcpyDeviceToHost, S0.st_main));
+    G16_CUDA(cudaMemcpyAsync(h, S0.d_h.p, sizeof(Fr) << L, cudaMemcpyDeviceToHost, S0.st_main));
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
     return G16_OK;
   }
@@ -1356,8 +1356,9 @@ struct Engine : IEngine {
     const uint32_t* zs = sl.d_z.template as<uint32_t>();
     const uint32_t* hs = sl.d_h.template as<uint32_t>();
     // scalar sources (prover.rs:63-85): H <- h ; L <- aux ; A, B1, B2 <- input[1..] ++ aux
-    const uint32_t* src[5] = {hs, zs + (size_t)num_inputs * 8, zs + 8, zs + 8, zs + 8};
-    const uint64_t stride[5] = {n * 8, nv * 8, nv * 8, nv * 8, nv * 8};   // 32-bit words between two proofs' scalars
+    constexpr int W = Fr::N;   // 32-bit words per scalar
+    const uint32_t* src[5] = {hs, zs + (size_t)num_inputs * W, zs + W, zs + W, zs + W};
+    const uint64_t stride[5] = {n * W, nv * W, nv * W, nv * W, nv * W};   // 32-bit words between two proofs' scalars
     // B in G1 and B in G2 run over the same scalars and identity pattern: one counting sort serves both.  B2 sorts
     // (its stream has the higher priority and its tail is the longest), B1 borrows the list.
     const bool share = share_b_sort && sl.run[M_B1] && sl.run[M_B2];
@@ -1370,7 +1371,7 @@ struct Engine : IEngine {
       if (!sl.serial) G16_CUDA(cudaStreamWaitEvent(st, m == M_H ? sl.ev_h : sl.ev_z, 0));
       G16_CUDA(cudaEventRecord(sl.ev_m0[m], st));
       if (sl.run[m]) {
-        const uint32_t* sc = src[m] + q[m].lo * 8;   // first owned scalar; the digit kernel strides by `world`
+        const uint32_t* sc = src[m] + q[m].lo * W;   // first owned scalar; the digit kernel strides by `world`
         cudaEvent_t gate = (wm_first && m != M_H) ? sl.ev_h : nullptr;
         cudaError_t e;
         if (m == M_B2 && share) { sl.b_sorted = MsmSorted{}; sl.b_sorted.ready = sl.ev_bsort; }
@@ -1461,10 +1462,10 @@ struct Engine : IEngine {
           if (m == M_B2) out.b2 = sl.run[m] ? msm_finish<Fq2>(sl.ws2, sl.geom[m]) : P2::inf();
           else *outs1[m] = sl.run[m] ? msm_finish<Fq>(sl.ws1[m], sl.geom[m]) : P1::inf();
           if (sl.have_s && (m == M_A || m == M_B1)) {       // prover.rs:94 / :114, distributed over the MSM result
-            uint32_t k[8];
+            uint32_t k[Fr::N];
             fr_to_canon(m == M_A ? sl.s : sl.r, k);
-            if (m == M_A) out.sa = out.a.mul_u32(k, 8);
-            else out.rb1 = out.b1.mul_u32(k, 8);
+            if (m == M_A) out.sa = out.a.mul_u32(k, Fr::N);
+            else out.rb1 = out.b1.mul_u32(k, Fr::N);
           }
         });
       }
@@ -1512,21 +1513,21 @@ struct Engine : IEngine {
   // The five key products of the proof tail (batch.cuh), for the single-proof paths: computed on the host by two pool
   // threads while the GPU works, split into halves of similar cost (a G2 product costs about three G1 products).
   void key_products_a(const Fr& r, const Fr& s, Products& p) const {
-    uint32_t rk[8], sk[8], rsk[8];
+    uint32_t rk[Fr::N], sk[Fr::N], rsk[Fr::N];
     fr_to_canon(r, rk);
     fr_to_canon(s, sk);
     fr_to_canon(Fr::mul(r, s), rsk);
     const P1 d1 = P1::from_affine(delta_g1);
-    p.r_d1 = d1.mul_u32(rk, 8);
-    p.rs_d1 = d1.mul_u32(rsk, 8);
-    p.s_pa = P1::from_affine(p_a).mul_u32(sk, 8);
+    p.r_d1 = d1.mul_u32(rk, Fr::N);
+    p.rs_d1 = d1.mul_u32(rsk, Fr::N);
+    p.s_pa = P1::from_affine(p_a).mul_u32(sk, Fr::N);
   }
   void key_products_b(const Fr& r, const Fr& s, Products& p) const {
-    uint32_t rk[8], sk[8];
+    uint32_t rk[Fr::N], sk[Fr::N];
     fr_to_canon(r, rk);
     fr_to_canon(s, sk);
-    p.r_pb = P1::from_affine(p_b).mul_u32(rk, 8);   // the identity when r == 0
-    p.s_d2 = P2::from_affine(delta_g2).mul_u32(sk, 8);
+    p.r_pb = P1::from_affine(p_b).mul_u32(rk, Fr::N);   // the identity when r == 0
+    p.s_d2 = P2::from_affine(delta_g2).mul_u32(sk, Fr::N);
   }
   Products key_products(const Fr& r, const Fr& s) const {
     Products p;
@@ -1536,9 +1537,9 @@ struct Engine : IEngine {
   }
   // this rank's contribution to g_c that depends on its MSM results: s A + r B1 + L + H
   P1 c_part(const Fr& r, const Fr& s, const Partials& x) const {
-    uint32_t k[8];
-    P1 c = x.scaled ? x.sa : (fr_to_canon(s, k), x.a.mul_u32(k, 8));
-    if (!r.is_zero()) c.add(x.scaled ? x.rb1 : (fr_to_canon(r, k), x.b1.mul_u32(k, 8)));
+    uint32_t k[Fr::N];
+    P1 c = x.scaled ? x.sa : (fr_to_canon(s, k), x.a.mul_u32(k, Fr::N));
+    if (!r.is_zero()) c.add(x.scaled ? x.rb1 : (fr_to_canon(r, k), x.b1.mul_u32(k, Fr::N)));
     c.add(x.l);
     c.add(x.h);
     return c;
@@ -1549,7 +1550,7 @@ struct Engine : IEngine {
     const ProofPoints<Fq, Fq2> pf = proof_tail(kp, p_a, p_2, a, b2, c);
     store_a1(proof, pf.g_a.to_affine());   // prover.rs:127-131
     store_a2(proof + 2 * NQ64, pf.g2_b.to_affine());
-    store_a1(proof + 6 * NQ64, pf.g_c.to_affine());
+    store_a1(proof + 2 * NQ64 + G2_64, pf.g_c.to_affine());
   }
   int prove_submit(int slot, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags) override {
     if (slot < 0 || slot >= NSLOTS) return fail(G16_ERR_BAD_ARGUMENT, "bad slot");
@@ -1575,7 +1576,7 @@ struct Engine : IEngine {
     auto t0 = std::chrono::steady_clock::now();
     store_proof(proof, sl.kp, x.a, x.b2, c_part(sl.r, sl.s, x));
     sl.tm.host_finish_ms += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    sl.tm.d2h_bytes += 8 * NQ64 * 8;
+    sl.tm.d2h_bytes += PROOF64 * 8;
     tm = sl.tm;
     return G16_OK;
   }
@@ -1604,7 +1605,7 @@ struct Engine : IEngine {
   // goes below the automatic floor), any round count and, for the B MSMs sharing one sorted list, any padding
   uint64_t batch_bytes_per_proof() const {
     const uint64_t n = 1ull << L;
-    uint64_t b = nvars() * 32 + 5 * n * 32 + 3 * 32 + 4 * sizeof(A1) + sizeof(A2);
+    uint64_t b = nvars() * sizeof(Fr) + 5 * n * sizeof(Fr) + 3 * sizeof(Fr) + 4 * sizeof(A1) + sizeof(A2);
     for (int m = 0; m < 5; m++) {
       if (q[m].hi <= q[m].lo) continue;
       const bool g2 = m == M_B2;
@@ -1626,10 +1627,10 @@ struct Engine : IEngine {
     if (tail_ready) return G16_OK;
     const A1 gens[3] = {delta_g1, p_a, p_b};   // TAB_D1, TAB_PA, TAB_PB
     for (int t = 0; t < 3; t++) {
-      G16_CUDA(tail_tab[t].reserve((size_t)FB_WINDOWS * 255 * sizeof(P1)));
+      G16_CUDA(tail_tab[t].reserve((size_t)fb_windows<Fr>() * 255 * sizeof(P1)));
       G16_CUDA((fb_batch_mul<Fq, Fr>(S0.st_main, gens[t], nullptr, 0, nullptr, tail_tab[t].template as<P1>())));
     }
-    G16_CUDA(tail_tab[TAB_D2].reserve((size_t)FB_WINDOWS * 255 * sizeof(P2)));
+    G16_CUDA(tail_tab[TAB_D2].reserve((size_t)fb_windows<Fr>() * 255 * sizeof(P2)));
     G16_CUDA((fb_batch_mul<Fq2, Fr>(S0.st_main, delta_g2, nullptr, 0, nullptr, tail_tab[TAB_D2].template as<P2>())));
     ctr.launches += 4;
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
@@ -1655,14 +1656,14 @@ struct Engine : IEngine {
     }
     Fr* hsc = reinterpret_cast<Fr*>(sl.h_tail);   // r[count], s[count], (r s)[count]
     for (uint32_t k = 0; k < count; k++) {
-      hsc[k] = load_fr(r + 4 * (size_t)(first + k));
-      hsc[count + k] = load_fr(s + 4 * (size_t)(first + k));
+      hsc[k] = load_fr(r + FR64 * (size_t)(first + k));
+      hsc[count + k] = load_fr(s + FR64 * (size_t)(first + k));
       hsc[2 * count + k] = Fr::mul(hsc[k], hsc[count + k]);
     }
     int rc;
     {
       NvtxSpan span_wm(SPAN_WITNESS_MAP);
-      rc = enqueue_witness_map(sl, z + (size_t)first * nv * 4, flags, count);
+      rc = enqueue_witness_map(sl, z + (size_t)first * nv * FR64, flags, count);
     }
     if (rc) return rc;
     // the five fixed-base products of every proof, after the witness map on its stream (the H MSM waits for ev_h only)
@@ -1705,8 +1706,8 @@ struct Engine : IEngine {
         P1* outs[4] = {&x.h, &x.l, &x.a, &x.b1};
         for (int m = 0; m < 4; m++) *outs[m] = sl.run[m] ? msm_finish<Fq>(sl.ws1[m], sl.geom[m], k) : P1::inf();
         x.b2 = sl.run[M_B2] ? msm_finish<Fq2>(sl.ws2, sl.geom[M_B2], k) : P2::inf();
-        const Fr rk = load_fr(r + 4 * (size_t)(first + k)), sk = load_fr(s + 4 * (size_t)(first + k));
-        store_proof(proofs + (size_t)(first + k) * 8 * NQ64, kp, x.a, x.b2, c_part(rk, sk, x));
+        const Fr rk = load_fr(r + FR64 * (size_t)(first + k)), sk = load_fr(s + FR64 * (size_t)(first + k));
+        store_proof(proofs + (size_t)(first + k) * PROOF64, kp, x.a, x.b2, c_part(rk, sk, x));
       });
     }
     for (auto& t : tk) t->wait();
@@ -1772,7 +1773,7 @@ struct Engine : IEngine {
   DevBuf d_comm_send, d_comm_recv;
   uint64_t* h_comm_send = nullptr;   // pinned
   uint64_t* h_comm_recv = nullptr;   // pinned, world records
-  static constexpr size_t REC_LIMBS = 2 * 4 * (size_t)NQ64 + 4 * 2 * (size_t)NQ64;   // A_k, C_k (XYZZ G1), B2_k (XYZZ G2)
+  static constexpr size_t REC_LIMBS = 2 * 4 * (size_t)NQ64 + sizeof(P2) / 8;   // A_k, C_k (XYZZ G1), B2_k (XYZZ G2)
   void comm_release() {
     if (nccl_comm && nccl_api().CommDestroy) nccl_api().CommDestroy(nccl_comm);
     if (nccl_comm_wm && nccl_api().CommDestroy) nccl_api().CommDestroy(nccl_comm_wm);
@@ -1913,7 +1914,7 @@ struct Engine : IEngine {
   G16_MSM_TEMPLATES(X, Fp<CP::FqP>, Fp<CP::FrP>)                                                  \
   G16_MSM_TEMPLATES(X, G16_FQ2(CP), Fp<CP::FrP>)                                                  \
   G16_SER_TEMPLATES(X, CP)
-#define G16_FQ2(CP) Fp2<CP::FqP, CP::FQ2_NONRESIDUE_NEG>
+#define G16_FQ2(CP) CP::G2F
 
 template <class CP>
 IEngine* make_engine(int device, int* rc) {

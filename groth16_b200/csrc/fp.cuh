@@ -62,7 +62,8 @@ inline void madc_hi(uint32_t& r, uint32_t a, uint32_t b, uint32_t c) { r = (uint
 // Curve base fields (Fq): their device products are out-of-line calls, see Fp::mul.  Scalar fields stay inlined.
 template <class P>
 constexpr bool is_base_field() {
-  return std::is_same<P, BLS381_FqP>::value || std::is_same<P, BN254_FqP>::value || std::is_same<P, BLS377_FqP>::value;
+  return std::is_same<P, BLS381_FqP>::value || std::is_same<P, BN254_FqP>::value || std::is_same<P, BLS377_FqP>::value ||
+         std::is_same<P, BW6_FqP>::value;
 }
 
 template <class P>

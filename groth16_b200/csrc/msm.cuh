@@ -120,10 +120,13 @@ __global__ void __launch_bounds__(256) msm_digits(const uint32_t* __restrict__ s
   bool live = i < g.n;
   FrF s = FrF::zero();
   if (live) {
-    const uint4* p = reinterpret_cast<const uint4*>(scalars) + (size_t)i * scalar_stride * 2;
-    uint4 lo = __ldg(p), hi = __ldg(p + 1);
-    s.v[0] = lo.x; s.v[1] = lo.y; s.v[2] = lo.z; s.v[3] = lo.w;
-    s.v[4] = hi.x; s.v[5] = hi.y; s.v[6] = hi.z; s.v[7] = hi.w;
+    constexpr int NV = FrF::N / 4;   // 16-byte words per scalar
+    const uint4* p = reinterpret_cast<const uint4*>(scalars) + (size_t)i * scalar_stride * NV;
+#pragma unroll
+    for (int j = 0; j < NV; j++) {
+      const uint4 x = __ldg(p + j);
+      s.v[4 * j] = x.x; s.v[4 * j + 1] = x.y; s.v[4 * j + 2] = x.z; s.v[4 * j + 3] = x.w;
+    }
     if (skip && skip[i]) live = false;
   }
   if (scalars_mont) s = FrF::from_mont(s);   // `into_bigint`, prover.rs:64,71,82
@@ -133,9 +136,9 @@ __global__ void __launch_bounds__(256) msm_digits(const uint32_t* __restrict__ s
     const int bit = w * g.c;
     const int limb = bit >> 5, sh = bit & 31;
     uint32_t raw = 0;
-    if (limb < 8) {
+    if (limb < FrF::N) {
       uint64_t two = s.v[limb];
-      if (limb + 1 < 8) two |= (uint64_t)s.v[limb + 1] << 32;
+      if (limb + 1 < FrF::N) two |= (uint64_t)s.v[limb + 1] << 32;
       raw = (uint32_t)(two >> sh) & ((1u << g.c) - 1);
     }
     raw += carry;
@@ -295,15 +298,15 @@ __device__ __forceinline__ Affine<F> load_affine(const Affine<F>* __restrict__ b
 }
 
 // Level 0: grid covers T0 = ceil(max_entries / K0) threads; threads past the real entry count only clear their slots.
-// Register budget: 3 resident blocks per SM for single-field points (G1), 2 for Fq2 points (G2).  (Staging the gathered
+// Register budget: 3 resident blocks per SM for narrow points (G1), 2 for wide ones (G2, BW6-761).  (Staging the gathered
 // bases through shared memory with cp.async was measured and is slower: with 3 warps per scheduler the gather latency
 // is already hidden and the kernel is bound by the IMAD.WIDE pipe.  Also measured and slower: the running sum
 // kept in shared memory for one more resident block per SM; lazily reduced double-width products.)
 template <class F>
-struct MsmAccumCfg { static constexpr int MIN_BLOCKS = sizeof(F) <= 48 ? 3 : 2; };
-// coordinates of the gathered base fetched on demand (x, then y) for Fq2 points: 24 fewer live registers at the peak
+struct MsmAccumCfg { static constexpr int MIN_BLOCKS = MsmWide<F>::value ? 2 : 3; };
+// coordinates of the gathered base fetched on demand (x, then y) for wide points: 24 fewer live registers at the peak
 template <class F>
-__host__ __device__ constexpr bool msm_lazy_load() { return sizeof(F) > 48; }
+__host__ __device__ constexpr bool msm_lazy_load() { return MsmWide<F>::value; }
 // `sidx` == nullptr: the entries are the points of `bases` themselves (last list of the batched-affine rounds) and the
 // key of entry e is skey[e << key_shift]; empty slots (MSM_INVALID index, or the point (0,0)) add nothing.
 template <class F>
@@ -766,7 +769,7 @@ struct MsmCounters {  // launch bookkeeping for bench.py's gpu_launches
 };
 
 // Enqueue one MSM on `st`.  d_bases holds g.copies * g.n affine points (copy-major); d_scalars / d_skip are device
-// pointers, pair i uses the scalar at d_scalars + 8 * i * scalar_stride (stride = world size for a sharded key); the leaf arrays of the bucket reduction land in ws.h_leaf once the stream is synchronised (msm_finish).
+// pointers, pair i uses the scalar at d_scalars + FrF::N * i * scalar_stride (stride = world size for a sharded key); the leaf arrays of the bucket reduction land in ws.h_leaf once the stream is synchronised (msm_finish).
 // The sorted (bucket-major, padded) entry list of an MSM, as another MSM over the SAME scalars, skip mask and geometry may
 // borrow it: B in G1 and B in G2 (prover.rs:101,113) share scalars, and their queries share the identity pattern
 // (b_g1_query[i] and b_g2_query[i] are both b_i(tau) times a generator), so one counting sort serves both.
@@ -1003,11 +1006,13 @@ cudaError_t msm_prepare_query(cudaStream_t st, Affine<F>* d_bases, uint32_t cnt,
 // ------------------------------------------------------------------------------------------------
 // fixed-base batch multiplication (BatchMulPreprocessing::batch_mul, generator.rs:129-183)
 // ------------------------------------------------------------------------------------------------
-static constexpr int FB_WINDOWS = 32;  // 8-bit windows over a 256-bit scalar
-template <class F>
-__global__ void fb_table_kernel(Affine<F> g, XYZZ<F>* table /* [32][255] */) {
+// 8-bit windows over the scalar's limbs: 32 for a 256-bit Fr, 48 for BW6-761's 384-bit one
+template <class FrF>
+constexpr int fb_windows() { return 4 * FrF::N; }
+template <class F, int NW>
+__global__ void fb_table_kernel(Affine<F> g, XYZZ<F>* table /* [NW][255] */) {
   const int w = threadIdx.x;
-  if (w >= FB_WINDOWS) return;
+  if (w >= NW) return;
   XYZZ<F> base = XYZZ<F>::from_affine(g);
   for (int i = 0; i < 8 * w; i++) base.dbl_inplace();
   XYZZ<F> acc = base;
@@ -1024,23 +1029,25 @@ __global__ void __launch_bounds__(128) fb_mul_kernel(const XYZZ<F>* __restrict__
   FrF s;
   {
     const uint4* p = reinterpret_cast<const uint4*>(scalars + i);
-    uint4 lo = __ldg(p), hi = __ldg(p + 1);
-    s.v[0] = lo.x; s.v[1] = lo.y; s.v[2] = lo.z; s.v[3] = lo.w;
-    s.v[4] = hi.x; s.v[5] = hi.y; s.v[6] = hi.z; s.v[7] = hi.w;
+#pragma unroll
+    for (int j = 0; j < FrF::N / 4; j++) {
+      const uint4 x = __ldg(p + j);
+      s.v[4 * j] = x.x; s.v[4 * j + 1] = x.y; s.v[4 * j + 2] = x.z; s.v[4 * j + 3] = x.w;
+    }
   }
   s = FrF::from_mont(s);
   XYZZ<F> acc = XYZZ<F>::inf();
-  for (int w = 0; w < FB_WINDOWS; w++) {
+  for (int w = 0; w < fb_windows<FrF>(); w++) {
     const uint32_t d = (s.v[w >> 2] >> (8 * (w & 3))) & 0xff;
     if (d) acc.add(table[w * 255 + d - 1]);
   }
   out[i] = acc.to_affine();
 }
-// d_table: FB_WINDOWS * 255 XYZZ points of scratch
+// d_table: fb_windows<FrF>() * 255 XYZZ points of scratch
 template <class F, class FrF>
 cudaError_t fb_batch_mul(cudaStream_t st, const Affine<F>& gen, const FrF* d_scalars, uint64_t cnt, Affine<F>* d_out,
                          XYZZ<F>* d_table) {
-  fb_table_kernel<F><<<1, 32, 0, st>>>(gen, d_table);
+  fb_table_kernel<F, fb_windows<FrF>()><<<1, fb_windows<FrF>(), 0, st>>>(gen, d_table);
   if (cnt) fb_mul_kernel<F, FrF><<<(unsigned)((cnt + 127) / 128), 128, 0, st>>>(d_table, d_scalars, (uint32_t)cnt, d_out);
   return cudaGetLastError();
 }

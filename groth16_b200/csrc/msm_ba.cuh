@@ -217,10 +217,10 @@ G16_HD void ba_backward(const BaRound<F>& a, uint64_t t) {
 }
 
 #ifdef __CUDACC__
-// Resident blocks per SM the register allocation aims at: single-field points ask for 3 and get 4 (~125 registers); Fq2
-// points 2 = the whole backward body in 254 registers (8 warps per SM).
+// Resident blocks per SM the register allocation aims at: narrow points ask for 3 and get 4 (~125 registers); wide points
+// (MsmWide: Fq2, BW6-761's Fq) 2 = the whole backward body in 254 registers (8 warps per SM).
 template <class F>
-struct BaCfg { static constexpr int MIN_BLOCKS = sizeof(F) <= 48 ? 3 : 2; };
+struct BaCfg { static constexpr int MIN_BLOCKS = MsmWide<F>::value ? 2 : 3; };
 template <class F>
 __global__ void __launch_bounds__(128, BaCfg<F>::MIN_BLOCKS) ba_forward_kernel(BaRound<F> a) {
   ba_forward<F>(a, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x);

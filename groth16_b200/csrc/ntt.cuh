@@ -55,16 +55,18 @@ template <class Fr>
 __device__ __forceinline__ Fr ntt_ldg(const Fr* p) {
   Fr r;
   const uint4* s = reinterpret_cast<const uint4*>(p);
-  uint4 a = __ldg(s), b = __ldg(s + 1);
-  r.v[0] = a.x; r.v[1] = a.y; r.v[2] = a.z; r.v[3] = a.w;
-  r.v[4] = b.x; r.v[5] = b.y; r.v[6] = b.z; r.v[7] = b.w;
+#pragma unroll
+  for (int j = 0; j < Fr::N / 4; j++) {
+    const uint4 a = __ldg(s + j);
+    r.v[4 * j] = a.x; r.v[4 * j + 1] = a.y; r.v[4 * j + 2] = a.z; r.v[4 * j + 3] = a.w;
+  }
   return r;
 }
 template <class Fr>
 __device__ __forceinline__ void ntt_stg(Fr* p, const Fr& r) {
   uint4* d = reinterpret_cast<uint4*>(p);
-  d[0] = make_uint4(r.v[0], r.v[1], r.v[2], r.v[3]);
-  d[1] = make_uint4(r.v[4], r.v[5], r.v[6], r.v[7]);
+#pragma unroll
+  for (int j = 0; j < Fr::N / 4; j++) d[j] = make_uint4(r.v[4 * j], r.v[4 * j + 1], r.v[4 * j + 2], r.v[4 * j + 3]);
 }
 
 static constexpr int NTT_TILE_LOG = 10;
@@ -74,8 +76,9 @@ static constexpr int NTT_TILE = 1 << NTT_TILE_LOG;
 // CIRCOM = false: the libsnark load / store modes; CIRCOM = true: NTT_LOAD_AB / NTT_STORE_AB_MINUS (plus plain / table loads)
 template <class Fr, bool CIRCOM>
 __global__ void __launch_bounds__(256) ntt_pass_kernel(NttPass<Fr> a) {
-  static_assert(Fr::N == 8, "Fr must be 8 x 32-bit limbs");
-  __shared__ uint32_t sm[8][NTT_TILE];
+  // 8 limbs (256-bit Fr): 32 KB of tile; 12 limbs (BW6-761's 377-bit Fr): 48 KB, the static shared-memory limit
+  static_assert(Fr::N == 8 || Fr::N == 12, "Fr must be 8 or 12 x 32-bit limbs");
+  __shared__ uint32_t sm[Fr::N][NTT_TILE];
   const int k = a.k, logC = a.logC;
   const uint32_t C = 1u << logC;
   const int tile_log = k + logC;
@@ -101,7 +104,7 @@ __global__ void __launch_bounds__(256) ntt_pass_kernel(NttPass<Fr> a) {
       x = Fr::mul(Fr::sub(Fr::mul(x, y), z), a.lcst);
     }
 #pragma unroll
-    for (int w = 0; w < 8; w++) sm[w][e] = x.v[w];
+    for (int w = 0; w < Fr::N; w++) sm[w][e] = x.v[w];
   }
   __syncthreads();
 
@@ -120,12 +123,12 @@ __global__ void __launch_bounds__(256) ntt_pass_kernel(NttPass<Fr> a) {
       const Fr w = ntt_ldg(a.tw + (jm << s));
       Fr x0, x1;
 #pragma unroll
-      for (int q = 0; q < 8; q++) { x0.v[q] = sm[q][e0]; x1.v[q] = sm[q][e1]; }
+      for (int q = 0; q < Fr::N; q++) { x0.v[q] = sm[q][e0]; x1.v[q] = sm[q][e1]; }
       const Fr u = Fr::add(x0, x1);
       Fr v = Fr::sub(x0, x1);
       if (s != a.L - 1) v = Fr::mul(v, w);   // the last stage of a transform only has the twiddle omega^0 = 1
 #pragma unroll
-      for (int q = 0; q < 8; q++) { sm[q][e0] = u.v[q]; sm[q][e1] = v.v[q]; }
+      for (int q = 0; q < Fr::N; q++) { sm[q][e0] = u.v[q]; sm[q][e1] = v.v[q]; }
     }
     __syncthreads();
   }
@@ -136,7 +139,7 @@ __global__ void __launch_bounds__(256) ntt_pass_kernel(NttPass<Fr> a) {
     uint64_t gi = gbase + ((uint64_t)mid << low_bits) + cl;
     Fr x;
 #pragma unroll
-    for (int w = 0; w < 8; w++) x.v[w] = sm[w][e];
+    for (int w = 0; w < Fr::N; w++) x.v[w] = sm[w][e];
     if (a.bitrev_store && a.L > 0) gi = __brevll(gi) >> (64 - a.L);
     if constexpr (CIRCOM) {
       if (a.store_mode == NTT_STORE_AB_MINUS) x = Fr::sub(Fr::mul(ntt_ldg(a.st_a + voff + gi), ntt_ldg(a.st_b + voff + gi)), x);

@@ -3,8 +3,8 @@
 // The formats are exactly groth16_b200/serialize.py's (ArkCodec.point / read_point):
 //   * BLS12-381: zcash / IETF, big-endian, three flag bits in the first byte (0x80 compressed, 0x40 infinity, 0x20 y is the
 //     larger of +-y), Fq2 as c1 || c0;
-//   * BN254, BLS12-377: generic short Weierstrass, little-endian, SWFlags in the two top bits of the last byte (0x80 y > -y,
-//     0x40 infinity), Fq2 as c0 || c1.
+//   * BN254, BLS12-377, BW6-761: generic short Weierstrass, little-endian, SWFlags in the two top bits of the last byte
+//     (0x80 y > -y, 0x40 infinity), Fq2 as c0 || c1.  BW6-761's G2 is over Fq: its points are encoded like G1 points.
 // A compressed point is x alone, an uncompressed one x || y.  Decoding checks what serialize.py checks: the flag bits, zero
 // bytes under the infinity flag, canonical coordinates (< q), that a compressed x has a curve point, that an uncompressed
 // point is on the curve, and with G16_SER_VALIDATE that [r]P = O (skipped for BN254 G1, whose cofactor is 1).
@@ -51,14 +51,15 @@ enum : uint32_t { SER_COMPRESSED = 1, SER_VALIDATE = 2 };
 template <class CP>
 struct SerFormat {
   static constexpr bool ZCASH = CP::CURVE_ID == 0;                           // BLS12-381
-  static constexpr int NB = 4 * CP::FqP::N;                                  // bytes per Fq: 48 (BLS12-*), 32 (BN254)
+  static constexpr int NB = 4 * CP::FqP::N;                                  // bytes per Fq: 48 (BLS12-*), 32 (BN254), 96 (BW6)
   static constexpr bool G1_COFACTOR_ONE = CP::CURVE_ID == 1;                 // BN254
+  static constexpr int G2_NC = sizeof(typename CP::G2F) / sizeof(Fp<typename CP::FqP>);   // Fq per G2 coordinate: 2 or 1
   static_assert(ZCASH || NB * 8 >= CP::FqP::BITS + 2, "no room for the SWFlags");
-  G16_HD static constexpr int point_bytes(bool g2, bool compress) { return NB * (g2 ? 2 : 1) * (compress ? 1 : 2); }
+  G16_HD static constexpr int point_bytes(bool g2, bool compress) { return NB * (g2 ? G2_NC : 1) * (compress ? 1 : 2); }
 };
 
 template <class CP, bool G2>
-using SerField = typename std::conditional<G2, Fp2<typename CP::FqP, CP::FQ2_NONRESIDUE_NEG>, Fp<typename CP::FqP>>::type;
+using SerField = typename std::conditional<G2, typename CP::G2F, Fp<typename CP::FqP>>::type;
 
 // ---- canonical integers ----------------------------------------------------------------------------------------------
 template <class P>
@@ -197,16 +198,17 @@ G16_HD bool ser_sqrt(const Fp2<P, NR>& a, Fp2<P, NR>& r) {
 }
 
 // ---- curve data -----------------------------------------------------------------------------------------------------
-template <class CP>
-G16_HD Fp<typename CP::FqP> ser_b(Fp<typename CP::FqP>*) {
-  Fp<typename CP::FqP> b;
-  for (int i = 0; i < CP::FqP::N; i++) b.v[i] = CP::FqP::curve_b(i);
-  return b;
-}
-template <class CP>
-G16_HD SerField<CP, true> ser_b(SerField<CP, true>*) {
-  SerField<CP, true> b;
-  for (int i = 0; i < CP::FqP::N; i++) { b.c0.v[i] = CP::FqP::twist_b0(i); b.c1.v[i] = CP::FqP::twist_b1(i); }
+// b of G1, or of G2 in G2's own coordinate field (twist_b0 alone when G2 is over Fq)
+template <class CP, bool G2>
+G16_HD SerField<CP, G2> ser_b() {
+  SerField<CP, G2> b;
+  if constexpr (!G2) {
+    for (int i = 0; i < CP::FqP::N; i++) b.v[i] = CP::FqP::curve_b(i);
+  } else if constexpr (SerFormat<CP>::G2_NC == 1) {
+    for (int i = 0; i < CP::FqP::N; i++) b.v[i] = CP::FqP::twist_b0(i);
+  } else {
+    for (int i = 0; i < CP::FqP::N; i++) { b.c0.v[i] = CP::FqP::twist_b0(i); b.c1.v[i] = CP::FqP::twist_b1(i); }
+  }
   return b;
 }
 // [r]P = O by left-to-right double-and-add over the bits of r in XYZZ.  XYZZ::madd / dbl_inplace handle every exceptional
@@ -221,10 +223,10 @@ G16_HD bool ser_in_subgroup(const Affine<F>& p) {
   return acc.is_inf();
 }
 
-// wire value k of the point -> field element (G1: x = value 0, y = value 1; G2: two values each)
+// wire value k of the point -> field element (G1: x = value 0, y = value 1; G2 over Fq2: two values each)
 template <class CP, bool G2>
 G16_HD SerField<CP, G2> ser_pick(const Fp<typename CP::FqP>* v, int k) {
-  if constexpr (G2) {
+  if constexpr (G2 && SerFormat<CP>::G2_NC == 2) {
     if (SerFormat<CP>::ZCASH) return {v[2 * k + 1], v[2 * k]};
     return {v[2 * k], v[2 * k + 1]};
   } else {
@@ -240,7 +242,7 @@ G16_HD uint32_t ser_decode(const uint8_t* raw, uint32_t flags, Affine<SerField<C
   using Fq = Fp<typename CP::FqP>;
   using F = SerField<CP, G2>;
   using Fmt = SerFormat<CP>;
-  constexpr int NB = Fmt::NB, NC = G2 ? 2 : 1, N = CP::FqP::N;
+  constexpr int NB = Fmt::NB, NC = G2 ? Fmt::G2_NC : 1, N = CP::FqP::N;
   const bool compress = flags & SER_COMPRESSED;
   const int nv = compress ? NC : 2 * NC;
   uint32_t fl;
@@ -276,7 +278,7 @@ G16_HD uint32_t ser_decode(const uint8_t* raw, uint32_t flags, Affine<SerField<C
 #pragma unroll
   for (int k = 0; k < 2 * NC; k++) v[k] = Fq::to_mont(v[k]);
   const F x = ser_pick<CP, G2>(v, 0);
-  const F rhs = F::add(F::mul(F::sqr(x), x), ser_b<CP>((F*)nullptr));
+  const F rhs = F::add(F::mul(F::sqr(x), x), ser_b<CP, G2>());
   F y;
   if (compress) {
     if (!ser_sqrt(rhs, y)) return SER_ERR_NO_ROOT;
@@ -297,7 +299,7 @@ template <class CP, bool G2>
 G16_HD void ser_encode(const Affine<SerField<CP, G2>>& p, uint32_t flags, uint8_t* out) {
   using Fq = Fp<typename CP::FqP>;
   using Fmt = SerFormat<CP>;
-  constexpr int NB = Fmt::NB, NC = G2 ? 2 : 1;
+  constexpr int NB = Fmt::NB, NC = G2 ? Fmt::G2_NC : 1;
   const bool compress = flags & SER_COMPRESSED;
   const int nv = compress ? NC : 2 * NC;
   const int size = nv * NB;
@@ -308,7 +310,7 @@ G16_HD void ser_encode(const Affine<SerField<CP, G2>>& p, uint32_t flags, uint8_
     return;
   }
   Fq v[2 * NC];
-  if constexpr (G2) {
+  if constexpr (NC == 2) {
     const Fq xs[4] = {p.x.c0, p.x.c1, p.y.c0, p.y.c1};
 #pragma unroll
     for (int k = 0; k < 4; k++) v[Fmt::ZCASH ? (k ^ 1) : k] = xs[k];
@@ -418,12 +420,13 @@ inline void ser_items(SerItem it[SER_ITEMS]) {
 }
 // Walks the structure from the length prefixes alone (every point has a fixed size once the flag is known): fills
 // it[].len / off / psize and returns "" or why the stream is malformed (truncated, trailing bytes, absurd prefix).
-inline std::string ser_walk(const uint8_t* bytes, uint64_t len, int nb, bool compress, SerItem it[SER_ITEMS]) {
+// g2_nc: Fq elements per G2 coordinate (SerFormat::G2_NC).
+inline std::string ser_walk(const uint8_t* bytes, uint64_t len, int nb, bool compress, SerItem it[SER_ITEMS], int g2_nc = 2) {
   ser_items(it);
   uint64_t pos = 0;
   for (int m = 0; m < SER_ITEMS; m++) {
     SerItem& x = it[m];
-    x.psize = (uint32_t)(nb * (x.g2 ? 2 : 1) * (compress ? 1 : 2));
+    x.psize = (uint32_t)(nb * (x.g2 ? g2_nc : 1) * (compress ? 1 : 2));
     if (x.vec) {
       if (len - pos < 8)
         return std::string("truncated input: wanted 8 bytes, got ") + std::to_string(len - pos) + " (length of " + x.name + ")";
@@ -445,11 +448,11 @@ inline std::string ser_walk(const uint8_t* bytes, uint64_t len, int nb, bool com
   return "";
 }
 // total size of a key with these lengths (g16_pk_export_serialized)
-inline uint64_t ser_size(SerItem it[SER_ITEMS], int nb, bool compress) {
+inline uint64_t ser_size(SerItem it[SER_ITEMS], int nb, bool compress, int g2_nc = 2) {
   uint64_t pos = 0;
   for (int m = 0; m < SER_ITEMS; m++) {
     SerItem& x = it[m];
-    x.psize = (uint32_t)(nb * (x.g2 ? 2 : 1) * (compress ? 1 : 2));
+    x.psize = (uint32_t)(nb * (x.g2 ? g2_nc : 1) * (compress ? 1 : 2));
     if (x.vec) pos += 8;
     x.off = pos;
     pos += x.len * x.psize;

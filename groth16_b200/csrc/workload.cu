@@ -35,14 +35,15 @@ static inline uint64_t splitmix(uint64_t& s) {
 template <class FrP>
 static int synth(uint32_t log_n, uint64_t seed, uint32_t* a_col, uint64_t* a_val, uint32_t* b_col, uint32_t* c_col, uint64_t* z_out) {
   using Fr = Fp<FrP>;
+  constexpr int W = Fr::N / 2;   // u64 limbs per Fr
   const uint64_t nc = (1ull << log_n) - 2;
   const uint32_t ninst = 2;
   uint64_t st = seed * 0x2545F4914F6CDD1Dull + 0x1234567ull;
   auto rand_fr = [&]() {   // uniform below 2^(BITS-1) < r: plenty for a workload
     Fr x;
-    for (int i = 0; i < 8; i += 2) { const uint64_t w = splitmix(st); x.v[i] = (uint32_t)w; x.v[i + 1] = (uint32_t)(w >> 32); }
-    const int top = FrP::BITS - 1 - 224;   // bits kept in limb 7
-    x.v[7] &= (top >= 32) ? 0xffffffffu : ((1u << top) - 1);
+    for (int i = 0; i < Fr::N; i += 2) { const uint64_t w = splitmix(st); x.v[i] = (uint32_t)w; x.v[i + 1] = (uint32_t)(w >> 32); }
+    const int top = FrP::BITS - 1 - 32 * (Fr::N - 1);   // bits kept in the top limb
+    x.v[Fr::N - 1] &= (top >= 32) ? 0xffffffffu : ((1u << top) - 1);
     return Fr::to_mont(x);
   };
   std::vector<Fr> vals(nc + 2);
@@ -64,14 +65,14 @@ static int synth(uint32_t log_n, uint64_t seed, uint32_t* a_col, uint64_t* a_val
     cols[i + 2] = (i == nc - 1) ? 1u : ninst + n_w++;
     a_col[2 * i] = cols[p];
     a_col[2 * i + 1] = 0;   // the constant One carries k_i
-    memcpy(a_val + 8 * i, one.v, 32);
-    memcpy(a_val + 8 * i + 4, km.v, 32);
+    memcpy(a_val + 2 * W * i, one.v, sizeof(Fr));
+    memcpy(a_val + 2 * W * i + W, km.v, sizeof(Fr));
     b_col[i] = cols[q];
     c_col[i] = cols[i + 2];
   }
   // full assignment: One, the public input, then the witnesses in column order
-  memcpy(z_out, one.v, 32);
-  for (uint64_t j = 0; j < nc + 2; j++) memcpy(z_out + 4 * (uint64_t)cols[j], vals[j].v, 32);
+  memcpy(z_out, one.v, sizeof(Fr));
+  for (uint64_t j = 0; j < nc + 2; j++) memcpy(z_out + W * (uint64_t)cols[j], vals[j].v, sizeof(Fr));
   return G16_OK;
 }
 }  // namespace g16
@@ -88,6 +89,7 @@ extern "C" int g16_synthetic_r1cs(int curve, uint32_t log_n, uint64_t seed, uint
     case G16_CURVE_BLS12_381: return synth<BLS381_FrP>(log_n, seed, a_col, a_val, b_col, c_col, full_assignment);
     case G16_CURVE_BN254: return synth<BN254_FrP>(log_n, seed, a_col, a_val, b_col, c_col, full_assignment);
     case G16_CURVE_BLS12_377: return synth<BLS377_FrP>(log_n, seed, a_col, a_val, b_col, c_col, full_assignment);
+    case G16_CURVE_BW6_761: return synth<BW6_FrP>(log_n, seed, a_col, a_val, b_col, c_col, full_assignment);
     default: return fail(G16_ERR_BAD_ARGUMENT, "unknown curve id");
   }
 }

@@ -1,4 +1,5 @@
-"""Field moduli and limb counts of the three supported pairing curves (SURVEY.md section 2b).
+"""Field moduli and limb counts of the supported curves: the pairing curves BLS12-381, BN254 and BLS12-377 (SURVEY.md
+section 2b) and BW6-761, the outer curve of BLS12-377 recursion.
 
 Only what the host-side codecs need; the CUDA side has its own generated table (csrc/g16_constants.h)."""
 from dataclasses import dataclass
@@ -12,10 +13,20 @@ class CurveParams:
     q: int              # base field modulus
     fr_generator: int   # Fr::GENERATOR (coset offset, r1cs_to_qap.rs:204)
     two_adicity: int
+    g2_over_fq: bool = False   # G2 coordinates in Fq itself (BW6-761) instead of Fq2
 
     @property
     def fq_limbs(self) -> int:
         return (self.q.bit_length() + 63) // 64
+
+    @property
+    def fr_limbs(self) -> int:
+        return (self.r.bit_length() + 63) // 64
+
+    @property
+    def g2_limbs(self) -> int:
+        """u64 limbs of one G2 affine point"""
+        return (2 if self.g2_over_fq else 4) * self.fq_limbs
 
 
 BLS12_381 = CurveParams(
@@ -34,7 +45,14 @@ BLS12_377 = CurveParams(
     258664426012969094010652733694893533536393512754914660539884262666720468348340822774968888139573360124440321458177,
     22, 47)
 
-CURVES = {c.name: c for c in (BLS12_381, BN254, BLS12_377)}
+# BW6-761: r is BLS12-377's q.  G1: y^2 = x^3 - 1, G2: y^2 = x^3 + 4, both over Fq.
+BW6_761 = CurveParams(
+    "bw6_761", 3,
+    BLS12_377.q,
+    0x122e824fb83ce0ad187c94004faff3eb926186a81d14688528275ef8087be41707ba638e584e91903cebaff25b423048689c8ed12f9fd9071dcd3dc73ebff2e98a116c25667a8f8160cf8aeeaf0a437e6913e6870000082f49d00000000008b,
+    15, 46, g2_over_fq=True)
+
+CURVES = {c.name: c for c in (BLS12_381, BN254, BLS12_377, BW6_761)}
 
 
 def get_curve(curve) -> CurveParams:
@@ -72,4 +90,12 @@ GENERATORS = {
              0x895a8006e7536bdf93f71f27bd5b280fa531cc66f63449312a91ec01c684a6ccff1ebd00e2931c19b0ac9bf61d4f68),
             (0x17663bd2b96d697799583fe676e7df81723dc2c223265cc2685c69e2b7d4c8464c342be5846f0eeeeec44de888db212,
              0x1b49e02eade86f46ff617db109925f68fc7bd69f1dbcbae76ff26e3388801324d585e56fbfb1cc438029a7a8b7f6b3))),
+    # G2 over Fq: g2 is an (x, y) pair like g1.  A recipe of its own, not the other curves' (a 256-bit hash, too short for a
+    # 761-bit x): x = the 1024-bit little-endian integer of sha512("bw6_761-g<k>:<i>") repeated twice, mod q, for the first i
+    # with a curve point (the smaller root y), times the 384-bit cofactor.  tests/test_bw6_cpu.py re-derives both.
+    "bw6_761": dict(
+        g1=(0xc4b9f2bdb719ce82628aeb2dce695848ccd7d8ada4eb2389732d498070cb23548fe3477cefa0b8a1189abe80b7350cec7944f4b1b70efd816a33f2f9cc136b6b7ff59253118d154eb7284e3321d6176fe081075ab3d349f5a74d54640a1b2f,
+            0x29430bee0dc548df82627abd2d312248f1bff387ad5c5f8197e50ae8e9d701b5f5ef655b751e9abaa61a3ada0864feb5e19972a3a1e38e501291719e1925ddcb209d8fdde82fc687daeefa1de84d80ded2f1bc29eb85547911897400f7dc23),
+        g2=(0x85ba4ee833fa16b37d0b1a861dc4caaa5b65ea073d65de92306440aa11225b1c66feb22afe5b2f76184642dd572e76be86b8f6e0a57af8864529d02b1cb6734209c828d3ff359daa153866695a707036dc8f13774c3178888713705752b8f1,
+            0xa5d36491ece4b262680ab6a294cc5b716290462eba70d0f42a2443599fa80df90c35fe3479e5e3159cfb60719ac1634eb415b9e088c315f506e6aec397a12a6c142c2fcb39d70fc2615d32ac1a2fae190dfaba433796f107f82b9cf2964035)),
 }

@@ -27,11 +27,14 @@ from .params import CurveParams, get_curve
 
 # Fq2 non-residues (u^2 = -NR) and curve coefficients needed to decompress
 _FQ2_NR = {"bls12_381": 1, "bn254": 1, "bls12_377": 5}
-_G1_B = {"bls12_381": 4, "bn254": 3, "bls12_377": 1}
+_G1_B = {"bls12_381": 4, "bn254": 3, "bls12_377": 1, "bw6_761": -1}
 
 
 def _g2_b(c: CurveParams):
+    """G2's coefficient b: an Fq2 pair, or one Fq element when G2 is over Fq (BW6-761: y^2 = x^3 + 4)"""
     q = c.q
+    if c.g2_over_fq:
+        return 4
     if c.name == "bls12_381":
         return (4, 4)
     if c.name == "bn254":  # 3 / (9 + u)
@@ -127,13 +130,14 @@ class ArkCodec:
         self.q = self.c.q
         self.zcash = self.c.name == "bls12_381"
         self.fq_bytes = (self.q.bit_length() + 2 + 7) // 8 if not self.zcash else 48
-        self.fq2 = _Fq2(self.q, _FQ2_NR[self.c.name])
+        self.g2_fq2 = not self.c.g2_over_fq   # G2 coordinates are Fq2 pairs (otherwise G2 points are encoded like G1's)
+        self.fq2 = _Fq2(self.q, _FQ2_NR[self.c.name]) if self.g2_fq2 else None
         self.b1 = _G1_B[self.c.name]
         self.b2 = _g2_b(self.c)
 
     # ---- scalars ----
     def fr(self, x: int) -> bytes:
-        return int(x % self.c.r).to_bytes(32, "little")
+        return int(x % self.c.r).to_bytes(8 * self.c.fr_limbs, "little")
 
     # ---- points ----
     def _coords(self, P, g2):
@@ -146,6 +150,7 @@ class ArkCodec:
 
     def point(self, P, g2: bool = False, compress: bool = True) -> bytes:
         nb, q = self.fq_bytes, self.q
+        g2 = g2 and self.g2_fq2   # from here on: "the coordinates are Fq2 pairs"
         ncomp = 2 if g2 else 1
         if self.zcash:
             size = nb * ncomp * (1 if compress else 2)
@@ -180,8 +185,8 @@ class ArkCodec:
 
     def _on_curve(self, x, y, g2) -> bool:
         q = self.q
-        if not g2:
-            return (y * y - x * x * x - self.b1) % q == 0
+        if not g2 or not self.g2_fq2:
+            return (y * y - x * x * x - (self.b2 if g2 else self.b1)) % q == 0
         f = self.fq2
         x3 = f.mul(f.mul(x, x), x)
         y2 = f.mul(y, y)
@@ -190,6 +195,7 @@ class ArkCodec:
     def _in_subgroup(self, P, g2) -> bool:
         """[r]P == O by double-and-add in affine coordinates (slow; opt-in)"""
         q, r = self.q, self.c.r
+        g2 = g2 and self.g2_fq2
         f = self.fq2
 
         def inv(a):
@@ -230,6 +236,8 @@ class ArkCodec:
 
     def read_point(self, buf: io.BytesIO, g2: bool = False, compress: bool = True):
         nb, q = self.fq_bytes, self.q
+        group2 = g2                 # which curve equation
+        g2 = g2 and self.g2_fq2     # the coordinates are Fq2 pairs
         ncomp = 2 if g2 else 1
         raw = self._read(buf, nb * ncomp * (1 if compress else 2))
         if self.zcash:
@@ -265,22 +273,22 @@ class ArkCodec:
             yraw = ((vals[2], vals[3]) if g2 else vals[1]) if not compress else None
             neg_flag = bool(flags & 0x80)
         if compress:
-            y = self._solve_y(x, g2)
+            y = self._solve_y(x, group2)
             if _neg_gt(y, q, g2) != neg_flag:
                 y = ((-y[0]) % q, (-y[1]) % q) if g2 else (-y) % q
         else:
             y = yraw
-            if not self._on_curve(x, y, g2):
+            if not self._on_curve(x, y, group2):
                 raise DeserializeError("point is not on the curve")
         P = (x, y)
-        if self.check_subgroup and not self._in_subgroup(P, g2):
+        if self.check_subgroup and not self._in_subgroup(P, group2):
             raise DeserializeError("point is not in the prime-order subgroup")
         return P
 
     def _solve_y(self, x, g2):
         q = self.q
-        if not g2:
-            y = _sqrt_fq((x * x * x + self.b1) % q, q)
+        if not g2 or not self.g2_fq2:
+            y = _sqrt_fq((x * x * x + (self.b2 if g2 else self.b1)) % q, q)
         else:
             f = self.fq2
             x3 = f.mul(f.mul(x, x), x)
@@ -300,7 +308,7 @@ class ArkCodec:
         return [self.read_point(buf, g2, compress) for _ in range(n)]
 
     def read_fr(self, buf) -> int:
-        v = int.from_bytes(self._read(buf, 32), "little")
+        v = int.from_bytes(self._read(buf, 8 * self.c.fr_limbs), "little")
         if v >= self.c.r:
             raise DeserializeError("non-canonical scalar (>= r)")
         return v

@@ -71,10 +71,10 @@ def synthetic_r1cs(curve, log_n: int, seed: int = 0, num_inputs: int = 1):
         raise ValueError("domain too small")
     nwit = nc + 1
     a_col = np.empty(2 * nc, dtype=np.uint32)
-    a_val = np.empty((2 * nc, 4), dtype=np.uint64)
+    a_val = np.empty((2 * nc, cd.fr.nl), dtype=np.uint64)
     b_col = np.empty(nc, dtype=np.uint32)
     c_col = np.empty(nc, dtype=np.uint32)
-    z = np.zeros((ninst + nwit, 4), dtype=np.uint64)
+    z = np.zeros((ninst + nwit, cd.fr.nl), dtype=np.uint64)
     vp = lambda x: x.ctypes.data_as(C.c_void_p)
     lib = _workload_lib()
     fn = (lib or _lib.load()).g16_synthetic_r1cs
@@ -90,7 +90,7 @@ def synthetic_r1cs(curve, log_n: int, seed: int = 0, num_inputs: int = 1):
     one = np.ascontiguousarray(cd.fr.enc1(1))
     a_rp = np.arange(0, 2 * nc + 1, 2, dtype=np.uint32)
     b_rp = np.arange(0, nc + 1, dtype=np.uint32)
-    ones = np.ascontiguousarray(np.broadcast_to(one, (nc, 4)))
+    ones = np.ascontiguousarray(np.broadcast_to(one, (nc, cd.fr.nl)))
     m = ConstraintMatrices(ninst, nwit, nc, (a_rp, a_col, a_val), (b_rp, b_col, ones), (b_rp.copy(), c_col, ones.copy()))
     return m, z, cd.fr.dec(z[1:ninst])
 

@@ -4,11 +4,15 @@
  * replaces; INTEGRATION.md shows the Rust `extern "C"` binding a maintainer would add.
  *
  * Data layout (SURVEY.md section 8b), identical to ark-ff / ark-ec in-memory values copied field-wise:
- *   Fr / Fq element : N64 little-endian uint64_t limbs in MONTGOMERY form (R = 2^(64*N64)); N64 = 4 for every Fr,
- *                     4 for BN254 Fq, 6 for BLS12-381 / BLS12-377 Fq.
- *   BigInt scalar   : 4 little-endian uint64_t limbs, canonical integer < r  (`PrimeField::into_bigint`).
+ *   Fr / Fq element : N64 little-endian uint64_t limbs in MONTGOMERY form (R = 2^(64*N64)).  Fr: g16_fr_limbs (4 for
+ *                     BLS12-381 / BN254 / BLS12-377, 6 for BW6-761).  Fq: g16_fq_limbs (4 for BN254, 6 for BLS12-381 /
+ *                     BLS12-377, 12 for BW6-761).  Every Fr array of this ABI (assignments, r, s, setup scalars, NTT
+ *                     and witness-map vectors, h_out) is g16_fr_limbs limbs per element.
+ *   BigInt scalar   : g16_fr_limbs little-endian uint64_t limbs, canonical integer < r  (`PrimeField::into_bigint`).
  *   G1 affine       : x || y                      (2*N64 limbs);  point at infinity = all-zero limbs.
- *   G2 affine       : x.c0 || x.c1 || y.c0 || y.c1 (4*N64 limbs); point at infinity = all-zero limbs.
+ *   G2 affine       : x.c0 || x.c1 || y.c0 || y.c1 (4*N64 limbs); point at infinity = all-zero limbs.  BW6-761's G2
+ *                     is over Fq: x || y (2*N64 limbs).  g16_g2_limbs gives the size for the context's curve.
+ *   Proof           : a (G1) || b (G2) || c (G1): 8*N64 limbs, 6*N64 on BW6-761.
  *   G1/G2 projective output : X || Y || Z Jacobian, normalised to Z = 1 (identity: X = Y = 1, Z = 0, as ark).
  * All functions return G16_OK (0) or an error code; they never unwind or abort across the ABI
  * (the reference builds with panic = 'abort' for FFI safety, Cargo.toml:61).  A context is used by one host
@@ -27,7 +31,8 @@ extern "C" {
 enum {
   G16_CURVE_BLS12_381 = 0,
   G16_CURVE_BN254 = 1,
-  G16_CURVE_BLS12_377 = 2
+  G16_CURVE_BLS12_377 = 2,
+  G16_CURVE_BW6_761 = 3   /* the outer curve of BLS12-377 recursion: its r is BLS12-377's q; G2 over Fq */
 };
 
 enum {
@@ -56,6 +61,9 @@ void g16_ctx_destroy(g16_ctx* ctx);
 const char* g16_last_error(void);
 /* sizes, in uint64_t limbs, for buffers of this context's curve */
 int g16_fq_limbs(const g16_ctx* ctx);
+/* one Fr element or BigInt scalar (4, or 6 on BW6-761); one G2 affine point (4*N64, or 2*N64 on BW6-761) */
+int g16_fr_limbs(const g16_ctx* ctx);
+int g16_g2_limbs(const g16_ctx* ctx);
 
 /* ---- NTT: ark-poly Radix2EvaluationDomain (un-vendored dependency), call sites r1cs_to_qap.rs:201-207,220-221,232
  * In-place transform of 2^log_n Montgomery Fr elements in host memory, natural order in and out.
@@ -178,7 +186,7 @@ int g16_prove(g16_ctx* ctx, const uint64_t* r, const uint64_t* s, const uint64_t
 
 /* Sharded proving (world > 1): every rank computes its partial MSM sums, the host plumbing (torch.distributed /
  * NCCL all_gather of 5 points per rank) exchanges them, every rank assembles the same proof.
- * partial_out / partials: [h, l, a, b_g1] as G1 affine (4 * 2*N64 limbs) followed by b_g2 as G2 affine (4*N64). */
+ * partial_out / partials: [h, l, a, b_g1] as G1 affine (4 * 2*N64 limbs) followed by b_g2 as G2 affine (g16_g2_limbs). */
 int g16_prove_partial(g16_ctx* ctx, const uint64_t* r, const uint64_t* full_assignment, uint32_t flags,
                       uint64_t* partial_out);
 int g16_prove_assemble(g16_ctx* ctx, const uint64_t* r, const uint64_t* s, const uint64_t* partials,
@@ -197,14 +205,15 @@ int g16_prove_submit(g16_ctx* ctx, int slot, const uint64_t* r, const uint64_t* 
 int g16_prove_wait(g16_ctx* ctx, int slot, uint64_t* proof_out);
 int g16_prove_partial_submit(g16_ctx* ctx, int slot, const uint64_t* r, const uint64_t* full_assignment, uint32_t flags);
 int g16_prove_partial_wait(g16_ctx* ctx, int slot, uint64_t* partial_out);
-/* limbs per partial record: 4*2*N64 + 4*N64 */
+/* limbs per partial record: 4*2*N64 + g16_g2_limbs */
 int g16_partial_limbs(const g16_ctx* ctx);
 
 /* Batch proving (no reference counterpart: ark-groth16 proves one proof per call): `count` proofs of the resident circuit
  * under the resident key, one call.  Proof i is bit-identical to
- * g16_prove(ctx, r + 4 i, s + 4 i, full_assignments + 4 i nv, flags, proofs_out + 8 N64 i), nv = num_inputs + num_witness.
+ * g16_prove(ctx, r + F i, s + F i, full_assignments + F i nv, flags, proofs_out + P i), nv = num_inputs + num_witness,
+ * F = g16_fr_limbs, P = the proof's limbs (8 N64, or 6 N64 on BW6-761).
  * r, s: count Montgomery Fr each.  full_assignments: count * nv Montgomery Fr (host, or device with
- * G16_ASSIGNMENT_ON_DEVICE).  proofs_out: count * 8 * N64 limbs.  group: at most this many proofs share one pass of the
+ * G16_ASSIGNMENT_ON_DEVICE).  proofs_out: count * P limbs.  group: at most this many proofs share one pass of the
  * kernels (0 = automatic: as many as fit); results never depend on it.  Sharded keys (world > 1) are refused, and so is a
  * call while a proof is in flight in either slot.  count == 0 returns G16_OK and touches nothing.  Afterwards
  * g16_get_timings describes the whole call: total_ms is its device span, msm_pairs / msm_entries are summed over the batch,

@@ -85,13 +85,14 @@ fn ser_status(rc: i32) -> Result<(), SerializationError> {
     }
 }
 
-/// Curve id of the C ABI from the scalar-field modulus (the three curves the library is built for).
+/// Curve id of the C ABI from the scalar-field modulus (the four curves the library is built for).
 pub fn curve_id<F: PrimeField>() -> Option<i32> {
     let m = F::MODULUS.as_ref();
     match (F::MODULUS_BIT_SIZE, m[0]) {
         (255, 0xffff_ffff_0000_0001) => Some(sys::G16_CURVE_BLS12_381),
         (254, 0x43e1_f593_f000_0001) => Some(sys::G16_CURVE_BN254),
         (253, 0x0a11_8000_0000_0001) => Some(sys::G16_CURVE_BLS12_377),
+        (377, 0x8508_c000_0000_0001) => Some(sys::G16_CURVE_BW6_761),
         _ => None,
     }
 }
@@ -163,7 +164,7 @@ pub struct Csr {
 impl Csr {
     pub fn new<F: PrimeField>(m: &Matrix<F>) -> Self {
         let nnz: usize = m.iter().map(|r| r.len()).sum();
-        let mut s = Csr { row_ptr: Vec::with_capacity(m.len() + 1), col: Vec::with_capacity(nnz), val: Vec::with_capacity(4 * nnz) };
+        let mut s = Csr { row_ptr: Vec::with_capacity(m.len() + 1), col: Vec::with_capacity(nnz), val: Vec::with_capacity(core::mem::size_of::<F>() / 8 * nnz) };
         s.row_ptr.push(0);
         for row in m {
             for (coeff, idx) in row {
@@ -203,6 +204,7 @@ pub struct B200Prover<E: SwPairing> {
     num_constraints: usize,
     num_variables: usize,
     fq_limbs: usize,
+    g2_limbs: usize,   // one G2 affine point: 4 * fq_limbs over Fq2, 2 * fq_limbs on BW6-761 (G2 over Fq)
     _e: PhantomData<E>,
 }
 // the context is used by one thread at a time (include/g16b200.h); moving it between threads is fine
@@ -242,6 +244,7 @@ impl<E: SwPairing> B200Prover<E> {
             num_constraints: matrices.num_constraints,
             num_variables: matrices.num_instance_variables + matrices.num_witness_variables,
             fq_limbs: unsafe { sys::g16_fq_limbs(ctx) } as usize,
+            g2_limbs: unsafe { sys::g16_g2_limbs(ctx) } as usize,
             _e: PhantomData,
         };
         let (a, b, c) = (Csr::new(&matrices.a), Csr::new(&matrices.b), Csr::new(&matrices.c));
@@ -318,6 +321,7 @@ impl<E: SwPairing> B200Prover<E> {
             num_constraints: matrices.num_constraints,
             num_variables: matrices.num_instance_variables + matrices.num_witness_variables,
             fq_limbs: unsafe { sys::g16_fq_limbs(ctx) } as usize,
+            g2_limbs: unsafe { sys::g16_g2_limbs(ctx) } as usize,
             _e: PhantomData,
         };
         let (a, b, c) = (Csr::new(&matrices.a), Csr::new(&matrices.b), Csr::new(&matrices.c));
@@ -391,9 +395,13 @@ impl<E: SwPairing> B200Prover<E> {
         Ok(out)
     }
 
+    /// a (G1) || b (G2) || c (G1): 8 * fq_limbs, or 6 * fq_limbs on BW6-761
+    fn proof_limbs(&self) -> usize {
+        4 * self.fq_limbs + self.g2_limbs
+    }
     fn proof_from_limbs(&self, out: &[u64]) -> Proof<E> {
-        let n = self.fq_limbs;
-        Proof { a: unpack_point(&out[..2 * n]), b: unpack_point(&out[2 * n..6 * n]), c: unpack_point(&out[6 * n..8 * n]) }
+        let (n, g) = (self.fq_limbs, self.g2_limbs);
+        Proof { a: unpack_point(&out[..2 * n]), b: unpack_point(&out[2 * n..2 * n + g]), c: unpack_point(&out[2 * n + g..4 * n + g]) }
     }
 
     /// Drop-in for `Groth16::<E>::create_proof_with_reduction_and_matrices` (src/prover.rs:26-51).  `pk` and `matrices` are
@@ -412,7 +420,7 @@ impl<E: SwPairing> B200Prover<E> {
         if num_inputs != self.num_inputs || num_constraints != self.num_constraints || full_assignment.len() != self.num_variables {
             return Err(SynthesisError::MalformedVerifyingKey);
         }
-        let mut out = ark_std::vec![0u64; 8 * self.fq_limbs];
+        let mut out = ark_std::vec![0u64; self.proof_limbs()];
         status(unsafe {
             sys::g16_prove(self.ctx, fp_limbs(&r).as_ptr(), fp_limbs(&s).as_ptr(), scalars_ptr(full_assignment), 0, out.as_mut_ptr())
         })?;
@@ -477,7 +485,7 @@ impl<E: SwPairing> B200Prover<E> {
             return Ok(Vec::new());
         }
         let z: Vec<E::ScalarField> = assignments.concat();
-        let w = 8 * self.fq_limbs;
+        let w = self.proof_limbs();
         let mut out = ark_std::vec![0u64; count * w];
         status(unsafe {
             sys::g16_prove_batch(self.ctx, count as u32, scalars_ptr(rs), scalars_ptr(ss), scalars_ptr(&z), 0, 0, out.as_mut_ptr())
@@ -503,7 +511,7 @@ impl<E: SwPairing> B200Prover<E> {
     }
     /// Multi-GPU, second half: all ranks' partial records (rank order), gathered by the caller (MPI / NCCL all-gather).
     pub fn prove_assemble(&self, r: E::ScalarField, s: E::ScalarField, partials: &[u64], nparts: u32) -> R1CSResult<Proof<E>> {
-        let mut out = ark_std::vec![0u64; 8 * self.fq_limbs];
+        let mut out = ark_std::vec![0u64; self.proof_limbs()];
         status(unsafe {
             sys::g16_prove_assemble(self.ctx, fp_limbs(&r).as_ptr(), fp_limbs(&s).as_ptr(), partials.as_ptr(), nparts, out.as_mut_ptr())
         })?;

@@ -11,6 +11,7 @@ pub struct g16_ctx {
 pub const G16_CURVE_BLS12_381: c_int = 0;
 pub const G16_CURVE_BN254: c_int = 1;
 pub const G16_CURVE_BLS12_377: c_int = 2;
+pub const G16_CURVE_BW6_761: c_int = 3;
 
 pub const G16_OK: c_int = 0;
 pub const G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE: c_int = 1;
@@ -113,6 +114,8 @@ extern "C" {
     pub fn g16_ctx_destroy(ctx: *mut g16_ctx);
     pub fn g16_last_error() -> *const c_char;
     pub fn g16_fq_limbs(ctx: *const g16_ctx) -> c_int;
+    pub fn g16_fr_limbs(ctx: *const g16_ctx) -> c_int;
+    pub fn g16_g2_limbs(ctx: *const g16_ctx) -> c_int;
     pub fn g16_partial_limbs(ctx: *const g16_ctx) -> c_int;
     pub fn g16_domain_log(ctx: *const g16_ctx) -> u32;
     pub fn g16_ntt(ctx: *mut g16_ctx, log_n: u32, inverse: c_int, coset: c_int, inout: *mut u64) -> c_int;
