@@ -246,11 +246,13 @@ struct Engine : IEngine {
   // resident proving key (this rank's shard)
   bool have_pk = false;
   uint32_t rank = 0, world = 1;
-  struct Query {
-    DevBuf bases, mask;   // bases: geom.copies * (hi - lo) affine points, copy-major (copy j = 2^(c*ne*j) * P)
+  struct Shard {
     uint64_t pairs = 0;   // full MSM length
     uint64_t lo = 0, hi = 0;   // this rank owns pairs lo, lo + world, lo + 2 world, ... : hi - lo of them (lo = rank)
     MsmGeom geom{};
+  };
+  struct Query : Shard {
+    DevBuf bases, mask;   // bases: geom.copies * (hi - lo) affine points, copy-major (copy j = 2^(c*ne*j) * P)
   } q[5];
   // Tuning options: defaults below (from sweeps of a full proof at 2^20, tools/sweep.py), overridden at context creation by
   // the environment and at run time by g16_set_option.  options() lists them.
@@ -545,35 +547,23 @@ struct Engine : IEngine {
     }
     return G16_OK;
   }
-  ~Engine() override {
+  ~Engine() override {   // the DevBuf and MsmWorkspace members free themselves after this body, on this device
     cudaSetDevice(device);
-    for (Slot& sl : slots) {
-      if (sl.helper) sl.helper->wait();
-      if (sl.helper2) sl.helper2->wait();
-    }
-    if (asm_helper) asm_helper->wait();
+    drop_key();   // waits for the pool tasks that read the key
     comm_release();
     pool.reset();
     cudaDeviceSynchronize();
     dom.release();
     dom_api.release();
     for (Slot& sl : slots) {
-      sl.d_z.release(); sl.d_a.release(); sl.d_b.release(); sl.d_c.release(); sl.d_t.release(); sl.d_h.release();
-      sl.d_tail.release();
       if (sl.h_tail) cudaFreeHost(sl.h_tail);
-      for (auto& w : sl.ws1) w.release();
-      sl.ws2.release();
       if (sl.st_main) cudaStreamDestroy(sl.st_main);
       for (auto s : sl.st_msm) if (s) cudaStreamDestroy(s);
       auto kill = [](cudaEvent_t ev) { if (ev) cudaEventDestroy(ev); };
       kill(sl.ev_start); kill(sl.ev_z); kill(sl.ev_h); kill(sl.ev_bsort);
       for (int i = 0; i < 5; i++) { kill(sl.ev_m0[i]); kill(sl.ev_m1[i]); kill(sl.ev_a0[i]); kill(sl.ev_a1[i]); }
     }
-    for (int m = 0; m < 3; m++) { csr_rp[m].release(); csr_col[m].release(); csr_val[m].release(); }
-    for (auto& x : q) { x.bases.release(); x.mask.release(); }
-    for (auto& t : tail_tab) t.release();
     if (ev_batch) cudaEventDestroy(ev_batch);
-    d_gamma_abc.release(); full_a.release(); full_b1.release(); full_b2.release();
   }
   int fq_limbs() const override { return NQ64; }
   int fr_limbs() const override { return FR64; }
@@ -791,11 +781,8 @@ struct Engine : IEngine {
       G16_CUDA(cudaMemcpyAsync(ds.p, scalars, n * sizeof(Fr), cudaMemcpyHostToDevice, S0.st_main));
       G16_CUDA(msm_prepare_query<F>(S0.st_main, db.template as<Affine<F>>(), (uint32_t)n, 1, 0, dm.template as<uint8_t>()));
       const MsmGeom g = with_k0(msm_geom(n, FR_BITS, (int)tune.c, 0), g2);   // caller-supplied bases: no precomputed copies
-      cudaError_t e = msm_enqueue<F, Fr>(S0.st_main, ws, g, db.template as<Affine<F>>(), dm.template as<uint8_t>(), ds.template as<uint32_t>(), 1, false, &ctr, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
-      if (e != cudaSuccess) { db.release(); ds.release(); dm.release(); return fail(G16_ERR_CUDA, std::string("msm_enqueue: ") + cudaGetErrorString(e)); }
-      e = cudaStreamSynchronize(S0.st_main);
-      db.release(); ds.release(); dm.release();
-      if (e != cudaSuccess) return fail(G16_ERR_CUDA, std::string("msm sync: ") + cudaGetErrorString(e));
+      G16_CUDA((msm_enqueue<F, Fr>(S0.st_main, ws, g, db.template as<Affine<F>>(), dm.template as<uint8_t>(), ds.template as<uint32_t>(), 1, false, &ctr, nullptr, nullptr, nullptr, nullptr, nullptr, 0)));
+      G16_CUDA(cudaStreamSynchronize(S0.st_main));
       res = msm_finish<F>(ws, g);
     }
     store_proj<F>(out, res);
@@ -820,14 +807,19 @@ struct Engine : IEngine {
     G16_CUDA(cudaSetDevice(device));
     const g16_csr* ms[3] = {a, b, c};
     const uint32_t nvars = ni + nw;
-    for (int m = 0; m < 3; m++) {
-      if (!ms[m]->row_ptr) return fail(G16_ERR_BAD_ARGUMENT, "null row_ptr");
-      if (ms[m]->row_ptr[0] != 0) return fail(G16_ERR_BAD_ARGUMENT, "row_ptr[0] must be 0");
+    for (const g16_csr* x : ms) {   // all three matrices pass before the resident circuit is touched
+      if (!x->row_ptr) return fail(G16_ERR_BAD_ARGUMENT, "null row_ptr");
+      if (x->row_ptr[0] != 0) return fail(G16_ERR_BAD_ARGUMENT, "row_ptr[0] must be 0");
       for (uint32_t i = 0; i < nc; i++)
-        if (ms[m]->row_ptr[i + 1] < ms[m]->row_ptr[i]) return fail(G16_ERR_BAD_ARGUMENT, "row_ptr must be non-decreasing");
+        if (x->row_ptr[i + 1] < x->row_ptr[i]) return fail(G16_ERR_BAD_ARGUMENT, "row_ptr must be non-decreasing");
+      const uint32_t nnz = x->row_ptr[nc];
+      if (nnz && (!x->col || !x->val)) return fail(G16_ERR_BAD_ARGUMENT, "null col/val");
+      for (uint32_t e = 0; e < nnz; e++) if (x->col[e] >= nvars) return fail(G16_ERR_BAD_ARGUMENT, "column index out of range");
+    }
+    drop_key();
+    have_circuit = false;
+    for (int m = 0; m < 3; m++) {
       const uint32_t nnz = ms[m]->row_ptr[nc];
-      if (nnz && (!ms[m]->col || !ms[m]->val)) return fail(G16_ERR_BAD_ARGUMENT, "null col/val");
-      for (uint32_t e = 0; e < nnz; e++) if (ms[m]->col[e] >= nvars) return fail(G16_ERR_BAD_ARGUMENT, "column index out of range");
       h_rp[m].assign(ms[m]->row_ptr, ms[m]->row_ptr + nc + 1);
       h_col[m].assign(ms[m]->col, ms[m]->col + nnz);
       h_val[m].resize(nnz);
@@ -846,39 +838,85 @@ struct Engine : IEngine {
     if ((rc = ensure_circuit_domain())) return rc;
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
     have_circuit = true;
-    have_pk = false;
-    tail_ready = false;
     return G16_OK;
   }
 
   // ---- proving key ----
-  void shard(Query& x, uint64_t pairs) {
-    x.pairs = pairs;
+  // A key is made resident in three steps, by g16_pk_load, g16_setup and g16_pk_load_serialized alike: begin_key checks
+  // the query lengths and only then drops the old key and reserves the new bases, the loader fills copy 0 of every query
+  // and sets the single points, commit_key finishes the queries and marks the key resident.  A failure between the two
+  // leaves no key resident.
+  //
+  // The only place the resident key and everything derived from it are dropped.  Waits first for the pool tasks that read
+  // the key points: the key products of g16_prove_assemble_prepare and of a slot's proof (also after a failed submit).
+  void drop_key() {
+    for (Slot& sl : slots)
+      for (auto* h : {&sl.helper, &sl.helper2})
+        if (*h) { (*h)->wait(); h->reset(); }
+    if (asm_helper) { asm_helper->wait(); asm_helper.reset(); }
+    have_pk = from_setup = tail_ready = asm_valid = share_b_sort = false;
+  }
+  Shard shard(uint64_t pairs, uint32_t rk, uint32_t wd, bool g2) const {
     // Interleaved (strided) split: rank k owns pairs k, k + world, ...  Contiguous ranges would be badly unbalanced
     // whenever the density of a query varies with the variable index (early variables of a circuit are used more often).
-    const uint64_t cnt = pairs > rank ? (pairs - rank + world - 1) / world : 0;
-    x.lo = rank;
-    x.hi = rank + cnt;
-    x.geom = with_k0(pick_geom(x.hi - x.lo), &x == &q[M_B2]);
+    const uint64_t cnt = pairs > rk ? (pairs - rk + wd - 1) / wd : 0;
+    return Shard{pairs, rk, rk + cnt, with_k0(pick_geom(cnt), g2)};
   }
   // sorted entries carry (copy * n + index) in 31 bits and offsets are 32-bit
-  bool geom_fits(const Query& x) const {
+  static bool geom_fits(const Shard& x) {
     return (uint64_t)x.geom.copies * (x.hi - x.lo) < (1ull << 31) && x.geom.max_entries < (1ull << 32);
+  }
+  // len: the raw lengths of the H, L, A, B1 and B2 queries (element 0 of A, B1 and B2 included).  Returns with nothing
+  // changed when the key cannot be made resident.
+  int begin_key(uint32_t rk, uint32_t wd, const uint64_t len[5]) {
+    if (len[M_A] < 1 || len[M_B1] < 1 || len[M_B2] < 1)
+      return fail(G16_ERR_MALFORMED_KEY, "a/b queries must hold at least the constant-one base");
+    // msm_bigint truncates to the shorter operand (SURVEY.md section 2a; relied upon at prover.rs:66)
+    const uint64_t nz1 = nvars() - 1;   // |input_assignment ++ aux_assignment|, prover.rs:85
+    const uint64_t pairs[5] = {std::min<uint64_t>(len[M_H], 1ull << L), std::min<uint64_t>(len[M_L], num_witness),
+                               std::min(len[M_A] - 1, nz1), std::min(len[M_B1] - 1, nz1), std::min(len[M_B2] - 1, nz1)};
+    Shard sh[5];
+    for (int m = 0; m < 5; m++) {
+      sh[m] = shard(pairs[m], rk, wd, m == M_B2);
+      if (!geom_fits(sh[m])) return fail(G16_ERR_BAD_ARGUMENT, "query too large for one GPU: shard it (world > 1) or raise G16_MSM_NE");
+    }
+    drop_key();
+    rank = rk; world = wd;
+    for (int m = 0; m < 5; m++) {
+      static_cast<Shard&>(q[m]) = sh[m];
+      const size_t esz = m == M_B2 ? sizeof(A2) : sizeof(A1);
+      G16_CUDA(q[m].bases.reserve((size_t)q[m].geom.copies * (q[m].hi - q[m].lo) * esz + 16));
+    }
+    return G16_OK;
+  }
+  // The only place a key becomes resident: copy 0 of every query's bases and alpha_g1, beta_g1, beta_g2 are in place.
+  int commit_key(const A1& a_q0, const A1& b1_q0, const A2& b2_q0, bool setup_key) {
+    int rc;
+    for (int m = 0; m < 5; m++)
+      if ((rc = (m == M_B2) ? finish_query<Fq2>(q[m]) : finish_query<Fq>(q[m]))) return rc;
+    set_tail_points(a_q0, b1_q0, b2_q0);
+    G16_CUDA(cudaStreamSynchronize(S0.st_main));
+    if ((rc = decide_b_sort_sharing())) return rc;
+    decide_ba_memory();
+    have_pk = true;
+    from_setup = setup_key;
+    return G16_OK;
   }
   template <class F>
   int upload_query(Query& x, const uint64_t* host_full, uint64_t skip_first) {
     using AT = Affine<F>;
     const uint64_t cnt = x.hi - x.lo;
-    G16_CUDA(x.bases.reserve((size_t)x.geom.copies * cnt * sizeof(AT) + 16));
     if (cnt) {
       const size_t limbs = sizeof(AT) / 8;
       // gather every world-th point of the full host array
       G16_CUDA(cudaMemcpy2DAsync(x.bases.p, sizeof(AT), host_full + (skip_first + x.lo) * limbs, (size_t)world * sizeof(AT), sizeof(AT), cnt,
                                  cudaMemcpyHostToDevice, S0.st_main));
     }
-    return finish_query<F>(x);
+    return G16_OK;
   }
   uint64_t nvars() const { return (uint64_t)num_inputs + num_witness; }
+  // H query length of the resident circuit's keys: n - 1 points, n under CircomReduction
+  uint64_t h_query_len() const { return qap == G16_QAP_CIRCOM ? 1ull << L : (1ull << L) - 1; }
   // a_q0, b1_q0, b2_q0: element 0 of a_query, b_g1_query, b_g2_query; alpha_g1, beta_g1, beta_g2 already set
   void set_tail_points(const A1& a_q0, const A1& b1_q0, const A2& b2_q0) {
     P1 pa = P1::from_affine(a_q0), pb = P1::from_affine(b1_q0);
@@ -896,22 +934,11 @@ struct Engine : IEngine {
     G16_NOT_BUSY();
     if (!pk->a_query || !pk->b_g1_query || !pk->b_g2_query || !pk->alpha_g1 || !pk->beta_g1 || !pk->delta_g1 || !pk->beta_g2 || !pk->delta_g2)
       return fail(G16_ERR_BAD_ARGUMENT, "null pk member");
-    if (pk->a_len < 1 || pk->b_g1_len < 1 || pk->b_g2_len < 1) return fail(G16_ERR_MALFORMED_KEY, "a/b queries must hold at least the constant-one base");
     if ((pk->h_len && !pk->h_query) || (pk->l_len && !pk->l_query)) return fail(G16_ERR_BAD_ARGUMENT, "null h/l query");
     G16_CUDA(cudaSetDevice(device));
-    tail_ready = false;
-    rank = rk; world = wd;
-    const uint64_t n = 1ull << L;
-    const uint64_t nz1 = nvars() - 1;  // |input_assignment ++ aux_assignment|, prover.rs:85
-    // msm_bigint truncates to the shorter operand (SURVEY.md section 2a; relied upon at prover.rs:66)
-    shard(q[M_H], std::min<uint64_t>(pk->h_len, n));
-    shard(q[M_L], std::min<uint64_t>(pk->l_len, num_witness));
-    shard(q[M_A], std::min<uint64_t>(pk->a_len - 1, nz1));
-    shard(q[M_B1], std::min<uint64_t>(pk->b_g1_len - 1, nz1));
-    shard(q[M_B2], std::min<uint64_t>(pk->b_g2_len - 1, nz1));
-    for (int m = 0; m < 5; m++)
-      if (!geom_fits(q[m])) return fail(G16_ERR_BAD_ARGUMENT, "query too large for one GPU: shard it (world > 1) or raise G16_MSM_NE");
-    int rc;
+    const uint64_t len[5] = {pk->h_len, pk->l_len, pk->a_len, pk->b_g1_len, pk->b_g2_len};
+    int rc = begin_key(rk, wd, len);
+    if (rc) return rc;
     if ((rc = upload_query<Fq>(q[M_H], pk->h_query, 0))) return rc;
     if ((rc = upload_query<Fq>(q[M_L], pk->l_query, 0))) return rc;
     if ((rc = upload_query<Fq>(q[M_A], pk->a_query, 1))) return rc;
@@ -919,13 +946,7 @@ struct Engine : IEngine {
     if ((rc = upload_query<Fq2>(q[M_B2], pk->b_g2_query, 1))) return rc;
     alpha_g1 = load_a1(pk->alpha_g1); beta_g1 = load_a1(pk->beta_g1); delta_g1 = load_a1(pk->delta_g1);
     beta_g2 = load_a2(pk->beta_g2); delta_g2 = load_a2(pk->delta_g2);
-    set_tail_points(load_a1(pk->a_query), load_a1(pk->b_g1_query), load_a2(pk->b_g2_query));
-    G16_CUDA(cudaStreamSynchronize(S0.st_main));
-    have_pk = true;
-    from_setup = false;
-    if ((rc = decide_b_sort_sharing())) return rc;
-    decide_ba_memory();
-    return G16_OK;
+    return commit_key(load_a1(pk->a_query), load_a1(pk->b_g1_query), load_a2(pk->b_g2_query), false);
   }
 
   // ---- setup (generator.rs:47-208) ----
@@ -981,7 +1002,7 @@ struct Engine : IEngine {
           dst = Fr::add(dst, Fr::mul(u[i], h_val[m][e]));                          // r1cs_to_qap.rs:157-167
         }
     const Fr gi = Fr::inv(gamma), di = Fr::inv(delta);
-    const uint64_t hn = circom ? n : n - 1;   // H query length
+    const uint64_t hn = h_query_len();
     std::vector<Fr> gabc(ni), lq(num_witness), hs(hn);
     for (uint64_t i = 0; i < nv; i++) {
       const Fr t = Fr::add(Fr::add(Fr::mul(beta, qa[i]), Fr::mul(alpha, qb[i])), qc[i]);
@@ -995,46 +1016,39 @@ struct Engine : IEngine {
       circom_h_scalars(tau, tn, di, hs);
     }
     // --- fixed-base batch multiplications on the GPU (generator.rs:129-183) ---
-    tail_ready = false;
-    rank = 0; world = 1;
-    DevBuf d_s, tab1, tab2;
-    const uint64_t maxs = std::max<uint64_t>(nv, n);
-    G16_CUDA(d_s.reserve(maxs * sizeof(Fr)));
-    int rc;
-    auto up = [&](const std::vector<Fr>& v) -> cudaError_t {
-      return v.empty() ? cudaSuccess : cudaMemcpyAsync(d_s.p, v.data(), v.size() * sizeof(Fr), cudaMemcpyHostToDevice, S0.st_main);
-    };
-    G16_CUDA(full_a.reserve(nv * sizeof(A1))); G16_CUDA(full_b1.reserve(nv * sizeof(A1))); G16_CUDA(full_b2.reserve(nv * sizeof(A2)));
-    G16_CUDA(d_gamma_abc.reserve((size_t)ni * sizeof(A1)));
-    shard(q[M_H], hn); shard(q[M_L], num_witness); shard(q[M_A], nv - 1); shard(q[M_B1], nv - 1); shard(q[M_B2], nv - 1);
-    G16_CUDA(q[M_H].bases.reserve((size_t)q[M_H].geom.copies * hn * sizeof(A1) + 16));
-    G16_CUDA(q[M_L].bases.reserve((size_t)q[M_L].geom.copies * num_witness * sizeof(A1) + 16));
-    // a_query / b_g1_query / b_g2_query
-    G16_CUDA(up(qa)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), nv, full_a.template as<A1>(), tab1))) return rc;
-    G16_CUDA(cudaStreamSynchronize(S0.st_main));
-    G16_CUDA(up(qb)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), nv, full_b1.template as<A1>(), tab1))) return rc;
-    if ((rc = batch_mul<Fq2>(g2, d_s.template as<Fr>(), nv, full_b2.template as<A2>(), tab2))) return rc;
-    G16_CUDA(cudaStreamSynchronize(S0.st_main));
-    G16_CUDA(up(hs)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), hn, q[M_H].bases.template as<A1>(), tab1))) return rc;
-    G16_CUDA(cudaStreamSynchronize(S0.st_main));
-    G16_CUDA(up(lq)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), num_witness, q[M_L].bases.template as<A1>(), tab1))) return rc;
-    G16_CUDA(cudaStreamSynchronize(S0.st_main));
-    G16_CUDA(up(gabc)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), ni, d_gamma_abc.template as<A1>(), tab1))) return rc;
-    G16_CUDA(cudaStreamSynchronize(S0.st_main));
-    // MSM views: query[1..]
-    auto view = [&](Query& x, DevBuf& full, size_t esz) -> int {
-      G16_CUDA(x.bases.reserve((size_t)x.geom.copies * (nv - 1) * esz + 16));
-      if (nv > 1) G16_CUDA(cudaMemcpyAsync(x.bases.p, (char*)full.p + esz, (nv - 1) * esz, cudaMemcpyDeviceToDevice, S0.st_main));
-      return G16_OK;
-    };
-    if ((rc = view(q[M_A], full_a, sizeof(A1)))) return rc;
-    if ((rc = view(q[M_B1], full_b1, sizeof(A1)))) return rc;
-    if ((rc = view(q[M_B2], full_b2, sizeof(A2)))) return rc;
-    for (int m = 0; m < 5; m++) {
-      if ((rc = (m == M_B2) ? finish_query<Fq2>(q[m]) : finish_query<Fq>(q[m]))) return rc;
-    }
+    const uint64_t len[5] = {hn, num_witness, nv, nv, nv};
+    int rc = begin_key(0, 1, len);
+    if (rc) return rc;
     A1 a_q0, b1_q0;
     A2 b2_q0;
+    {   // the scalars and tables are freed before commit_key weighs the free memory
+      DevBuf d_s, tab1, tab2;
+      G16_CUDA(d_s.reserve(std::max<uint64_t>(nv, n) * sizeof(Fr)));
+      auto up = [&](const std::vector<Fr>& v) -> cudaError_t {
+        return v.empty() ? cudaSuccess : cudaMemcpyAsync(d_s.p, v.data(), v.size() * sizeof(Fr), cudaMemcpyHostToDevice, S0.st_main);
+      };
+      G16_CUDA(full_a.reserve(nv * sizeof(A1))); G16_CUDA(full_b1.reserve(nv * sizeof(A1))); G16_CUDA(full_b2.reserve(nv * sizeof(A2)));
+      G16_CUDA(d_gamma_abc.reserve((size_t)ni * sizeof(A1)));
+      // a_query / b_g1_query / b_g2_query
+      G16_CUDA(up(qa)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), nv, full_a.template as<A1>(), tab1))) return rc;
+      G16_CUDA(cudaStreamSynchronize(S0.st_main));
+      G16_CUDA(up(qb)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), nv, full_b1.template as<A1>(), tab1))) return rc;
+      if ((rc = batch_mul<Fq2>(g2, d_s.template as<Fr>(), nv, full_b2.template as<A2>(), tab2))) return rc;
+      G16_CUDA(cudaStreamSynchronize(S0.st_main));
+      G16_CUDA(up(hs)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), hn, q[M_H].bases.template as<A1>(), tab1))) return rc;
+      G16_CUDA(cudaStreamSynchronize(S0.st_main));
+      G16_CUDA(up(lq)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), num_witness, q[M_L].bases.template as<A1>(), tab1))) return rc;
+      G16_CUDA(cudaStreamSynchronize(S0.st_main));
+      G16_CUDA(up(gabc)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), ni, d_gamma_abc.template as<A1>(), tab1))) return rc;
+      G16_CUDA(cudaStreamSynchronize(S0.st_main));
+    }
+    // MSM views: query[1..]
+    auto view = [&](Query& x, const DevBuf& full, size_t esz) {
+      return nv > 1 ? cudaMemcpyAsync(x.bases.p, (char*)full.p + esz, (nv - 1) * esz, cudaMemcpyDeviceToDevice, S0.st_main) : cudaSuccess;
+    };
+    G16_CUDA(view(q[M_A], full_a, sizeof(A1)));
+    G16_CUDA(view(q[M_B1], full_b1, sizeof(A1)));
+    G16_CUDA(view(q[M_B2], full_b2, sizeof(A2)));
     G16_CUDA(cudaMemcpyAsync(&a_q0, full_a.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
     G16_CUDA(cudaMemcpyAsync(&b1_q0, full_b1.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
     G16_CUDA(cudaMemcpyAsync(&b2_q0, full_b2.p, sizeof(A2), cudaMemcpyDeviceToHost, S0.st_main));
@@ -1045,13 +1059,7 @@ struct Engine : IEngine {
     auto mul2 = [&](const Fr& s) { fr_to_canon(s, k); return P2::from_affine(g2).mul_u32(k, Fr::N).to_affine(); };
     alpha_g1 = mul1(alpha); beta_g1 = mul1(beta); delta_g1 = mul1(delta);
     beta_g2 = mul2(beta); gamma_g2 = mul2(gamma); delta_g2 = mul2(delta);
-    set_tail_points(a_q0, b1_q0, b2_q0);
-    d_s.release(); tab1.release(); tab2.release();
-    have_pk = true;
-    from_setup = true;
-    if ((rc = decide_b_sort_sharing())) return rc;
-    decide_ba_memory();
-    return G16_OK;
+    return commit_key(a_q0, b1_q0, b2_q0, true);
   }
   // CircomReduction::h_query_scalars(n - 1, tau, _, delta^-1): the odd entries 1, 3, .., 2n - 1 of the size-2n ifft of
   // v[i] = delta^-1 tau^i (i < 2n - 1), v[2n - 1] = 0.  With w = omega_2n, k = 2j + 1 and the geometric sum in closed form:
@@ -1083,21 +1091,24 @@ struct Engine : IEngine {
     if (!have_pk || !from_setup) return fail(G16_ERR_BAD_ARGUMENT, "g16_pk_export needs a key produced by g16_setup");
     if (!o) return fail(G16_ERR_BAD_ARGUMENT, "null");
     G16_CUDA(cudaSetDevice(device));
-    const uint64_t nv = nvars(), n = 1ull << L;
+    const uint64_t nv = nvars(), hn = h_query_len();
     if (o->a_query) G16_CUDA(cudaMemcpy(o->a_query, full_a.p, nv * sizeof(A1), cudaMemcpyDeviceToHost));
     if (o->b_g1_query) G16_CUDA(cudaMemcpy(o->b_g1_query, full_b1.p, nv * sizeof(A1), cudaMemcpyDeviceToHost));
     if (o->b_g2_query) G16_CUDA(cudaMemcpy(o->b_g2_query, full_b2.p, nv * sizeof(A2), cudaMemcpyDeviceToHost));
-    const uint64_t hn = qap == G16_QAP_CIRCOM ? n : n - 1;
     if (o->h_query && hn) G16_CUDA(cudaMemcpy(o->h_query, q[M_H].bases.p, hn * sizeof(A1), cudaMemcpyDeviceToHost));
     if (o->l_query && num_witness) G16_CUDA(cudaMemcpy(o->l_query, q[M_L].bases.p, (size_t)num_witness * sizeof(A1), cudaMemcpyDeviceToHost));
     if (o->gamma_abc_g1) G16_CUDA(cudaMemcpy(o->gamma_abc_g1, d_gamma_abc.p, (size_t)num_inputs * sizeof(A1), cudaMemcpyDeviceToHost));
+    store_vk_points(o, gamma_g2);
+    return G16_OK;
+  }
+  // the verifying key's six single points into the non-null members of o
+  void store_vk_points(const g16_pk_export_desc* o, const A2& gamma) const {
     if (o->alpha_g1) store_a1(o->alpha_g1, alpha_g1);
     if (o->beta_g1) store_a1(o->beta_g1, beta_g1);
     if (o->delta_g1) store_a1(o->delta_g1, delta_g1);
     if (o->beta_g2) store_a2(o->beta_g2, beta_g2);
-    if (o->gamma_g2) store_a2(o->gamma_g2, gamma_g2);
+    if (o->gamma_g2) store_a2(o->gamma_g2, gamma);
     if (o->delta_g2) store_a2(o->delta_g2, delta_g2);
-    return G16_OK;
   }
 
   // ---- ark-serialized proving keys (ser.cuh) ----
@@ -1116,12 +1127,9 @@ struct Engine : IEngine {
         if (ev_h2d[k]) cudaEventDestroy(ev_h2d[k]);
         if (ev_dec[k]) cudaEventDestroy(ev_dec[k]);
         if (host[k]) cudaFreeHost(host[k]);
-        dev[k].release();
       }
       if (st_dec) cudaStreamDestroy(st_dec);
       if (st_copy) cudaStreamDestroy(st_copy);
-      aux.release();
-      err.release();
     }
   };
   int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rk, uint32_t wd,
@@ -1134,32 +1142,16 @@ struct Engine : IEngine {
       return fail(G16_ERR_BAD_ARGUMENT, "vk_out receives the verifying key only: its query members must be NULL");
     G16_NOT_BUSY();
     G16_CUDA(cudaSetDevice(device));
-    // from here on a rejected key leaves no key resident
-    have_pk = false;
-    from_setup = false;
-    tail_ready = false;
+    drop_key();   // from here on a rejected key leaves no key resident
     SerItem it[SER_ITEMS];
     const std::string why = ser_walk(bytes, len, Fmt::NB, flags & G16_SER_COMPRESSED, it, Fmt::G2_NC);
     if (!why.empty()) return fail(G16_ERR_INVALID_DATA, why);
-    if (it[SER_A].len < 1 || it[SER_B_G1].len < 1 || it[SER_B_G2].len < 1)
-      return fail(G16_ERR_MALFORMED_KEY, "a/b queries must hold at least the constant-one base");
     if (it[SER_GAMMA_ABC].len != num_inputs)
       return fail(G16_ERR_MALFORMED_KEY, "vk.gamma_abc_g1 holds " + std::to_string(it[SER_GAMMA_ABC].len) +
                                              " points, the circuit has " + std::to_string(num_inputs) + " instance variables");
-    rank = rk; world = wd;
-    const uint64_t n = 1ull << L;
-    const uint64_t nz1 = nvars() - 1;
-    // the same truncation and shards as g16_pk_load
-    shard(q[M_H], std::min<uint64_t>(it[SER_H].len, n));
-    shard(q[M_L], std::min<uint64_t>(it[SER_L].len, num_witness));
-    shard(q[M_A], std::min<uint64_t>(it[SER_A].len - 1, nz1));
-    shard(q[M_B1], std::min<uint64_t>(it[SER_B_G1].len - 1, nz1));
-    shard(q[M_B2], std::min<uint64_t>(it[SER_B_G2].len - 1, nz1));
-    for (int m = 0; m < 5; m++) {
-      if (!geom_fits(q[m])) return fail(G16_ERR_BAD_ARGUMENT, "query too large for one GPU: shard it (world > 1) or raise G16_MSM_NE");
-      const size_t esz = m == M_B2 ? sizeof(A2) : sizeof(A1);
-      G16_CUDA(q[m].bases.reserve((size_t)q[m].geom.copies * (q[m].hi - q[m].lo) * esz + 16));
-    }
+    const uint64_t qlen[5] = {it[SER_H].len, it[SER_L].len, it[SER_A].len, it[SER_B_G1].len, it[SER_B_G2].len};
+    int rc = begin_key(rk, wd, qlen);   // the same truncation and shards as g16_pk_load
+    if (rc) return rc;
     // host-bound points: the seven single points, element 0 of a / b_g1 / b_g2, gamma_abc_g1
     enum { AUX_A0 = 7, AUX_B10 = 8, AUX_B20 = 9, AUX_ABC = 10 };
     const size_t aux_bytes = AUX_ABC * sizeof(A2) + (size_t)num_inputs * sizeof(A1);
@@ -1226,21 +1218,9 @@ struct Engine : IEngine {
     auto a2 = [&](int slot) { A2 r; memcpy(&r, aux.data() + (size_t)slot * sizeof(A2), sizeof(A2)); return r; };
     alpha_g1 = a1(SER_ALPHA_G1); beta_g1 = a1(SER_BETA_G1); delta_g1 = a1(SER_DELTA_G1);
     beta_g2 = a2(SER_BETA_G2); delta_g2 = a2(SER_DELTA_G2);
-    int rc;
-    for (int m = 0; m < 5; m++)
-      if ((rc = (m == M_B2) ? finish_query<Fq2>(q[m]) : finish_query<Fq>(q[m]))) return rc;
-    set_tail_points(a1(AUX_A0), a1(AUX_B10), a2(AUX_B20));
-    G16_CUDA(cudaStreamSynchronize(S0.st_main));
-    have_pk = true;
-    if ((rc = decide_b_sort_sharing())) return rc;
-    decide_ba_memory();
+    if ((rc = commit_key(a1(AUX_A0), a1(AUX_B10), a2(AUX_B20), false))) return rc;
     if (vk) {
-      if (vk->alpha_g1) store_a1(vk->alpha_g1, alpha_g1);
-      if (vk->beta_g1) store_a1(vk->beta_g1, beta_g1);
-      if (vk->delta_g1) store_a1(vk->delta_g1, delta_g1);
-      if (vk->beta_g2) store_a2(vk->beta_g2, beta_g2);
-      if (vk->gamma_g2) store_a2(vk->gamma_g2, a2(SER_GAMMA_G2));
-      if (vk->delta_g2) store_a2(vk->delta_g2, delta_g2);
+      store_vk_points(vk, a2(SER_GAMMA_G2));
       if (vk->gamma_abc_g1)
         for (uint32_t i = 0; i < num_inputs; i++) {
           A1 p;
@@ -1256,12 +1236,12 @@ struct Engine : IEngine {
     if (!len_out) return fail(G16_ERR_BAD_ARGUMENT, "null len_out");
     if (flags & ~(uint32_t)G16_SER_COMPRESSED) return fail(G16_ERR_BAD_ARGUMENT, "export takes G16_SER_COMPRESSED only");
     G16_NOT_BUSY();
-    const uint64_t nv = nvars(), n = 1ull << L;
+    const uint64_t nv = nvars();
     SerItem it[SER_ITEMS];
     ser_items(it);
     it[SER_GAMMA_ABC].len = num_inputs;
     it[SER_A].len = it[SER_B_G1].len = it[SER_B_G2].len = nv;
-    it[SER_H].len = qap == G16_QAP_CIRCOM ? n : n - 1;
+    it[SER_H].len = h_query_len();
     it[SER_L].len = num_witness;
     const uint64_t size = ser_size(it, Fmt::NB, flags & G16_SER_COMPRESSED, Fmt::G2_NC);
     *len_out = size;
@@ -1275,8 +1255,8 @@ struct Engine : IEngine {
     src[SER_GAMMA_ABC] = d_gamma_abc.p; src[SER_A] = full_a.p; src[SER_B_G1] = full_b1.p; src[SER_B_G2] = full_b2.p;
     src[SER_H] = q[M_H].bases.p; src[SER_L] = q[M_L].bases.p;
     DevBuf stage;
-    int rc = G16_OK;
-    for (int m = 0; m < SER_ITEMS && rc == G16_OK; m++) {
+    G16_CUDA(stage.reserve((size_t)SER_CHUNK * 4 * Fmt::NB));
+    for (int m = 0; m < SER_ITEMS; m++) {
       const SerItem& x = it[m];
       if (!x.vec) {   // a single point: encoded here, with the kernel's own function
         if (x.g2) ser_encode<CP, true>(g2s[m], flags, out + x.off);
@@ -1285,21 +1265,16 @@ struct Engine : IEngine {
       }
       for (int k = 0; k < 8; k++) out[x.off - 8 + k] = (uint8_t)(x.len >> (8 * k));
       const size_t esz = x.g2 ? sizeof(A2) : sizeof(A1);
-      for (uint64_t f = 0; f < x.len && rc == G16_OK; f += SER_CHUNK) {
+      for (uint64_t f = 0; f < x.len; f += SER_CHUNK) {
         const uint32_t cnt = (uint32_t)std::min<uint64_t>(SER_CHUNK, x.len - f);
-        cudaError_t e = stage.reserve((size_t)SER_CHUNK * 4 * Fmt::NB);
         const void* s = (const char*)src[m] + f * esz;
-        if (e == cudaSuccess)
-          e = x.g2 ? ser_encode_enqueue<CP, true>(S0.st_main, s, cnt, flags, stage.template as<uint8_t>())
-                   : ser_encode_enqueue<CP, false>(S0.st_main, s, cnt, flags, stage.template as<uint8_t>());
-        if (e == cudaSuccess)
-          e = cudaMemcpyAsync(out + x.off + f * x.psize, stage.p, (size_t)cnt * x.psize, cudaMemcpyDeviceToHost, S0.st_main);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(S0.st_main);
-        if (e != cudaSuccess) rc = fail(G16_ERR_CUDA, std::string("pk_export_serialized: ") + cudaGetErrorString(e));
+        G16_CUDA((x.g2 ? ser_encode_enqueue<CP, true>(S0.st_main, s, cnt, flags, stage.template as<uint8_t>())
+                       : ser_encode_enqueue<CP, false>(S0.st_main, s, cnt, flags, stage.template as<uint8_t>())));
+        G16_CUDA(cudaMemcpyAsync(out + x.off + f * x.psize, stage.p, (size_t)cnt * x.psize, cudaMemcpyDeviceToHost, S0.st_main));
+        G16_CUDA(cudaStreamSynchronize(S0.st_main));
       }
     }
-    stage.release();
-    return rc;
+    return G16_OK;
   }
 
   // ---- proving ----
@@ -1874,7 +1849,7 @@ struct Engine : IEngine {
   // (g16_prove_assemble_prepare), so that they overlap the GPU work and the gather; prove_assemble picks them up.
   Fr asm_r, asm_s;
   Products asm_kp;
-  bool asm_valid = false;
+  bool asm_valid = false;   // asm_kp belongs to (asm_r, asm_s) under the resident key
   std::shared_ptr<HostPool::Ticket> asm_helper;
   int assemble_prepare(const uint64_t* r, const uint64_t* s) override {
     if (!have_pk) return fail(G16_ERR_BAD_ARGUMENT, "no proving key resident");
@@ -1902,7 +1877,6 @@ struct Engine : IEngine {
     }
     const Fr rr = load_fr(r), ss = load_fr(s);
     const bool prepared = asm_valid && rr == asm_r && ss == asm_s;
-    if (prepared) asm_valid = false;
     store_proof(proof, prepared ? asm_kp : key_products(rr, ss), x.a, x.b2, c_part(rr, ss, x));
     return G16_OK;
   }

@@ -573,9 +573,22 @@ __global__ void __launch_bounds__(128) msm_precompute(const Affine<F>* in, uint3
 // ------------------------------------------------------------------------------------------------
 // host driver
 // ------------------------------------------------------------------------------------------------
-struct DevBuf {
+struct DevBuf {   // owns one device allocation: freed when the buffer goes out of scope, moved but never copied
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) {
+      release();
+      p = o.p; cap = o.cap;
+      o.p = nullptr; o.cap = 0;
+    }
+    return *this;
+  }
+  ~DevBuf() { release(); }
   cudaError_t reserve(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
     if (p) cudaFree(p);
@@ -751,16 +764,9 @@ struct MsmWorkspace {
 #undef G16_TRY
     return cudaSuccess;
   }
-  void release() {
-    counters.release(); offsets.release(); blocktot.release(); sidx.release(); skey.release(); buckets.release();
-    pk0.release(); pp0.release(); pk1.release(); pp1.release(); pending.release(); red_inner.release(); red_leaf.release();
-    ba_pre.release(); ba_prod.release(); ba_pre2.release();
-    ba_l0.release(); ba_l1.release();
+  ~MsmWorkspace() {   // the DevBuf members free themselves
     if (h_leaf) cudaFreeHost(h_leaf);
     if (h_total) cudaFreeHost(h_total);
-    h_leaf = nullptr;
-    h_total = nullptr;
-    h_cap = 0;
   }
 };
 

@@ -86,7 +86,10 @@ int g16_msm_g2(g16_ctx* ctx, const uint64_t* bases, const uint64_t* scalars, uin
 /* ---- constraint matrices: ark-relations ConstraintMatrices as consumed by
  * R1CSToQAP::witness_map_from_matrices (r1cs_to_qap.rs:172-199,213-218).  CSR per matrix: row_ptr has
  * num_constraints+1 entries, col[e] indexes the full assignment (instance first), val[e] is Montgomery Fr.
- * Uploaded once per circuit and kept resident. */
+ * Uploaded once per circuit and kept resident.  g16_circuit_load checks all three matrices (row_ptr starts at 0 and never
+ * decreases, col / val are not null where entries exist, every column is below num_inputs + num_witness) before it
+ * touches anything resident: a rejected circuit leaves the previous circuit and its key resident.  A circuit that passes
+ * drops the resident key; a failure while it is uploaded leaves neither a circuit nor a key resident. */
 typedef struct {
   const uint32_t* row_ptr;
   const uint32_t* col;
@@ -119,7 +122,10 @@ int g16_circuit_load_qap(g16_ctx* ctx, int qap, uint32_t num_inputs, uint32_t nu
 
 /* ---- proving key: data_structures.rs:126-143.  Query arrays are the FULL ark vectors (a_query[0] included).
  * With world > 1 the context keeps only the index range of every query owned by `rank` (SURVEY.md section 8e):
- * round-robin split of each MSM's (base, scalar) pairs: pair i belongs to rank i mod world. */
+ * round-robin split of each MSM's (base, scalar) pairs: pair i belongs to rank i mod world.
+ * g16_pk_load and g16_setup check their arguments and the query lengths (an empty a/b query is G16_ERR_MALFORMED_KEY) before
+ * they release the resident key: a key rejected there leaves the previous key resident.  A failure after that leaves no key
+ * resident. */
 typedef struct {
   const uint64_t* a_query;    uint64_t a_len;     /* G1, num_inputs + num_witness      (generator.rs:155) */
   const uint64_t* b_g1_query; uint64_t b_g1_len;  /* G1, same length                   (generator.rs:161) */
@@ -192,7 +198,8 @@ int g16_prove_partial(g16_ctx* ctx, const uint64_t* r, const uint64_t* full_assi
 int g16_prove_assemble(g16_ctx* ctx, const uint64_t* r, const uint64_t* s, const uint64_t* partials,
                        uint32_t nparts, uint64_t* proof_out);
 /* Optional: start the (r, s)-only scalar multiplications of prover.rs:76,90,100,112 on a helper thread before the partial
- * sums exist; the next g16_prove_assemble with the same (r, s) picks the result up instead of computing it inline. */
+ * sums exist; the next g16_prove_assemble with the same (r, s) picks the result up instead of computing it inline.
+ * Loading a circuit or a key (g16_circuit_load, g16_pk_load, g16_setup, g16_pk_load_serialized) discards the result. */
 int g16_prove_assemble_prepare(g16_ctx* ctx, const uint64_t* r, const uint64_t* s);
 /* Pipelined proving: a context owns two proof slots (0 and 1), each with its own streams and work buffers.
  * g16_prove_submit enqueues a whole proof asynchronously and returns; g16_prove_wait blocks until that slot's GPU
