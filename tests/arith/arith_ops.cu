@@ -20,15 +20,16 @@ using namespace g16;
 
 namespace {
 
-// fields: 0..5 Fp (Fr, Fq of BLS12-381, BN254, BLS12-377), 6..8 Fq2 of the same three curves; the point ops run on G1
-// (coordinates in fields 1, 3, 5) and G2 (fields 6, 7, 8)
+// fields: 0..5 Fp (Fr, Fq of BLS12-381, BN254, BLS12-377), 6..8 Fq2 of the same three curves, 9 and 10 Fp (Fr, Fq of
+// BW6-761); the point ops run on G1 (coordinates in fields 1, 3, 5, 10) and G2 (fields 6, 7, 8, and 10: BW6-761's G2 is
+// over Fq)
 enum Op {
   ADD = 0, SUB = 1, NEG = 2, DBL = 3, MUL = 4, SQR = 5, MUL_SMALL = 6, FROM_MONT = 7, TO_MONT = 8, POW_U64 = 9, INV = 10,
   INV_GCD = 11, MUL_NR = 12, BA_INV = 13,
   MADD = 20, MADD_NEG = 21, MADD_LAZY = 22, MADD_LAZY_NEG = 23, PADD = 24, PDBL = 25, PDBL_AFFINE = 26, PMUL_U32 = 27,
   TO_AFFINE = 28,
 };
-constexpr int NUM_FIELDS = 9;
+constexpr int NUM_FIELDS = 11;
 
 template <class T>
 G16_HD T ld(const uint32_t* p) {
@@ -43,8 +44,9 @@ G16_HD void st(uint32_t* p, const T& t) {
   for (int i = 0; i < (int)(sizeof(T) / 4); i++) p[i] = s[i];
 }
 
-// Vector layouts (E = words of one coordinate):  XYZZ = X Y ZZ ZZZ (4E), affine = x y (2E), scalar = 8 words LE.
-template <class F>
+// Vector layouts (E = words of one coordinate):  XYZZ = X Y ZZ ZZZ (4E), affine = x y (2E), scalar = SW words LE (the
+// curve's Fr::N, as the engine passes to mul_u32).
+template <class F, int SW>
 G16_HD bool point_op(int op, const uint32_t* in, uint32_t* out) {
   constexpr int E = sizeof(F) / 4;
   using X = XYZZ<F>;
@@ -78,13 +80,14 @@ G16_HD bool point_op(int op, const uint32_t* in, uint32_t* out) {
       return true;
     }
     case PDBL_AFFINE: st(out, X::dbl_affine(ld<A>(in))); return true;
-    case PMUL_U32: st(out, ld<X>(in).mul_u32(in + 4 * E, 8)); return true;
+    case PMUL_U32: st(out, ld<X>(in).mul_u32(in + 4 * E, SW)); return true;
     case TO_AFFINE: st(out, ld<X>(in).to_affine()); return true;
   }
   return false;
 }
 
-template <class P>
+// SW: scalar words of the curve over a base field P (0 for a scalar field)
+template <class P, int SW = 0>
 G16_HD bool fp_op(int op, const uint32_t* in, uint32_t* out) {
   using F = Fp<P>;
   constexpr int E = P::N;
@@ -102,11 +105,14 @@ G16_HD bool fp_op(int op, const uint32_t* in, uint32_t* out) {
     case INV: st(out, F::inv(ld<F>(in))); return true;
     case INV_GCD: st(out, fp_inv_safegcd<P>(ld<F>(in))); return true;
   }
-  if constexpr (is_base_field<P>()) return point_op<F>(op, in, out);
+  if constexpr (is_base_field<P>()) {
+    if (op == BA_INV) { st(out, ba_inv(ld<F>(in), in[E] != 0)); return true; }
+    return point_op<F, SW>(op, in, out);
+  }
   return false;
 }
 
-template <class P, int NR>
+template <class P, int NR, int SW>
 G16_HD bool fq2_op(int op, const uint32_t* in, uint32_t* out) {
   using F = Fp2<P, NR>;
   constexpr int E = 2 * P::N;
@@ -121,25 +127,31 @@ G16_HD bool fq2_op(int op, const uint32_t* in, uint32_t* out) {
     case MUL_NR: st(out, F::mul_nr(ld<Fp<P>>(in))); return true;
     case BA_INV: st(out, ba_inv(ld<F>(in), in[E] != 0)); return true;
   }
-  return point_op<F>(op, in, out);
+  return point_op<F, SW>(op, in, out);
 }
 
 template <int FIELD>
 G16_HD bool run_one(int op, const uint32_t* in, uint32_t* out) {
   if constexpr (FIELD == 0) return fp_op<BLS381_FrP>(op, in, out);
-  else if constexpr (FIELD == 1) return fp_op<BLS381_FqP>(op, in, out);
+  else if constexpr (FIELD == 1) return fp_op<BLS381_FqP, BLS381_FrP::N>(op, in, out);
   else if constexpr (FIELD == 2) return fp_op<BN254_FrP>(op, in, out);
-  else if constexpr (FIELD == 3) return fp_op<BN254_FqP>(op, in, out);
+  else if constexpr (FIELD == 3) return fp_op<BN254_FqP, BN254_FrP::N>(op, in, out);
   else if constexpr (FIELD == 4) return fp_op<BLS377_FrP>(op, in, out);
-  else if constexpr (FIELD == 5) return fp_op<BLS377_FqP>(op, in, out);
-  else if constexpr (FIELD == 6) return fq2_op<BLS381_FqP, BLS381_Params::FQ2_NONRESIDUE_NEG>(op, in, out);
-  else if constexpr (FIELD == 7) return fq2_op<BN254_FqP, BN254_Params::FQ2_NONRESIDUE_NEG>(op, in, out);
-  else return fq2_op<BLS377_FqP, BLS377_Params::FQ2_NONRESIDUE_NEG>(op, in, out);
+  else if constexpr (FIELD == 5) return fp_op<BLS377_FqP, BLS377_FrP::N>(op, in, out);
+  else if constexpr (FIELD == 6) return fq2_op<BLS381_FqP, BLS381_Params::FQ2_NONRESIDUE_NEG, BLS381_FrP::N>(op, in, out);
+  else if constexpr (FIELD == 7) return fq2_op<BN254_FqP, BN254_Params::FQ2_NONRESIDUE_NEG, BN254_FrP::N>(op, in, out);
+  else if constexpr (FIELD == 8) return fq2_op<BLS377_FqP, BLS377_Params::FQ2_NONRESIDUE_NEG, BLS377_FrP::N>(op, in, out);
+  else if constexpr (FIELD == 9) return fp_op<BW6_FrP>(op, in, out);
+  else return fp_op<BW6_FqP, BW6_FrP::N>(op, in, out);
 }
 
 // words per element of each field
 constexpr int ELEM_WORDS[NUM_FIELDS] = {BLS381_FrP::N, BLS381_FqP::N, BN254_FrP::N, BN254_FqP::N, BLS377_FrP::N,
-                                        BLS377_FqP::N, 2 * BLS381_FqP::N, 2 * BN254_FqP::N, 2 * BLS377_FqP::N};
+                                        BLS377_FqP::N, 2 * BLS381_FqP::N, 2 * BN254_FqP::N, 2 * BLS377_FqP::N,
+                                        BW6_FrP::N, BW6_FqP::N};
+// words of a point-op scalar (the curve's Fr::N) for the fields that carry points, 0 for the others
+constexpr int SCALAR_WORDS[NUM_FIELDS] = {0, BLS381_FrP::N, 0, BN254_FrP::N, 0, BLS377_FrP::N, BLS381_FrP::N, BN254_FrP::N,
+                                          BLS377_FrP::N, 0, BW6_FrP::N};
 
 #ifdef __CUDACC__
 template <int FIELD>
@@ -177,8 +189,8 @@ int g16t_backend() {
 // words per vector of (field, op); returns -1 for a pair the harness does not run
 int g16t_shape(int field, int op, int* in_words, int* out_words) {
   if (field < 0 || field >= NUM_FIELDS) return -1;
-  const int E = ELEM_WORDS[field];
-  const bool fp = field < 6, fq2 = field >= 6, curve = fq2 || (field & 1);
+  const int E = ELEM_WORDS[field], SW = SCALAR_WORDS[field];
+  const bool fq2 = field >= 6 && field <= 8, fp = !fq2, curve = SW > 0;
   int i = -1, o = E;
   switch (op) {
     case ADD: case SUB: case MUL: i = 2 * E; break;
@@ -187,12 +199,12 @@ int g16t_shape(int field, int op, int* in_words, int* out_words) {
     case FROM_MONT: case TO_MONT: case INV_GCD: if (fp) i = E; break;
     case POW_U64: if (fp) i = E + 2; break;
     case MUL_NR: if (fq2) { i = E / 2; o = E / 2; } break;
-    case BA_INV: if (fq2) i = E + 1; break;
+    case BA_INV: if (curve) i = E + 1; break;
     case MADD: case MADD_NEG: case MADD_LAZY: case MADD_LAZY_NEG: if (curve) { i = 6 * E; o = 4 * E; } break;
     case PADD: if (curve) { i = 8 * E; o = 4 * E; } break;
     case PDBL: if (curve) { i = 4 * E; o = 4 * E; } break;
     case PDBL_AFFINE: if (curve) { i = 2 * E; o = 4 * E; } break;
-    case PMUL_U32: if (curve) { i = 4 * E + 8; o = 4 * E; } break;
+    case PMUL_U32: if (curve) { i = 4 * E + SW; o = 4 * E; } break;
     case TO_AFFINE: if (curve) { i = 4 * E; o = 2 * E; } break;
   }
   if (i < 0) return -1;
@@ -208,7 +220,8 @@ int g16t_run(int field, int op, const uint32_t* in, uint32_t* out, int64_t n) {
   if (n == 0) return 0;
   const size_t ib = (size_t)n * iw * 4, ob = (size_t)n * ow * 4;
   using Exec = void (*)(int, const uint32_t*, uint32_t*, int64_t, int, int);
-  static const Exec table[NUM_FIELDS] = {exec<0>, exec<1>, exec<2>, exec<3>, exec<4>, exec<5>, exec<6>, exec<7>, exec<8>};
+  static const Exec table[NUM_FIELDS] = {exec<0>, exec<1>, exec<2>, exec<3>, exec<4>, exec<5>,
+                                         exec<6>, exec<7>, exec<8>, exec<9>, exec<10>};
   const Exec run = table[field];
 #ifdef __CUDACC__
   uint32_t *din = nullptr, *dout = nullptr;

@@ -93,6 +93,50 @@ def msm(bases, scalars):
     return acc
 
 
+def _jdbl(X, Y, Z):
+    """2 (X : Y : Z) in Jacobian coordinates (a = 0; Z = 0 is the identity)"""
+    A, B = X * X % Q, Y * Y % Q
+    C = B * B % Q
+    D = 2 * ((X + B) ** 2 - A - C) % Q
+    E = 3 * A % Q
+    X3 = (E * E - 2 * D) % Q
+    return X3, (E * (D - X3) - 8 * C) % Q, 2 * Y * Z % Q
+
+
+def mul_proj(k, P):
+    """k P for any k >= 0 with one inversion: left-to-right double-and-add in Jacobian coordinates, adding the affine P"""
+    if P is None or k == 0:
+        return None
+    x, y = P
+    X, Y, Z = 0, 1, 0
+    for bit in bin(k)[2:]:
+        if Z:
+            X, Y, Z = _jdbl(X, Y, Z)
+        if bit == "1":
+            if not Z:
+                X, Y, Z = x, y, 1
+                continue
+            ZZ = Z * Z % Q
+            H = (x * ZZ - X) % Q
+            S = (y * ZZ * Z - Y) % Q
+            if H == 0:
+                if S == 0:
+                    X, Y, Z = _jdbl(X, Y, Z)
+                else:
+                    X, Y, Z = 0, 1, 0
+                continue
+            HH = H * H % Q
+            HHH = H * HH % Q
+            V = X * HH % Q
+            X3 = (S * S - HHH - 2 * V) % Q
+            X, Y, Z = X3, (S * (V - X3) - Y * HHH) % Q, Z * H % Q
+    if not Z:
+        return None
+    zi = pow(Z, -1, Q)
+    zi2 = zi * zi % Q
+    return X * zi2 % Q, Y * zi2 * zi % Q
+
+
 def sqrt_fq(a):
     y = pow(a, (Q + 1) // 4, Q)
     return y if y * y % Q == a % Q else None
@@ -178,35 +222,168 @@ def lagrange_at(tau, log_n):
     return out
 
 
-def expected_proof(rows, num_inputs, z, alpha, beta, delta, tau, r, s, g1, g2):
-    """A, B, C of a Groth16 proof (libsnark QAP; CircomReduction gives the same points) from the toxic waste:
-    A = [alpha + a(tau) + r delta]_1, B = [beta + b(tau) + s delta]_2,
-    C = [(sum_{i >= ni} z_i (beta a_i + alpha b_i + c_i)(tau) + a(tau) b(tau) - c(tau)) / delta + s A + r B - r s delta]_1
-    with x(tau) = sum_i z_i x_i(tau).  rows = (A, B, C), each a list of constraints [(coeff, var), ...]."""
-    nc = len(rows[0])
+def fft(vals, inverse=False, coset=False):
+    """the same transforms as `ntt` in O(n log n): iterative radix-2 over the bit-reversed input"""
+    n = len(vals)
+    L = n.bit_length() - 1
+    a = [v % R for v in vals]
+    if coset and not inverse:
+        gp = 1
+        for i in range(n):
+            a[i] = a[i] * gp % R
+            gp = gp * FR_GENERATOR % R
+    j = 0
+    for i in range(1, n):
+        bit = n >> 1
+        while j & bit:
+            j ^= bit
+            bit >>= 1
+        j |= bit
+        if i < j:
+            a[i], a[j] = a[j], a[i]
+    w = domain_root(L)
+    if inverse:
+        w = pow(w, -1, R)
+    m = 1
+    while m < n:
+        wm = pow(w, n // (2 * m), R)
+        tw = [1] * m
+        for k in range(1, m):
+            tw[k] = tw[k - 1] * wm % R
+        for st in range(0, n, 2 * m):
+            for k in range(m):
+                u, t = a[st + k], a[st + k + m] * tw[k] % R
+                a[st + k], a[st + k + m] = (u + t) % R, (u - t) % R
+        m *= 2
+    if inverse:
+        ni, gi = pow(n, -1, R), pow(FR_GENERATOR, -1, R) if coset else 1
+        c = ni
+        for i in range(n):
+            a[i] = a[i] * c % R
+            c = c * gi % R
+    return a
+
+
+def domain_size(rows, num_inputs):
+    """(n, log n) of the QAP domain: the constraints plus one instance copy per input"""
     n, L = 1, 0
-    while n < nc + num_inputs:
+    while n < len(rows[0]) + num_inputs:
         n, L = 2 * n, L + 1
-    lag = lagrange_at(tau, L)
-    ev = []       # a(tau), b(tau), c(tau)
-    inst = []     # sum_{i < ni} z_i x_i(tau)
+    return n, L
+
+
+def row_evals(rows, num_inputs, z):
+    """LibsnarkReduction's evaluations of A, B, C on the domain: row j of each matrix at z, the instance copy
+    a[nc + i] = z_i (r1cs_to_qap.rs), zero above"""
+    n, _ = domain_size(rows, num_inputs)
+    nc = len(rows[0])
+    out = []
     for m, mat in enumerate(rows):
-        tot, ins = 0, 0
-        for j, row in enumerate(mat):
-            v = sum(cf * z[var] for cf, var in row) % R
-            tot += lag[j] * v
-            ins += lag[j] * sum(cf * z[var] for cf, var in row if var < num_inputs)
-        if m == 0:   # the instance copy a[nc + i] = z_i (r1cs_to_qap.rs)
+        ev = [sum(cf * z[var] for cf, var in row) % R for row in mat] + [0] * (n - nc)
+        if m == 0:
             for i in range(num_inputs):
-                tot += lag[nc + i] * z[i]
-                ins += lag[nc + i] * z[i]
-        ev.append(tot % R)
-        inst.append(ins % R)
-    a_s = (alpha + ev[0] + r * delta) % R
-    b_s = (beta + ev[1] + s * delta) % R
-    wit = (beta * (ev[0] - inst[0]) + alpha * (ev[1] - inst[1]) + (ev[2] - inst[2])) % R
-    c_s = ((wit + ev[0] * ev[1] - ev[2]) * pow(delta, -1, R) + s * a_s + r * b_s - r * s * delta) % R
-    return mul(a_s, g1), mul(b_s, g2), mul(c_s, g1)
+                ev[nc + i] = z[i] % R
+        out.append(ev)
+    return out
+
+
+def witness_map(a, b, c):
+    """LibsnarkReduction's h (n coefficients) from the row evaluations: coset-ifft((A B - C) / Z) with X = coset-fft(ifft(x));
+    Z is g^n - 1 at every point of the coset"""
+    n = len(a)
+    ac, bc, cc = (fft(fft(x, inverse=True), coset=True) for x in (a, b, c))
+    zi = pow((pow(FR_GENERATOR, n, R) - 1) % R, -1, R)
+    return fft([(x * y - z) * zi % R for x, y, z in zip(ac, bc, cc)], inverse=True, coset=True)
+
+
+def query_exponents(rows, num_inputs, num_vars, alpha, beta, delta, tau):
+    """The discrete logs of the five queries of a key g16_setup makes from this toxic waste: every point is [d]G with
+    a: a_i(tau) and b: b_i(tau) for every variable (b_g1_query and b_g2_query alike), l: (beta a_i + alpha b_i + c_i)(tau) /
+    delta for i >= num_inputs, h: tau^i Z(tau) / delta for i < n - 1."""
+    n, L = domain_size(rows, num_inputs)
+    nc = len(rows[0])
+    lag = lagrange_at(tau, L)
+    q = [[0] * num_vars for _ in range(3)]
+    for m, mat in enumerate(rows):
+        for j, row in enumerate(mat):
+            for cf, var in row:
+                q[m][var] += lag[j] * cf
+    for i in range(num_inputs):
+        q[0][i] += lag[nc + i]
+    qa, qb, qc = ([v % R for v in x] for x in q)
+    di = pow(delta, -1, R)
+    zd = (pow(tau, n, R) - 1) * di % R
+    h, p = [], zd
+    for _ in range(n - 1):
+        h.append(p)
+        p = p * tau % R
+    return dict(a=qa, b=qb, l=[(beta * qa[i] + alpha * qb[i] + qc[i]) * di % R for i in range(num_inputs, num_vars)], h=h)
+
+
+def msm_exponents(d, h, z, num_inputs):
+    """The exponents of the prover's five MSMs over a key with discrete logs d (`query_exponents`, possibly edited): H over
+    the first n - 1 coefficients of h, L over the witness, A, B in G1 and B in G2 over every variable but the constant One"""
+    dot = lambda xs, ys: sum(x * y for x, y in zip(xs, ys)) % R
+    b1, b2 = (d[k] if k in d else d["b"] for k in ("b_g1", "b_g2"))   # one b for both groups unless edited apart
+    return dict(h=dot(d["h"], h), l=dot(d["l"], z[num_inputs:]), a=dot(d["a"][1:], z[1:]), b_g1=dot(b1[1:], z[1:]),
+                b_g2=dot(b2[1:], z[1:]))
+
+
+def proof_from_msms(e, d0, alpha, beta, delta, r, s):
+    """A, B, C exponents as the prover assembles them from its MSM exponents e and the first entries d0 = (a_0, b_g1_0,
+    b_g2_0) of the queries (the constant One): A = alpha + a + r delta, B = beta + b + s delta, C = h + l + s A + r B_1 -
+    r s delta"""
+    a_s = (alpha + d0[0] + e["a"] + r * delta) % R
+    b1 = (beta + d0[1] + e["b_g1"] + s * delta) % R
+    b_s = (beta + d0[2] + e["b_g2"] + s * delta) % R
+    return a_s, b_s, (e["h"] + e["l"] + s * a_s + r * b1 - r * s * delta) % R
+
+
+def proof_exponents(rows, num_inputs, z, alpha, beta, delta, tau, r, s):
+    """A, B, C of a Groth16 proof (libsnark QAP) as exponents of the generators, for ANY assignment z, in O(n):
+    A = alpha + a(tau) + r delta, B = beta + b(tau) + s delta, with x(tau) = sum_i z_i x_i(tau), and
+    C = sum_{i >= ni} z_i (beta a_i + alpha b_i + c_i)(tau) / delta + H + s A + r B - r s delta.
+    H is what the prover's H MSM gives, sum_{i < n-1} h_i tau^i Z(tau) / delta.  With the row evaluations e_j = a_j b_j - c_j
+    and rem(X) = sum_j e_j L_j(X) (a b - c mod Z), the witness map's h interpolates (a b - c) / (g^n - 1) on the coset, so
+    h = (a b - c - rem) / Z + rem / (g^n - 1), of degree < n, with top coefficient h_{n-1} = (sum_j e_j w^j) / (n (g^n - 1));
+    h_query has n - 1 points, so H = (h(tau) - h_{n-1} tau^{n-1}) Z(tau) / delta.  For a satisfying z, rem = 0 and
+    H = (a(tau) b(tau) - c(tau)) / delta."""
+    n, L = domain_size(rows, num_inputs)
+    lag = lagrange_at(tau, L)
+    ev = row_evals(rows, num_inputs, z)
+    at, bt, ct = (sum(l * v for l, v in zip(lag, e)) % R for e in ev)
+    # the instance part of a(tau), b(tau), c(tau): only z_i with i < ni, the instance copies included
+    inst = []
+    nc = len(rows[0])
+    for m, mat in enumerate(rows):
+        tot = sum(lag[j] * sum(cf * z[var] for cf, var in row if var < num_inputs) for j, row in enumerate(mat))
+        if m == 0:
+            tot += sum(lag[nc + i] * z[i] for i in range(num_inputs))
+        inst.append(tot % R)
+    e = [(x * y - w) % R for x, y, w in zip(*ev)]
+    rem = sum(l * v for l, v in zip(lag, e)) % R
+    w, wp, top = domain_root(L), 1, 0
+    for v in e:
+        top += v * wp
+        wp = wp * w % R
+    gn1 = (pow(FR_GENERATOR, n, R) - 1) % R
+    top = top * pow(n * gn1, -1, R) % R
+    zt = (pow(tau, n, R) - 1) % R
+    h_tau = ((at * bt - ct - rem) * pow(zt, -1, R) + rem * pow(gn1, -1, R)) % R
+    di = pow(delta, -1, R)
+    hh = (h_tau - top * pow(tau, n - 1, R)) * zt % R
+    a_s = (alpha + at + r * delta) % R
+    b_s = (beta + bt + s * delta) % R
+    wit = (beta * (at - inst[0]) + alpha * (bt - inst[1]) + (ct - inst[2])) % R
+    c_s = ((wit + hh) * di + s * a_s + r * b_s - r * s * delta) % R
+    return a_s, b_s, c_s
+
+
+def expected_proof(rows, num_inputs, z, alpha, beta, delta, tau, r, s, g1, g2):
+    """A, B, C of a Groth16 proof from the toxic waste (`proof_exponents`; CircomReduction gives the same points for a
+    satisfying z).  rows = (A, B, C), each a list of constraints [(coeff, var), ...]."""
+    a_s, b_s, c_s = proof_exponents(rows, num_inputs, z, alpha, beta, delta, tau, r, s)
+    return mul_proj(a_s, g1), mul_proj(b_s, g2), mul_proj(c_s, g1)
 
 
 def csr_rows(m):

@@ -1,5 +1,6 @@
-"""Element-level checks of the product arithmetic against Python big integers: every Fp operation of the six fields, the
-three Fq2 towers and the XYZZ point operations of G1 and G2, one operation per vector, compared bit for bit.
+"""Element-level checks of the product arithmetic against Python big integers: every Fp operation of the eight fields (Fr
+and Fq of BLS12-381, BN254, BLS12-377 and BW6-761), the three Fq2 towers and the XYZZ point operations of G1 and G2 of
+all four curves, one operation per vector, compared bit for bit.
 
 tests/arith/arith_ops.cu runs the templates of fp.cuh, ec.cuh, fp_inv.cuh and msm_ba.cuh themselves, built three ways:
 the plain 64-bit host back-end and the device algorithm under emulated PTX carries (CPU tests, built here with g++), and
@@ -11,7 +12,10 @@ They are chosen where this kind of arithmetic breaks -- 0, p - 1, (p +- 1)/2, R,
 p - 2^k, limb patterns, pairs whose top-limb partial product is 0xffffffff -- plus random values.  Point results are
 normalised here (x = X/ZZ, y = Y/ZZZ, identity <=> ZZ == 0, and ZZ^3 == ZZZ^2 for every finite result); the accumulators
 carry ZZ != 1 so that the doubling and inverse branches of the additions are reached from general projective inputs.
-Vectors are generated once per process from fixed seeds, and every (field, op) asserts a minimum vector count."""
+Vectors are generated once per process from fixed seeds, and every (field, op) asserts a minimum vector count.
+
+BW6-761 (12-limb Fr, 24-limb Fq, G1 and G2 both over Fq) has no pyref curve: its points are checked in value space over
+tests/bw6_ref.py, and its Fp cases run the same operand sets at 24 limbs."""
 import ctypes as C
 import functools
 import glob
@@ -23,7 +27,9 @@ import subprocess
 import numpy as np
 import pytest
 
+import bw6_ref as ref
 import pyref as P
+from groth16_b200.params import GENERATORS
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ARITH = os.path.join(ROOT, "tests", "arith")
@@ -31,12 +37,16 @@ SRC = os.path.join(ARITH, "arith_ops.cu")
 DEVICE_LIB = os.path.join(ARITH, "libg16arith.so")
 CSRC = os.path.join(ROOT, "groth16_b200", "csrc")
 
-CURVES = ("bls12_381", "bn254", "bls12_377")
+CURVES = ("bls12_381", "bn254", "bls12_377")   # the pairing curves (pyref)
+BW6 = "bw6_761"
+POINT_CURVES = CURVES + (BW6,)
 # op ids of arith_ops.cu
 ADD, SUB, NEG, DBL, MUL, SQR, MUL_SMALL, FROM_MONT, TO_MONT, POW_U64, INV, INV_GCD, MUL_NR, BA_INV = range(14)
 MADD, MADD_NEG, MADD_LAZY, MADD_LAZY_NEG, PADD, PDBL, PDBL_AFFINE, PMUL_U32, TO_AFFINE = range(20, 29)
 FP_OPS = {"add": ADD, "sub": SUB, "neg": NEG, "dbl": DBL, "mul": MUL, "sqr": SQR, "mul_small": MUL_SMALL,
-          "from_mont": FROM_MONT, "to_mont": TO_MONT, "pow_u64": POW_U64, "inv": INV, "inv_safegcd": INV_GCD}
+          "from_mont": FROM_MONT, "to_mont": TO_MONT, "pow_u64": POW_U64, "inv": INV, "inv_safegcd": INV_GCD,
+          "ba_inv": BA_INV}
+BASE_ONLY = {"ba_inv"}   # Fp ops that run on the base fields only (the batched-affine inversion of a G1 / BW6 G2 combine)
 FQ2_OPS = {"add": ADD, "sub": SUB, "neg": NEG, "dbl": DBL, "mul": MUL, "sqr": SQR, "mul_nr": MUL_NR, "inv": INV,
            "ba_inv": BA_INV}
 POINT_OPS = {"madd": MADD, "madd_neg": MADD_NEG, "madd_lazy": MADD_LAZY, "madd_lazy_neg": MADD_LAZY_NEG, "add": PADD,
@@ -44,7 +54,7 @@ POINT_OPS = {"madd": MADD, "madd_neg": MADD_NEG, "madd_lazy": MADD_LAZY, "madd_l
 # minimum vectors per case: a change to the generator must not quietly shrink the coverage
 MIN_FP = {"add": 100_000, "sub": 100_000, "mul": 100_000, "neg": 1 << 16, "dbl": 1 << 16, "sqr": 1 << 16,
           "from_mont": 1 << 16, "to_mont": 1 << 16, "mul_small": 10_000, "pow_u64": 5_000, "inv": 2_500,
-          "inv_safegcd": 2_500}
+          "inv_safegcd": 2_500, "ba_inv": 5_000}
 MIN_FQ2 = {"add": 30_000, "sub": 30_000, "mul": 30_000, "neg": 10_000, "dbl": 10_000, "sqr": 10_000, "mul_nr": 8_000,
            "inv": 3_000, "ba_inv": 6_000}
 MIN_POINT = {"madd": 150, "madd_neg": 150, "madd_lazy": 150, "madd_lazy_neg": 150, "add": 200, "dbl_inplace": 20,
@@ -59,19 +69,23 @@ def _field_ids():
         fp[f"{name}_fr"] = (2 * i, c.r)
         fp[f"{name}_fq"] = (2 * i + 1, c.q)
         fq2[f"{name}_fq2"] = (6 + i, c.q, -c.beta)   # Fq2 = Fq[u]/(u^2 + NR), NR = -beta
+    fp[f"{BW6}_fr"] = (9, ref.R)
+    fp[f"{BW6}_fq"] = (10, ref.Q)
     return fp, fq2
 
 
 FP_FIELDS, FQ2_FIELDS = _field_ids()
-CASES = ([f"fp-{f}-{o}" for f in FP_FIELDS for o in FP_OPS] + [f"fq2-{f}-{o}" for f in FQ2_FIELDS for o in FQ2_OPS]
-         + [f"pt-{c}_{g}-{o}" for c in CURVES for g in ("g1", "g2") for o in POINT_OPS])
+CASES = ([f"fp-{f}-{o}" for f in FP_FIELDS for o in FP_OPS if f.endswith("_fq") or o not in BASE_ONLY]
+         + [f"fq2-{f}-{o}" for f in FQ2_FIELDS for o in FQ2_OPS]
+         + [f"pt-{c}_{g}-{o}" for c in POINT_CURVES for g in ("g1", "g2") for o in POINT_OPS])
 
 
 # ------------------------------------------------------------------------------------------------------------------
 # limbs
 # ------------------------------------------------------------------------------------------------------------------
 def _nw(p):
-    return 8 if p.bit_length() <= 256 else 12
+    nb = p.bit_length()
+    return 8 if nb <= 256 else 12 if nb <= 384 else 24
 
 
 def _pack(vals, nw):
@@ -233,6 +247,11 @@ def _fp_case(name, field, opname):
         a = _fp_singles(p, field, 2048)
         # value x R^-1 -> R x^-1, in Montgomery form R^2 x^-1; the inverse of zero is zero
         return _exact_case(name, fid, FP_OPS[opname], [a], [R * R * pow(x, -1, p) % p if x else 0 for x in a], [nw], nw)
+    if opname == "ba_inv":
+        a = _fp_singles(p, f"{field}:ba_inv", 2048)
+        gcd = np.array([g for _ in a for g in (0, 1)], dtype=np.uint32)[:, None]   # Fermat and safegcd
+        a2 = [x for x in a for _ in (0, 1)]
+        return _exact_case(name, fid, BA_INV, [a2, gcd], [R * R * pow(x, -1, p) % p if x else 0 for x in a2], [nw, 1], nw)
     raise KeyError(opname)
 
 
@@ -281,20 +300,50 @@ def _fq2_case(name, field, opname):
     raise KeyError(opname)
 
 
+class _Bw6Group:
+    """BW6-761's G1 (b = -1) or G2 (b = 4), both over Fq, with the methods of pyref.Group, over tests/bw6_ref.py"""
+
+    def __init__(self, b):
+        self.b = b
+
+    def add(self, p, q):
+        return ref.add(p, q)
+
+    def dbl(self, p):
+        return ref.add(p, p)     # (x, 0): 2 y = 0, the identity
+
+    def neg(self, p):
+        return ref.neg(p)
+
+    def mul(self, p, k):
+        return ref.mul_proj(k, p)
+
+
 class _Group:
-    """G1 or G2 of a curve in value space (pyref), with the raw Montgomery encoding of its coordinates"""
+    """G1 or G2 of a curve in value space (pyref, or bw6_ref for BW6-761), with the raw Montgomery encoding of its
+    coordinates"""
 
     def __init__(self, curve, g2):
-        c = P.CURVES[curve]
-        cx = P.ctx(c)
-        self.q, self.r, self.nw = c.q, c.r, _nw(c.q)
+        if curve == BW6:
+            self.q, self.r = ref.Q, ref.R
+            self.F, self.G = P.FqOps(ref.Q), _Bw6Group(ref.B2 if g2 else ref.B1)
+            self.gen = GENERATORS[BW6]["g2" if g2 else "g1"]
+            self.fq2 = False                        # G2 over Fq
+            self.fid = FP_FIELDS[f"{BW6}_fq"][0]
+            self.sw = 12                            # Fr::N: 377-bit scalars in 12 words
+        else:
+            c = P.CURVES[curve]
+            cx = P.ctx(c)
+            self.q, self.r = c.q, c.r
+            self.F, self.G = (cx.Fq2, cx.G2) if g2 else (cx.Fq, cx.G1)
+            self.gen = cx.g2_gen() if g2 else cx.g1_gen()
+            self.fq2 = g2
+            self.fid = FQ2_FIELDS[f"{curve}_fq2"][0] if g2 else FP_FIELDS[f"{curve}_fq"][0]
+            self.sw = 8
+        self.nw = _nw(self.q)
         self.R = 1 << (32 * self.nw)
-        self.Ri = pow(self.R, -1, c.q)
-        self.g2 = g2
-        self.F, self.G = (cx.Fq2, cx.G2) if g2 else (cx.Fq, cx.G1)
-        self.gen = cx.g2_gen() if g2 else cx.g1_gen()
-        self.ew = 2 * self.nw if g2 else self.nw      # words per coordinate
-        self.fid = FQ2_FIELDS[f"{curve}_fq2"][0] if g2 else FP_FIELDS[f"{curve}_fq"][0]
+        self.Ri = pow(self.R, -1, self.q)
+        self.ew = 2 * self.nw if self.fq2 else self.nw      # words per coordinate
 
     @functools.lru_cache(None)
     def pool(self, seed):
@@ -308,16 +357,16 @@ class _Group:
         return out
 
     def rand(self, rng):
-        return rng.randrange(1, self.q) if not self.g2 else (rng.randrange(self.q), rng.randrange(1, self.q))
+        return rng.randrange(1, self.q) if not self.fq2 else (rng.randrange(self.q), rng.randrange(1, self.q))
 
     def raw(self, v):
-        if not self.g2:
+        if not self.fq2:
             return v * self.R % self.q
         return (v[0] * self.R % self.q) | ((v[1] * self.R % self.q) << (32 * self.nw))
 
     def val(self, w):
         """raw limbs -> value, None if a component is not below q"""
-        if not self.g2:
+        if not self.fq2:
             return w * self.Ri % self.q if w < self.q else None
         lo, hi = w & ((1 << (32 * self.nw)) - 1), w >> (32 * self.nw)
         return (lo * self.Ri % self.q, hi * self.Ri % self.q) if lo < self.q and hi < self.q else None
@@ -362,8 +411,9 @@ def _pt_case(name, curve, grp, opname):
     Pp, Q = rng.sample(pool, 2)
     P2, Pn = G.dbl(Pp), G.neg(Pp)
     lams = [F.one, F.neg(F.one), F.add(F.one, F.one), g.rand(rng)]
-    # (0, sqrt(b)) where it exists: x == 0 on a finite point; (x, 0): a point whose doubling is the identity
-    # (off the curve, but the doubling and addition formulas never read b)
+    # (0, sqrt(b)) where it exists: x == 0 on a finite point (not on BW6-761's G1: b = -1 is a non-residue, q = 3 mod 4;
+    # (0, 2) on its G2, b = 4); (x, 0): a point whose doubling is the identity (off the curve, but the doubling and
+    # addition formulas never read b)
     y0 = F.sqrt(G.b)
     specials = [(F.zero, y0)] if y0 is not None else []
     T = (g.rand(rng), F.zero)
@@ -406,13 +456,16 @@ def _pt_case(name, curve, grp, opname):
             want.append(G.dbl(a))
         sizes = [ew] * 2
     elif opname == "mul_u32":
-        r = g.r
-        ks = [0, 1, 2, r - 1, r, r + 1, (1 << 255) - 1, (1 << 256) - 1] + [rng.randrange(1 << 256) for _ in range(6)]
+        # scalars of Fr::N words, as the engine's proof tail passes them: all ones below the top bit of r, all ones in
+        # every word, r and its neighbours, random values over the whole width
+        r, sb = g.r, 32 * g.sw
+        top = (1 << 255) - 1 if g.sw == 8 else (1 << (r.bit_length() - 1)) - 1
+        ks = [0, 1, 2, r - 1, r, r + 1, top, (1 << sb) - 1] + [rng.randrange(1 << sb) for _ in range(6)]
         for a, lam in [(None, F.one), (Pp, F.one), (Pp, g.rand(rng)), (Q, F.neg(F.one))]:
             for k in ks:
                 vecs.append(g.xyzz(a, lam) + [k])
                 want.append(G.mul(a, k))
-        sizes = [ew] * 4 + [8]
+        sizes = [ew] * 4 + [g.sw]
     elif opname == "to_affine":
         pts = accs + [(rpt(), g.rand(rng)) for _ in range(64)]
         for a, lam in pts:

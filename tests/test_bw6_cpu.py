@@ -143,3 +143,65 @@ def test_ntt_reference_round_trip():
     for coset in (False, True):
         assert ref.ntt(ref.ntt(x, coset=coset), inverse=True, coset=coset) == x
     assert pow(ref.domain_root(4), 16, ref.R) == 1 and pow(ref.domain_root(4), 8, ref.R) != 1
+
+
+def test_projective_mul_and_fast_ntt():
+    """mul_proj (one inversion) against the affine double-and-add, at scalars beyond r too; fft against the naive ntt"""
+    rng = random.Random(4)
+    for name in ("g1", "g2"):
+        g = GENERATORS["bw6_761"][name]
+        for k in (0, 1, 2, 3, ref.R - 1, ref.R, ref.R + 1, (1 << 384) - 1, rng.randrange(1 << 40)):
+            assert ref.mul_proj(k, g) == ref.mul(k, g), (name, k)
+    assert ref.mul_proj(2, (7, 0)) is None and ref.mul_proj(5, None) is None
+    for log_n in range(7):
+        x = [rng.randrange(ref.R) for _ in range(1 << log_n)]
+        x[0] = ref.R - 1
+        for inverse in (False, True):
+            for coset in (False, True):
+                assert ref.fft(x, inverse, coset) == ref.ntt(x, inverse, coset), (log_n, inverse, coset)
+
+
+def _random_r1cs(rng, nc, ni, nw):
+    """nc random constraints over One, ni - 1 inputs and nw witnesses: one to three terms per row, coefficients at the
+    edges (1, r - 1) and random"""
+    nv = ni + nw
+    coeff = lambda: rng.choice([1, ref.R - 1, rng.randrange(ref.R)])
+    rows = tuple([[(coeff(), rng.randrange(nv)) for _ in range(rng.randrange(1, 4))] for _ in range(nc)] for _ in range(3))
+    return rows, nv
+
+
+def _witness_map_naive(a, b, c):
+    n = len(a)
+    ac, bc, cc = (ref.ntt(ref.ntt(x, inverse=True), coset=True) for x in (a, b, c))
+    zi = pow((pow(ref.FR_GENERATOR, n, ref.R) - 1) % ref.R, -1, ref.R)
+    return ref.ntt([(x * y - z) * zi % ref.R for x, y, z in zip(ac, bc, cc)], inverse=True, coset=True)
+
+
+@pytest.mark.parametrize("nc,ni,nw", [(1, 1, 1), (2, 2, 3), (5, 2, 6), (13, 3, 9), (29, 2, 20), (60, 4, 40)])
+def test_closed_form_proof_any_assignment(nc, ni, nw):
+    """proof_exponents (O(n) closed form, for any assignment) against the prover's definition: the five MSMs over the
+    key's discrete logs with h from the naive-NTT witness map, at domains 2 .. 2^6 and random assignments that do not
+    satisfy the circuit; a satisfying assignment (c = a * b by construction) as well"""
+    rng = random.Random(nc * 100 + ni)
+    rows, nv = _random_r1cs(rng, nc, ni, nw)
+    alpha, beta, _gamma, delta, tau = (rng.randrange(1, ref.R) for _ in range(5))
+    d = ref.query_exponents(rows, ni, nv, alpha, beta, delta, tau)
+    n, _ = ref.domain_size(rows, ni)
+    assert len(d["a"]) == len(d["b"]) == nv and len(d["l"]) == nv - ni and len(d["h"]) == n - 1
+    for k in range(4):
+        z = [1] + [rng.randrange(ref.R) for _ in range(nv - 1)]
+        if k == 3:   # satisfy every row: a fresh witness variable per row would be needed, so make C's rows A * B directly
+            ev = ref.row_evals(rows, ni, z)
+            rows = (rows[0], rows[1], [[(ev[0][j] * ev[1][j] % ref.R, 0)] for j in range(nc)])
+            d = ref.query_exponents(rows, ni, nv, alpha, beta, delta, tau)
+        ev = ref.row_evals(rows, ni, z)
+        h = _witness_map_naive(*ev)
+        assert h == ref.witness_map(*ev)
+        if k == 3:
+            assert all((x * y - w) % ref.R == 0 for x, y, w in zip(*ev)) and h[-1] == 0
+        else:
+            assert any((x * y - w) % ref.R for x, y, w in zip(*ev))
+        r, s = (0, rng.randrange(ref.R)) if k == 1 else (rng.randrange(ref.R), rng.randrange(ref.R))
+        e = ref.msm_exponents(d, h, z, ni)
+        want = ref.proof_from_msms(e, (d["a"][0], d["b"][0], d["b"][0]), alpha, beta, delta, r, s)
+        assert ref.proof_exponents(rows, ni, z, alpha, beta, delta, tau, r, s) == want, k

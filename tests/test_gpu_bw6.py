@@ -2,13 +2,11 @@
 curve's definition.  BW6-761 has no pairing here, so a proof is checked by the closed form "proof in the exponent":
 with the toxic waste known, A, B and C are fixed multiples of the generators (bw6_ref.expected_proof), independently of
 any MSM."""
-import os
 import random
 
 import numpy as np
 import pytest
 
-import bw6_arith
 import bw6_ref as ref
 from groth16_b200 import ConstraintMatrices, Groth16, _lib
 from groth16_b200.params import GENERATORS
@@ -90,7 +88,8 @@ def mimc(rounds=40, seed=3):
     return m, z
 
 
-def prove_and_check(g, m, z, tw, r_, s_, expect_valid=True):
+def prove_and_check(g, m, z, tw, r_, s_):
+    """the proof equals the closed form, for satisfying and unsatisfying assignments alike"""
     pk = g.generate_parameters_with_qap(m, *tw, G1, G2)
     zl = np.ascontiguousarray(g.codec.fr.enc(z))
     pf = g.create_proof_with_reduction_and_matrices(None, r_, s_, None, m.num_instance_variables, m.num_constraints, zl)
@@ -98,18 +97,8 @@ def prove_and_check(g, m, z, tw, r_, s_, expect_valid=True):
     got = (cd.dec_g1(pf.a)[0], cd.dec_g2(pf.b)[0], cd.dec_g1(pf.c)[0])
     alpha, beta, _gamma, delta, tau = tw
     want = ref.expected_proof(ref.csr_rows(m), m.num_instance_variables, z, alpha, beta, delta, tau, r_, s_, G1, G2)
-    if expect_valid:
-        assert got == want
-    else:
-        assert got[0] == want[0] and got[1] == want[1] and got[2] != want[2]
+    assert got == want
     return pk, pf, zl
-
-
-def test_device_arithmetic():
-    """the device build of tests/arith_bw6 (PTX carry chains, out-of-line 24-limb product, safegcd) at the edge operands"""
-    so = os.path.join(os.path.dirname(os.path.abspath(__file__)), "arith_bw6", "libg16bw6arith.so")
-    bad = bw6_arith.check_all(bw6_arith.load(so))
-    assert not bad, bad[:5]
 
 
 def _witness_map_ref(a, b, c):
@@ -250,7 +239,7 @@ def test_silly_and_mimc_proofs():
         prove_and_check(g, m, z, tw, 0, rng_fr(rng))          # r = 0
         bad = list(z)
         bad[2] = (bad[2] + 1) % ref.R                          # an assignment that does not satisfy the circuit
-        prove_and_check(g, m, bad, tw, rng_fr(rng), rng_fr(rng), expect_valid=False)
+        prove_and_check(g, m, bad, tw, rng_fr(rng), rng_fr(rng))
 
 
 @pytest.mark.parametrize("log_n", [6, 8, 10, 12])
