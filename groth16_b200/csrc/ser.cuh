@@ -9,7 +9,8 @@
 // bytes under the infinity flag, canonical coordinates (< q), that a compressed x has a curve point, that an uncompressed
 // point is on the curve, and with G16_SER_VALIDATE that [r]P = O (skipped for BN254 G1, whose cofactor is 1).
 //
-// ser_decode / ser_encode are per-point host/device functions (tests/host/ser_check.cu runs them on the CPU); the kernels
+// ser_decode / ser_encode are per-point host/device functions (tests/test_ser_codec.py runs them, and ser_sqrt, point by
+// point in the host, emulated-PTX and device builds of tests/arith/arith_ops.cu); the kernels
 // run one thread per point.  The host walk of the stream and the chunk planner are at the end.
 #pragma once
 #include <algorithm>

@@ -1,6 +1,8 @@
 // Element-level harness of the product arithmetic: one field, Fq2 or point operation per vector, run through the very
 // templates of fp.cuh, ec.cuh, fp_inv.cuh and msm_ba.cuh (no copies of their code).  tests/test_arith_ops.py feeds it
-// raw Montgomery limbs and compares every output with Python big integers.
+// raw Montgomery limbs and compares every output with Python big integers.  The proving-key point codec of ser.cuh
+// (ser_decode, ser_encode, ser_sqrt) runs through the same ABI; tests/test_ser_codec.py checks it against
+// groth16_b200.serialize.ArkCodec.
 //
 // Built three ways from this one file:
 //   nvcc (Makefile)             : libg16arith.so, one device thread per vector -- the PTX carry chains, the out-of-line
@@ -15,6 +17,7 @@
 #include <cstdlib>
 #include <cstring>
 #include "../../groth16_b200/csrc/msm_ba.cuh"
+#include "../../groth16_b200/csrc/ser.cuh"
 
 using namespace g16;
 
@@ -28,6 +31,7 @@ enum Op {
   INV_GCD = 11, MUL_NR = 12, BA_INV = 13,
   MADD = 20, MADD_NEG = 21, MADD_LAZY = 22, MADD_LAZY_NEG = 23, PADD = 24, PDBL = 25, PDBL_AFFINE = 26, PMUL_U32 = 27,
   TO_AFFINE = 28,
+  SER_DECODE_G1 = 30, SER_DECODE_G2 = 31, SER_ENCODE_G1 = 32, SER_ENCODE_G2 = 33, SQRT = 34,
 };
 constexpr int NUM_FIELDS = 11;
 
@@ -130,8 +134,86 @@ G16_HD bool fq2_op(int op, const uint32_t* in, uint32_t* out) {
   return point_op<F, SW>(op, in, out);
 }
 
+// ---- the proving-key point codec (ser.cuh) ----------------------------------------------------------------------------
+// Canonical integers in and out (the wire format's values), C = words of one coordinate:
+//   SER_DECODE_*: flags (G16_SER_*), then the encoding's bytes packed little-endian in u32 words, 2C of them (a compressed
+//                 encoding fills the first C, the rest is zero) -> result code, x, y (all zero unless the code is SER_OK;
+//                 the identity is all zero too)
+//   SER_ENCODE_*: flags, x, y (all zero: the identity) -> the encoding's bytes in 2C words (compressed: the first C, the
+//                 rest zero)
+//   SQRT:         a -> 1 and the root ser_sqrt returns, or 0 and zero
+template <class P>
+G16_HD Fp<P> mont(const Fp<P>& a, bool to) { return to ? Fp<P>::to_mont(a) : Fp<P>::from_mont(a); }
+template <class P, int NR>
+G16_HD Fp2<P, NR> mont(const Fp2<P, NR>& a, bool to) { return {mont(a.c0, to), mont(a.c1, to)}; }
+
+template <class CP, bool G2>
+G16_HD void ser_op(bool decode, const uint32_t* in, uint32_t* out) {
+  using F = SerField<CP, G2>;
+  using A = Affine<F>;
+  constexpr int C = sizeof(F) / 4, NBYTES = 8 * C;   // the uncompressed encoding: 2C words
+  static_assert(NBYTES == SerFormat<CP>::point_bytes(G2, false), "encoding size");
+  uint8_t raw[NBYTES];
+  if (decode) {
+    for (int i = 0; i < NBYTES; i++) raw[i] = (uint8_t)(in[1 + i / 4] >> (8 * (i % 4)));
+    A p;
+    const uint32_t code = ser_decode<CP, G2>(raw, in[0], p);
+    if (code) p = A::inf();
+    out[0] = code;
+    st(out + 1, mont(p.x, false));
+    st(out + 1 + C, mont(p.y, false));
+  } else {
+    const A p = {mont(ld<F>(in + 1), true), mont(ld<F>(in + 1 + C), true)};
+    for (int i = 0; i < NBYTES; i++) raw[i] = 0;
+    ser_encode<CP, G2>(p, in[0], raw);
+    for (int i = 0; i < 2 * C; i++)
+      out[i] = raw[4 * i] | (uint32_t)raw[4 * i + 1] << 8 | (uint32_t)raw[4 * i + 2] << 16 | (uint32_t)raw[4 * i + 3] << 24;
+  }
+}
+
+// the curve of a base field (its G1, and BW6-761's G2) or of an Fq2 field (its G2); void for the scalar fields
+template <int FIELD>
+struct SerCurve { using CP = void; };
+template <> struct SerCurve<1> { using CP = BLS381_Params; };
+template <> struct SerCurve<3> { using CP = BN254_Params; };
+template <> struct SerCurve<5> { using CP = BLS377_Params; };
+template <> struct SerCurve<6> { using CP = BLS381_Params; };
+template <> struct SerCurve<7> { using CP = BN254_Params; };
+template <> struct SerCurve<8> { using CP = BLS377_Params; };
+template <> struct SerCurve<10> { using CP = BW6_Params; };
+
+template <int FIELD>
+G16_HD bool codec_op(int op, const uint32_t* in, uint32_t* out) {
+  using CP = typename SerCurve<FIELD>::CP;
+  if constexpr (std::is_void<CP>::value) {
+    return false;
+  } else {
+    constexpr bool fq2 = FIELD >= 6 && FIELD <= 8, g1 = !fq2, g2 = fq2 || FIELD == 10;
+    switch (op) {
+      case SER_DECODE_G1:
+      case SER_ENCODE_G1:
+        if constexpr (g1) { ser_op<CP, false>(op == SER_DECODE_G1, in, out); return true; }
+        break;
+      case SER_DECODE_G2:
+      case SER_ENCODE_G2:
+        if constexpr (g2) { ser_op<CP, true>(op == SER_DECODE_G2, in, out); return true; }
+        break;
+      case SQRT: {
+        using F = SerField<CP, fq2>;
+        F r;
+        const bool ok = ser_sqrt(mont(ld<F>(in), true), r);
+        out[0] = ok;
+        st(out + 1, ok ? mont(r, false) : F::zero());
+        return true;
+      }
+    }
+    return false;
+  }
+}
+
 template <int FIELD>
 G16_HD bool run_one(int op, const uint32_t* in, uint32_t* out) {
+  if (op >= SER_DECODE_G1) return codec_op<FIELD>(op, in, out);
   if constexpr (FIELD == 0) return fp_op<BLS381_FrP>(op, in, out);
   else if constexpr (FIELD == 1) return fp_op<BLS381_FqP, BLS381_FrP::N>(op, in, out);
   else if constexpr (FIELD == 2) return fp_op<BN254_FrP>(op, in, out);
@@ -191,6 +273,7 @@ int g16t_shape(int field, int op, int* in_words, int* out_words) {
   if (field < 0 || field >= NUM_FIELDS) return -1;
   const int E = ELEM_WORDS[field], SW = SCALAR_WORDS[field];
   const bool fq2 = field >= 6 && field <= 8, fp = !fq2, curve = SW > 0;
+  const bool ser_g1 = field == 1 || field == 3 || field == 5 || field == 10, ser_g2 = fq2 || field == 10;
   int i = -1, o = E;
   switch (op) {
     case ADD: case SUB: case MUL: i = 2 * E; break;
@@ -206,6 +289,11 @@ int g16t_shape(int field, int op, int* in_words, int* out_words) {
     case PDBL_AFFINE: if (curve) { i = 2 * E; o = 4 * E; } break;
     case PMUL_U32: if (curve) { i = 4 * E + SW; o = 4 * E; } break;
     case TO_AFFINE: if (curve) { i = 4 * E; o = 2 * E; } break;
+    case SER_DECODE_G1: if (ser_g1) { i = 1 + 2 * E; o = 1 + 2 * E; } break;
+    case SER_DECODE_G2: if (ser_g2) { i = 1 + 2 * E; o = 1 + 2 * E; } break;
+    case SER_ENCODE_G1: if (ser_g1) { i = 1 + 2 * E; o = 2 * E; } break;
+    case SER_ENCODE_G2: if (ser_g2) { i = 1 + 2 * E; o = 2 * E; } break;
+    case SQRT: if (ser_g1 || ser_g2) { i = E; o = 1 + E; } break;
   }
   if (i < 0) return -1;
   *in_words = i;

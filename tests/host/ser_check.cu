@@ -1,14 +1,9 @@
-// Host-only check (built by nvcc, runs without a GPU) of the proving-key wire format code of groth16_b200/csrc/ser.cuh:
-//   1. the chunk planner and the placement rule: for chunk sizes 1, 2, 7, 1000, odd vector lengths and world 1 .. 3, every
-//      point is visited once, at its byte offset, and every MSM pair has exactly one owner, in the slot g16_pk_load uses;
-//   2. ser_decode / ser_encode, the per-point functions the kernels run, on cases read from stdin (tests/test_ser_host.py
-//      writes them and compares the answers with groth16_b200.serialize.ArkCodec):
-//        D <curve> <g2> <flags> <hex bytes>                 ->  "ERR <code>" | "INF" | "PT <hex canonical coordinates>"
-//        E <curve> <g2> <flags> INF | <hex coordinates>     ->  "BYTES <hex>"
-//      curve: 0 BLS12-381, 1 BN254, 2 BLS12-377; coordinates x y (G1) or x0 x1 y0 y1 (G2).
+// Host-only check (built by nvcc, runs without a GPU) of the proving-key stream code of groth16_b200/csrc/ser.cuh: the
+// walk of the length prefixes, the chunk planner and the placement rule.  For chunk sizes 1, 2, 7, 1000, odd vector lengths
+// and world 1 .. 3, every point is visited once, at its byte offset, and every MSM pair has exactly one owner, in the slot
+// g16_pk_load uses.  The per-point functions ser_decode / ser_encode / ser_sqrt are checked in all three builds of the
+// element harness (tests/arith/arith_ops.cu, tests/test_ser_codec.py).
 #include <cstdio>
-#include <iostream>
-#include <sstream>
 #include <string>
 #include <vector>
 #include "../../groth16_b200/csrc/ser.cuh"
@@ -28,27 +23,28 @@ static int bad = 0, cases = 0;
 static void check_planner() {
   const uint64_t lens[][5] = {{3, 5, 5, 7, 2}, {1, 1, 1, 1, 0}, {9, 1001, 1001, 1999, 17}, {0, 2, 2, 2, 0}};
   for (auto& L : lens)
-    for (int nb : {32, 48})
+    for (int nb : {32, 48, 96})   // 96: BW6-761, whose G2 points are over Fq (one value per coordinate)
       for (bool compress : {true, false}) {
+        const int g2_nc = nb == 96 ? 1 : 2;
         // build the stream skeleton with these lengths: gamma_abc = L[0], a = b1 = b2 = L[1..3]... and h, l
         SerItem it[SER_ITEMS];
         ser_items(it);
         it[SER_GAMMA_ABC].len = L[0];
         it[SER_A].len = L[1]; it[SER_B_G1].len = L[1]; it[SER_B_G2].len = L[2];
         it[SER_H].len = L[3]; it[SER_L].len = L[4];
-        const uint64_t total = ser_size(it, nb, compress);
+        const uint64_t total = ser_size(it, nb, compress, g2_nc);
         std::vector<uint8_t> bytes(total, 0);
         for (int m = 0; m < SER_ITEMS; m++)
           if (it[m].vec)
             for (int k = 0; k < 8; k++) bytes[it[m].off - 8 + k] = (uint8_t)(it[m].len >> (8 * k));
         SerItem w[SER_ITEMS];
-        CHECK(ser_walk(bytes.data(), total, nb, compress, w).empty(), "walk rejected a well-formed skeleton");
+        CHECK(ser_walk(bytes.data(), total, nb, compress, w, g2_nc).empty(), "walk rejected a well-formed skeleton");
         for (int m = 0; m < SER_ITEMS; m++)
           CHECK(w[m].len == it[m].len && w[m].off == it[m].off && w[m].psize == it[m].psize, "walk: member %d", m);
-        CHECK(!ser_walk(bytes.data(), total - 1, nb, compress, w).empty(), "walk accepted a truncated stream");
+        CHECK(!ser_walk(bytes.data(), total - 1, nb, compress, w, g2_nc).empty(), "walk accepted a truncated stream");
         std::vector<uint8_t> more(bytes);
         more.push_back(0);
-        CHECK(ser_walk(more.data(), total + 1, nb, compress, w) == "trailing bytes after the proving key", "trailing bytes");
+        CHECK(ser_walk(more.data(), total + 1, nb, compress, w, g2_nc) == "trailing bytes after the proving key", "trailing bytes");
         for (uint32_t chunk : {1u, 2u, 7u, 1000u}) {
           const std::vector<SerChunk> plan = ser_plan(it, chunk);
           std::vector<std::vector<int>> seen(SER_ITEMS);
@@ -103,97 +99,8 @@ static void check_planner() {
   CHECK(ser_walk(b.data(), b.size(), 48, true, w).find("exceeds the limit") != std::string::npos, "absurd prefix");
 }
 
-// ---- per-point functions --------------------------------------------------------------------------------------------
-template <class P>
-static Fp<P> parse_fq(const std::string& hex) {
-  Fp<P> r = Fp<P>::zero();
-  int bit = 0;
-  for (int k = (int)hex.size() - 1; k >= 0; k--, bit += 4) {
-    const char ch = hex[k];
-    const uint32_t d = ch <= '9' ? ch - '0' : (ch | 0x20) - 'a' + 10;
-    if (bit < 32 * P::N) r.v[bit / 32] |= d << (bit % 32);
-  }
-  return r;
-}
-template <class P>
-static std::string hex_fq(const Fp<P>& a) {
-  std::string s;
-  char buf[16];
-  for (int i = P::N - 1; i >= 0; i--) { snprintf(buf, sizeof buf, "%08x", a.v[i]); s += buf; }
-  return s;
-}
-static std::vector<uint8_t> parse_bytes(const std::string& hex) {
-  std::vector<uint8_t> out(hex.size() / 2);
-  for (size_t i = 0; i < out.size(); i++) out[i] = (uint8_t)std::stoul(hex.substr(2 * i, 2), nullptr, 16);
-  return out;
-}
-
-template <class CP, bool G2>
-static std::string run(char op, uint32_t flags, std::istringstream& in) {
-  using P = typename CP::FqP;
-  using Fq = Fp<P>;
-  using A = Affine<SerField<CP, G2>>;
-  constexpr int NC = G2 ? 2 : 1;
-  if (op == 'D') {
-    std::string hex;
-    in >> hex;
-    const std::vector<uint8_t> raw = parse_bytes(hex);
-    if ((int)raw.size() != SerFormat<CP>::point_bytes(G2, flags & SER_COMPRESSED)) return "BADLEN";
-    A p;
-    const uint32_t code = ser_decode<CP, G2>(raw.data(), flags, p);
-    if (code) return "ERR " + std::to_string(code);
-    if (p.is_inf()) return "INF";
-    Fq c[4];
-    if constexpr (G2) { c[0] = p.x.c0; c[1] = p.x.c1; c[2] = p.y.c0; c[3] = p.y.c1; }
-    else { c[0] = p.x; c[1] = p.y; }
-    std::string s = "PT";
-    for (int k = 0; k < 2 * NC; k++) s += " " + hex_fq(Fq::from_mont(c[k]));
-    return s;
-  }
-  std::string first;
-  in >> first;
-  A p = A::inf();
-  if (first != "INF") {
-    Fq c[4];
-    c[0] = Fq::to_mont(parse_fq<P>(first));
-    for (int k = 1; k < 2 * NC; k++) { std::string h; in >> h; c[k] = Fq::to_mont(parse_fq<P>(h)); }
-    if constexpr (G2) p = A{{c[0], c[1]}, {c[2], c[3]}};
-    else p = A{c[0], c[1]};
-  }
-  std::vector<uint8_t> out(SerFormat<CP>::point_bytes(G2, flags & SER_COMPRESSED), 0xAA);
-  ser_encode<CP, G2>(p, flags, out.data());
-  std::string s = "BYTES ";
-  char buf[4];
-  for (uint8_t b : out) { snprintf(buf, sizeof buf, "%02x", b); s += buf; }
-  return s;
-}
-
-template <class CP>
-static std::string run_curve(char op, bool g2, uint32_t flags, std::istringstream& in) {
-  return g2 ? run<CP, true>(op, flags, in) : run<CP, false>(op, flags, in);
-}
-
 int main() {
   check_planner();
   printf("planner: %d checks, %d mismatches\n", cases, bad);
-  std::string line;
-  int points = 0;
-  while (std::getline(std::cin, line)) {
-    if (line.empty()) continue;
-    std::istringstream in(line);
-    char op;
-    int curve, g2;
-    uint32_t flags;
-    in >> op >> curve >> g2 >> flags;
-    std::string r;
-    switch (curve) {
-      case 0: r = run_curve<BLS381_Params>(op, g2, flags, in); break;
-      case 1: r = run_curve<BN254_Params>(op, g2, flags, in); break;
-      default: r = run_curve<BLS377_Params>(op, g2, flags, in); break;
-    }
-    printf("%s\n", r.c_str());
-    points++;
-  }
-  fprintf(stderr, "%d point cases\n", points);
   return bad ? 1 : 0;
 }

@@ -6,7 +6,9 @@
   * 2^20 keys on each curve round-trip (export, validated load, same proof) and load sharded over 3 emulated ranks;
   * rejections name the first bad item in stream order, with serialize.py's reason: every malformation in every member at
     its first and last index, and in every query at a chunk boundary of a 2^20 key; no key is resident afterwards;
-  * small-order and cofactor-torsion points fail the subgroup check and pass without it."""
+  * small-order and cofactor-torsion points fail the subgroup check and pass without it.
+The rejection and subgroup tests run on BW6-761 too (its G2 points are over Fq, encoded like G1 points), with a key made by
+g16_setup whose export is checked against ArkCodec first."""
 import io
 import os
 
@@ -15,10 +17,11 @@ import pytest
 
 import pyref as P
 from groth16_b200 import Groth16, MalformedKey, Proof
-from groth16_b200.params import GENERATORS
+from groth16_b200.codec import CurveCodec
+from groth16_b200.params import GENERATORS, get_curve
 from groth16_b200.serialize import ArkCodec, DeserializeError
 from groth16_b200.workload import synthetic_r1cs
-from test_ser_host import _special_points, _torsion_points
+from test_ser_codec import _special_points, _torsion_points
 from util import ALL_CURVES, matrices_from_r1cs, pk_from_abi, proof_from_abi, toxic
 
 pytestmark = pytest.mark.gpu
@@ -28,6 +31,7 @@ MEMBERS = ["vk.alpha_g1", "vk.beta_g2", "vk.gamma_g2", "vk.delta_g2", "vk.gamma_
            "b_g1_query", "b_g2_query", "h_query", "l_query"]
 G2_MEMBERS = {"vk.beta_g2", "vk.gamma_g2", "vk.delta_g2", "b_g2_query"}
 VECS = {"vk.gamma_abc_g1", "a_query", "b_g1_query", "b_g2_query", "h_query", "l_query"}
+BW6 = "bw6_761"
 _ENG = {}
 _KEYS = {}
 
@@ -52,7 +56,7 @@ def layout(k: ArkCodec, data: bytes, compress: bool):
     """member -> (byte offset of element 0, length, bytes per point), from the length prefixes"""
     out, pos = {}, 0
     for name in MEMBERS:
-        ps = k.fq_bytes * (2 if name in G2_MEMBERS else 1) * (1 if compress else 2)
+        ps = k.fq_bytes * (2 if name in G2_MEMBERS and k.g2_fq2 else 1) * (1 if compress else 2)
         n = 1
         if name in VECS:
             n = int.from_bytes(data[pos:pos + 8], "little")
@@ -64,11 +68,14 @@ def layout(k: ArkCodec, data: bytes, compress: bool):
 
 
 def ark_bytes(curve, pk_abi, compress):
-    opk = pk_from_abi(curve, pk_abi)
-    k = ArkCodec(curve)
-    vk = opk.vk
-    return k.proving_key((vk.alpha_g1, vk.beta_g2, vk.gamma_g2, vk.delta_g2, vk.gamma_abc_g1), opk.beta_g1, opk.delta_g1,
-                         opk.a_query, opk.b_g1_query, opk.b_g2_query, opk.h_query, opk.l_query, compress=compress)
+    cd = CurveCodec(get_curve(curve))
+    g1 = lambda v: cd.dec_g1(v)[0]
+    g2 = lambda v: cd.dec_g2(v)[0]
+    vk = pk_abi.vk
+    return ArkCodec(curve).proving_key(
+        (g1(vk.alpha_g1), g2(vk.beta_g2), g2(vk.gamma_g2), g2(vk.delta_g2), cd.dec_g1(vk.gamma_abc_g1)), g1(pk_abi.beta_g1),
+        g1(pk_abi.delta_g1), cd.dec_g1(pk_abi.a_query), cd.dec_g1(pk_abi.b_g1_query), cd.dec_g2(pk_abi.b_g2_query),
+        cd.dec_g1(pk_abi.h_query), cd.dec_g1(pk_abi.l_query), compress=compress)
 
 
 def prove(g, m, z, r, s):
@@ -80,6 +87,14 @@ def prove(g, m, z, r, s):
 def small_key(curve, kind):
     """(engine, matrices, assignment, setup key limbs, oracle circuit or None) for one of the small circuits"""
     key = (curve, kind)
+    if key not in _KEYS and curve == BW6:
+        g = engine(curve)
+        m, z, _ = synthetic_r1cs(curve, {"2p6": 6, "2p10": 10}[kind], seed=9)
+        tw = toxic(get_curve(curve), 31)
+        pk = g.generate_parameters_with_qap(m, *tw, GENERATORS[curve]["g1"], GENERATORS[curve]["g2"])
+        for compress in (True, False):   # g16_setup's key, exported on the GPU, is ArkCodec's encoding of it
+            assert g.export_proving_key_bytes(compress) == ark_bytes(curve, pk, compress), compress
+        _KEYS[key] = (g, m, z, pk, None, tw)
     if key not in _KEYS:
         c = P.CURVES[curve]
         cx = P.ctx(c)
@@ -247,10 +262,9 @@ def _corruptions(k, compress, g2):
 
 
 @pytest.mark.parametrize("compress", [True, False])
-@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("curve", ALL_CURVES + [BW6])
 def test_rejections_name_the_first_bad_item(curve, compress):
     g, m, z, pk, cs, tw = small_key(curve, "2p6")
-    c = P.CURVES[curve]
     k = ArkCodec(curve)
     data = ark_bytes(curve, pk, compress)
     lay = layout(k, data, compress)
@@ -288,7 +302,7 @@ def test_rejections_name_the_first_bad_item(curve, compress):
         prove(g, m, z, r, s)
 
 
-@pytest.mark.parametrize("curve", ALL_CURVES)
+@pytest.mark.parametrize("curve", ALL_CURVES + [BW6])
 def test_subgroup_check_small_order_and_torsion(curve):
     g, m, z, pk, cs, tw = small_key(curve, "2p6")
     for compress in (True, False):
