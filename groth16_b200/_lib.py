@@ -39,6 +39,10 @@ class Config(C.Structure):
                                          "ba_inv_gcd", "acc_block", "sm_count", "rank", "world")] + [("reserved", C.c_int32 * 4)]
 
 
+class WitnessReport(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("first_unsatisfied", "num_unsatisfied", "first_malformed")]
+
+
 # every symbol include/g16b200.h declares: (name, restype, argtypes)
 SIGNATURES = [
     ("g16_ctx_create", C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
@@ -72,6 +76,7 @@ SIGNATURES = [
     ("g16_prove_partial_submit", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_uint32]),
     ("g16_prove_partial_wait", C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     ("g16_witness_map", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
+    ("g16_check_witness", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(WitnessReport)]),
     ("g16_get_timings", C.c_int, [C.c_void_p, C.POINTER(Timings)]),
     ("g16_comm_unique_id", C.c_int, [C.c_void_p]),
     ("g16_comm_init", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]),
@@ -90,10 +95,13 @@ ERR_BAD_ARGUMENT = 2
 ERR_CUDA = 3
 ERR_MALFORMED_KEY = 4
 ERR_INVALID_DATA = 5
+ERR_UNSATISFIED = 6
 SER_COMPRESSED = 1
 SER_VALIDATE = 2
 ASSIGNMENT_ON_DEVICE = 1
 SERIAL_MSMS = 2
+CHECK_WITNESS = 4
+NONE = (1 << 64) - 1   # G16_NONE
 QAP_LIBSNARK = 0
 QAP_CIRCOM = 1
 QAPS = {"libsnark": QAP_LIBSNARK, "circom": QAP_CIRCOM}

@@ -35,6 +35,10 @@ class MalformedKey(SynthesisError):
     pass
 
 
+class Unsatisfiable(SynthesisError):
+    """SynthesisError::Unsatisfiable: CHECK_WITNESS refused an assignment; the message names the constraint or element"""
+
+
 class CudaError(RuntimeError):
     pass
 
@@ -51,6 +55,8 @@ def _check(rc: int):
         raise CudaError(msg)
     if rc == _lib.ERR_INVALID_DATA:
         raise DeserializeError(msg)
+    if rc == _lib.ERR_UNSATISFIED:
+        raise Unsatisfiable(msg)
     raise ValueError(msg)
 
 
@@ -122,6 +128,18 @@ class ProvingKey:
     b_g2_query: np.ndarray
     h_query: np.ndarray
     l_query: np.ndarray
+
+
+@dataclass
+class WitnessReport:
+    """g16_witness_report of one assignment, None where the library reports G16_NONE"""
+    first_unsatisfied: Optional[int]   # lowest constraint i with <A_i,z><B_i,z> != <C_i,z>
+    num_unsatisfied: int
+    first_malformed: Optional[int]     # lowest element with limbs >= r, or 0 when z[0] is not One; rows not evaluated then
+
+    @property
+    def ok(self) -> bool:
+        return self.first_malformed is None and self.num_unsatisfied == 0
 
 
 @dataclass
@@ -479,9 +497,9 @@ class Groth16:
         return self._lib.g16_partial_limbs(self._ctx)
 
     def witness_map_from_matrices(self, matrices: Optional[ConstraintMatrices], num_inputs: int, num_constraints: int,
-                                  full_assignment: np.ndarray) -> np.ndarray:
+                                  full_assignment: np.ndarray, flags: int = 0) -> np.ndarray:
         """R1CSToQAP::witness_map_from_matrices (r1cs_to_qap.rs:172-235) -> domain_size Montgomery Fr coefficients; with
-        qap="circom", CircomReduction's domain_size evaluations at the odd powers of omega_2n."""
+        qap="circom", CircomReduction's domain_size evaluations at the odd powers of omega_2n.  flags: 0 or CHECK_WITNESS."""
         if matrices is not None and matrices is not self._matrices:
             self.load_matrices(matrices)
         m = self._matrices
@@ -490,8 +508,45 @@ class Groth16:
             raise ValueError("full_assignment has the wrong length")
         n = 1 << self._lib.g16_domain_log(self._ctx)
         h = np.zeros((n, self.nr), dtype=np.uint64)
-        _check(self._lib.g16_witness_map(self._ctx, _ptr(z), 0, _ptr(h)))
+        _check(self._lib.g16_witness_map(self._ctx, _ptr(z), flags, _ptr(h)))
         return h
+
+    # ---- R1CS satisfiability (ark-relations ConstraintSystem::is_satisfied / which_is_unsatisfied), on the GPU ----
+    def check_witness(self, full_assignments, count: Optional[int] = None, flags: int = 0) -> List[WitnessReport]:
+        """g16_check_witness on the resident circuit: one report per assignment.  `full_assignments`: (nv, F) or (K, nv, F)
+        Montgomery limbs, or a device address of `count` assignments together with flags = ASSIGNMENT_ON_DEVICE."""
+        m = self._matrices
+        if m is None:
+            raise ValueError("load_matrices must come first")
+        nv = m.num_instance_variables + m.num_witness_variables
+        if isinstance(full_assignments, np.ndarray):
+            z = np.ascontiguousarray(full_assignments, dtype=np.uint64)
+            if z.ndim == 2:
+                z = z.reshape(1, *z.shape)
+            if z.ndim != 3 or z.shape[1:] != (nv, self.nr):
+                raise ValueError(f"full_assignments must have shape (nv, {self.nr}) or (K, {nv}, {self.nr})")
+            count, ptr = z.shape[0], z.ctypes.data
+        else:
+            if count is None:
+                raise ValueError("a device address needs `count`")
+            ptr = int(full_assignments)
+        out = (_lib.WitnessReport * max(count, 1))()
+        _check(self._lib.g16_check_witness(self._ctx, count, C.c_void_p(ptr), flags, out))
+        none = lambda v: None if v == _lib.NONE else int(v)
+        return [WitnessReport(none(w.first_unsatisfied), int(w.num_unsatisfied), none(w.first_malformed)) for w in out[:count]]
+
+    def is_satisfied(self, full_assignment: np.ndarray) -> bool:
+        """ConstraintSystem::is_satisfied for one assignment (a malformed element counts as unsatisfied)"""
+        return self.check_witness(full_assignment)[0].ok
+
+    def which_is_unsatisfied(self, full_assignment: np.ndarray) -> Optional[int]:
+        """ConstraintSystem::which_is_unsatisfied: the lowest unsatisfied constraint, or None (there are no constraint
+        names at this boundary).  A malformed assignment raises Unsatisfiable naming the element."""
+        w = self.check_witness(full_assignment)[0]
+        if w.first_malformed is not None:
+            raise Unsatisfiable(f"assignment element {w.first_malformed} is " +
+                                ("not One" if w.first_malformed == 0 else "not a canonical Fr"))
+        return w.first_unsatisfied
 
     def timings(self) -> dict:
         t = _lib.Timings()

@@ -195,6 +195,11 @@ int g16_witness_map(g16_ctx* ctx, const uint64_t* full_assignment, uint32_t flag
   CTX_OR_FAIL(ctx);
   return ctx->eng->witness_map(full_assignment, flags, h_out);
 }
+int g16_check_witness(g16_ctx* ctx, uint32_t count, const uint64_t* full_assignments, uint32_t flags,
+                      g16_witness_report* reports_out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->check_witness(count, full_assignments, flags, reports_out);
+}
 int g16_get_timings(const g16_ctx* ctx, g16_timings* out) {
   CTX_OR_FAIL(ctx);
   if (!out) return fail(G16_ERR_BAD_ARGUMENT, "null out");

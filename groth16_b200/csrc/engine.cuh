@@ -156,6 +156,7 @@ struct IEngine {
   virtual int partial_submit(int slot, const uint64_t* r, const uint64_t* z, uint32_t flags) = 0;
   virtual int partial_wait(int slot, uint64_t* partial) = 0;
   virtual int witness_map(const uint64_t* z, uint32_t flags, uint64_t* h) = 0;
+  virtual int check_witness(uint32_t count, const uint64_t* z, uint32_t flags, g16_witness_report* out) = 0;
   virtual uint32_t domain_log() const = 0;
   virtual int comm_init(const uint8_t* id128, uint32_t rank, uint32_t world) = 0;
   virtual int sharded_submit(int slot, const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags) = 0;
@@ -222,6 +223,12 @@ struct Engine : IEngine {
     DevBuf d_tail;          // per proof: r, s, r s (Fr), then r d1, (r s) d1, s P_a, r P_b (G1 affine), s d2 (G2 affine)
     uint64_t* h_tail = nullptr;   // pinned copy of d_tail
     size_t h_tail_cap = 0;
+    // G16_CHECK_WITNESS: the submission checks its assignments (r1cs_check); d_check -> h_check (pinned) after the witness
+    // map, read where the results are collected
+    bool check = false;
+    DevBuf d_check;
+    uint32_t* h_check = nullptr;
+    size_t h_check_cap = 0;
   };
   static constexpr int NSLOTS = 2;
   Slot slots[NSLOTS];
@@ -557,6 +564,7 @@ struct Engine : IEngine {
     dom_api.release();
     for (Slot& sl : slots) {
       if (sl.h_tail) cudaFreeHost(sl.h_tail);
+      if (sl.h_check) cudaFreeHost(sl.h_check);
       if (sl.st_main) cudaStreamDestroy(sl.st_main);
       for (auto s : sl.st_msm) if (s) cudaStreamDestroy(s);
       auto kill = [](cudaEvent_t ev) { if (ev) cudaEventDestroy(ev); };
@@ -1297,7 +1305,21 @@ struct Engine : IEngine {
     G16_CUDA(cudaEventRecord(sl.ev_z, sl.st_main));
     const uint32_t n = 1u << L;
     CsrDev cs[3];
-    for (int m = 0; m < 3; m++) cs[m] = CsrDev{csr_rp[m].template as<uint32_t>(), csr_col[m].template as<uint32_t>(), csr_val[m].p};
+    csr_dev(cs);
+    sl.check = (flags & G16_CHECK_WITNESS) != 0;
+    if (sl.check) {   // on the main stream only: the MSMs, which wait for ev_z, run beside it
+      const size_t bytes = (size_t)count * 3 * sizeof(uint32_t);
+      G16_CUDA(sl.d_check.reserve(bytes));
+      if (sl.h_check_cap < bytes) {
+        if (sl.h_check) cudaFreeHost(sl.h_check);
+        sl.h_check = nullptr;
+        sl.h_check_cap = 0;
+        G16_CUDA(cudaMallocHost(&sl.h_check, bytes));
+        sl.h_check_cap = bytes;
+      }
+      G16_CUDA(r1cs_check<Fr>(sl.st_main, cs, sl.d_z.template as<Fr>(), num_constraints, (uint32_t)nv, count,
+                              sl.d_check.template as<uint32_t>(), &ntt_launches));
+    }
     r1cs_matvec<Fr>(sl.st_main, cs, sl.d_z.template as<Fr>(), num_constraints, num_inputs, n, sl.d_a.template as<Fr>(),
                     sl.d_b.template as<Fr>(), sl.d_c.template as<Fr>(), count, (uint32_t)nv, qap == G16_QAP_LIBSNARK);
     ntt_launches++;
@@ -1310,6 +1332,71 @@ struct Engine : IEngine {
     }
     G16_CUDA(cudaGetLastError());
     G16_CUDA(cudaEventRecord(sl.ev_h, sl.st_main));
+    if (sl.check)   // after ev_h: the H MSM does not wait for the copy
+      G16_CUDA(cudaMemcpyAsync(sl.h_check, sl.d_check.p, (size_t)count * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, sl.st_main));
+    return G16_OK;
+  }
+  void csr_dev(CsrDev cs[3]) const {
+    for (int m = 0; m < 3; m++) cs[m] = CsrDev{csr_rp[m].template as<uint32_t>(), csr_col[m].template as<uint32_t>(), csr_val[m].p};
+  }
+  // One r1cs_check record (lowest unsatisfied row, ~count, lowest malformed element) as the ABI reports it: a malformed
+  // element leaves the rows unevaluated
+  static g16_witness_report report_of(const uint32_t* x) {
+    g16_witness_report w;
+    w.first_malformed = x[2] == UINT32_MAX ? G16_NONE : x[2];
+    const bool rows = w.first_malformed == G16_NONE;
+    w.first_unsatisfied = rows && x[0] != UINT32_MAX ? x[0] : G16_NONE;
+    w.num_unsatisfied = rows ? (uint32_t)~x[1] : 0;
+    return w;
+  }
+  static bool report_ok(const g16_witness_report& w) { return w.first_malformed == G16_NONE && w.num_unsatisfied == 0; }
+  static std::string report_reason(const g16_witness_report& w) {
+    if (w.first_malformed == 0) return "assignment element 0 is not One";
+    if (w.first_malformed != G16_NONE)
+      return "assignment element " + std::to_string(w.first_malformed) + " is not a canonical Fr";
+    return "constraint " + std::to_string(w.first_unsatisfied) + " unsatisfied (" + std::to_string(w.num_unsatisfied) + " in all)";
+  }
+  // The verdict of a single-proof submission, once its main stream has drained: G16_OK, or G16_ERR_UNSATISFIED naming why
+  int slot_verdict(const Slot& sl) const {
+    if (!sl.check) return G16_OK;
+    const g16_witness_report w = report_of(sl.h_check);
+    return report_ok(w) ? G16_OK : fail(G16_ERR_UNSATISFIED, report_reason(w));
+  }
+  // g16_check_witness: slot 0's main stream, one launch per chunk of at most R1CS_CHECK_MAX_Y assignments; host assignments
+  // go up chunk by chunk, each chunk at most half the free device memory
+  int check_witness(uint32_t count, const uint64_t* z, uint32_t flags, g16_witness_report* out) override {
+    if (count == 0) return G16_OK;
+    if (flags & ~(uint32_t)G16_ASSIGNMENT_ON_DEVICE) return fail(G16_ERR_BAD_ARGUMENT, "g16_check_witness takes G16_ASSIGNMENT_ON_DEVICE only");
+    if (!z || !out) return fail(G16_ERR_BAD_ARGUMENT, "null buffer");
+    if (!have_circuit) return fail(G16_ERR_BAD_ARGUMENT, "no circuit resident");
+    if (S0.busy) return fail(G16_ERR_BAD_ARGUMENT, "slot 0 has a proof in flight");
+    G16_CUDA(cudaSetDevice(device));
+    const bool on_device = (flags & G16_ASSIGNMENT_ON_DEVICE) != 0;
+    const uint64_t nv = nvars();
+    const size_t zb = (size_t)nv * sizeof(Fr);
+    uint64_t chunk = std::min<uint64_t>(count, R1CS_CHECK_MAX_Y);
+    DevBuf dz, dres;
+    if (!on_device) {
+      size_t free_b = 0, total_b = 0;
+      G16_CUDA(cudaMemGetInfo(&free_b, &total_b));
+      chunk = std::max<uint64_t>(1, std::min<uint64_t>(chunk, free_b / 2 / zb));
+      G16_CUDA(dz.reserve(chunk * zb));
+    }
+    G16_CUDA(dres.reserve(chunk * 3 * sizeof(uint32_t)));
+    std::vector<uint32_t> res(chunk * 3);
+    CsrDev cs[3];
+    csr_dev(cs);
+    cudaStream_t st = S0.st_main;
+    for (uint64_t first = 0; first < count; first += chunk) {
+      const uint32_t k = (uint32_t)std::min<uint64_t>(chunk, count - first);
+      const uint64_t* src = z + first * nv * FR64;
+      if (!on_device) G16_CUDA(cudaMemcpyAsync(dz.p, src, k * zb, cudaMemcpyHostToDevice, st));
+      const Fr* zk = on_device ? reinterpret_cast<const Fr*>(src) : dz.template as<Fr>();
+      G16_CUDA(r1cs_check<Fr>(st, cs, zk, num_constraints, (uint32_t)nv, k, dres.template as<uint32_t>(), &ntt_launches));
+      G16_CUDA(cudaMemcpyAsync(res.data(), dres.p, (size_t)k * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+      G16_CUDA(cudaStreamSynchronize(st));
+      for (uint32_t i = 0; i < k; i++) out[first + i] = report_of(&res[3 * (size_t)i]);
+    }
     return G16_OK;
   }
   int witness_map(const uint64_t* z, uint32_t flags, uint64_t* h) override {
@@ -1319,6 +1406,10 @@ struct Engine : IEngine {
     G16_CUDA(cudaSetDevice(device));
     int rc = enqueue_witness_map(S0, z, flags);
     if (rc) return rc;
+    if (S0.check) {   // a rejected assignment writes nothing to h
+      G16_CUDA(cudaStreamSynchronize(S0.st_main));
+      if ((rc = slot_verdict(S0))) return rc;
+    }
     G16_CUDA(cudaMemcpyAsync(h, S0.d_h.p, sizeof(Fr) << L, cudaMemcpyDeviceToHost, S0.st_main));
     G16_CUDA(cudaStreamSynchronize(S0.st_main));
     return G16_OK;
@@ -1469,7 +1560,7 @@ struct Engine : IEngine {
     int rc = submit(S0, r, nullptr, z, flags);
     if (rc) return rc;
     Partials x;
-    if ((rc = wait_partials(S0, x))) return rc;
+    if ((rc = wait_partials(S0, x)) || (rc = slot_verdict(S0))) return rc;
     store_partials(partial, x);
     return G16_OK;
   }
@@ -1481,7 +1572,7 @@ struct Engine : IEngine {
     if (slot < 0 || slot >= NSLOTS || !partial) return fail(G16_ERR_BAD_ARGUMENT, "bad slot / null buffer");
     Partials x;
     int rc = wait_partials(slots[slot], x);
-    if (rc) return rc;
+    if (rc || (rc = slot_verdict(slots[slot]))) return rc;
     store_partials(partial, x);
     return G16_OK;
   }
@@ -1547,7 +1638,7 @@ struct Engine : IEngine {
     Slot& sl = slots[slot];
     Partials x;
     int rc = wait_proof(sl, x);
-    if (rc) return rc;
+    if (rc || (rc = slot_verdict(sl))) return rc;
     auto t0 = std::chrono::steady_clock::now();
     store_proof(proof, sl.kp, x.a, x.b2, c_part(sl.r, sl.s, x));
     sl.tm.host_finish_ms += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
@@ -1663,8 +1754,11 @@ struct Engine : IEngine {
     batch_geoms(count, share_b_sort && sl.run[M_B1] && sl.run[M_B2], sl.geom);
     return enqueue_msms(sl);
   }
-  // wait for the slot's group, then finish its proofs on the pool (one proof per task); adds the group to `acc`
-  int batch_finish(Slot& sl, const uint64_t* r, const uint64_t* s, uint64_t* proofs, g16_timings& acc, float* host_ms) {
+  // wait for the slot's group, then finish its proofs on the pool (one proof per task); adds the group to `acc`.  Under
+  // G16_CHECK_WITNESS a rejected proof is written as all-zero limbs, and the first one of the call is kept in *rejected
+  // (index, reason)
+  int batch_finish(Slot& sl, const uint64_t* r, const uint64_t* s, uint64_t* proofs, g16_timings& acc, float* host_ms,
+                   std::pair<int64_t, std::string>* rejected) {
     const uint32_t count = sl.batch_count, first = sl.batch_first;
     sl.batch_count = 0;
     for (int m = 0; m < 5 && !sl.serial; m++) G16_CUDA(cudaStreamSynchronize(sl.st_msm[m]));
@@ -1674,6 +1768,14 @@ struct Engine : IEngine {
     const A2* o2 = reinterpret_cast<const A2*>(o1 + 4 * (size_t)count);
     std::vector<std::shared_ptr<HostPool::Ticket>> tk(count);
     for (uint32_t k = 0; k < count; k++) {
+      if (sl.check) {
+        const g16_witness_report w = report_of(sl.h_check + 3 * (size_t)k);
+        if (!report_ok(w)) {
+          memset(proofs + (size_t)(first + k) * PROOF64, 0, PROOF64 * sizeof(uint64_t));   // three identity points
+          if (rejected->first < 0) *rejected = {(int64_t)(first + k), report_reason(w)};   // groups finish in order
+          continue;
+        }
+      }
       tk[k] = pool->submit([&, k]() {
         const Products kp{P1::from_affine(o1[k]), P1::from_affine(o1[count + k]), P1::from_affine(o1[2 * (size_t)count + k]),
                           P1::from_affine(o1[3 * (size_t)count + k]), P2::from_affine(o2[k])};
@@ -1685,7 +1787,7 @@ struct Engine : IEngine {
         store_proof(proofs + (size_t)(first + k) * PROOF64, kp, x.a, x.b2, c_part(rk, sk, x));
       });
     }
-    for (auto& t : tk) t->wait();
+    for (auto& t : tk) if (t) t->wait();
     *host_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
     add_timings(sl, ev_batch, first == 0, acc);
     acc.d2h_bytes += tail_point_bytes(count);
@@ -1711,12 +1813,13 @@ struct Engine : IEngine {
     G16_CUDA(cudaEventRecord(ev_batch, slots[0].st_main));
     g16_timings acc{};
     float host_ms = 0;
+    std::pair<int64_t, std::string> rejected{-1, std::string()};   // lowest proof rejected by G16_CHECK_WITNESS
     int order[NSLOTS] = {-1, -1};   // slots holding a group, oldest first
     auto finish_oldest = [&]() -> int {
       const int si = order[0];
       order[0] = order[1];
       order[1] = -1;
-      return batch_finish(slots[si], r, s, proofs, acc, &host_ms);
+      return batch_finish(slots[si], r, s, proofs, acc, &host_ms, &rejected);
     };
     for (uint32_t first = 0, gi = 0; first < count && !rc; first += G, gi++) {
       const int si = nslots > 1 ? (int)(gi & 1) : 0;
@@ -1733,6 +1836,7 @@ struct Engine : IEngine {
     acc.host_finish_ms = host_ms;   // host work after the last group's GPU work
     acc.launches = ctr.launches + ntt_launches - launches0;
     tm = acc;
+    if (rejected.first >= 0) return fail(G16_ERR_UNSATISFIED, "proof " + std::to_string(rejected.first) + ": " + rejected.second);
     return G16_OK;
   }
   // ---- sharded proof with the exchange inside the library (g16_comm_init + g16_prove_sharded*) ----
@@ -1825,6 +1929,9 @@ struct Engine : IEngine {
     if (rc != 0) return fail(G16_ERR_CUDA, std::string("ncclAllGather: ") + api.GetErrorString(rc));
     G16_CUDA(cudaMemcpyAsync(h_comm_recv, d_comm_recv.p, REC_LIMBS * 8 * comm_world, cudaMemcpyDeviceToHost, st_comm));
     G16_CUDA(cudaStreamSynchronize(st_comm));
+    // every rank checked the same assignment and reaches the same verdict, but only after its part of every exchange: a
+    // rank that left one out would leave the others waiting
+    if ((rc = slot_verdict(sl))) return rc;
     P1 a_sum = P1::inf(), c_sum = P1::inf();
     P2 b2_sum = P2::inf();
     for (uint32_t k = 0; k < comm_world; k++) {           // fixed rank order; the sum is order-independent anyway

@@ -174,6 +174,16 @@ struct CsrDev {
   const uint32_t* col;
   const void* val;          // Fr, Montgomery
 };
+// <M_i, z>: row i of one CSR matrix times the assignment
+template <class Fr>
+__device__ __forceinline__ Fr r1cs_row_dot(const CsrDev& M, uint32_t i, const Fr* __restrict__ z) {
+  const uint32_t lo = M.row_ptr[i], hi = M.row_ptr[i + 1];
+  const Fr* vals = reinterpret_cast<const Fr*>(M.val);
+  Fr acc = Fr::zero();
+  for (uint32_t e = lo; e < hi; e++) acc = Fr::add(acc, Fr::mul(ntt_ldg(vals + e), ntt_ldg(z + M.col[e])));
+  return acc;
+}
+
 template <class Fr, bool WITH_C>
 __global__ void __launch_bounds__(256) r1cs_matvec_kernel(CsrDev A, CsrDev B, CsrDev Cm, const Fr* __restrict__ z,
                                                           uint32_t nc, uint32_t num_inputs, uint32_t n, Fr* a, Fr* b,
@@ -186,22 +196,63 @@ __global__ void __launch_bounds__(256) r1cs_matvec_kernel(CsrDev A, CsrDev B, Cs
   c += (size_t)blockIdx.y * n;
   Fr ra = Fr::zero(), rb = Fr::zero(), rc = Fr::zero();
   if (i < nc) {
-    const CsrDev* ms[3] = {&A, &B, &Cm};
-    Fr* outs[3] = {&ra, &rb, &rc};
-#pragma unroll
-    for (int m = 0; m < (WITH_C ? 3 : 2); m++) {
-      const uint32_t lo = ms[m]->row_ptr[i], hi = ms[m]->row_ptr[i + 1];
-      const Fr* vals = reinterpret_cast<const Fr*>(ms[m]->val);
-      Fr acc = Fr::zero();
-      for (uint32_t e = lo; e < hi; e++) acc = Fr::add(acc, Fr::mul(ntt_ldg(vals + e), ntt_ldg(z + ms[m]->col[e])));
-      *outs[m] = acc;
-    }
+    ra = r1cs_row_dot(A, i, z);
+    rb = r1cs_row_dot(B, i, z);
+    if (WITH_C) rc = r1cs_row_dot(Cm, i, z);
   } else if (i < nc + num_inputs) {
     ra = ntt_ldg(z + (i - nc));
   }
   ntt_stg(a + i, ra);
   ntt_stg(b + i, rb);
   if (WITH_C) ntt_stg(c + i, rc);
+}
+
+// The limbs of x, read as an integer, are >= the modulus: x is not a canonical field element
+template <class Fr>
+__device__ __forceinline__ bool fr_noncanonical(const Fr& x) {
+  const Fr p = Fr::modulus();
+  bool ge = true;   // equal so far
+#pragma unroll
+  for (int w = 0; w < Fr::N; w++) ge = x.v[w] > p.v[w] || (x.v[w] == p.v[w] && ge);   // little-endian limbs
+  return ge;
+}
+
+// R1CS satisfiability of `count` assignments (ark-relations ConstraintSystem::is_satisfied / which_is_unsatisfied), one
+// launch for rows and elements.  blockIdx.y = proof k: it reads z + k * nv and writes out[3k .. 3k + 2].
+//   rows     thread i < nc: constraint i is unsatisfied when <A_i,z> <B_i,z> != <C_i,z> (values are fully reduced, so ==
+//            compares them).  Only constraint rows: the instance rows the witness map appends are not constraints.
+//   elements grid-stride over j < nv: z[j] is malformed when its limbs are >= r, z[0] also when it is not One.
+// out[3k] = lowest unsatisfied row, out[3k + 1] = ~(unsatisfied rows), out[3k + 2] = lowest malformed element.  All three
+// start at 0xffffffff (one memset), which is why the count is kept as its complement and counted down.  The lanes of a warp
+// hold consecutive indices, so a warp's lowest index is its base plus the first set bit of its ballot: one atomic per warp
+// and value.  Malformed limbs make the row values meaningless (the field operations assume inputs < p) but never an index:
+// the columns were checked at g16_circuit_load.
+template <class Fr>
+__global__ void __launch_bounds__(256) r1cs_check_kernel(CsrDev A, CsrDev B, CsrDev Cm, const Fr* __restrict__ z,
+                                                         uint32_t nc, uint32_t nv, uint32_t* out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+  z += (size_t)blockIdx.y * nv;
+  out += 3 * (size_t)blockIdx.y;
+  const bool bad = i < nc && Fr::mul(r1cs_row_dot(A, i, z), r1cs_row_dot(B, i, z)) != r1cs_row_dot(Cm, i, z);
+  const uint32_t rows = __ballot_sync(0xffffffffu, bad);
+  if (rows && lane == 0) {
+    atomicMin(out, i + __ffs(rows) - 1);
+    atomicSub(out + 1, (uint32_t)__popc(rows));
+  }
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t j0 = i - lane; j0 < nv; j0 += stride) {   // j0: the warp's base, so every lane runs the same iterations
+    const uint64_t j = j0 + lane;
+    bool mal = false;
+    if (j < nv) {
+      const Fr x = ntt_ldg(z + j);
+      mal = j == 0 ? x != Fr::one() : fr_noncanonical(x);
+    }
+    const uint32_t els = __ballot_sync(0xffffffffu, mal);
+    if (els) {   // later iterations of this warp only see higher indices
+      if (lane == 0) atomicMin(out + 2, (uint32_t)j0 + __ffs(els) - 1);
+      break;
+    }
+  }
 }
 
 // h[i] = a[i] * b[i] - c[i], i < n: the pointwise step of CircomReduction when a, b, c were transformed on different GPUs
@@ -391,6 +442,23 @@ void r1cs_matvec(cudaStream_t st, const CsrDev* cs, const Fr* z, uint32_t nc, ui
   else r1cs_matvec_kernel<Fr, false><<<grid, 256, 0, st>>>(cs[0], cs[1], cs[2], z, nc, num_inputs, n, a, b, c, nv);
 }
 
+// Satisfiability of `count` assignments (z, nv elements apart) into out (count * 3 u32, device; see r1cs_check_kernel):
+// the memset, then one launch per 65535 proofs (the grid-y limit)
+static constexpr uint32_t R1CS_CHECK_MAX_Y = 65535;
+template <class Fr>
+cudaError_t r1cs_check(cudaStream_t st, const CsrDev* cs, const Fr* z, uint32_t nc, uint32_t nv, uint32_t count, uint32_t* out,
+                       unsigned long long* launches) {
+  cudaError_t e = cudaMemsetAsync(out, 0xff, (size_t)count * 3 * sizeof(uint32_t), st);
+  if (e != cudaSuccess) return e;
+  const unsigned bx = (nc > 0 ? (nc + 255) / 256 : 1u);
+  for (uint32_t k = 0; k < count; k += R1CS_CHECK_MAX_Y) {
+    const uint32_t ky = count - k < R1CS_CHECK_MAX_Y ? count - k : R1CS_CHECK_MAX_Y;
+    r1cs_check_kernel<Fr><<<dim3(bx, ky), 256, 0, st>>>(cs[0], cs[1], cs[2], z + (size_t)k * nv, nc, nv, out + 3 * (size_t)k);
+    if (launches) (*launches)++;
+  }
+  return cudaGetLastError();
+}
+
 // h = a o b - c over `count` vectors of n elements (one launch)
 template <class Fr>
 void ntt_ab_minus_c(cudaStream_t st, const Fr* a, const Fr* b, const Fr* c, Fr* h, uint64_t n) {
@@ -404,6 +472,8 @@ void ntt_ab_minus_c(cudaStream_t st, const Fr* a, const Fr* b, const Fr* c, Fr* 
   X cudaError_t ntt_domain_build_odd<Fr>(NttDomain<Fr>&, cudaStream_t, unsigned long long*);                           \
   X void r1cs_matvec<Fr>(cudaStream_t, const CsrDev*, const Fr*, uint32_t, uint32_t, uint32_t, Fr*, Fr*, Fr*, uint32_t, uint32_t, \
                          bool);                                                                                         \
+  X cudaError_t r1cs_check<Fr>(cudaStream_t, const CsrDev*, const Fr*, uint32_t, uint32_t, uint32_t, uint32_t*,            \
+                               unsigned long long*);                                                                    \
   X void ntt_ab_minus_c<Fr>(cudaStream_t, const Fr*, const Fr*, const Fr*, Fr*, uint64_t);
 
 }  // namespace g16

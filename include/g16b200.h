@@ -41,8 +41,10 @@ enum {
   G16_ERR_BAD_ARGUMENT = 2,                /* null pointer / inconsistent length / unknown curve               */
   G16_ERR_CUDA = 3,                        /* CUDA failure or no usable sm_90 device; see g16_last_error()     */
   G16_ERR_MALFORMED_KEY = 4,               /* SynthesisError::MalformedVerifyingKey-class length mismatch      */
-  G16_ERR_INVALID_DATA = 5                 /* ark_serialize::SerializationError::{InvalidData, UnexpectedFlags,
+  G16_ERR_INVALID_DATA = 5,                /* ark_serialize::SerializationError::{InvalidData, UnexpectedFlags,
                                               NotEnoughSpace}: a rejected serialized key                         */
+  G16_ERR_UNSATISFIED = 6                  /* SynthesisError::Unsatisfiable: G16_CHECK_WITNESS rejected the assignment;
+                                              g16_last_error() names the constraint or element                  */
 };
 
 typedef struct g16_ctx g16_ctx;
@@ -50,7 +52,8 @@ typedef struct g16_ctx g16_ctx;
 /* Flags for g16_prove* (bitwise or) */
 enum {
   G16_ASSIGNMENT_ON_DEVICE = 1, /* `full_assignment` is a device pointer (bench.py's resident-input measurement) */
-  G16_SERIAL_MSMS = 2           /* run the five MSMs one after another on one stream (kernel-level profiling)    */
+  G16_SERIAL_MSMS = 2,          /* run the five MSMs one after another on one stream (kernel-level profiling)    */
+  G16_CHECK_WITNESS = 4         /* refuse an assignment that does not satisfy the circuit: see g16_check_witness  */
 };
 
 /* ---- context ----------------------------------------------------------------------------------------------- */
@@ -251,6 +254,45 @@ int g16_prove_sharded_wait(g16_ctx* ctx, int slot, uint64_t* proof_out);
 /* ---- witness map alone on the resident circuit (R1CSToQAP::witness_map_from_matrices, r1cs_to_qap.rs:172-235):
  * h_out receives domain_size Montgomery Fr coefficients (G16_QAP_CIRCOM: domain_size evaluations, see above). */
 int g16_witness_map(g16_ctx* ctx, const uint64_t* full_assignment, uint32_t flags, uint64_t* h_out);
+
+/* ---- R1CS satisfiability of assignments of the resident circuit: ark-relations ConstraintSystem::is_satisfied /
+ * which_is_unsatisfied (ark-groth16 checks it only as debug_assert!, prover.rs:193).  A GPU pass over the resident
+ * matrices, independent of the reduction (matrix C is read under G16_QAP_CIRCOM too, whose witness map never reads it).
+ * Per assignment z:
+ *   first_malformed   lowest j whose limbs, read as an integer, are >= r, or 0 when z[0] is not One (Montgomery R mod r);
+ *                     G16_NONE if none.  When set, the rows are not evaluated: first_unsatisfied = G16_NONE and
+ *                     num_unsatisfied = 0 (the field arithmetic assumes canonical inputs).
+ *   first_unsatisfied lowest constraint i < num_constraints with <A_i,z> <B_i,z> != <C_i,z>, or G16_NONE.  Only the
+ *                     constraints: the instance rows LibsnarkReduction appends are not checked.
+ *   num_unsatisfied   how many constraints are unsatisfied.
+ * g16_check_witness: `count` assignments of nv = num_inputs + num_witness Montgomery Fr each (host, or device with
+ * G16_ASSIGNMENT_ON_DEVICE, the only flag it takes) -> reports_out[count].  Needs a resident circuit, no key.  Returns
+ * G16_OK whatever the verdicts; an unknown flag, a null pointer, no circuit or a proof in flight in slot 0 is
+ * G16_ERR_BAD_ARGUMENT; count == 0 returns G16_OK and touches nothing.  Runs on slot 0; host assignments are uploaded in
+ * chunks bounded by the free device memory.  Results never depend on the chunking, the reduction or the options.
+ *
+ * G16_CHECK_WITNESS, a flag of g16_prove, g16_prove_submit, g16_prove_batch, g16_prove_partial (+ submit), g16_prove_sharded
+ * (+ submit) and g16_witness_map, runs the same check on the device copy of the assignment, as one more kernel launch per
+ * proof or batch group (g16_get_timings' launches grows by exactly 1; by one more per 65535 proofs of a group).  The check
+ * never changes what else is enqueued: a rejected proof's GPU work, and a sharded proof's NCCL exchanges, run to completion,
+ * and the slot is free after its wait.  The verdict is read where the results are collected (g16_prove_wait,
+ * g16_prove_partial_wait, g16_prove_sharded_wait, the end of g16_prove_batch):
+ *   single proof, partial, witness map: G16_ERR_UNSATISFIED and nothing written to proof_out / partial_out / h_out;
+ *     g16_last_error() names the reason, e.g. "constraint 1234 unsatisfied (17 in all)" or "assignment element 5 is not a
+ *     canonical Fr".
+ *   batch: every proof is computed; a rejected proof's entry of proofs_out is all-zero limbs (three identity points, which
+ *     never verify), every other entry is what the call without the flag writes.  The call returns G16_ERR_UNSATISFIED
+ *     naming the lowest rejected proof and its reason ("proof 3: constraint 0 unsatisfied (1 in all)"); g16_check_witness
+ *     gives every proof's report.
+ * Without the flag nothing is launched or copied: outputs and launch counts are those of the call without it. */
+#define G16_NONE UINT64_MAX
+typedef struct {
+  uint64_t first_unsatisfied;
+  uint64_t num_unsatisfied;
+  uint64_t first_malformed;
+} g16_witness_report;
+int g16_check_witness(g16_ctx* ctx, uint32_t count, const uint64_t* full_assignments, uint32_t flags,
+                      g16_witness_report* reports_out);
 
 /* ---- measurement hooks (bench.py) ---------------------------------------------------------------------------- */
 typedef struct {

@@ -42,7 +42,7 @@ use ark_relations::r1cs::{
     Result as R1CSResult, SynthesisError,
 };
 use ark_std::{
-    cell::RefCell,
+    cell::{Cell, RefCell},
     collections::BTreeMap,
     marker::PhantomData,
     rand::{Rng, RngCore},
@@ -58,6 +58,12 @@ fn status(rc: i32) -> R1CSResult<()> {
         sys::G16_OK => Ok(()),
         sys::G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE => Err(SynthesisError::PolynomialDegreeTooLarge), // r1cs_to_qap.rs:134,179
         sys::G16_ERR_MALFORMED_KEY => Err(SynthesisError::MalformedVerifyingKey),                  // verifier.rs:30
+        sys::G16_ERR_UNSATISFIED => {
+            // G16_CHECK_WITNESS refused the assignment; the message names the constraint or element
+            let msg = unsafe { CStr::from_ptr(sys::g16_last_error()) }.to_string_lossy().into_owned();
+            eprintln!("libg16b200: {msg}");
+            Err(SynthesisError::Unsatisfiable)
+        },
         _ => {
             // G16_ERR_BAD_ARGUMENT / G16_ERR_CUDA carry a message; SynthesisError has no string variant
             let msg = unsafe { CStr::from_ptr(sys::g16_last_error()) }.to_string_lossy().into_owned();
@@ -205,6 +211,7 @@ pub struct B200Prover<E: SwPairing> {
     num_variables: usize,
     fq_limbs: usize,
     g2_limbs: usize,   // one G2 affine point: 4 * fq_limbs over Fq2, 2 * fq_limbs on BW6-761 (G2 over Fq)
+    flags: Cell<u32>,  // ored into every prove call: G16_CHECK_WITNESS after set_check_witness(true)
     _e: PhantomData<E>,
 }
 // the context is used by one thread at a time (include/g16b200.h); moving it between threads is fine
@@ -245,6 +252,7 @@ impl<E: SwPairing> B200Prover<E> {
             num_variables: matrices.num_instance_variables + matrices.num_witness_variables,
             fq_limbs: unsafe { sys::g16_fq_limbs(ctx) } as usize,
             g2_limbs: unsafe { sys::g16_g2_limbs(ctx) } as usize,
+            flags: Cell::new(0),
             _e: PhantomData,
         };
         let (a, b, c) = (Csr::new(&matrices.a), Csr::new(&matrices.b), Csr::new(&matrices.c));
@@ -322,6 +330,7 @@ impl<E: SwPairing> B200Prover<E> {
             num_variables: matrices.num_instance_variables + matrices.num_witness_variables,
             fq_limbs: unsafe { sys::g16_fq_limbs(ctx) } as usize,
             g2_limbs: unsafe { sys::g16_g2_limbs(ctx) } as usize,
+            flags: Cell::new(0),
             _e: PhantomData,
         };
         let (a, b, c) = (Csr::new(&matrices.a), Csr::new(&matrices.b), Csr::new(&matrices.c));
@@ -404,6 +413,52 @@ impl<E: SwPairing> B200Prover<E> {
         Proof { a: unpack_point(&out[..2 * n]), b: unpack_point(&out[2 * n..2 * n + g]), c: unpack_point(&out[2 * n + g..4 * n + g]) }
     }
 
+    /// Check every assignment against the circuit on the GPU before proving it (`G16_CHECK_WITNESS` on every prove call of
+    /// this prover).  Off by default.  A refused proof is `SynthesisError::Unsatisfiable`, with the constraint or element
+    /// on stderr; in `create_proofs_batch` the whole call fails (`check_witness` tells which assignments were bad).
+    pub fn set_check_witness(&self, on: bool) {
+        let f = self.flags.get() & !sys::G16_CHECK_WITNESS;
+        self.flags.set(if on { f | sys::G16_CHECK_WITNESS } else { f });
+    }
+
+    /// g16_check_witness: one report per assignment (fields as in the header; `sys::G16_NONE` where there is none).
+    pub fn check_witness(&self, assignments: &[Vec<E::ScalarField>]) -> R1CSResult<Vec<sys::g16_witness_report>> {
+        if assignments.iter().any(|z| z.len() != self.num_variables) || assignments.len() > u32::MAX as usize {
+            return Err(SynthesisError::MalformedVerifyingKey);
+        }
+        let mut out = ark_std::vec![sys::g16_witness_report::default(); assignments.len()];
+        if assignments.is_empty() {
+            return Ok(out);
+        }
+        let z: Vec<E::ScalarField> = assignments.concat();
+        status(unsafe { sys::g16_check_witness(self.ctx, assignments.len() as u32, scalars_ptr(&z), 0, out.as_mut_ptr()) })?;
+        Ok(out)
+    }
+    fn check_one(&self, full_assignment: &[E::ScalarField]) -> R1CSResult<sys::g16_witness_report> {
+        if full_assignment.len() != self.num_variables {
+            return Err(SynthesisError::MalformedVerifyingKey);
+        }
+        let mut w = sys::g16_witness_report::default();
+        status(unsafe { sys::g16_check_witness(self.ctx, 1, scalars_ptr(full_assignment), 0, &mut w) })?;
+        Ok(w)
+    }
+    /// `ConstraintSystem::is_satisfied` of `full_assignment` (instance || witness) on the resident circuit.  An element that
+    /// is not a canonical field element, or a first element other than One, is unsatisfied.
+    pub fn is_satisfied(&self, full_assignment: &[E::ScalarField]) -> R1CSResult<bool> {
+        let w = self.check_one(full_assignment)?;
+        Ok(w.first_malformed == sys::G16_NONE && w.num_unsatisfied == 0)
+    }
+    /// `ConstraintSystem::which_is_unsatisfied`, by index: the lowest unsatisfied constraint (there are no constraint
+    /// names at this boundary).  A malformed assignment is `SynthesisError::Unsatisfiable`.
+    pub fn which_is_unsatisfied(&self, full_assignment: &[E::ScalarField]) -> R1CSResult<Option<usize>> {
+        let w = self.check_one(full_assignment)?;
+        if w.first_malformed != sys::G16_NONE {
+            eprintln!("libg16b200: assignment element {} is malformed", w.first_malformed);
+            return Err(SynthesisError::Unsatisfiable);
+        }
+        Ok(if w.first_unsatisfied == sys::G16_NONE { None } else { Some(w.first_unsatisfied as usize) })
+    }
+
     /// Drop-in for `Groth16::<E>::create_proof_with_reduction_and_matrices` (src/prover.rs:26-51).  `pk` and `matrices` are
     /// the ones made resident by `new`; they are accepted (and their sizes checked) so that call sites read the same.
     #[allow(clippy::too_many_arguments)]
@@ -422,7 +477,7 @@ impl<E: SwPairing> B200Prover<E> {
         }
         let mut out = ark_std::vec![0u64; self.proof_limbs()];
         status(unsafe {
-            sys::g16_prove(self.ctx, fp_limbs(&r).as_ptr(), fp_limbs(&s).as_ptr(), scalars_ptr(full_assignment), 0, out.as_mut_ptr())
+            sys::g16_prove(self.ctx, fp_limbs(&r).as_ptr(), fp_limbs(&s).as_ptr(), scalars_ptr(full_assignment), self.flags.get(), out.as_mut_ptr())
         })?;
         Ok(self.proof_from_limbs(&out))
     }
@@ -488,7 +543,7 @@ impl<E: SwPairing> B200Prover<E> {
         let w = self.proof_limbs();
         let mut out = ark_std::vec![0u64; count * w];
         status(unsafe {
-            sys::g16_prove_batch(self.ctx, count as u32, scalars_ptr(rs), scalars_ptr(ss), scalars_ptr(&z), 0, 0, out.as_mut_ptr())
+            sys::g16_prove_batch(self.ctx, count as u32, scalars_ptr(rs), scalars_ptr(ss), scalars_ptr(&z), 0, self.flags.get(), out.as_mut_ptr())
         })?;
         Ok(out.chunks(w).map(|p| self.proof_from_limbs(p)).collect())
     }
@@ -506,7 +561,7 @@ impl<E: SwPairing> B200Prover<E> {
     /// Multi-GPU, first half: this rank's five partial MSM sums ([h, l, a, b_g1] G1 affine, then b_g2 G2 affine).
     pub fn prove_partial(&self, r: E::ScalarField, full_assignment: &[E::ScalarField]) -> R1CSResult<Vec<u64>> {
         let mut out = ark_std::vec![0u64; unsafe { sys::g16_partial_limbs(self.ctx) } as usize];
-        status(unsafe { sys::g16_prove_partial(self.ctx, fp_limbs(&r).as_ptr(), scalars_ptr(full_assignment), 0, out.as_mut_ptr()) })?;
+        status(unsafe { sys::g16_prove_partial(self.ctx, fp_limbs(&r).as_ptr(), scalars_ptr(full_assignment), self.flags.get(), out.as_mut_ptr()) })?;
         Ok(out)
     }
     /// Multi-GPU, second half: all ranks' partial records (rank order), gathered by the caller (MPI / NCCL all-gather).

@@ -19,6 +19,7 @@ pub const G16_ERR_BAD_ARGUMENT: c_int = 2;
 pub const G16_ERR_CUDA: c_int = 3;
 pub const G16_ERR_MALFORMED_KEY: c_int = 4;
 pub const G16_ERR_INVALID_DATA: c_int = 5;
+pub const G16_ERR_UNSATISFIED: c_int = 6;
 
 pub const G16_SER_COMPRESSED: u32 = 1;
 pub const G16_SER_VALIDATE: u32 = 2;
@@ -28,6 +29,17 @@ pub const G16_QAP_CIRCOM: c_int = 1;
 
 pub const G16_ASSIGNMENT_ON_DEVICE: u32 = 1;
 pub const G16_SERIAL_MSMS: u32 = 2;
+pub const G16_CHECK_WITNESS: u32 = 4;
+
+pub const G16_NONE: u64 = u64::MAX;
+
+#[repr(C)]
+#[derive(Default, Clone, Copy, Debug, PartialEq, Eq)]
+pub struct g16_witness_report {
+    pub first_unsatisfied: u64,
+    pub num_unsatisfied: u64,
+    pub first_malformed: u64,
+}
 
 #[repr(C)]
 pub struct g16_csr {
@@ -144,6 +156,7 @@ extern "C" {
     pub fn g16_prove_sharded_submit(ctx: *mut g16_ctx, slot: c_int, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32) -> c_int;
     pub fn g16_prove_sharded_wait(ctx: *mut g16_ctx, slot: c_int, proof_out: *mut u64) -> c_int;
     pub fn g16_witness_map(ctx: *mut g16_ctx, full_assignment: *const u64, flags: u32, h_out: *mut u64) -> c_int;
+    pub fn g16_check_witness(ctx: *mut g16_ctx, count: u32, full_assignments: *const u64, flags: u32, reports_out: *mut g16_witness_report) -> c_int;
     pub fn g16_get_timings(ctx: *const g16_ctx, out: *mut g16_timings) -> c_int;
     pub fn g16_synthetic_r1cs(curve: c_int, log_n: u32, seed: u64, a_col: *mut u32, a_val: *mut u64, b_col: *mut u32, c_col: *mut u32, full_assignment: *mut u64) -> c_int;
     pub fn g16_get_config(ctx: *const g16_ctx, out: *mut g16_config) -> c_int;
