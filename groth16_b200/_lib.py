@@ -27,6 +27,16 @@ class PkExportDesc(C.Structure):
                                     "beta_g1", "delta_g1", "beta_g2", "gamma_g2", "delta_g2", "gamma_abc_g1")]
 
 
+class SrsDesc(C.Structure):
+    _fields_ = [("tau_g1", u64p), ("tau_g1_len", C.c_uint64), ("tau_g2", u64p), ("tau_g2_len", C.c_uint64),
+                ("alpha_tau_g1", u64p), ("alpha_tau_g1_len", C.c_uint64), ("beta_tau_g1", u64p),
+                ("beta_tau_g1_len", C.c_uint64), ("beta_g2", u64p)]
+
+
+class SrsOut(C.Structure):
+    _fields_ = SrsDesc._fields_
+
+
 class Timings(C.Structure):
     _fields_ = [("total_ms", C.c_float), ("h2d_ms", C.c_float), ("witness_map_ms", C.c_float),
                 ("msm_ms", C.c_float * 5), ("msm_accum_ms", C.c_float * 5), ("host_finish_ms", C.c_float),
@@ -63,6 +73,9 @@ SIGNATURES = [
     ("g16_pk_load", C.c_int, [C.c_void_p, C.POINTER(PkDesc), C.c_uint32, C.c_uint32]),
     ("g16_setup", C.c_int, [C.c_void_p] + [C.c_void_p] * 7),
     ("g16_pk_export", C.c_int, [C.c_void_p, C.POINTER(PkExportDesc)]),
+    ("g16_setup_from_srs", C.c_int, [C.c_void_p, C.POINTER(SrsDesc), C.c_uint32]),
+    ("g16_setup_contribute", C.c_int, [C.c_void_p, C.c_void_p]),
+    ("g16_srs_from_secrets", C.c_int, [C.c_void_p] + [C.c_void_p] * 5 + [C.POINTER(SrsOut)]),
     ("g16_pk_load_serialized", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
                                          C.POINTER(PkExportDesc)]),
     ("g16_pk_export_serialized", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),

@@ -131,6 +131,18 @@ class ProvingKey:
 
 
 @dataclass
+class Srs:
+    """A powers-of-tau transcript (phase 1 of a Groth16 ceremony) as affine Montgomery limbs, identity = all-zero limbs:
+    tau_g1[i] = [tau^i]G1, tau_g2[i] = [tau^i]G2, alpha_tau_g1[i] = [alpha tau^i]G1, beta_tau_g1[i] = [beta tau^i]G1,
+    beta_g2 = [beta]G2.  A circuit with domain size n needs at least 2n - 1, n, n and n points."""
+    tau_g1: np.ndarray
+    tau_g2: np.ndarray
+    alpha_tau_g1: np.ndarray
+    beta_tau_g1: np.ndarray
+    beta_g2: np.ndarray
+
+
+@dataclass
 class WitnessReport:
     """g16_witness_report of one assignment, None where the library reports G16_NONE"""
     first_unsatisfied: Optional[int]   # lowest constraint i with <A_i,z><B_i,z> != <C_i,z>
@@ -321,6 +333,67 @@ class Groth16:
         self.world = 1
         self._pk_obj = self.export_proving_key() if export else None
         return self._pk_obj
+
+    # ---- keys from a powers-of-tau transcript (g16_setup_from_srs) and phase-2 contributions ----
+    def srs_from_secrets(self, g1_len: int, g2_len: int, tau, alpha, beta, g1_generator, g2_generator) -> Srs:
+        """g16_srs_from_secrets, for tests and benchmarks: the transcript of known secrets (Python ints), with g1_len points in
+        tau_g1 and g2_len in tau_g2, alpha_tau_g1 and beta_tau_g1."""
+        cd = self.codec
+        z = lambda rows, w: np.zeros((rows, w), dtype=np.uint64)
+        srs = Srs(z(g1_len, 2 * self.nq), z(g2_len, self.ng2), z(g2_len, 2 * self.nq), z(g2_len, 2 * self.nq),
+                  np.zeros(self.ng2, dtype=np.uint64))
+        d = _lib.SrsOut()
+        for k in ("tau_g1", "tau_g2", "alpha_tau_g1", "beta_tau_g1"):
+            v = getattr(srs, k)
+            setattr(d, k, _u64p(v) if v.size else None)
+            setattr(d, k + "_len", v.shape[0])
+        d.beta_g2 = _u64p(srs.beta_g2)
+        sc = [np.ascontiguousarray(cd.fr.enc1(x)) for x in (tau, alpha, beta)]
+        g1 = np.ascontiguousarray(cd.enc_g1([g1_generator])[0])
+        g2 = np.ascontiguousarray(cd.enc_g2([g2_generator])[0])
+        _check(self._lib.g16_srs_from_secrets(self._ctx, *[_ptr(x) for x in sc], _ptr(g1), _ptr(g2), C.byref(d)))
+        return srs
+
+    def generate_parameters_from_srs(self, matrices: Optional[ConstraintMatrices], srs: Srs, validate: bool = False,
+                                     export: bool = True) -> Optional[ProvingKey]:
+        """g16_setup_from_srs: the proving key of `matrices` (None: the resident circuit) derived on the GPU from a
+        powers-of-tau transcript, with gamma = delta = 1 until contribute_delta.  The key becomes resident; a point the checks
+        refuse raises serialize.DeserializeError naming it, and leaves no key resident."""
+        if matrices is not None:
+            self.load_matrices(matrices)
+        d = _lib.SrsDesc()
+        keep = []
+        for k in ("tau_g1", "tau_g2", "alpha_tau_g1", "beta_tau_g1"):
+            v = getattr(srs, k)
+            v = None if v is None else np.ascontiguousarray(v, dtype=np.uint64)
+            keep.append(v)
+            setattr(d, k, _u64p(v) if v is not None and v.size else None)
+            width = self.ng2 if k == "tau_g2" else 2 * self.nq
+            setattr(d, k + "_len", 0 if v is None else v.size // width)
+        bg2 = None if srs.beta_g2 is None else np.ascontiguousarray(srs.beta_g2, dtype=np.uint64)
+        d.beta_g2 = _u64p(bg2)
+        rc = self._lib.g16_setup_from_srs(self._ctx, C.byref(d), _lib.SER_VALIDATE if validate else 0)
+        self._after_key_change(rc)
+        self._pk_resident = True
+        self.world = 1
+        self._pk_obj = self.export_proving_key() if export else None
+        return self._pk_obj
+
+    def contribute_delta(self, delta, export: bool = True) -> Optional[ProvingKey]:
+        """g16_setup_contribute: one phase-2 contribution delta (Python int) to the resident key made by
+        generate_parameters_with_qap or generate_parameters_from_srs.  Returns the new key when `export`."""
+        dl = np.ascontiguousarray(self.codec.fr.enc1(delta))
+        self._after_key_change(self._lib.g16_setup_contribute(self._ctx, _ptr(dl)))
+        self._pk_obj = self.export_proving_key() if export else None
+        return self._pk_obj
+
+    def _after_key_change(self, rc: int):
+        """Status of g16_setup_from_srs / g16_setup_contribute: argument errors (G16_ERR_BAD_ARGUMENT,
+        G16_ERR_MALFORMED_KEY) leave the previous key resident, any other failure happens after it was released."""
+        if rc not in (_lib.G16_OK, _lib.ERR_BAD_ARGUMENT, _lib.ERR_MALFORMED_KEY):
+            self._pk_resident = False
+            self._pk_obj = None
+        _check(rc)
 
     def export_proving_key(self) -> ProvingKey:
         m = self._matrices

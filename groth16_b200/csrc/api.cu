@@ -145,6 +145,19 @@ int g16_pk_export(g16_ctx* ctx, const g16_pk_export_desc* out) {
   CTX_OR_FAIL(ctx);
   return ctx->eng->pk_export(out);
 }
+int g16_setup_from_srs(g16_ctx* ctx, const g16_srs_desc* srs, uint32_t flags) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->setup_from_srs(srs, flags);
+}
+int g16_setup_contribute(g16_ctx* ctx, const uint64_t* delta) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->setup_contribute(delta);
+}
+int g16_srs_from_secrets(g16_ctx* ctx, const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta, const uint64_t* g1,
+                         const uint64_t* g2, const g16_srs_out* out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->srs_from_secrets(tau, alpha, beta, g1, g2, out);
+}
 int g16_pk_load_serialized(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                            const g16_pk_export_desc* vk_out) {
   CTX_OR_FAIL(ctx);

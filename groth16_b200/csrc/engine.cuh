@@ -9,6 +9,7 @@
 #include <nvtx3/nvToolsExt.h>       // header-only NVTX v3: no-ops unless a profiler injects itself
 #include <nvtx3/nvToolsExtCudaRt.h>
 #include <algorithm>
+#include <array>
 #include <cctype>
 #include <cerrno>
 #include <chrono>
@@ -29,6 +30,7 @@
 #include "msm.cuh"
 #include "ntt.cuh"
 #include "ser.cuh"
+#include "srs.cuh"
 
 namespace g16 {
 
@@ -142,6 +144,10 @@ struct IEngine {
   virtual int setup(const uint64_t* alpha, const uint64_t* beta, const uint64_t* gamma, const uint64_t* delta,
                     const uint64_t* tau, const uint64_t* g1, const uint64_t* g2) = 0;
   virtual int pk_export(const g16_pk_export_desc* out) = 0;
+  virtual int setup_from_srs(const g16_srs_desc* srs, uint32_t flags) = 0;
+  virtual int setup_contribute(const uint64_t* delta) = 0;
+  virtual int srs_from_secrets(const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta, const uint64_t* g1,
+                               const uint64_t* g2, const g16_srs_out* out) = 0;
   virtual int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                                  const g16_pk_export_desc* vk_out) = 0;
   virtual int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) = 0;
@@ -1027,8 +1033,6 @@ struct Engine : IEngine {
     const uint64_t len[5] = {hn, num_witness, nv, nv, nv};
     int rc = begin_key(0, 1, len);
     if (rc) return rc;
-    A1 a_q0, b1_q0;
-    A2 b2_q0;
     {   // the scalars and tables are freed before commit_key weighs the free memory
       DevBuf d_s, tab1, tab2;
       G16_CUDA(d_s.reserve(std::max<uint64_t>(nv, n) * sizeof(Fr)));
@@ -1050,24 +1054,312 @@ struct Engine : IEngine {
       G16_CUDA(up(gabc)); if ((rc = batch_mul<Fq>(g1, d_s.template as<Fr>(), ni, d_gamma_abc.template as<A1>(), tab1))) return rc;
       G16_CUDA(cudaStreamSynchronize(S0.st_main));
     }
-    // MSM views: query[1..]
-    auto view = [&](Query& x, const DevBuf& full, size_t esz) {
-      return nv > 1 ? cudaMemcpyAsync(x.bases.p, (char*)full.p + esz, (nv - 1) * esz, cudaMemcpyDeviceToDevice, S0.st_main) : cudaSuccess;
-    };
-    G16_CUDA(view(q[M_A], full_a, sizeof(A1)));
-    G16_CUDA(view(q[M_B1], full_b1, sizeof(A1)));
-    G16_CUDA(view(q[M_B2], full_b2, sizeof(A2)));
-    G16_CUDA(cudaMemcpyAsync(&a_q0, full_a.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
-    G16_CUDA(cudaMemcpyAsync(&b1_q0, full_b1.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
-    G16_CUDA(cudaMemcpyAsync(&b2_q0, full_b2.p, sizeof(A2), cudaMemcpyDeviceToHost, S0.st_main));
-    G16_CUDA(cudaStreamSynchronize(S0.st_main));
     // single points on the host (generator.rs:147-151,182)
     uint32_t k[Fr::N];
     auto mul1 = [&](const Fr& s) { fr_to_canon(s, k); return P1::from_affine(g1).mul_u32(k, Fr::N).to_affine(); };
     auto mul2 = [&](const Fr& s) { fr_to_canon(s, k); return P2::from_affine(g2).mul_u32(k, Fr::N).to_affine(); };
     alpha_g1 = mul1(alpha); beta_g1 = mul1(beta); delta_g1 = mul1(delta);
     beta_g2 = mul2(beta); gamma_g2 = mul2(gamma); delta_g2 = mul2(delta);
+    return commit_setup_key();
+  }
+  // The last step of every key this library derives itself (g16_setup, g16_setup_from_srs, g16_setup_contribute): full_a,
+  // full_b1, full_b2, d_gamma_abc, copy 0 of the H and L bases and the single points are in place.  Copies the MSM views
+  // query[1..] of A and B and commits the key.
+  int commit_setup_key() {
+    const uint64_t nv = nvars();
+    auto view = [&](Query& x, const DevBuf& full, size_t esz) {
+      return nv > 1 ? cudaMemcpyAsync(x.bases.p, (char*)full.p + esz, (nv - 1) * esz, cudaMemcpyDeviceToDevice, S0.st_main) : cudaSuccess;
+    };
+    G16_CUDA(view(q[M_A], full_a, sizeof(A1)));
+    G16_CUDA(view(q[M_B1], full_b1, sizeof(A1)));
+    G16_CUDA(view(q[M_B2], full_b2, sizeof(A2)));
+    A1 a_q0, b1_q0;
+    A2 b2_q0;
+    G16_CUDA(cudaMemcpyAsync(&a_q0, full_a.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
+    G16_CUDA(cudaMemcpyAsync(&b1_q0, full_b1.p, sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
+    G16_CUDA(cudaMemcpyAsync(&b2_q0, full_b2.p, sizeof(A2), cudaMemcpyDeviceToHost, S0.st_main));
+    G16_CUDA(cudaStreamSynchronize(S0.st_main));
     return commit_key(a_q0, b1_q0, b2_q0, true);
+  }
+
+  // ---- proving keys from a powers-of-tau transcript (srs.cuh) ----
+  enum { SRS_TAU_G1 = 0, SRS_TAU_G2, SRS_ALPHA, SRS_BETA, SRS_BETA_G2, SRS_MEMBERS };
+  static const char* srs_member(int m) {
+    static const char* t[SRS_MEMBERS] = {"tau_g1", "tau_g2", "alpha_tau_g1", "beta_tau_g1", "beta_g2"};
+    return t[m];
+  }
+  // Stage times of the last g16_setup_from_srs (host clock around work that ends in a stream synchronise), read by
+  // tools/bench_srs_setup.py through g16_get_timings: h2d_ms = upload and point checks, witness_map_ms = the group inverse
+  // transforms, msm_ms[0] = the H query, msm_ms[1] = the sparse sums, total_ms = the whole call.
+  int setup_from_srs(const g16_srs_desc* srs, uint32_t flags) override {
+    if (!have_circuit) return fail(G16_ERR_BAD_ARGUMENT, "g16_circuit_load must precede g16_setup_from_srs");
+    if (!srs) return fail(G16_ERR_BAD_ARGUMENT, "null srs");
+    if (flags & ~(uint32_t)G16_SER_VALIDATE) return fail(G16_ERR_BAD_ARGUMENT, "g16_setup_from_srs takes 0 or G16_SER_VALIDATE");
+    G16_NOT_BUSY();
+    const uint64_t n = 1ull << L;
+    const uint64_t* ptr[SRS_MEMBERS] = {srs->tau_g1, srs->tau_g2, srs->alpha_tau_g1, srs->beta_tau_g1, srs->beta_g2};
+    const uint64_t have[SRS_MEMBERS] = {srs->tau_g1_len, srs->tau_g2_len, srs->alpha_tau_g1_len, srs->beta_tau_g1_len, 1};
+    const uint64_t need[SRS_MEMBERS] = {2 * n - 1, n, n, n, 1};
+    for (int m = 0; m < SRS_MEMBERS; m++) {
+      if (!ptr[m]) return fail(G16_ERR_BAD_ARGUMENT, std::string("null srs member ") + srs_member(m));
+      if (have[m] < need[m])
+        return fail(G16_ERR_BAD_ARGUMENT, std::string(srs_member(m)) + " holds " + std::to_string(have[m]) +
+                                              " points, the circuit (domain 2^" + std::to_string(L) + ") needs at least " +
+                                              std::to_string(need[m]));
+    }
+    G16_CUDA(cudaSetDevice(device));
+    int rc = ensure_circuit_domain();   // dom.tw_inv: the circuit's omega^-i
+    if (rc) return rc;
+    const auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point a) {
+      return (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count();
+    };
+    tm = g16_timings{};
+    const bool circom = qap == G16_QAP_CIRCOM;
+    const uint32_t nc = num_constraints, ni = num_inputs, nw = num_witness;
+    const uint64_t nv = nvars(), hn = h_query_len();
+    const uint64_t len[5] = {hn, nw, nv, nv, nv};
+    if ((rc = begin_key(0, 1, len))) return rc;   // from here on a failure leaves no key resident
+    G16_CUDA(full_a.reserve(nv * sizeof(A1))); G16_CUDA(full_b1.reserve(nv * sizeof(A1))); G16_CUDA(full_b2.reserve(nv * sizeof(A2)));
+    G16_CUDA(d_gamma_abc.reserve((size_t)ni * sizeof(A1)));
+    cudaStream_t st = S0.st_main;
+    {   // transcript buffers and scratch are freed before commit_key weighs the free memory
+      // --- upload and check the prefixes ---
+      DevBuf up[SRS_MEMBERS], err;
+      const size_t esz[SRS_MEMBERS] = {sizeof(A1), sizeof(A2), sizeof(A1), sizeof(A1), sizeof(A2)};
+      G16_CUDA(err.reserve(8));
+      G16_CUDA(cudaMemsetAsync(err.p, 0xff, 8, st));
+      for (int m = 0; m < SRS_MEMBERS; m++) {
+        G16_CUDA(up[m].reserve(need[m] * esz[m]));
+        G16_CUDA(cudaMemcpyAsync(up[m].p, ptr[m], need[m] * esz[m], cudaMemcpyHostToDevice, st));
+        const bool g2 = m == SRS_TAU_G2 || m == SRS_BETA_G2;
+        G16_CUDA((g2 ? srs_check<CP, true>(st, up[m].p, (uint32_t)need[m], flags, m, err.template as<unsigned long long>())
+                     : srs_check<CP, false>(st, up[m].p, (uint32_t)need[m], flags, m, err.template as<unsigned long long>())));
+      }
+      unsigned long long first_err = 0;
+      G16_CUDA(cudaMemcpyAsync(&first_err, err.p, 8, cudaMemcpyDeviceToHost, st));
+      G16_CUDA(cudaStreamSynchronize(st));
+      if (first_err != ~0ull)
+        return fail(G16_ERR_INVALID_DATA, std::string(srs_member((int)(first_err >> 48))) + "[" +
+                                              std::to_string((first_err >> 8) & ((1ull << 40) - 1)) + "]: " +
+                                              ser_reason(first_err & 0xff));
+      tm.h2d_ms = ms_since(t0);
+      // --- H query: [tau^(n+i)] - [tau^i] (LibsnarkReduction), or the odd entries of the size-2n inverse transform of
+      // [tau^i], i < 2n - 1: 1/(2n) times the size-n transform of omega_2n^-i ([tau^i] - [tau^(i+n)]) (CircomReduction) ---
+      auto t1 = std::chrono::steady_clock::now();
+      const A1* t1p = up[SRS_TAU_G1].template as<A1>();
+      DevBuf hpts, dfr;
+      G16_CUDA(hpts.reserve(n * sizeof(P1)));
+      G16_CUDA(dfr.reserve(n * sizeof(Fr)));
+      if (!circom) {
+        G16_CUDA(srs_diff<Fq>(st, t1p, (uint32_t)(2 * n - 1), (uint32_t)n, 0, (uint32_t)(n - 1), hpts.template as<P1>()));
+      } else {
+        G16_CUDA(srs_diff<Fq>(st, t1p, (uint32_t)(2 * n - 1), 0, (uint32_t)n, (uint32_t)n, hpts.template as<P1>()));
+        std::vector<Fr> s(n);
+        const Fr w_inv = Fr::inv(fr_domain_root<Fr>(L + 1));
+        Fr c = Fr::inv(fr_from_u64<Fr>(2 * n));
+        for (uint64_t i = 0; i < n; i++) { s[i] = c; c = Fr::mul(c, w_inv); }
+        G16_CUDA(cudaMemcpyAsync(dfr.p, s.data(), n * sizeof(Fr), cudaMemcpyHostToDevice, st));
+        G16_CUDA((srs_scale<Fq, Fr>(st, hpts.template as<P1>(), (uint32_t)n, dfr.template as<Fr>(), 1)));
+        G16_CUDA((srs_ifft<Fq, Fr>(st, hpts.template as<P1>(), L, dom.tw_inv, &ntt_launches)));
+        G16_CUDA(cudaStreamSynchronize(st));   // s is read by the copy above
+      }
+      G16_CUDA(srs_affine<Fq>(st, hpts.template as<P1>(), (uint32_t)hn, q[M_H].bases.template as<A1>()));
+      G16_CUDA(cudaStreamSynchronize(st));
+      hpts.release();
+      tm.msm_ms[M_H] = ms_since(t1);
+      // --- Lagrange points: [L_i], [alpha L_i], [beta L_i] in G1 (s1 = three blocks of n) and [L_i] in G2: unscaled
+      // inverse transforms of the first n powers, then times n^-1 ---
+      t1 = std::chrono::steady_clock::now();
+      DevBuf s1, s2;
+      G16_CUDA(s1.reserve(3 * n * sizeof(P1)));
+      G16_CUDA(s2.reserve(n * sizeof(P2)));
+      P1* s1p = s1.template as<P1>();
+      P2* s2p = s2.template as<P2>();
+      const int src1[3] = {SRS_TAU_G1, SRS_ALPHA, SRS_BETA};
+      for (int b = 0; b < 3; b++) {
+        G16_CUDA(srs_load<Fq>(st, up[src1[b]].template as<A1>(), (uint32_t)n, s1p + b * n));
+        G16_CUDA((srs_ifft<Fq, Fr>(st, s1p + b * n, L, dom.tw_inv, &ntt_launches)));
+      }
+      G16_CUDA(srs_load<Fq2>(st, up[SRS_TAU_G2].template as<A2>(), (uint32_t)n, s2p));
+      G16_CUDA((srs_ifft<Fq2, Fr>(st, s2p, L, dom.tw_inv, &ntt_launches)));
+      G16_CUDA(cudaMemcpyAsync(dfr.p, &dom.n_inv, sizeof(Fr), cudaMemcpyHostToDevice, st));
+      G16_CUDA((srs_scale<Fq, Fr>(st, s1p, (uint32_t)(3 * n), dfr.template as<Fr>(), 0)));
+      G16_CUDA((srs_scale<Fq2, Fr>(st, s2p, (uint32_t)n, dfr.template as<Fr>(), 0)));
+      G16_CUDA(cudaStreamSynchronize(st));
+      for (DevBuf& u : up) u.release();
+      tm.witness_map_ms = ms_since(t1);
+      // --- sparse sums (r1cs_to_qap.rs:150-167, generator.rs:113-123 with gamma = delta = 1) over the CSC of the matrices:
+      // G1 columns [a_query | b_g1_query | gamma_abc_g1 ++ l_query] (3 nv), G2 columns b_g2_query (nv) ---
+      t1 = std::chrono::steady_clock::now();
+      struct Csc {
+        std::vector<uint64_t> cp;
+        std::vector<uint32_t> idx;
+        std::vector<Fr> coeff;
+      } c1, c2;
+      const Fr one = Fr::one();
+      // (matrix, column offset, source offset) of every term; instance rows L_(nc + j) added with coefficient One
+      auto build = [&](Csc& c, uint64_t cols, std::initializer_list<std::array<uint64_t, 3>> parts,
+                       std::initializer_list<std::array<uint64_t, 2>> inst) {
+        c.cp.assign(cols + 1, 0);
+        for (const auto& p : parts)
+          for (uint32_t col : h_col[p[0]]) c.cp[p[1] + col + 1]++;
+        for (const auto& p : inst)
+          for (uint32_t j = 0; j < ni; j++) c.cp[p[0] + j + 1]++;
+        for (uint64_t j = 0; j < cols; j++) c.cp[j + 1] += c.cp[j];
+        std::vector<uint64_t> at(c.cp.begin(), c.cp.end() - 1);
+        c.idx.resize(c.cp[cols]);
+        c.coeff.resize(c.cp[cols]);
+        for (const auto& p : parts)
+          for (uint32_t i = 0; i < nc; i++)
+            for (uint32_t e = h_rp[p[0]][i]; e < h_rp[p[0]][i + 1]; e++) {
+              const uint64_t k = at[p[1] + h_col[p[0]][e]]++;
+              c.idx[k] = (uint32_t)(p[2] + i);
+              c.coeff[k] = h_val[p[0]][e];
+            }
+        for (const auto& p : inst)
+          for (uint32_t j = 0; j < ni; j++) {
+            const uint64_t k = at[p[0] + j]++;
+            c.idx[k] = (uint32_t)(p[1] + nc + j);
+            c.coeff[k] = one;
+          }
+      };
+      build(c1, 3 * nv, {{0, 0, 0}, {1, nv, 0}, {0, 2 * nv, 2 * n}, {1, 2 * nv, n}, {2, 2 * nv, 0}}, {{0, 0}, {2 * nv, 2 * n}});
+      build(c2, nv, {{1, 0, 0}}, {});
+      SrsSumPlan p1, p2;
+      p1.make(c1.cp);
+      p2.make(c2.cp);
+      // level 1 writes at most entries / 16 + columns items and every later level fewer: the ping-pong buffer `tmp` holds the
+      // largest level, `terms` (level 0's output) receives the levels after it
+      size_t chunk_max = 1, tmp_bytes = sizeof(P2);
+      for (const SrsSumPlan* p : {&p1, &p2})
+        for (const auto& lv : p->levels) {
+          chunk_max = std::max(chunk_max, lv.size());
+          tmp_bytes = std::max(tmp_bytes, (lv.size() - 1) * (p == &p1 ? sizeof(P1) : sizeof(P2)));
+        }
+      DevBuf didx, dco, terms, tmp, dchunk, dlast, out1;
+      const uint64_t e_max = std::max<uint64_t>(c1.idx.size(), c2.idx.size());
+      G16_CUDA(didx.reserve(e_max * 4 + 4));
+      G16_CUDA(dco.reserve(e_max * sizeof(Fr) + sizeof(Fr)));
+      G16_CUDA(terms.reserve(std::max(c1.idx.size() * sizeof(P1), c2.idx.size() * sizeof(P2)) + sizeof(P2)));
+      G16_CUDA(tmp.reserve(tmp_bytes));
+      G16_CUDA(dchunk.reserve(chunk_max * 8));
+      G16_CUDA(dlast.reserve((3 * nv + 1) * 8));
+      G16_CUDA(out1.reserve(3 * nv * sizeof(A1)));
+      auto upload = [&](const Csc& c) -> cudaError_t {
+        cudaError_t e = cudaSuccess;
+        if (c.idx.empty()) return e;
+        if ((e = cudaMemcpyAsync(didx.p, c.idx.data(), c.idx.size() * 4, cudaMemcpyHostToDevice, st))) return e;
+        return cudaMemcpyAsync(dco.p, c.coeff.data(), c.coeff.size() * sizeof(Fr), cudaMemcpyHostToDevice, st);
+      };
+      G16_CUDA(upload(c1));
+      G16_CUDA((srs_sum<Fq, Fr>(st, s1p, didx.template as<uint32_t>(), dco.template as<Fr>(), (uint32_t)c1.idx.size(), p1,
+                                terms.template as<P1>(), tmp.template as<P1>(), dchunk.template as<uint64_t>(),
+                                dlast.template as<uint64_t>(), (uint32_t)(3 * nv), out1.template as<A1>())));
+      G16_CUDA(cudaStreamSynchronize(st));
+      G16_CUDA(upload(c2));
+      G16_CUDA((srs_sum<Fq2, Fr>(st, s2p, didx.template as<uint32_t>(), dco.template as<Fr>(), (uint32_t)c2.idx.size(), p2,
+                                 terms.template as<P2>(), tmp.template as<P2>(), dchunk.template as<uint64_t>(),
+                                 dlast.template as<uint64_t>(), (uint32_t)nv, full_b2.template as<A2>())));
+      const A1* o1 = out1.template as<A1>();
+      G16_CUDA(cudaMemcpyAsync(full_a.p, o1, nv * sizeof(A1), cudaMemcpyDeviceToDevice, st));
+      G16_CUDA(cudaMemcpyAsync(full_b1.p, o1 + nv, nv * sizeof(A1), cudaMemcpyDeviceToDevice, st));
+      if (ni) G16_CUDA(cudaMemcpyAsync(d_gamma_abc.p, o1 + 2 * nv, ni * sizeof(A1), cudaMemcpyDeviceToDevice, st));
+      if (nw) G16_CUDA(cudaMemcpyAsync(q[M_L].bases.p, o1 + 2 * nv + ni, nw * sizeof(A1), cudaMemcpyDeviceToDevice, st));
+      G16_CUDA(cudaStreamSynchronize(st));
+      tm.msm_ms[M_L] = ms_since(t1);
+    }
+    // single points (gamma = delta = 1)
+    alpha_g1 = load_a1(srs->alpha_tau_g1);
+    beta_g1 = load_a1(srs->beta_tau_g1);
+    delta_g1 = load_a1(srs->tau_g1);
+    beta_g2 = load_a2(srs->beta_g2);
+    gamma_g2 = delta_g2 = load_a2(srs->tau_g2);
+    rc = commit_setup_key();
+    tm.total_ms = ms_since(t0);
+    return rc;
+  }
+  // One phase-2 contribution: delta_g1, delta_g2 times delta; the H and L queries times delta^-1; the key re-committed.
+  int setup_contribute(const uint64_t* delta_) override {
+    if (!delta_) return fail(G16_ERR_BAD_ARGUMENT, "null delta");
+    G16_NOT_BUSY();
+    if (!have_pk || !from_setup || world != 1)
+      return fail(G16_ERR_BAD_ARGUMENT, "g16_setup_contribute needs a resident key made by g16_setup or g16_setup_from_srs (world 1)");
+    const Fr d = load_fr(delta_);
+    if (d.is_zero()) return fail(G16_ERR_BAD_ARGUMENT, "delta must be invertible (UnexpectedIdentity)");
+    G16_CUDA(cudaSetDevice(device));
+    const Fr di = Fr::inv(d);
+    const uint64_t nv = nvars(), hn = h_query_len(), nw = num_witness, cnt = hn + nw;
+    cudaStream_t st = S0.st_main;
+    {
+      DevBuf aff, pts, ds;
+      G16_CUDA(aff.reserve(cnt * sizeof(A1) + sizeof(A1)));
+      G16_CUDA(pts.reserve(cnt * sizeof(P1) + sizeof(P1)));
+      G16_CUDA(ds.reserve(sizeof(Fr)));
+      A1* a = aff.template as<A1>();
+      if (hn) G16_CUDA(cudaMemcpyAsync(a, q[M_H].bases.p, hn * sizeof(A1), cudaMemcpyDeviceToDevice, st));
+      if (nw) G16_CUDA(cudaMemcpyAsync(a + hn, q[M_L].bases.p, nw * sizeof(A1), cudaMemcpyDeviceToDevice, st));
+      G16_CUDA(cudaMemcpyAsync(ds.p, &di, sizeof(Fr), cudaMemcpyHostToDevice, st));
+      G16_CUDA(srs_load<Fq>(st, a, (uint32_t)cnt, pts.template as<P1>()));
+      G16_CUDA((srs_scale<Fq, Fr>(st, pts.template as<P1>(), (uint32_t)cnt, ds.template as<Fr>(), 0)));
+      G16_CUDA(srs_affine<Fq>(st, pts.template as<P1>(), (uint32_t)cnt, a));
+      G16_CUDA(cudaStreamSynchronize(st));
+      const uint64_t len[5] = {hn, nw, nv, nv, nv};
+      int rc = begin_key(0, 1, len);
+      if (rc) return rc;
+      if (hn) G16_CUDA(cudaMemcpyAsync(q[M_H].bases.p, a, hn * sizeof(A1), cudaMemcpyDeviceToDevice, st));
+      if (nw) G16_CUDA(cudaMemcpyAsync(q[M_L].bases.p, a + hn, nw * sizeof(A1), cudaMemcpyDeviceToDevice, st));
+      G16_CUDA(cudaStreamSynchronize(st));
+    }
+    uint32_t k[Fr::N];
+    fr_to_canon(d, k);
+    delta_g1 = P1::from_affine(delta_g1).mul_u32(k, Fr::N).to_affine();
+    delta_g2 = P2::from_affine(delta_g2).mul_u32(k, Fr::N).to_affine();
+    return commit_setup_key();
+  }
+  // g16_srs_from_secrets: member i of each vector is tau^i times [1]G1, [1]G2, [alpha]G1, [beta]G1
+  int srs_from_secrets(const uint64_t* tau_, const uint64_t* alpha_, const uint64_t* beta_, const uint64_t* g1_,
+                       const uint64_t* g2_, const g16_srs_out* out) override {
+    if (!tau_ || !alpha_ || !beta_ || !g1_ || !g2_ || !out || !out->beta_g2) return fail(G16_ERR_BAD_ARGUMENT, "null argument");
+    if ((out->tau_g1_len && !out->tau_g1) || (out->tau_g2_len && !out->tau_g2) || (out->alpha_tau_g1_len && !out->alpha_tau_g1) ||
+        (out->beta_tau_g1_len && !out->beta_tau_g1))
+      return fail(G16_ERR_BAD_ARGUMENT, "null srs output member");
+    const uint64_t mx = std::max(std::max(out->tau_g1_len, out->tau_g2_len), std::max(out->alpha_tau_g1_len, out->beta_tau_g1_len));
+    if (mx >= (1ull << 31)) return fail(G16_ERR_BAD_ARGUMENT, "srs member too long");
+    G16_NOT_BUSY();
+    G16_CUDA(cudaSetDevice(device));
+    const Fr tau = load_fr(tau_);
+    const A1 g1 = load_a1(g1_);
+    const A2 g2 = load_a2(g2_);
+    uint32_t k[Fr::N];
+    auto mul1 = [&](const Fr& s) { fr_to_canon(s, k); return P1::from_affine(g1).mul_u32(k, Fr::N).to_affine(); };
+    auto mul2 = [&](const Fr& s) { fr_to_canon(s, k); return P2::from_affine(g2).mul_u32(k, Fr::N).to_affine(); };
+    std::vector<Fr> pw(mx);
+    Fr p = Fr::one();
+    for (uint64_t i = 0; i < mx; i++) { pw[i] = p; p = Fr::mul(p, tau); }
+    DevBuf ds, dout, tab;
+    G16_CUDA(ds.reserve(mx * sizeof(Fr) + sizeof(Fr)));
+    G16_CUDA(dout.reserve(mx * sizeof(A2) + sizeof(A2)));
+    if (mx) G16_CUDA(cudaMemcpyAsync(ds.p, pw.data(), mx * sizeof(Fr), cudaMemcpyHostToDevice, S0.st_main));
+    auto run1 = [&](const A1& gen, uint64_t* dst, uint64_t cnt) -> int {
+      if (!cnt) return G16_OK;
+      int rc = batch_mul<Fq>(gen, ds.template as<Fr>(), cnt, dout.template as<A1>(), tab);
+      if (rc) return rc;
+      G16_CUDA(cudaMemcpyAsync(dst, dout.p, cnt * sizeof(A1), cudaMemcpyDeviceToHost, S0.st_main));
+      G16_CUDA(cudaStreamSynchronize(S0.st_main));
+      return G16_OK;
+    };
+    int rc;
+    if ((rc = run1(g1, out->tau_g1, out->tau_g1_len))) return rc;
+    if ((rc = run1(mul1(load_fr(alpha_)), out->alpha_tau_g1, out->alpha_tau_g1_len))) return rc;
+    if ((rc = run1(mul1(load_fr(beta_)), out->beta_tau_g1, out->beta_tau_g1_len))) return rc;
+    if (out->tau_g2_len) {
+      if ((rc = batch_mul<Fq2>(g2, ds.template as<Fr>(), out->tau_g2_len, dout.template as<A2>(), tab))) return rc;
+      G16_CUDA(cudaMemcpyAsync(out->tau_g2, dout.p, out->tau_g2_len * sizeof(A2), cudaMemcpyDeviceToHost, S0.st_main));
+      G16_CUDA(cudaStreamSynchronize(S0.st_main));
+    }
+    store_a2(out->beta_g2, mul2(load_fr(beta_)));
+    return G16_OK;
   }
   // CircomReduction::h_query_scalars(n - 1, tau, _, delta^-1): the odd entries 1, 3, .., 2n - 1 of the size-2n ifft of
   // v[i] = delta^-1 tau^i (i < 2n - 1), v[2n - 1] = 0.  With w = omega_2n, k = 2j + 1 and the geometric sum in closed form:
@@ -1994,7 +2286,9 @@ struct Engine : IEngine {
   G16_NTT_TEMPLATES(X, Fp<CP::FrP>)                                                               \
   G16_MSM_TEMPLATES(X, Fp<CP::FqP>, Fp<CP::FrP>)                                                  \
   G16_MSM_TEMPLATES(X, G16_FQ2(CP), Fp<CP::FrP>)                                                  \
-  G16_SER_TEMPLATES(X, CP)
+  G16_SER_TEMPLATES(X, CP)                                                                        \
+  G16_SRS_TEMPLATES(X, CP)                                                                        \
+  G16_SRS_POINT_TEMPLATES(X, G16_FQ2(CP), Fp<CP::FrP>)
 #define G16_FQ2(CP) CP::G2F
 
 template <class CP>

@@ -162,6 +162,47 @@ typedef struct {
 } g16_pk_export_desc;
 int g16_pk_export(g16_ctx* ctx, const g16_pk_export_desc* out);
 
+/* ---- proving keys from a powers-of-tau transcript, with nobody holding tau: phase 2 of Bowe-Gabizon-Miers ("Scalable
+ * Multi-Party Computation for zk-SNARK Parameters in the Random Beacon Model"), as snarkjs keys are made.
+ * The transcript of a circuit with domain size n = 2^g16_domain_log holds, as affine Montgomery limbs (all-zero limbs for
+ * the identity): tau_g1 = [tau^i]G1 (at least 2n - 1 points), tau_g2 = [tau^i]G2 (at least n), alpha_tau_g1 = [alpha
+ * tau^i]G1 and beta_tau_g1 = [beta tau^i]G1 (at least n each), beta_g2 = [beta]G2.  Longer members are allowed (ceremonies
+ * are sized for the largest circuit); only the prefixes above are read, checked and used.
+ * g16_setup_from_srs derives the key of the resident circuit under its reduction on the GPU (four group inverse FFTs, the
+ * sparse sums of the queries, the H query) and makes it resident as g16_setup does (rank 0 / world 1; g16_pk_export,
+ * g16_pk_export_serialized and every prover path take it).  gamma = 1, and with no contribution delta = 1: the key equals
+ * g16_setup(alpha, beta, 1, 1, tau, tau_g1[0], tau_g2[0]) point for point.  flags: 0 or G16_SER_VALIDATE (adds the
+ * subgroup check [r]P = O of every point read; always checked: coordinates below q and on the curve).
+ * Argument errors leave the previous key resident: a null pointer, unknown flags, no circuit, a member shorter than it
+ * must be (G16_ERR_BAD_ARGUMENT naming the member and the length it needs), a proof in flight.  A point the checks refuse is
+ * G16_ERR_INVALID_DATA, g16_last_error() naming the first one by member and index ("alpha_tau_g1[17]: point is not on the
+ * curve"), and no key is resident afterwards.
+ * g16_setup_contribute applies one phase-2 contribution delta (Montgomery Fr, non-zero) to the resident key: delta_g1 and
+ * delta_g2 times delta, every h_query and l_query point times delta^-1.  After contributions delta_1 .. delta_k the key equals
+ * g16_setup(alpha, beta, 1, delta_1 ... delta_k, tau, g1, g2); on a g16_setup key made with delta it equals g16_setup with
+ * delta delta'.  It needs a key made by g16_setup or g16_setup_from_srs (world 1); any other, no key, or delta = 0 is
+ * G16_ERR_BAD_ARGUMENT with the key unchanged.  The key is re-committed, so everything derived from it is rebuilt.
+ * After g16_setup_from_srs, g16_get_timings describes that call instead of the last proof (the fields keep their types, not
+ * their prover meaning; every other field is 0): total_ms = the whole call, h2d_ms = upload and point checks, witness_map_ms
+ * = the four group inverse transforms, msm_ms[0] = the H query, msm_ms[1] = the sparse sums of the other queries. */
+typedef struct {
+  const uint64_t* tau_g1;       uint64_t tau_g1_len;
+  const uint64_t* tau_g2;       uint64_t tau_g2_len;       /* g16_g2_limbs per point */
+  const uint64_t* alpha_tau_g1; uint64_t alpha_tau_g1_len;
+  const uint64_t* beta_tau_g1;  uint64_t beta_tau_g1_len;
+  const uint64_t* beta_g2;
+} g16_srs_desc;
+int g16_setup_from_srs(g16_ctx* ctx, const g16_srs_desc* srs, uint32_t flags);
+int g16_setup_contribute(g16_ctx* ctx, const uint64_t* delta);
+/* Test and benchmark helper, no reference counterpart: the transcript of explicit secrets tau, alpha, beta (Montgomery Fr)
+ * over the affine generators g1, g2, each member as long as the caller's *_len (fixed-base multiplications on the GPU).
+ * Needs no circuit and leaves the resident circuit and key alone. */
+typedef struct { uint64_t* tau_g1; uint64_t tau_g1_len; uint64_t* tau_g2; uint64_t tau_g2_len;
+                 uint64_t* alpha_tau_g1; uint64_t alpha_tau_g1_len; uint64_t* beta_tau_g1; uint64_t beta_tau_g1_len;
+                 uint64_t* beta_g2; } g16_srs_out;
+int g16_srs_from_secrets(g16_ctx* ctx, const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta,
+                         const uint64_t* g1, const uint64_t* g2, const g16_srs_out* out);
+
 /* ---- ark-serialized proving keys: `ProvingKey::serialize_{compressed,uncompressed}` / `deserialize_with_mode`
  * (data_structures.rs:125 derives them).  The bytes are a whole ProvingKey<E> as ark-serialize 0.5 writes it: vk {alpha_g1,
  * beta_g2, gamma_g2, delta_g2, gamma_abc_g1}, beta_g1, delta_g1, a_query, b_g1_query, b_g2_query, h_query, l_query; vectors
@@ -202,7 +243,8 @@ int g16_prove_assemble(g16_ctx* ctx, const uint64_t* r, const uint64_t* s, const
                        uint32_t nparts, uint64_t* proof_out);
 /* Optional: start the (r, s)-only scalar multiplications of prover.rs:76,90,100,112 on a helper thread before the partial
  * sums exist; the next g16_prove_assemble with the same (r, s) picks the result up instead of computing it inline.
- * Loading a circuit or a key (g16_circuit_load, g16_pk_load, g16_setup, g16_pk_load_serialized) discards the result. */
+ * Loading a circuit or a key (g16_circuit_load, g16_pk_load, g16_setup, g16_pk_load_serialized, g16_setup_from_srs,
+ * g16_setup_contribute) discards the result. */
 int g16_prove_assemble_prepare(g16_ctx* ctx, const uint64_t* r, const uint64_t* s);
 /* Pipelined proving: a context owns two proof slots (0 and 1), each with its own streams and work buffers.
  * g16_prove_submit enqueues a whole proof asynchronously and returns; g16_prove_wait blocks until that slot's GPU

@@ -393,6 +393,46 @@ impl<E: SwPairing> B200Prover<E> {
         })
     }
 
+    /// Derives the resident circuit's proving key on the GPU from a powers-of-tau transcript (g16_setup_from_srs) and makes
+    /// it resident: gamma = 1, delta = 1 until `contribute_delta`.  `tau_g1` holds at least 2n - 1 points, `tau_g2`,
+    /// `alpha_tau_g1` and `beta_tau_g1` at least n (n = the circuit's domain size); longer transcripts are fine.
+    /// `validate` adds the subgroup check of every point read.  Export the key with `export_proving_key_bytes`.
+    pub fn setup_from_srs(
+        &self,
+        tau_g1: &[Affine<E::G1Config>],
+        tau_g2: &[Affine<E::G2Config>],
+        alpha_tau_g1: &[Affine<E::G1Config>],
+        beta_tau_g1: &[Affine<E::G1Config>],
+        beta_g2: &Affine<E::G2Config>,
+        validate: Validate,
+    ) -> Result<(), SerializationError> {
+        let (t1, t2, a1, b1) = (pack_points(tau_g1), pack_points(tau_g2), pack_points(alpha_tau_g1), pack_points(beta_tau_g1));
+        let bg2 = pack_points(core::slice::from_ref(beta_g2));
+        let desc = sys::g16_srs_desc {
+            tau_g1: t1.as_ptr(),
+            tau_g1_len: tau_g1.len() as u64,
+            tau_g2: t2.as_ptr(),
+            tau_g2_len: tau_g2.len() as u64,
+            alpha_tau_g1: a1.as_ptr(),
+            alpha_tau_g1_len: alpha_tau_g1.len() as u64,
+            beta_tau_g1: b1.as_ptr(),
+            beta_tau_g1_len: beta_tau_g1.len() as u64,
+            beta_g2: bg2.as_ptr(),
+        };
+        let flags = if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 };
+        ser_status(unsafe { sys::g16_setup_from_srs(self.ctx, &desc, flags) })
+    }
+
+    /// One phase-2 contribution to the resident key (g16_setup_contribute): delta_g1, delta_g2 times `delta`, the H and L
+    /// queries times delta^-1.  delta = 0 is SynthesisError::UnexpectedIdentity.
+    pub fn contribute_delta(&self, delta: E::ScalarField) -> R1CSResult<()> {
+        if delta.is_zero() {
+            return Err(SynthesisError::UnexpectedIdentity);
+        }
+        let d = [delta];
+        status(unsafe { sys::g16_setup_contribute(self.ctx, scalars_ptr(&d)) })
+    }
+
     /// `ProvingKey::serialize_with_mode(compress)` of the resident key, encoded on the GPU (g16_pk_export_serialized).  Only
     /// a key made by the library's own setup can be exported.
     pub fn export_proving_key_bytes(&self, compress: Compress) -> Result<Vec<u8>, SerializationError> {

@@ -67,6 +67,34 @@ pub struct g16_pk_desc {
     pub delta_g2: *const u64,
 }
 
+/// g16_srs_desc: a powers-of-tau transcript, affine Montgomery limbs (g16_setup_from_srs)
+#[repr(C)]
+pub struct g16_srs_desc {
+    pub tau_g1: *const u64,
+    pub tau_g1_len: u64,
+    pub tau_g2: *const u64,
+    pub tau_g2_len: u64,
+    pub alpha_tau_g1: *const u64,
+    pub alpha_tau_g1_len: u64,
+    pub beta_tau_g1: *const u64,
+    pub beta_tau_g1_len: u64,
+    pub beta_g2: *const u64,
+}
+
+/// g16_srs_out: where g16_srs_from_secrets writes a transcript
+#[repr(C)]
+pub struct g16_srs_out {
+    pub tau_g1: *mut u64,
+    pub tau_g1_len: u64,
+    pub tau_g2: *mut u64,
+    pub tau_g2_len: u64,
+    pub alpha_tau_g1: *mut u64,
+    pub alpha_tau_g1_len: u64,
+    pub beta_tau_g1: *mut u64,
+    pub beta_tau_g1_len: u64,
+    pub beta_g2: *mut u64,
+}
+
 #[repr(C)]
 pub struct g16_pk_export_desc {
     pub a_query: *mut u64,
@@ -139,6 +167,9 @@ extern "C" {
     pub fn g16_pk_load(ctx: *mut g16_ctx, pk: *const g16_pk_desc, rank: u32, world: u32) -> c_int;
     pub fn g16_setup(ctx: *mut g16_ctx, alpha: *const u64, beta: *const u64, gamma: *const u64, delta: *const u64, tau: *const u64, g1: *const u64, g2: *const u64) -> c_int;
     pub fn g16_pk_export(ctx: *mut g16_ctx, out: *const g16_pk_export_desc) -> c_int;
+    pub fn g16_setup_from_srs(ctx: *mut g16_ctx, srs: *const g16_srs_desc, flags: u32) -> c_int;
+    pub fn g16_setup_contribute(ctx: *mut g16_ctx, delta: *const u64) -> c_int;
+    pub fn g16_srs_from_secrets(ctx: *mut g16_ctx, tau: *const u64, alpha: *const u64, beta: *const u64, g1: *const u64, g2: *const u64, out: *const g16_srs_out) -> c_int;
     pub fn g16_pk_load_serialized(ctx: *mut g16_ctx, bytes: *const u8, len: u64, flags: u32, rank: u32, world: u32, vk_out: *const g16_pk_export_desc) -> c_int;
     pub fn g16_pk_export_serialized(ctx: *mut g16_ctx, flags: u32, out: *mut u8, cap: u64, len_out: *mut u64) -> c_int;
     pub fn g16_prove(ctx: *mut g16_ctx, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32, proof_out: *mut u64) -> c_int;
