@@ -142,6 +142,37 @@ class Srs:
     beta_g2: np.ndarray
 
 
+SRS_VECTORS = ("tau_g1", "tau_g2", "alpha_tau_g1", "beta_tau_g1")
+
+
+def srs_arrays(srs: Srs, g1_width: int, g2_width: int, in_place: bool = False) -> dict:
+    """The members of `srs` as C-contiguous uint64 arrays, as Groth16.contribute_srs hands them to the library: the vectors
+    as (points, limbs) (None: no points), beta_g2 as one point of g2_width limbs.  ValueError names a member that is not
+    made of whole points, a missing beta_g2, and with `in_place` a member that cannot be written where it is (not a
+    C-contiguous, writable uint64 array)."""
+    out = {}
+    for k in SRS_VECTORS + ("beta_g2",):
+        v = getattr(srs, k)
+        w = g2_width if k in ("tau_g2", "beta_g2") else g1_width
+        if v is None:
+            if k == "beta_g2":
+                raise ValueError("srs.beta_g2 is missing: it is always read and written")
+            out[k] = np.zeros((0, w), dtype=np.uint64)
+            continue
+        a = np.ascontiguousarray(v, dtype=np.uint64)
+        if in_place and (a is not v or not a.flags["WRITEABLE"]):
+            raise ValueError(f"in_place needs srs.{k} to be a C-contiguous, writable uint64 array")
+        if k == "beta_g2":
+            if a.size != w:
+                raise ValueError(f"srs.beta_g2 holds {a.size} limbs, one G2 point is {w}")
+            out[k] = a.reshape(w)
+        else:
+            if a.ndim not in (1, 2) or a.size % w or (a.ndim == 2 and a.shape[1] != w):
+                raise ValueError(f"srs.{k} of shape {a.shape} is not a list of points of {w} limbs")
+            out[k] = a.reshape(-1, w)
+    return out
+
+
 @dataclass
 class WitnessReport:
     """g16_witness_report of one assignment, None where the library reports G16_NONE"""
@@ -386,6 +417,32 @@ class Groth16:
         self._after_key_change(self._lib.g16_setup_contribute(self._ctx, _ptr(dl)))
         self._pk_obj = self.export_proving_key() if export else None
         return self._pk_obj
+
+    def contribute_srs(self, srs: Srs, tau, alpha, beta, validate: bool = False, chunk_points: int = 0,
+                       in_place: bool = False) -> Srs:
+        """g16_srs_contribute: one phase-1 contribution of the secrets tau, alpha, beta (Python ints) to the transcript `srs`,
+        on the GPU: point i of tau_g1 and tau_g2 times tau^i, of alpha_tau_g1 times alpha tau^i, of beta_tau_g1 times
+        beta tau^i, and beta_g2 times beta.  Returns the new transcript; with `in_place` it is written into srs's own arrays
+        (each then a C-contiguous, writable uint64 array) and srs is returned.  `validate` adds the subgroup check of every
+        point; `chunk_points` caps the points per chunk (0: as many as the free device memory holds).  A refused point raises
+        serialize.DeserializeError naming it, with nothing written.  Needs no circuit or key and leaves the resident ones
+        alone."""
+        ins = srs_arrays(srs, 2 * self.nq, self.ng2, in_place)
+        chunk_points = int(chunk_points)
+        if not 0 <= chunk_points < 1 << 64:
+            raise ValueError(f"chunk_points must be in [0, 2^64), not {chunk_points}")
+        outs = ins if in_place else {k: np.empty_like(v) for k, v in ins.items()}
+        d_in, d_out = _lib.SrsDesc(), _lib.SrsOut()
+        for d, arrs in ((d_in, ins), (d_out, outs)):
+            for k in SRS_VECTORS:
+                v = arrs[k]
+                setattr(d, k, _u64p(v) if v.size else None)
+                setattr(d, k + "_len", v.shape[0])
+            d.beta_g2 = _u64p(arrs["beta_g2"])
+        sc = [np.ascontiguousarray(self.codec.fr.enc1(x)) for x in (tau, alpha, beta)]
+        _check(self._lib.g16_srs_contribute(self._ctx, C.byref(d_in), *[_ptr(x) for x in sc],
+                                            _lib.SER_VALIDATE if validate else 0, chunk_points, C.byref(d_out)))
+        return srs if in_place else Srs(**outs)
 
     def _after_key_change(self, rc: int):
         """Status of g16_setup_from_srs / g16_setup_contribute: argument errors (G16_ERR_BAD_ARGUMENT,

@@ -158,6 +158,11 @@ int g16_srs_from_secrets(g16_ctx* ctx, const uint64_t* tau, const uint64_t* alph
   CTX_OR_FAIL(ctx);
   return ctx->eng->srs_from_secrets(tau, alpha, beta, g1, g2, out);
 }
+int g16_srs_contribute(g16_ctx* ctx, const g16_srs_desc* in, const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta,
+                       uint32_t flags, uint64_t chunk_points, const g16_srs_out* out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->srs_contribute(in, tau, alpha, beta, flags, chunk_points, out);
+}
 int g16_pk_load_serialized(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                            const g16_pk_export_desc* vk_out) {
   CTX_OR_FAIL(ctx);

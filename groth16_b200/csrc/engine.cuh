@@ -148,6 +148,8 @@ struct IEngine {
   virtual int setup_contribute(const uint64_t* delta) = 0;
   virtual int srs_from_secrets(const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta, const uint64_t* g1,
                                const uint64_t* g2, const g16_srs_out* out) = 0;
+  virtual int srs_contribute(const g16_srs_desc* in, const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta,
+                             uint32_t flags, uint64_t chunk_points, const g16_srs_out* out) = 0;
   virtual int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                                  const g16_pk_export_desc* vk_out) = 0;
   virtual int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) = 0;
@@ -1359,6 +1361,118 @@ struct Engine : IEngine {
       G16_CUDA(cudaStreamSynchronize(S0.st_main));
     }
     store_a2(out->beta_g2, mul2(load_fr(beta_)));
+    return G16_OK;
+  }
+  // g16_srs_contribute: one phase-1 contribution (tau, alpha, beta).  Point i of tau_g1 and tau_g2 times tau^i, of
+  // alpha_tau_g1 times alpha tau^i, of beta_tau_g1 times beta tau^i; beta_g2 times beta.  Two passes over the members in
+  // chunks of at most `cap` points through one device buffer: every point is uploaded and checked before anything is written
+  // to `out`, then every chunk is uploaded again, transformed in place on the device (srs_contribute_kernel) and copied out.
+  // Timings (host clock around work that ends in a stream synchronise): h2d_ms = the check pass, msm_ms[m] = the transform
+  // of member m < 4, total_ms = the whole call.
+  int srs_contribute(const g16_srs_desc* in, const uint64_t* tau_, const uint64_t* alpha_, const uint64_t* beta_, uint32_t flags,
+                     uint64_t chunk_points, const g16_srs_out* out) override {
+    if (!in || !out || !tau_ || !alpha_ || !beta_) return fail(G16_ERR_BAD_ARGUMENT, "null argument");
+    if (flags & ~(uint32_t)G16_SER_VALIDATE) return fail(G16_ERR_BAD_ARGUMENT, "g16_srs_contribute takes 0 or G16_SER_VALIDATE");
+    const uint64_t* src[SRS_MEMBERS] = {in->tau_g1, in->tau_g2, in->alpha_tau_g1, in->beta_tau_g1, in->beta_g2};
+    uint64_t* dst[SRS_MEMBERS] = {out->tau_g1, out->tau_g2, out->alpha_tau_g1, out->beta_tau_g1, out->beta_g2};
+    const uint64_t len[SRS_MEMBERS] = {in->tau_g1_len, in->tau_g2_len, in->alpha_tau_g1_len, in->beta_tau_g1_len, 1};
+    const uint64_t olen[SRS_MEMBERS] = {out->tau_g1_len, out->tau_g2_len, out->alpha_tau_g1_len, out->beta_tau_g1_len, 1};
+    const uint64_t esz[SRS_MEMBERS] = {sizeof(A1), sizeof(A2), sizeof(A1), sizeof(A1), sizeof(A2)};
+    for (int m = 0; m < SRS_MEMBERS; m++) {
+      const std::string name = srs_member(m);
+      if (olen[m] != len[m])
+        return fail(G16_ERR_BAD_ARGUMENT, "out " + name + " holds " + std::to_string(olen[m]) + " points, in " + name + " " +
+                                              std::to_string(len[m]) + ": the lengths must be equal");
+      if (len[m] >> 32)
+        return fail(G16_ERR_BAD_ARGUMENT, name + " holds " + std::to_string(len[m]) + " points, at most 2^32 - 1 are allowed");
+      if (len[m] && (!src[m] || !dst[m])) return fail(G16_ERR_BAD_ARGUMENT, "null srs member " + name);
+    }
+    // an output range may be its own input range (in place) and must overlap no other input or output range
+    auto overlap = [&](const void* a, int ma, const void* b, int mb) {
+      const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
+      return len[ma] && len[mb] && a0 < b0 + len[mb] * esz[mb] && b0 < a0 + len[ma] * esz[ma];
+    };
+    for (int o = 0; o < SRS_MEMBERS; o++)
+      for (int m = 0; m < SRS_MEMBERS; m++) {
+        if (overlap(dst[o], o, src[m], m) && !(o == m && (const void*)dst[o] == (const void*)src[m]))
+          return fail(G16_ERR_BAD_ARGUMENT, std::string("out ") + srs_member(o) + " overlaps in " + srs_member(m) +
+                                                ": an output may only be the very same array as its own input");
+        if (m > o && overlap(dst[o], o, dst[m], m))
+          return fail(G16_ERR_BAD_ARGUMENT, std::string("out ") + srs_member(o) + " overlaps out " + srs_member(m));
+      }
+    const Fr tau = load_fr(tau_), alpha = load_fr(alpha_), beta = load_fr(beta_);
+    if (tau.is_zero() || alpha.is_zero() || beta.is_zero())
+      return fail(G16_ERR_BAD_ARGUMENT, "tau, alpha and beta must be non-zero (UnexpectedIdentity)");
+    G16_NOT_BUSY();
+    G16_CUDA(cudaSetDevice(device));
+    const auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point a) {
+      return (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count();
+    };
+    tm = g16_timings{};
+    cudaStream_t st = S0.st_main;
+    const uint64_t big = std::max(sizeof(A1), sizeof(A2));
+    size_t free_b = 0, total_b = 0;
+    G16_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const uint64_t longest = *std::max_element(len, len + SRS_MEMBERS);
+    const uint64_t cap = srs_chunk_cap(chunk_points, longest, free_b, big);
+    DevBuf buf, err, dtab;
+    G16_CUDA(buf.reserve(cap * big));
+    G16_CUDA(err.reserve(8));
+    auto part = [&](int m, uint64_t i0) { return i0 * esz[m]; };   // byte offset of point i0 of member m
+    // --- check pass: every point, chunk by chunk; the first bad one by member, then index ---
+    for (int m = 0; m < SRS_MEMBERS; m++) {
+      const bool g2 = m == SRS_TAU_G2 || m == SRS_BETA_G2;
+      for (uint64_t i0 = 0; i0 < len[m];) {
+        const uint32_t cnt = srs_chunk_len(len[m], i0, cap);
+        G16_CUDA(cudaMemcpyAsync(buf.p, (const char*)src[m] + part(m, i0), cnt * esz[m], cudaMemcpyHostToDevice, st));
+        G16_CUDA(cudaMemsetAsync(err.p, 0xff, 8, st));
+        unsigned long long* e = err.template as<unsigned long long>();
+        G16_CUDA((g2 ? srs_check<CP, true>(st, buf.p, cnt, flags, m, e) : srs_check<CP, false>(st, buf.p, cnt, flags, m, e)));
+        unsigned long long first_err = 0;
+        G16_CUDA(cudaMemcpyAsync(&first_err, err.p, 8, cudaMemcpyDeviceToHost, st));
+        G16_CUDA(cudaStreamSynchronize(st));
+        tm.h2d_bytes += cnt * esz[m];
+        tm.d2h_bytes += 8;
+        tm.launches++;
+        if (first_err != ~0ull)
+          return fail(G16_ERR_INVALID_DATA, std::string(srs_member(m)) + "[" +
+                                                std::to_string(i0 + ((first_err >> 8) & ((1ull << 40) - 1))) + "]: " +
+                                                ser_reason(first_err & 0xff));
+        i0 += cnt;
+      }
+    }
+    tm.h2d_ms = ms_since(t0);
+    // --- transform pass: chunk [i0, i0 + cnt) of member m times x tau^(i0 + j), x = 1, 1, alpha, beta ---
+    Fr tab[32];
+    tab[0] = tau;
+    for (int k = 1; k < 32; k++) tab[k] = Fr::sqr(tab[k - 1]);
+    G16_CUDA(dtab.reserve(sizeof(tab)));
+    G16_CUDA(cudaMemcpyAsync(dtab.p, tab, sizeof(tab), cudaMemcpyHostToDevice, st));
+    tm.h2d_bytes += sizeof(tab);
+    const Fr x[4] = {Fr::one(), Fr::one(), alpha, beta};
+    for (int m = 0; m < 4; m++) {
+      const auto t1 = std::chrono::steady_clock::now();
+      for (uint64_t i0 = 0; i0 < len[m];) {
+        const uint32_t cnt = srs_chunk_len(len[m], i0, cap);
+        const Fr c = srs_power(x[m], tab, i0);
+        G16_CUDA(cudaMemcpyAsync(buf.p, (const char*)src[m] + part(m, i0), cnt * esz[m], cudaMemcpyHostToDevice, st));
+        G16_CUDA((m == SRS_TAU_G2 ? g16::srs_contribute<Fq2, Fr>(st, buf.template as<A2>(), cnt, dtab.template as<Fr>(), c)
+                                  : g16::srs_contribute<Fq, Fr>(st, buf.template as<A1>(), cnt, dtab.template as<Fr>(), c)));
+        G16_CUDA(cudaMemcpyAsync((char*)dst[m] + part(m, i0), buf.p, cnt * esz[m], cudaMemcpyDeviceToHost, st));
+        tm.h2d_bytes += cnt * esz[m];
+        tm.d2h_bytes += cnt * esz[m];
+        tm.launches++;
+        i0 += cnt;
+      }
+      G16_CUDA(cudaStreamSynchronize(st));
+      tm.msm_ms[m] = ms_since(t1);
+    }
+    // beta_g2 is one point: on the host, as g16_setup_contribute does for delta_g2
+    uint32_t k[Fr::N];
+    fr_to_canon(beta, k);
+    store_a2(dst[SRS_BETA_G2], P2::from_affine(load_a2(src[SRS_BETA_G2])).mul_u32(k, Fr::N).to_affine());
+    tm.total_ms = ms_since(t0);
     return G16_OK;
   }
   // CircomReduction::h_query_scalars(n - 1, tau, _, delta^-1): the odd entries 1, 3, .., 2n - 1 of the size-2n ifft of

@@ -1,6 +1,7 @@
 // srs.cuh -- proving keys from a powers-of-tau transcript (g16_setup_from_srs) and phase-2 delta contributions
 // (g16_setup_contribute): the group-valued inverse FFT, sparse sums of points, one scalar times many points, and the
-// transcript point checks.
+// transcript point checks; and phase-1 contributions to a transcript (g16_srs_contribute): every point times its own power
+// of the secret.
 //
 // Every kernel works on XYZZ points in global memory, one point (or one butterfly, or one chunk of a sum) per thread.  The
 // scalar multiplications are left-to-right double-and-add over the canonical scalar (XYZZ::mul_u32); a windowed form would
@@ -53,6 +54,28 @@ struct SrsSumPlan {
     last = seg;
   }
 };
+
+// ---- phase-1 contributions (g16_srs_contribute) -------------------------------------------------------------------------
+// A member of `len` points runs in chunks of at most `cap` points; the chunk starting at point i0 holds
+// srs_chunk_len(len, i0, cap) of them.  len < 2^32 and 1 <= cap < 2^32, so a chunk's count and every index fit in 32 bits.
+inline uint32_t srs_chunk_len(uint64_t len, uint64_t i0, uint64_t cap) { return (uint32_t)std::min<uint64_t>(cap, len - i0); }
+// Points per chunk: as many points of `esz` bytes as `free_bytes` of device memory hold after a 512 MiB margin, and no more
+// than `chunk_points` (0: no cap of its own), `longest` (the longest member) or 2^32 - 1; at least 1.
+inline uint64_t srs_chunk_cap(uint64_t chunk_points, uint64_t longest, uint64_t free_bytes, uint64_t esz) {
+  const uint64_t margin = 512ull << 20;
+  uint64_t cap = free_bytes > margin ? (free_bytes - margin) / esz : 0;
+  if (chunk_points) cap = std::min(cap, chunk_points);
+  cap = std::min(cap, std::min<uint64_t>(longest, 0xffffffffull));
+  return std::max<uint64_t>(cap, 1);
+}
+// c tau^j from tab[k] = tau^(2^k): one Fr product per set bit of j (at most 32).  The kernel forms its point's scalar this
+// way with c = x tau^i0 and j = the point's index in its chunk; the host forms c itself the same way with j = i0.
+template <class FrF>
+G16_HD FrF srs_power(FrF c, const FrF* tab, uint64_t j) {
+  for (int k = 0; j; k++, j >>= 1)
+    if (j & 1) c = FrF::mul(c, tab[k]);
+  return c;
+}
 
 // ---- device functions -----------------------------------------------------------------------------------------------
 template <class P>
@@ -127,6 +150,15 @@ template <class F, class FrF>
 __global__ void __launch_bounds__(128) srs_scale_kernel(XYZZ<F>* p, uint32_t cnt, const FrF* s, uint32_t stride) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < cnt) p[i] = srs_mul(p[i], s[(uint64_t)i * stride]);
+}
+// One chunk of a phase-1 contribution, in place: p[j] *= c tau^j (tab[k] = tau^(2^k)), affine in and out; the identity
+// stays the identity.  j in 64 bits: a chunk may hold up to 2^32 - 1 points.
+template <class F, class FrF>
+__global__ void __launch_bounds__(128) srs_contribute_kernel(Affine<F>* p, uint32_t cnt, const FrF* tab, FrF c) {
+  const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= cnt) return;
+  const XYZZ<F> r = srs_mul(XYZZ<F>::from_affine(p[j]), srs_power(c, tab, j));
+  srs_store_affine(&r, p + j);
 }
 // in-place bit-reversal permutation of 2^log_n points
 template <class F>
@@ -213,6 +245,11 @@ cudaError_t srs_scale(cudaStream_t st, XYZZ<F>* p, uint32_t cnt, const FrF* s, u
   if (cnt) srs_scale_kernel<F, FrF><<<srs_blocks(cnt), 128, 0, st>>>(p, cnt, s, stride);
   return cudaGetLastError();
 }
+template <class F, class FrF>
+cudaError_t srs_contribute(cudaStream_t st, Affine<F>* p, uint32_t cnt, const FrF* tab, FrF c) {
+  if (cnt) srs_contribute_kernel<F, FrF><<<srs_blocks(cnt), 128, 0, st>>>(p, cnt, tab, c);
+  return cudaGetLastError();
+}
 // the unscaled inverse transform of 2^log_n points in place: out[j] = sum_i omega^(-ij) in[i]
 template <class F, class FrF>
 cudaError_t srs_ifft(cudaStream_t st, XYZZ<F>* p, int log_n, const FrF* tw_inv, unsigned long long* launches) {
@@ -250,6 +287,7 @@ cudaError_t srs_sum(cudaStream_t st, const XYZZ<F>* src, const uint32_t* d_idx, 
   X cudaError_t srs_load<F>(cudaStream_t, const Affine<F>*, uint32_t, XYZZ<F>*);                                      \
   X cudaError_t srs_affine<F>(cudaStream_t, const XYZZ<F>*, uint32_t, Affine<F>*);                                    \
   X cudaError_t srs_scale<F, FrF>(cudaStream_t, XYZZ<F>*, uint32_t, const FrF*, uint32_t);                            \
+  X cudaError_t srs_contribute<F, FrF>(cudaStream_t, Affine<F>*, uint32_t, const FrF*, FrF);                          \
   X cudaError_t srs_ifft<F, FrF>(cudaStream_t, XYZZ<F>*, int, const FrF*, unsigned long long*);                       \
   X cudaError_t srs_sum<F, FrF>(cudaStream_t, const XYZZ<F>*, const uint32_t*, const FrF*, uint32_t, const SrsSumPlan&, \
                                 XYZZ<F>*, XYZZ<F>*, uint64_t*, uint64_t*, uint32_t, Affine<F>*);

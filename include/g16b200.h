@@ -202,6 +202,30 @@ typedef struct { uint64_t* tau_g1; uint64_t tau_g1_len; uint64_t* tau_g2; uint64
                  uint64_t* beta_g2; } g16_srs_out;
 int g16_srs_from_secrets(g16_ctx* ctx, const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta,
                          const uint64_t* g1, const uint64_t* g2, const g16_srs_out* out);
+/* Phase 1 of the ceremony, the contributor's side (snarkjs `powersoftau contribute`): one contribution tau, alpha, beta
+ * (Montgomery Fr, g16_fr_limbs limbs each, all non-zero) to the transcript `in`, written to `out`.  Point i of each member is
+ * the input point i times its own scalar: tau_g1[i] and tau_g2[i] times tau^i, alpha_tau_g1[i] times alpha tau^i,
+ * beta_tau_g1[i] times beta tau^i, beta_g2 times beta; the identity (all-zero limbs) stays the identity.  After
+ * contributions (tau_k, alpha_k, beta_k) to g16_srs_from_secrets(1, 1, 1, g1, g2) the transcript equals
+ * g16_srs_from_secrets(prod tau_k, prod alpha_k, prod beta_k, g1, g2) limb for limb.  Phase 1 knows no circuit: any length
+ * from 0 to 2^32 - 1 per member, out->*_len equal to in->*_len; a member of length 0 may be null and is skipped; beta_g2
+ * (one point) is always read and written.  out->m may be the very same pointer as in->m (in place); any other overlap of an
+ * output range with an input or another output range is refused.  The result does not depend on chunk_points, on in place
+ * or not, or on flags.
+ * Two passes over the members in chunks of at most chunk_points points (0: as many as the free device memory holds; any
+ * value is also capped by it), so a transcript larger than the device streams through: first every point is uploaded and
+ * checked (coordinates below q, on the curve; G16_SER_VALIDATE adds [r]P = O), and only when all have passed is each chunk
+ * uploaded again, multiplied on the GPU (one thread per point, its scalar formed on the device from tau^(2^k)) and written
+ * to out.  A refused point returns G16_ERR_INVALID_DATA with g16_last_error() naming the first one by member and then index
+ * ("beta_tau_g1[70001]: point is not on the curve") and nothing written to out, so an in-place transcript is intact.
+ * G16_ERR_BAD_ARGUMENT, decided before any point is read: a null pointer where a point or scalar is needed, flags other
+ * than 0 or G16_SER_VALIDATE, a secret equal to 0 ("UnexpectedIdentity"), in and out lengths that differ, a length of 2^32
+ * or more, overlapping ranges, a proof in flight.  Needs no circuit or key and leaves the resident ones and everything
+ * derived from them alone.  Afterwards g16_get_timings describes this call (every other field 0): total_ms = the whole
+ * call, h2d_ms = the check pass, msm_ms[0..3] = the transform of tau_g1, tau_g2, alpha_tau_g1, beta_tau_g1 (host clock
+ * around work that ends in a stream synchronise), h2d_bytes / d2h_bytes = bytes copied each way, launches = kernels. */
+int g16_srs_contribute(g16_ctx* ctx, const g16_srs_desc* in, const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta,
+                       uint32_t flags, uint64_t chunk_points, const g16_srs_out* out);
 
 /* ---- ark-serialized proving keys: `ProvingKey::serialize_{compressed,uncompressed}` / `deserialize_with_mode`
  * (data_structures.rs:125 derives them).  The bytes are a whole ProvingKey<E> as ark-serialize 0.5 writes it: vk {alpha_g1,

@@ -201,6 +201,16 @@ where
     type G2Config = P2;
 }
 
+/// A powers-of-tau transcript (phase 1 of a Groth16 ceremony): tau_g1[i] = [tau^i]G1, tau_g2[i] = [tau^i]G2,
+/// alpha_tau_g1[i] = [alpha tau^i]G1, beta_tau_g1[i] = [beta tau^i]G1, beta_g2 = [beta]G2.
+pub struct PowersOfTau<E: SwPairing> {
+    pub tau_g1: Vec<Affine<E::G1Config>>,
+    pub tau_g2: Vec<Affine<E::G2Config>>,
+    pub alpha_tau_g1: Vec<Affine<E::G1Config>>,
+    pub beta_tau_g1: Vec<Affine<E::G1Config>>,
+    pub beta_g2: Affine<E::G2Config>,
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // the prover: one context = one curve on one GPU with ONE circuit and ONE proving key resident
 // ---------------------------------------------------------------------------------------------------------------------
@@ -421,6 +431,67 @@ impl<E: SwPairing> B200Prover<E> {
         };
         let flags = if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 };
         ser_status(unsafe { sys::g16_setup_from_srs(self.ctx, &desc, flags) })
+    }
+
+    /// One phase-1 contribution (g16_srs_contribute, snarkjs `powersoftau contribute`) to a powers-of-tau transcript, on the
+    /// GPU: point i of `tau_g1` and `tau_g2` times tau^i, of `alpha_tau_g1` times alpha tau^i, of `beta_tau_g1` times
+    /// beta tau^i, and `beta_g2` times beta.  Members may have any length below 2^32 and may be empty.  `validate` adds the
+    /// subgroup check of every point; `chunk_points` caps the points per chunk (0: as many as the free device memory holds).
+    /// A refused point is `InvalidData` (the message naming member and index goes to stderr); a zero secret is an `IoError`
+    /// carrying "UnexpectedIdentity".  Needs no circuit or key and leaves the resident ones alone.
+    #[allow(clippy::too_many_arguments)]
+    pub fn contribute_srs(
+        &self,
+        tau_g1: &[Affine<E::G1Config>],
+        tau_g2: &[Affine<E::G2Config>],
+        alpha_tau_g1: &[Affine<E::G1Config>],
+        beta_tau_g1: &[Affine<E::G1Config>],
+        beta_g2: &Affine<E::G2Config>,
+        tau: E::ScalarField,
+        alpha: E::ScalarField,
+        beta: E::ScalarField,
+        validate: Validate,
+        chunk_points: u64,
+    ) -> Result<PowersOfTau<E>, SerializationError> {
+        // packed copies, transformed in place by the library
+        let (mut t1, mut t2, mut a1, mut b1) =
+            (pack_points(tau_g1), pack_points(tau_g2), pack_points(alpha_tau_g1), pack_points(beta_tau_g1));
+        let mut bg2 = pack_points(core::slice::from_ref(beta_g2));
+        let desc = sys::g16_srs_desc {
+            tau_g1: t1.as_ptr(),
+            tau_g1_len: tau_g1.len() as u64,
+            tau_g2: t2.as_ptr(),
+            tau_g2_len: tau_g2.len() as u64,
+            alpha_tau_g1: a1.as_ptr(),
+            alpha_tau_g1_len: alpha_tau_g1.len() as u64,
+            beta_tau_g1: b1.as_ptr(),
+            beta_tau_g1_len: beta_tau_g1.len() as u64,
+            beta_g2: bg2.as_ptr(),
+        };
+        let out = sys::g16_srs_out {
+            tau_g1: t1.as_mut_ptr(),
+            tau_g1_len: tau_g1.len() as u64,
+            tau_g2: t2.as_mut_ptr(),
+            tau_g2_len: tau_g2.len() as u64,
+            alpha_tau_g1: a1.as_mut_ptr(),
+            alpha_tau_g1_len: alpha_tau_g1.len() as u64,
+            beta_tau_g1: b1.as_mut_ptr(),
+            beta_tau_g1_len: beta_tau_g1.len() as u64,
+            beta_g2: bg2.as_mut_ptr(),
+        };
+        let (t, a, b) = ([tau], [alpha], [beta]);
+        let flags = if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 };
+        ser_status(unsafe {
+            sys::g16_srs_contribute(self.ctx, &desc, scalars_ptr(&t), scalars_ptr(&a), scalars_ptr(&b), flags, chunk_points, &out)
+        })?;
+        let (w1, w2) = (point_limbs::<E::G1Config>(), point_limbs::<E::G2Config>());
+        Ok(PowersOfTau {
+            tau_g1: t1.chunks(w1).map(|l| unpack_point(l)).collect(),
+            tau_g2: t2.chunks(w2).map(|l| unpack_point(l)).collect(),
+            alpha_tau_g1: a1.chunks(w1).map(|l| unpack_point(l)).collect(),
+            beta_tau_g1: b1.chunks(w1).map(|l| unpack_point(l)).collect(),
+            beta_g2: unpack_point(&bg2),
+        })
     }
 
     /// One phase-2 contribution to the resident key (g16_setup_contribute): delta_g1, delta_g2 times `delta`, the H and L
