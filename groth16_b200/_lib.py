@@ -78,6 +78,8 @@ SIGNATURES = [
     ("g16_srs_from_secrets", C.c_int, [C.c_void_p] + [C.c_void_p] * 5 + [C.POINTER(SrsOut)]),
     ("g16_srs_contribute", C.c_int, [C.c_void_p, C.POINTER(SrsDesc)] + [C.c_void_p] * 3 + [C.c_uint32, C.c_uint64,
                                                                                           C.POINTER(SrsOut)]),
+    ("g16_srs_verify_pairs", C.c_int, [C.c_void_p, C.POINTER(SrsDesc)] + [C.c_void_p] * 3 + [C.c_uint32, C.c_uint64]
+     + [C.c_void_p] * 2),
     ("g16_pk_load_serialized", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
                                          C.POINTER(PkExportDesc)]),
     ("g16_pk_export_serialized", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),

@@ -19,7 +19,7 @@ import numpy as np
 
 from . import _lib
 from .codec import CurveCodec
-from .params import CurveParams, get_curve
+from .params import GENERATORS, CurveParams, get_curve
 from .serialize import DeserializeError
 
 
@@ -171,6 +171,46 @@ def srs_arrays(srs: Srs, g1_width: int, g2_width: int, in_place: bool = False) -
                 raise ValueError(f"srs.{k} of shape {a.shape} is not a list of points of {w} limbs")
             out[k] = a.reshape(-1, w)
     return out
+
+
+SRS_EQUATIONS = ("tau_g1", "tau_g2", "alpha_tau_g1", "beta_tau_g1", "beta_g2")
+
+
+@dataclass
+class SrsPairs:
+    """g16_srs_verify_pairs: the five pairing equations of a transcript check.  Equation k (the member members[k]) holds iff
+    e(g1[2k], g2[2k]) = e(g1[2k + 1], g2[2k + 1]); g1 is (10, G1 limbs) and g2 is (10, G2 limbs), affine Montgomery limbs."""
+    g1: np.ndarray
+    g2: np.ndarray
+    members: Tuple[str, ...] = SRS_EQUATIONS
+
+    def equation(self, k: int) -> tuple:
+        """(P_k, Q_k, P'_k, Q'_k) of equation k, as limb arrays"""
+        return self.g1[2 * k], self.g2[2 * k], self.g1[2 * k + 1], self.g2[2 * k + 1]
+
+
+SRS_VERIFY_MIN = dict(tau_g1=2, tau_g2=2, alpha_tau_g1=1, beta_tau_g1=1)
+
+
+def srs_verify_args(srs: Srs, rho, r: int, g1_width: int, g2_width: int, chunk_points: int = 0) -> tuple:
+    """The arguments of Groth16.srs_verification_pairs as the library takes them: (the members as srs_arrays gives them,
+    rho mod r, chunk_points).  ValueError, before any device work: a member that is not made of whole points, a member
+    shorter than the check needs (tau_g1 and tau_g2 two points, alpha_tau_g1 and beta_tau_g1 one) or of 2^32 points or
+    more, rho = 0 mod r, chunk_points outside [0, 2^64)."""
+    arrs = srs_arrays(srs, g1_width, g2_width)
+    for k, need in SRS_VERIFY_MIN.items():
+        have = arrs[k].shape[0]
+        if have < need:
+            raise ValueError(f"srs.{k} holds {have} points, the check needs at least {need}")
+        if have >= 1 << 32:
+            raise ValueError(f"srs.{k} holds {have} points, at most 2^32 - 1 are allowed")
+    rho = int(rho) % r
+    if rho == 0:
+        raise ValueError("the challenge rho must be non-zero mod r")
+    chunk_points = int(chunk_points)
+    if not 0 <= chunk_points < 1 << 64:
+        raise ValueError(f"chunk_points must be in [0, 2^64), not {chunk_points}")
+    return arrs, rho, chunk_points
 
 
 @dataclass
@@ -443,6 +483,39 @@ class Groth16:
         _check(self._lib.g16_srs_contribute(self._ctx, C.byref(d_in), *[_ptr(x) for x in sc],
                                             _lib.SER_VALIDATE if validate else 0, chunk_points, C.byref(d_out)))
         return srs if in_place else Srs(**outs)
+
+    def srs_verification_pairs(self, srs: Srs, rho, g1=None, g2=None, validate: bool = True,
+                               chunk_points: int = 0) -> SrsPairs:
+        """g16_srs_verify_pairs: the GPU part of checking that `srs` is a powers-of-tau transcript T(tau, alpha, beta) over
+        the generators g1, g2 (affine int tuples; default params.GENERATORS[curve]).  rho (a Python int, non-zero mod r) is
+        the challenge: draw it after the transcript is fixed, so that whoever made the transcript cannot predict it (e.g.
+        secrets.randbelow(r - 1) + 1, or a hash of the transcript).
+
+        The library checks every point (canonical, on the curve, and with `validate` in the prime-order subgroup), refuses
+        the identity anywhere and checks tau_g1[0] = g1 and tau_g2[0] = g2; a refused point raises
+        serialize.DeserializeError naming it.  It returns five equations, one per member (SrsPairs): with
+        (P, Q, P', Q') = pairs.equation(k), the caller evaluates e(P, Q) = e(P', Q') with its own pairing, e.g.
+        multi_pairing([P, -P'], [Q, Q']) == 1.  The transcript is accepted iff all five hold; then, with probability at
+        least 1 - N/r over rho, it is T(tau, alpha, beta) for non-zero tau, alpha, beta with one tau in both groups.
+        `validate` defaults to True: without the subgroup check the answer means nothing on a curve whose cofactor is not
+        1.  `chunk_points` caps the points per chunk (0: as many as the free device memory holds).  Needs no circuit or key
+        and leaves the resident ones alone."""
+        arrs, rho, chunk_points = srs_verify_args(srs, rho, self.curve.r, 2 * self.nq, self.ng2, chunk_points)
+        G = GENERATORS[self.curve.name]
+        cd = self.codec
+        g1 = np.ascontiguousarray(cd.enc_g1([G["g1"] if g1 is None else g1])[0])
+        g2 = np.ascontiguousarray(cd.enc_g2([G["g2"] if g2 is None else g2])[0])
+        d = _lib.SrsDesc()
+        for k in SRS_VECTORS:
+            setattr(d, k, _u64p(arrs[k]))
+            setattr(d, k + "_len", arrs[k].shape[0])
+        d.beta_g2 = _u64p(arrs["beta_g2"])
+        out1 = np.zeros((10, 2 * self.nq), dtype=np.uint64)
+        out2 = np.zeros((10, self.ng2), dtype=np.uint64)
+        r_ = np.ascontiguousarray(cd.fr.enc1(rho))
+        _check(self._lib.g16_srs_verify_pairs(self._ctx, C.byref(d), _ptr(g1), _ptr(g2), _ptr(r_),
+                                              _lib.SER_VALIDATE if validate else 0, chunk_points, _ptr(out1), _ptr(out2)))
+        return SrsPairs(out1, out2)
 
     def _after_key_change(self, rc: int):
         """Status of g16_setup_from_srs / g16_setup_contribute: argument errors (G16_ERR_BAD_ARGUMENT,

@@ -150,6 +150,8 @@ struct IEngine {
                                const uint64_t* g2, const g16_srs_out* out) = 0;
   virtual int srs_contribute(const g16_srs_desc* in, const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta,
                              uint32_t flags, uint64_t chunk_points, const g16_srs_out* out) = 0;
+  virtual int srs_verify_pairs(const g16_srs_desc* srs, const uint64_t* g1, const uint64_t* g2, const uint64_t* rho,
+                               uint32_t flags, uint64_t chunk_points, uint64_t* pairs_g1, uint64_t* pairs_g2) = 0;
   virtual int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                                  const g16_pk_export_desc* vk_out) = 0;
   virtual int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) = 0;
@@ -1475,6 +1477,172 @@ struct Engine : IEngine {
     tm.total_ms = ms_since(t0);
     return G16_OK;
   }
+  // The MSM geometry of one chunk of a transcript check: caller-supplied bases, as msm_host runs them
+  MsmGeom srs_verify_geom(uint64_t cnt, bool g2) const { return with_k0(msm_geom(cnt, FR_BITS, (int)tune.c, 0), g2); }
+  // One member of g16_srs_verify_pairs: sum = sum_i rho^i X_i over its len points, in chunks of at most cap points through
+  // buf (points), dsc (scalars) and dmask (identity mask).  Each chunk is uploaded and checked (the identity refused, and
+  // with gen the first point must be that generator) and its error word read before its scalars and MSM are enqueued, so a
+  // refusal stops the call before a later chunk is read.  The chunk's MSM result is added to sum on the host.
+  template <class F>
+  int srs_verify_member(int m, bool g2, const uint64_t* src, uint64_t len, const uint64_t* gen, uint32_t flags, uint64_t cap,
+                        DevBuf& buf, DevBuf& dsc, DevBuf& dmask, DevBuf& err, const Fr* dtab, const Fr* tab, XYZZ<F>& sum) {
+    cudaStream_t st = S0.st_main;
+    MsmWorkspace<F> ws;   // this call's own: the prover's workspaces keep their sizes
+    MsmCounters mc;
+    sum = XYZZ<F>::inf();
+    for (uint64_t i0 = 0; i0 < len;) {
+      const uint32_t cnt = srs_chunk_len(len, i0, cap);
+      G16_CUDA(cudaMemcpyAsync(buf.p, src + i0 * (sizeof(Affine<F>) / 8), cnt * sizeof(Affine<F>), cudaMemcpyHostToDevice, st));
+      G16_CUDA(cudaMemsetAsync(err.p, 0xff, 8, st));
+      unsigned long long* e = err.template as<unsigned long long>();
+      const uint32_t fl = flags | SRS_REFUSE_IDENTITY;
+      G16_CUDA((g2 ? srs_check<CP, true>(st, buf.p, cnt, fl, m, e) : srs_check<CP, false>(st, buf.p, cnt, fl, m, e)));
+      unsigned long long first_err = 0;
+      G16_CUDA(cudaMemcpyAsync(&first_err, err.p, 8, cudaMemcpyDeviceToHost, st));
+      G16_CUDA(cudaStreamSynchronize(st));
+      tm.h2d_bytes += cnt * sizeof(Affine<F>);
+      tm.d2h_bytes += 8;
+      tm.launches++;
+      const uint64_t bad_at = first_err == ~0ull ? ~0ull : i0 + ((first_err >> 8) & ((1ull << 40) - 1));
+      // point 0 first: a failed check there is named as such, else a wrong generator comes before any later bad point
+      if (bad_at != 0 && i0 == 0 && gen && memcmp(src, gen, sizeof(Affine<F>)))
+        return fail(G16_ERR_INVALID_DATA, std::string(srs_member(m)) + "[0]: not the generator " + (g2 ? "g2" : "g1"));
+      if (first_err != ~0ull)
+        return fail(G16_ERR_INVALID_DATA, std::string(srs_member(m)) + "[" + std::to_string(bad_at) + "]: " +
+                                              srs_reason(first_err & 0xff));
+      // scalars rho^(i0 + j), then the chunk's MSM
+      G16_CUDA(srs_powers<Fr>(st, dtab, srs_power(Fr::one(), tab, i0), cnt, dsc.template as<Fr>()));
+      G16_CUDA(msm_prepare_query<F>(st, buf.template as<Affine<F>>(), cnt, 1, 0, dmask.template as<uint8_t>()));
+      const MsmGeom g = srs_verify_geom(cnt, g2);
+      G16_CUDA((msm_enqueue<F, Fr>(st, ws, g, buf.template as<Affine<F>>(), dmask.template as<uint8_t>(), dsc.template as<uint32_t>(),
+                                   1, true, &mc, nullptr, nullptr, nullptr, nullptr, nullptr, 0)));
+      G16_CUDA(cudaStreamSynchronize(st));
+      sum.add(msm_finish<F>(ws, g));
+      tm.launches += 2;
+      tm.d2h_bytes += 4 + ws.plan.leaf_pts * g.sets() * sizeof(XYZZ<F>);   // msm_enqueue's slot total and leaf arrays
+      i0 += cnt;
+    }
+    tm.launches += mc.launches;
+    return G16_OK;
+  }
+  // g16_srs_verify_pairs: the five pairing equations of a powers-of-tau transcript under the challenge rho, after every
+  // point passed the checks (srs_verify_member).  For a member X of N points, S = sum_{i<N} rho^i X_i is one MSM per member;
+  // lo = S - rho^(N-1) X_(N-1) and hi = rho^-1 (S - X_0) are formed on the host.  Nothing is written until every check passed.
+  // Timings (host clock around work that ends in a stream synchronise): msm_ms[m] = member m's chunk loop, total_ms = the
+  // whole call.
+  int srs_verify_pairs(const g16_srs_desc* srs, const uint64_t* g1_, const uint64_t* g2_, const uint64_t* rho_, uint32_t flags,
+                       uint64_t chunk_points, uint64_t* pairs_g1, uint64_t* pairs_g2) override {
+    if (!srs || !g1_ || !g2_ || !rho_ || !pairs_g1 || !pairs_g2) return fail(G16_ERR_BAD_ARGUMENT, "null argument");
+    const uint64_t* src[SRS_MEMBERS] = {srs->tau_g1, srs->tau_g2, srs->alpha_tau_g1, srs->beta_tau_g1, srs->beta_g2};
+    const uint64_t len[SRS_MEMBERS] = {srs->tau_g1_len, srs->tau_g2_len, srs->alpha_tau_g1_len, srs->beta_tau_g1_len, 1};
+    for (int m = 0; m < SRS_MEMBERS; m++)
+      if (!src[m]) return fail(G16_ERR_BAD_ARGUMENT, std::string("null srs member ") + srs_member(m));
+    if (flags & ~(uint32_t)G16_SER_VALIDATE) return fail(G16_ERR_BAD_ARGUMENT, "g16_srs_verify_pairs takes 0 or G16_SER_VALIDATE");
+    const Fr rho = load_fr(rho_);
+    if (rho.is_zero()) return fail(G16_ERR_BAD_ARGUMENT, "the challenge rho must be non-zero");
+    const uint64_t need[SRS_MEMBERS] = {2, 2, 1, 1, 1};
+    for (int m = 0; m < SRS_MEMBERS; m++) {
+      if (len[m] < need[m])
+        return fail(G16_ERR_BAD_ARGUMENT, std::string(srs_member(m)) + " holds " + std::to_string(len[m]) + " points, at least " +
+                                              std::to_string(need[m]) + " are needed");
+      if (len[m] >> 32)
+        return fail(G16_ERR_BAD_ARGUMENT, std::string(srs_member(m)) + " holds " + std::to_string(len[m]) +
+                                              " points, at most 2^32 - 1 are allowed");
+    }
+    G16_NOT_BUSY();
+    G16_CUDA(cudaSetDevice(device));
+    const auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point a) {
+      return (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count();
+    };
+    tm = g16_timings{};
+    cudaStream_t st = S0.st_main;
+    size_t free_b = 0, total_b = 0;
+    G16_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const uint64_t longest = *std::max_element(len, len + SRS_BETA_G2);
+    // one workspace is alive at a time (per member), so a chunk needs the larger of the two groups' workspaces
+    auto ws_bytes = [&](uint64_t cnt) {
+      MsmGeom g[2] = {srs_verify_geom(cnt, false), srs_verify_geom(cnt, true)};
+      MsmBaPlan bap[2];
+      MsmRedPlan plan[2];
+      for (int k = 0; k < 2; k++) { bap[k].make(g[k]); plan[k].make(g[k].c - 1); }
+      return std::max(msm_ws_bytes<Fq>(g[0], bap[0], plan[0]).total(), msm_ws_bytes<Fq2>(g[1], bap[1], plan[1]).total());
+    };
+    const uint64_t per_point = std::max(sizeof(A1), sizeof(A2)) + sizeof(Fr) + 1;
+    const uint64_t cap = srs_verify_chunk_cap(chunk_points, longest, free_b, per_point, ws_bytes);
+    DevBuf buf, dsc, dmask, err, dtab;
+    G16_CUDA(buf.reserve(cap * std::max(sizeof(A1), sizeof(A2))));
+    G16_CUDA(dsc.reserve(cap * sizeof(Fr)));
+    G16_CUDA(dmask.reserve(cap));
+    G16_CUDA(err.reserve(8));
+    Fr tab[32];
+    tab[0] = rho;
+    for (int k = 1; k < 32; k++) tab[k] = Fr::sqr(tab[k - 1]);
+    G16_CUDA(dtab.reserve(sizeof(tab)));
+    G16_CUDA(cudaMemcpyAsync(dtab.p, tab, sizeof(tab), cudaMemcpyHostToDevice, st));
+    tm.h2d_bytes += sizeof(tab);
+    P1 s1[4];
+    P2 s2;
+    int rc;
+    for (int m = 0; m < 4; m++) {
+      const auto t1 = std::chrono::steady_clock::now();
+      if (m == SRS_TAU_G2)
+        rc = srs_verify_member<Fq2>(m, true, src[m], len[m], g2_, flags, cap, buf, dsc, dmask, err, dtab.template as<Fr>(), tab, s2);
+      else
+        rc = srs_verify_member<Fq>(m, false, src[m], len[m], m == SRS_TAU_G1 ? g1_ : nullptr, flags, cap, buf, dsc, dmask, err,
+                                   dtab.template as<Fr>(), tab, s1[m]);
+      if (rc) return rc;
+      tm.msm_ms[m] = ms_since(t1);
+      tm.msm_pairs[m] = len[m];
+    }
+    // beta_g2 is one point: checked on the device with the others, used on the host
+    G16_CUDA(cudaMemcpyAsync(buf.p, src[SRS_BETA_G2], sizeof(A2), cudaMemcpyHostToDevice, st));
+    G16_CUDA(cudaMemsetAsync(err.p, 0xff, 8, st));
+    G16_CUDA((srs_check<CP, true>(st, buf.p, 1, flags | SRS_REFUSE_IDENTITY, SRS_BETA_G2, err.template as<unsigned long long>())));
+    unsigned long long first_err = 0;
+    G16_CUDA(cudaMemcpyAsync(&first_err, err.p, 8, cudaMemcpyDeviceToHost, st));
+    G16_CUDA(cudaStreamSynchronize(st));
+    tm.h2d_bytes += sizeof(A2);
+    tm.d2h_bytes += 8;
+    tm.launches++;
+    if (first_err != ~0ull) return fail(G16_ERR_INVALID_DATA, std::string("beta_g2[0]: ") + srs_reason(first_err & 0xff));
+    // lo and hi of every member: two scalar multiplications and one shared inversion
+    const Fr rho_inv = Fr::inv(rho);
+    uint32_t k[Fr::N];
+    auto lo_hi = [&](auto S, auto pt, int m, auto& lo, auto& hi) {
+      using PT = decltype(S);
+      const uint64_t w = srs_point_limbs(m);
+      const PT x0 = PT::from_affine(pt(src[m])), xl = PT::from_affine(pt(src[m] + (len[m] - 1) * w));
+      fr_to_canon(srs_power(Fr::one(), tab, len[m] - 1), k);
+      PT t = xl.mul_u32(k, Fr::N);
+      t.negate();
+      lo = S;
+      lo.add(t);
+      PT d = x0;
+      d.negate();
+      d.add(S);
+      fr_to_canon(rho_inv, k);
+      hi = d.mul_u32(k, Fr::N);
+    };
+    P1 lo1[4], hi1[4];
+    P2 lo2, hi2;
+    for (int m : {SRS_TAU_G1, SRS_ALPHA, SRS_BETA}) lo_hi(s1[m], load_a1, m, lo1[m], hi1[m]);
+    lo_hi(s2, load_a2, SRS_TAU_G2, lo2, hi2);
+    const A1 g1 = load_a1(g1_), t1 = load_a1(src[SRS_TAU_G1] + 2 * NQ64), b0 = load_a1(src[SRS_BETA]);
+    const A2 g2 = load_a2(g2_), t2 = load_a2(src[SRS_TAU_G2] + G2_64), bg2 = load_a2(src[SRS_BETA_G2]);
+    // equation k: e(P_k, Q_k) = e(P'_k, Q'_k), written as P_0, P'_0, .., P_4, P'_4 and Q_0, Q'_0, .., Q_4, Q'_4
+    const A1 ps[10] = {hi1[SRS_TAU_G1].to_affine(), lo1[SRS_TAU_G1].to_affine(), g1, t1, hi1[SRS_ALPHA].to_affine(),
+                       lo1[SRS_ALPHA].to_affine(), hi1[SRS_BETA].to_affine(), lo1[SRS_BETA].to_affine(), b0, g1};
+    const A2 qs[10] = {g2, t2, hi2.to_affine(), lo2.to_affine(), g2, t2, g2, t2, g2, bg2};
+    for (int i = 0; i < 10; i++) {
+      store_a1(pairs_g1 + (size_t)i * 2 * NQ64, ps[i]);
+      store_a2(pairs_g2 + (size_t)i * G2_64, qs[i]);
+    }
+    tm.total_ms = ms_since(t0);
+    return G16_OK;
+  }
+  // u64 limbs of one point of transcript member m
+  static uint64_t srs_point_limbs(int m) { return (m == SRS_TAU_G2 || m == SRS_BETA_G2) ? (uint64_t)G2_64 : (uint64_t)(2 * NQ64); }
   // CircomReduction::h_query_scalars(n - 1, tau, _, delta^-1): the odd entries 1, 3, .., 2n - 1 of the size-2n ifft of
   // v[i] = delta^-1 tau^i (i < 2n - 1), v[2n - 1] = 0.  With w = omega_2n, k = 2j + 1 and the geometric sum in closed form:
   //   out[j] = delta^-1 / (2n) * [ (tau^2n - 1) / (tau w^-k - 1) - tau^(2n-1) w^k ]

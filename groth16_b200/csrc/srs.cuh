@@ -1,7 +1,7 @@
 // srs.cuh -- proving keys from a powers-of-tau transcript (g16_setup_from_srs) and phase-2 delta contributions
 // (g16_setup_contribute): the group-valued inverse FFT, sparse sums of points, one scalar times many points, and the
-// transcript point checks; and phase-1 contributions to a transcript (g16_srs_contribute): every point times its own power
-// of the secret.
+// transcript point checks; phase-1 contributions to a transcript (g16_srs_contribute): every point times its own power
+// of the secret; and the scalars of the transcript check (g16_srs_verify_pairs): one power of the challenge per point.
 //
 // Every kernel works on XYZZ points in global memory, one point (or one butterfly, or one chunk of a sum) per thread.  The
 // scalar multiplications are left-to-right double-and-add over the canonical scalar (XYZZ::mul_u32); a windowed form would
@@ -77,17 +77,46 @@ G16_HD FrF srs_power(FrF c, const FrF* tab, uint64_t j) {
   return c;
 }
 
+// ---- transcript checks (g16_srs_verify_pairs) ---------------------------------------------------------------------------
+// The largest chunk one MSM of caller-supplied bases takes (the stand-alone MSM refuses n >= 2^27).
+static constexpr uint64_t SRS_VERIFY_MSM_MAX = (1ull << 27) - 1;
+// Points per chunk of the transcript check: the most that `free_bytes` of device memory hold after the 512 MiB margin, a
+// chunk of cnt points needing cnt * per_point bytes (the point, its Fr scalar, its byte of the identity mask) and
+// ws_bytes(cnt) for the MSM workspace of its geometry; and no more than `chunk_points` (0: no cap of its own), `longest`
+// or SRS_VERIFY_MSM_MAX; at least 1.  The workspace is not linear in cnt (the window grows with it), so the largest chunk
+// that fits is found by bisection.
+template <class WsBytes>
+uint64_t srs_verify_chunk_cap(uint64_t chunk_points, uint64_t longest, uint64_t free_bytes, uint64_t per_point, WsBytes ws_bytes) {
+  const uint64_t margin = 512ull << 20;
+  const uint64_t avail = free_bytes > margin ? free_bytes - margin : 0;
+  auto fits = [&](uint64_t cnt) { return cnt * per_point + (uint64_t)ws_bytes(cnt) <= avail; };
+  uint64_t cap = std::min(longest, SRS_VERIFY_MSM_MAX);
+  if (chunk_points) cap = std::min(cap, chunk_points);
+  if (cap <= 1 || fits(cap)) return std::max<uint64_t>(cap, 1);
+  uint64_t lo = 1, hi = cap;   // hi does not fit; lo fits, or is the floor of 1
+  while (hi - lo > 1) {
+    const uint64_t mid = lo + (hi - lo) / 2;
+    (fits(mid) ? lo : hi) = mid;
+  }
+  return lo;
+}
+
 // ---- device functions -----------------------------------------------------------------------------------------------
 template <class P>
 G16_HD bool srs_canonical(const Fp<P>& a) { return ser_lt_mod(a); }
 template <class P, int NR>
 G16_HD bool srs_canonical(const Fp2<P, NR>& a) { return ser_lt_mod(a.c0) && ser_lt_mod(a.c1); }
+// Check flag of the transcript check alone (beside SER_VALIDATE): the identity is refused, with its own result code.
+enum : uint32_t { SRS_REFUSE_IDENTITY = 1u << 8 };
+enum : uint32_t { SRS_ERR_IDENTITY = 9 };   // after the SER_ERR_* codes of ser.cuh
+inline const char* srs_reason(uint32_t code) { return code == SRS_ERR_IDENTITY ? "point is the identity" : ser_reason(code); }
 // A transcript point: Montgomery limbs below q, on the curve, and with G16_SER_VALIDATE in the prime-order subgroup (the
-// check ser.cuh runs on decoded keys; skipped for BN254 G1, whose cofactor is 1).  All-zero limbs are the identity.
+// check ser.cuh runs on decoded keys; skipped for BN254 G1, whose cofactor is 1).  All-zero limbs are the identity, accepted
+// unless SRS_REFUSE_IDENTITY is set.
 template <class CP, bool G2>
 G16_HD uint32_t srs_check_point(const Affine<SerField<CP, G2>>& p, uint32_t flags) {
   using F = SerField<CP, G2>;
-  if (p.is_inf()) return SER_OK;
+  if (p.is_inf()) return (flags & SRS_REFUSE_IDENTITY) ? (uint32_t)SRS_ERR_IDENTITY : (uint32_t)SER_OK;
   if (!srs_canonical(p.x) || !srs_canonical(p.y)) return SER_ERR_NONCANONICAL;
   if (F::sqr(p.y) != F::add(F::mul(F::sqr(p.x), p.x), ser_b<CP, G2>())) return SER_ERR_OFF_CURVE;
   if ((flags & SER_VALIDATE) && !(!G2 && SerFormat<CP>::G1_COFACTOR_ONE) && !ser_in_subgroup<typename CP::FrP>(p))
@@ -159,6 +188,12 @@ __global__ void __launch_bounds__(128) srs_contribute_kernel(Affine<F>* p, uint3
   if (j >= cnt) return;
   const XYZZ<F> r = srs_mul(XYZZ<F>::from_affine(p[j]), srs_power(c, tab, j));
   srs_store_affine(&r, p + j);
+}
+// The scalars of one chunk of a transcript check: out[j] = c rho^j (tab[k] = rho^(2^k), c = rho^i0), Montgomery form.
+template <class FrF>
+__global__ void __launch_bounds__(128) srs_powers_kernel(const FrF* tab, FrF c, uint32_t cnt, FrF* out) {
+  const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < cnt) out[j] = srs_power(c, tab, j);
 }
 // in-place bit-reversal permutation of 2^log_n points
 template <class F>
@@ -250,6 +285,11 @@ cudaError_t srs_contribute(cudaStream_t st, Affine<F>* p, uint32_t cnt, const Fr
   if (cnt) srs_contribute_kernel<F, FrF><<<srs_blocks(cnt), 128, 0, st>>>(p, cnt, tab, c);
   return cudaGetLastError();
 }
+template <class FrF>
+cudaError_t srs_powers(cudaStream_t st, const FrF* tab, FrF c, uint32_t cnt, FrF* out) {
+  if (cnt) srs_powers_kernel<FrF><<<srs_blocks(cnt), 128, 0, st>>>(tab, c, cnt, out);
+  return cudaGetLastError();
+}
 // the unscaled inverse transform of 2^log_n points in place: out[j] = sum_i omega^(-ij) in[i]
 template <class F, class FrF>
 cudaError_t srs_ifft(cudaStream_t st, XYZZ<F>* p, int log_n, const FrF* tw_inv, unsigned long long* launches) {
@@ -294,6 +334,7 @@ cudaError_t srs_sum(cudaStream_t st, const XYZZ<F>* src, const uint32_t* d_idx, 
 #define G16_SRS_TEMPLATES(X, CP)                                                                                     \
   X cudaError_t srs_check<CP, false>(cudaStream_t, const void*, uint32_t, uint32_t, uint32_t, unsigned long long*);  \
   X cudaError_t srs_check<CP, true>(cudaStream_t, const void*, uint32_t, uint32_t, uint32_t, unsigned long long*);   \
+  X cudaError_t srs_powers<Fp<CP::FrP>>(cudaStream_t, const Fp<CP::FrP>*, Fp<CP::FrP>, uint32_t, Fp<CP::FrP>*);     \
   G16_SRS_POINT_TEMPLATES(X, Fp<CP::FqP>, Fp<CP::FrP>)
 #endif
 

@@ -226,6 +226,43 @@ int g16_srs_from_secrets(g16_ctx* ctx, const uint64_t* tau, const uint64_t* alph
  * around work that ends in a stream synchronise), h2d_bytes / d2h_bytes = bytes copied each way, launches = kernels. */
 int g16_srs_contribute(g16_ctx* ctx, const g16_srs_desc* in, const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta,
                        uint32_t flags, uint64_t chunk_points, const g16_srs_out* out);
+/* Phase 1 of the ceremony, the checker's side (snarkjs `powersoftau verify`, without the contributions' proofs of knowledge):
+ * the GPU part of checking that `srs` is a powers-of-tau transcript T(tau, alpha, beta) over the agreed affine generators g1,
+ * g2.  rho (Montgomery Fr, non-zero) is a challenge the caller draws after the transcript is fixed, which whoever made the
+ * transcript cannot predict (a CSPRNG, or a hash of the transcript).  For a member X of N points let
+ *   S_X = sum_{i<N} rho^i X_i        (one MSM per member, on the GPU)
+ *   lo_X = S_X - rho^(N-1) X_(N-1) = sum_{i<N-1} rho^i X_i,   hi_X = rho^-1 (S_X - X_0) = sum_{i<N-1} rho^i X_(i+1)
+ * (a member of one point has lo = hi = the identity).  The call writes ten affine G1 points P_0, P'_0, .., P_4, P'_4 to
+ * pairs_g1 and ten affine G2 points Q_0, Q'_0, .., Q_4, Q'_4 to pairs_g2; equation k holds iff e(P_k, Q_k) = e(P'_k, Q'_k):
+ *   k = 0  tau_g1        (hi_T1, g2)               = (lo_T1, tau_g2[1])
+ *   k = 1  tau_g2        (g1, hi_T2)               = (tau_g1[1], lo_T2)
+ *   k = 2  alpha_tau_g1  (hi_A, g2)                = (lo_A, tau_g2[1])
+ *   k = 3  beta_tau_g1   (hi_B, g2)                = (lo_B, tau_g2[1])
+ *   k = 4  beta_g2       (beta_tau_g1[0], g2)      = (g1, beta_g2)
+ * The pairings are the caller's: this library has none.  The call itself checks every point (coordinates below q, on the
+ * curve; G16_SER_VALIDATE adds [r]P = O, without which the answer means nothing on a curve whose cofactor is not 1), that no
+ * point is the identity (it would mean tau, alpha or beta = 0), and that tau_g1[0] = g1 and tau_g2[0] = g2.  If those pass
+ * and all five equations hold, then with probability at least 1 - N/r over rho (N the longest member) the transcript is
+ * T(tau, alpha, beta) for some non-zero tau, alpha, beta with the same tau in both groups: a member that is not geometric
+ * with ratio tau makes sum_i rho^i (X_(i+1) - tau X_i) a non-zero polynomial in rho of degree at most N - 2 (Schwartz-Zippel).
+ * alpha has no G2 counterpart in a transcript, so its chain is checked against tau only, which is all Groth16 needs.
+ * Lengths: tau_g1 and tau_g2 at least 2 points, alpha_tau_g1 and beta_tau_g1 at least 1, each below 2^32; beta_g2 is one
+ * point.  One pass over the members in chunks of at most chunk_points points (0: as many as the free device memory holds,
+ * counting the points, their scalars and the MSM workspace; any value is also capped by it and by 2^27 - 1), so a
+ * transcript larger than the device streams through: each chunk is uploaded and checked, and only then are its scalars
+ * rho^i formed on the device (one thread per point, from rho^(2^k)) and its MSM run.  A refused point returns
+ * G16_ERR_INVALID_DATA with g16_last_error() naming the first one by member and then index ("tau_g2[5]: point is the
+ * identity", "tau_g1[0]: not the generator g1") and nothing written; later chunks are not read.  The identity is refused by
+ * this call only: g16_setup_from_srs and g16_srs_contribute accept it.
+ * G16_ERR_BAD_ARGUMENT, decided before any point is read, with nothing written: a null pointer, flags other than 0 or
+ * G16_SER_VALIDATE, rho = 0, a member shorter than the lengths above or of 2^32 points or more, a proof in flight.  Needs no
+ * circuit or key and leaves the resident ones and everything derived from them alone.  The result does not depend on
+ * chunk_points or on flags.  Afterwards g16_get_timings describes this call (every other field 0): total_ms = the whole
+ * call, msm_ms[0..3] = the chunk loop (upload, check, scalars, MSM) of tau_g1, tau_g2, alpha_tau_g1, beta_tau_g1 (host
+ * clock around work that ends in a stream synchronise), msm_pairs[0..3] = the points of each member's MSM, h2d_bytes /
+ * d2h_bytes = bytes copied each way, launches = kernels. */
+int g16_srs_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const uint64_t* g1, const uint64_t* g2, const uint64_t* rho,
+                         uint32_t flags, uint64_t chunk_points, uint64_t* pairs_g1, uint64_t* pairs_g2);
 
 /* ---- ark-serialized proving keys: `ProvingKey::serialize_{compressed,uncompressed}` / `deserialize_with_mode`
  * (data_structures.rs:125 derives them).  The bytes are a whole ProvingKey<E> as ark-serialize 0.5 writes it: vk {alpha_g1,

@@ -494,6 +494,85 @@ impl<E: SwPairing> B200Prover<E> {
         })
     }
 
+    /// The GPU part of checking a powers-of-tau transcript (g16_srs_verify_pairs, snarkjs `powersoftau verify` without the
+    /// proofs of knowledge): every point is checked (curve, with `validate` the subgroup, never the identity), tau_g1[0] must
+    /// be `g1` and tau_g2[0] must be `g2`, and one MSM per member under the challenge `rho` (non-zero, drawn after the
+    /// transcript is fixed) reduces each member's chain to one pairing equation.  Returns the five equations as
+    /// (P, Q, P', Q'); equation k holds iff e(P, Q) = e(P', Q').  A refused point is `InvalidData` (the message naming
+    /// member and index goes to stderr); an argument error (a member too short, rho = 0) is an `IoError` carrying it.
+    #[allow(clippy::type_complexity)]
+    pub fn srs_verification_pairs(
+        &self,
+        srs: &PowersOfTau<E>,
+        g1: &Affine<E::G1Config>,
+        g2: &Affine<E::G2Config>,
+        rho: E::ScalarField,
+        validate: Validate,
+        chunk_points: u64,
+    ) -> Result<[(Affine<E::G1Config>, Affine<E::G2Config>, Affine<E::G1Config>, Affine<E::G2Config>); 5], SerializationError>
+    {
+        let (t1, t2, a1, b1) =
+            (pack_points(&srs.tau_g1), pack_points(&srs.tau_g2), pack_points(&srs.alpha_tau_g1), pack_points(&srs.beta_tau_g1));
+        let bg2 = pack_points(core::slice::from_ref(&srs.beta_g2));
+        let desc = sys::g16_srs_desc {
+            tau_g1: t1.as_ptr(),
+            tau_g1_len: srs.tau_g1.len() as u64,
+            tau_g2: t2.as_ptr(),
+            tau_g2_len: srs.tau_g2.len() as u64,
+            alpha_tau_g1: a1.as_ptr(),
+            alpha_tau_g1_len: srs.alpha_tau_g1.len() as u64,
+            beta_tau_g1: b1.as_ptr(),
+            beta_tau_g1_len: srs.beta_tau_g1.len() as u64,
+            beta_g2: bg2.as_ptr(),
+        };
+        let (gp1, gp2) = (pack_points(core::slice::from_ref(g1)), pack_points(core::slice::from_ref(g2)));
+        let (w1, w2) = (point_limbs::<E::G1Config>(), point_limbs::<E::G2Config>());
+        let (mut o1, mut o2) = (vec![0u64; 10 * w1], vec![0u64; 10 * w2]);
+        let r = [rho];
+        let flags = if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 };
+        ser_status(unsafe {
+            sys::g16_srs_verify_pairs(
+                self.ctx,
+                &desc,
+                gp1.as_ptr(),
+                gp2.as_ptr(),
+                scalars_ptr(&r),
+                flags,
+                chunk_points,
+                o1.as_mut_ptr(),
+                o2.as_mut_ptr(),
+            )
+        })?;
+        let p = |i: usize| unpack_point::<E::G1Config>(&o1[i * w1..(i + 1) * w1]);
+        let q = |i: usize| unpack_point::<E::G2Config>(&o2[i * w2..(i + 1) * w2]);
+        Ok(core::array::from_fn(|k| (p(2 * k), q(2 * k), p(2 * k + 1), q(2 * k + 1))))
+    }
+
+    /// Checks a powers-of-tau transcript over the generators `g1`, `g2`: `srs_verification_pairs` under a challenge drawn
+    /// from `rng`, then each equation as `E::multi_pairing([P, -P'], [Q, Q']).is_zero()`.  Ok(true): with probability at
+    /// least 1 - N/r the transcript is T(tau, alpha, beta) for non-zero tau, alpha, beta with one tau in both groups.
+    /// Ok(false): an equation fails.  A point the library refuses (off the curve, outside the subgroup with `validate`,
+    /// the identity, a wrong generator) is `InvalidData`.  `validate` should be `Yes` unless the points were checked
+    /// already: without it the answer means nothing on a curve whose cofactor is not 1.
+    pub fn verify_srs<R: RngCore>(
+        &self,
+        srs: &PowersOfTau<E>,
+        g1: &Affine<E::G1Config>,
+        g2: &Affine<E::G2Config>,
+        rng: &mut R,
+        validate: Validate,
+        chunk_points: u64,
+    ) -> Result<bool, SerializationError> {
+        let rho = loop {
+            let x = E::ScalarField::rand(rng);
+            if !x.is_zero() {
+                break x;
+            }
+        };
+        let eqs = self.srs_verification_pairs(srs, g1, g2, rho, validate, chunk_points)?;
+        Ok(eqs.iter().all(|(p, q, p2, q2)| E::multi_pairing([*p, -*p2], [*q, *q2]).is_zero()))
+    }
+
     /// One phase-2 contribution to the resident key (g16_setup_contribute): delta_g1, delta_g2 times `delta`, the H and L
     /// queries times delta^-1.  delta = 0 is SynthesisError::UnexpectedIdentity.
     pub fn contribute_delta(&self, delta: E::ScalarField) -> R1CSResult<()> {

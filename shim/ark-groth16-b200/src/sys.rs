@@ -171,6 +171,7 @@ extern "C" {
     pub fn g16_setup_contribute(ctx: *mut g16_ctx, delta: *const u64) -> c_int;
     pub fn g16_srs_from_secrets(ctx: *mut g16_ctx, tau: *const u64, alpha: *const u64, beta: *const u64, g1: *const u64, g2: *const u64, out: *const g16_srs_out) -> c_int;
     pub fn g16_srs_contribute(ctx: *mut g16_ctx, srs_in: *const g16_srs_desc, tau: *const u64, alpha: *const u64, beta: *const u64, flags: u32, chunk_points: u64, out: *const g16_srs_out) -> c_int;
+    pub fn g16_srs_verify_pairs(ctx: *mut g16_ctx, srs: *const g16_srs_desc, g1: *const u64, g2: *const u64, rho: *const u64, flags: u32, chunk_points: u64, pairs_g1: *mut u64, pairs_g2: *mut u64) -> c_int;
     pub fn g16_pk_load_serialized(ctx: *mut g16_ctx, bytes: *const u8, len: u64, flags: u32, rank: u32, world: u32, vk_out: *const g16_pk_export_desc) -> c_int;
     pub fn g16_pk_export_serialized(ctx: *mut g16_ctx, flags: u32, out: *mut u8, cap: u64, len_out: *mut u64) -> c_int;
     pub fn g16_prove(ctx: *mut g16_ctx, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32, proof_out: *mut u64) -> c_int;
