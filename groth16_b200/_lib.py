@@ -27,6 +27,10 @@ class PkExportDesc(C.Structure):
                                     "beta_g1", "delta_g1", "beta_g2", "gamma_g2", "delta_g2", "gamma_abc_g1")]
 
 
+class PkCheckDesc(C.Structure):
+    _fields_ = PkExportDesc._fields_
+
+
 class SrsDesc(C.Structure):
     _fields_ = [("tau_g1", u64p), ("tau_g1_len", C.c_uint64), ("tau_g2", u64p), ("tau_g2_len", C.c_uint64),
                 ("alpha_tau_g1", u64p), ("alpha_tau_g1_len", C.c_uint64), ("beta_tau_g1", u64p),
@@ -80,6 +84,8 @@ SIGNATURES = [
                                                                                           C.POINTER(SrsOut)]),
     ("g16_srs_verify_pairs", C.c_int, [C.c_void_p, C.POINTER(SrsDesc)] + [C.c_void_p] * 3 + [C.c_uint32, C.c_uint64]
      + [C.c_void_p] * 2),
+    ("g16_pk_verify_pairs", C.c_int, [C.c_void_p, C.POINTER(SrsDesc), C.POINTER(PkCheckDesc), C.c_void_p, C.c_uint32]
+     + [C.c_void_p] * 2),
     ("g16_pk_load_serialized", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
                                          C.POINTER(PkExportDesc)]),
     ("g16_pk_export_serialized", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
@@ -118,6 +124,7 @@ SER_VALIDATE = 2
 ASSIGNMENT_ON_DEVICE = 1
 SERIAL_MSMS = 2
 CHECK_WITNESS = 4
+PK_UNCONTRIBUTED = 4   # a flag of g16_pk_verify_pairs
 NONE = (1 << 64) - 1   # G16_NONE
 QAP_LIBSNARK = 0
 QAP_CIRCOM = 1

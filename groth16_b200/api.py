@@ -213,6 +213,69 @@ def srs_verify_args(srs: Srs, rho, r: int, g1_width: int, g2_width: int, chunk_p
     return arrs, rho, chunk_points
 
 
+KEY_EQUATIONS = ("delta", "h_query", "l_query", "gamma_abc_g1")
+
+
+@dataclass
+class KeyPairs:
+    """g16_pk_verify_pairs: the four pairing equations of a key check.  Equation k (members[k]) holds iff
+    e(g1[2k], g2[2k]) = e(g1[2k + 1], g2[2k + 1]); g1 is (8, G1 limbs) and g2 is (8, G2 limbs), affine Montgomery limbs."""
+    g1: np.ndarray
+    g2: np.ndarray
+    members: Tuple[str, ...] = KEY_EQUATIONS
+
+    def equation(self, k: int) -> tuple:
+        """(P_k, Q_k, P'_k, Q'_k) of equation k, as limb arrays"""
+        return self.g1[2 * k], self.g2[2 * k], self.g1[2 * k + 1], self.g2[2 * k + 1]
+
+
+KEY_VECTORS = ("a_query", "b_g1_query", "b_g2_query", "h_query", "l_query", "gamma_abc_g1")
+KEY_POINTS = ("alpha_g1", "beta_g1", "delta_g1", "beta_g2", "gamma_g2", "delta_g2")
+
+
+def key_members(pk: ProvingKey) -> dict:
+    """the members of g16_pk_check_desc, by name, as `pk` holds them (None where it has none)"""
+    vk = pk.vk
+    return dict(a_query=pk.a_query, b_g1_query=pk.b_g1_query, b_g2_query=pk.b_g2_query, h_query=pk.h_query,
+                l_query=pk.l_query, gamma_abc_g1=vk.gamma_abc_g1, alpha_g1=vk.alpha_g1, beta_g1=pk.beta_g1,
+                delta_g1=pk.delta_g1, beta_g2=vk.beta_g2, gamma_g2=vk.gamma_g2, delta_g2=vk.delta_g2)
+
+
+def pk_verify_args(pk: ProvingKey, srs: Srs, rho, r: int, g1_width: int, g2_width: int, num_inputs: int, num_witness: int,
+                   log_n: int, qap: str = "libsnark") -> tuple:
+    """The arguments of Groth16.key_verification_pairs as the library takes them: (the key's members as (points, limbs)
+    arrays, the transcript's as srs_arrays gives them, rho mod r).  ValueError, before any device work: a key member missing
+    or not of exactly the length g16_pk_export writes for the circuit (num_inputs + num_witness points in a_query,
+    b_g1_query, b_g2_query; n - 1 in h_query, n under qap="circom"; num_witness in l_query; num_inputs in gamma_abc_g1;
+    one point each for the others), a transcript member that is not made of whole points or is shorter than the circuit
+    needs (tau_g1 2n - 1 points, the other vectors n), rho = 0 mod r."""
+    n = 1 << log_n
+    nv = num_inputs + num_witness
+    want = dict(a_query=nv, b_g1_query=nv, b_g2_query=nv, h_query=n if qap == "circom" else n - 1, l_query=num_witness,
+                gamma_abc_g1=num_inputs)
+    keys = {}
+    for k, v in key_members(pk).items():
+        w = g2_width if k in ("b_g2_query", "beta_g2", "gamma_g2", "delta_g2") else g1_width
+        if v is None:
+            raise ValueError(f"the key has no {k}")
+        a = np.ascontiguousarray(v, dtype=np.uint64)
+        if a.size % w or (a.ndim == 2 and a.shape[1] != w) or a.ndim > 2:
+            raise ValueError(f"{k} of shape {a.shape} is not made of points of {w} limbs")
+        a = a.reshape(-1, w)
+        need = want.get(k, 1)
+        if a.shape[0] != need:
+            raise ValueError(f"{k} holds {a.shape[0]} points, the circuit's key has {need}")
+        keys[k] = a
+    arrs = srs_arrays(srs, g1_width, g2_width)
+    for k, need in zip(SRS_VECTORS, (2 * n - 1, n, n, n)):
+        if arrs[k].shape[0] < need:
+            raise ValueError(f"srs.{k} holds {arrs[k].shape[0]} points, the circuit (domain 2^{log_n}) needs at least {need}")
+    rho = int(rho) % r
+    if rho == 0:
+        raise ValueError("the challenge rho must be non-zero mod r")
+    return keys, arrs, rho
+
+
 @dataclass
 class WitnessReport:
     """g16_witness_report of one assignment, None where the library reports G16_NONE"""
@@ -516,6 +579,40 @@ class Groth16:
         _check(self._lib.g16_srs_verify_pairs(self._ctx, C.byref(d), _ptr(g1), _ptr(g2), _ptr(r_),
                                               _lib.SER_VALIDATE if validate else 0, chunk_points, _ptr(out1), _ptr(out2)))
         return SrsPairs(out1, out2)
+
+    def key_verification_pairs(self, pk: ProvingKey, srs: Srs, rho, validate: bool = True,
+                               uncontributed: bool = False) -> KeyPairs:
+        """g16_pk_verify_pairs: the GPU part of checking that `pk` is the key of the resident circuit (under this instance's
+        reduction) made from the transcript `srs`: g16_setup(alpha, beta, gamma, delta, tau) for the transcript's tau,
+        alpha, beta.  rho (a Python int, non-zero mod r) is the challenge: draw it after the key and transcript are fixed.
+
+        The library checks every point (canonical, on the curve, and with `validate` in the prime-order subgroup), that
+        alpha_g1, beta_g1 and beta_g2 are the transcript's, that delta and gamma are not the identity, that gamma_g2 !=
+        delta_g2 (`uncontributed` accepts gamma = delta, the key generate_parameters_from_srs makes before any
+        contribution), and that the a_query, b_g1_query and b_g2_query combinations match the transcript's; a refusal raises
+        serialize.DeserializeError naming the member.  It returns four equations (KeyPairs): with (P, Q, P', Q') =
+        pairs.equation(k), the caller evaluates e(P, Q) = e(P', Q') with its own pairing.  The key is accepted iff all four
+        hold; then, with probability at least 1 - 6 max(nv, n) / r over rho, it is that setup point for point.  Needs a
+        resident circuit, no key, and leaves the resident key alone."""
+        m = self._matrices
+        if m is None:
+            raise ValueError("load_matrices must come first")
+        keys, arrs, rho = pk_verify_args(pk, srs, rho, self.curve.r, 2 * self.nq, self.ng2, m.num_instance_variables,
+                                         m.num_witness_variables, self._lib.g16_domain_log(self._ctx), self.qap)
+        d = _lib.PkCheckDesc()
+        for k, v in keys.items():
+            setattr(d, k, _u64p(v) if v.size else None)
+        s = _lib.SrsDesc()
+        for k in SRS_VECTORS:
+            setattr(s, k, _u64p(arrs[k]))
+            setattr(s, k + "_len", arrs[k].shape[0])
+        s.beta_g2 = _u64p(arrs["beta_g2"])
+        out1 = np.zeros((8, 2 * self.nq), dtype=np.uint64)
+        out2 = np.zeros((8, self.ng2), dtype=np.uint64)
+        r_ = np.ascontiguousarray(self.codec.fr.enc1(rho))
+        flags = (_lib.SER_VALIDATE if validate else 0) | (_lib.PK_UNCONTRIBUTED if uncontributed else 0)
+        _check(self._lib.g16_pk_verify_pairs(self._ctx, C.byref(s), C.byref(d), _ptr(r_), flags, _ptr(out1), _ptr(out2)))
+        return KeyPairs(out1, out2)
 
     def _after_key_change(self, rc: int):
         """Status of g16_setup_from_srs / g16_setup_contribute: argument errors (G16_ERR_BAD_ARGUMENT,

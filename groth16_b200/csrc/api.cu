@@ -168,6 +168,11 @@ int g16_srs_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const uint64_t* 
   CTX_OR_FAIL(ctx);
   return ctx->eng->srs_verify_pairs(srs, g1, g2, rho, flags, chunk_points, pairs_g1, pairs_g2);
 }
+int g16_pk_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const g16_pk_check_desc* pk, const uint64_t* rho, uint32_t flags,
+                        uint64_t* pairs_g1, uint64_t* pairs_g2) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->pk_verify_pairs(srs, pk, rho, flags, pairs_g1, pairs_g2);
+}
 int g16_pk_load_serialized(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                            const g16_pk_export_desc* vk_out) {
   CTX_OR_FAIL(ctx);

@@ -152,6 +152,8 @@ struct IEngine {
                              uint32_t flags, uint64_t chunk_points, const g16_srs_out* out) = 0;
   virtual int srs_verify_pairs(const g16_srs_desc* srs, const uint64_t* g1, const uint64_t* g2, const uint64_t* rho,
                                uint32_t flags, uint64_t chunk_points, uint64_t* pairs_g1, uint64_t* pairs_g2) = 0;
+  virtual int pk_verify_pairs(const g16_srs_desc* srs, const g16_pk_check_desc* pk, const uint64_t* rho, uint32_t flags,
+                              uint64_t* pairs_g1, uint64_t* pairs_g2) = 0;
   virtual int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                                  const g16_pk_export_desc* vk_out) = 0;
   virtual int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) = 0;
@@ -1512,17 +1514,33 @@ struct Engine : IEngine {
                                               srs_reason(first_err & 0xff));
       // scalars rho^(i0 + j), then the chunk's MSM
       G16_CUDA(srs_powers<Fr>(st, dtab, srs_power(Fr::one(), tab, i0), cnt, dsc.template as<Fr>()));
-      G16_CUDA(msm_prepare_query<F>(st, buf.template as<Affine<F>>(), cnt, 1, 0, dmask.template as<uint8_t>()));
-      const MsmGeom g = srs_verify_geom(cnt, g2);
-      G16_CUDA((msm_enqueue<F, Fr>(st, ws, g, buf.template as<Affine<F>>(), dmask.template as<uint8_t>(), dsc.template as<uint32_t>(),
-                                   1, true, &mc, nullptr, nullptr, nullptr, nullptr, nullptr, 0)));
-      G16_CUDA(cudaStreamSynchronize(st));
-      sum.add(msm_finish<F>(ws, g));
-      tm.launches += 2;
-      tm.d2h_bytes += 4 + ws.plan.leaf_pts * g.sets() * sizeof(XYZZ<F>);   // msm_enqueue's slot total and leaf arrays
+      tm.launches++;
+      int rc = msm_device<F>(ws, mc, g2, buf.template as<Affine<F>>(), dsc.template as<Fr>(), cnt, dmask.template as<uint8_t>(), sum);
+      if (rc) return rc;
       i0 += cnt;
     }
     tm.launches += mc.launches;
+    return G16_OK;
+  }
+  // acc += sum_{i<cnt} s_i P_i over device bases and device Montgomery scalars, on the main stream through a workspace the
+  // calling entry point owns (the prover's keep their sizes): the identity mask into dmask (cnt bytes), then the prover's
+  // MSM pipeline, in pieces of at most SRS_VERIFY_MSM_MAX pairs; the host waits for each.  Counts the mask launches and the
+  // bytes msm_enqueue copies back in tm, the pipeline's launches in mc.
+  template <class F>
+  int msm_device(MsmWorkspace<F>& ws, MsmCounters& mc, bool g2, Affine<F>* bases, const Fr* sc, uint64_t cnt, uint8_t* dmask,
+                 XYZZ<F>& acc) {
+    cudaStream_t st = S0.st_main;
+    for (uint64_t i0 = 0; i0 < cnt; i0 += SRS_VERIFY_MSM_MAX) {
+      const uint32_t c = (uint32_t)std::min<uint64_t>(SRS_VERIFY_MSM_MAX, cnt - i0);
+      G16_CUDA(msm_prepare_query<F>(st, bases + i0, c, 1, 0, dmask));
+      const MsmGeom g = srs_verify_geom(c, g2);
+      G16_CUDA((msm_enqueue<F, Fr>(st, ws, g, bases + i0, dmask, reinterpret_cast<const uint32_t*>(sc + i0), 1, true, &mc, nullptr,
+                                   nullptr, nullptr, nullptr, nullptr, 0)));
+      G16_CUDA(cudaStreamSynchronize(st));
+      acc.add(msm_finish<F>(ws, g));
+      tm.launches++;
+      tm.d2h_bytes += 4 + ws.plan.leaf_pts * g.sets() * sizeof(XYZZ<F>);   // msm_enqueue's slot total and leaf arrays
+    }
     return G16_OK;
   }
   // g16_srs_verify_pairs: the five pairing equations of a powers-of-tau transcript under the challenge rho, after every
@@ -1643,6 +1661,200 @@ struct Engine : IEngine {
   }
   // u64 limbs of one point of transcript member m
   static uint64_t srs_point_limbs(int m) { return (m == SRS_TAU_G2 || m == SRS_BETA_G2) ? (uint64_t)G2_64 : (uint64_t)(2 * NQ64); }
+
+  // ---- checking a proving key against the resident circuit and a transcript (g16_pk_verify_pairs) ----
+  // Members of the key in the order their points are checked; the error word names transcript member m as PKV_SRS + m, so
+  // that the first bad point is the key's before the transcript's.
+  enum { PKV_A = 0, PKV_B1, PKV_B2, PKV_H, PKV_L, PKV_ABC, PKV_ALPHA, PKV_BETA, PKV_DELTA1, PKV_BETA2, PKV_GAMMA2, PKV_DELTA2,
+         PKV_MEMBERS, PKV_SRS = 16 };
+  static const char* pkv_member(int m) {
+    static const char* t[PKV_MEMBERS] = {"a_query", "b_g1_query", "b_g2_query", "h_query",  "l_query",  "gamma_abc_g1",
+                                         "alpha_g1", "beta_g1",   "delta_g1",   "beta_g2", "gamma_g2", "delta_g2"};
+    return m >= PKV_SRS ? srs_member(m - PKV_SRS) : t[m];
+  }
+  static bool pkv_g2(int m) { return m == PKV_B2 || m == PKV_BETA2 || m == PKV_GAMMA2 || m == PKV_DELTA2; }
+  // g16_pk_verify_pairs.  With z_j = rho^j (j < nv), z^I = z on the instance variables and 0 elsewhere, z^L = z - z^I, the
+  // combination sum_j rho^j K_j of each key member equals one MSM per transcript member over the transcript-side weights,
+  // which are field transforms of z (DESIGN.md section 16):
+  //   a_query, b_g1_query, b_g2_query  tau_g1 / tau_g2 [0, n) by the inverse transforms a^, b^ of A z, B z (instance rows
+  //                                    included, as the witness map forms them)
+  //   l_query (x delta), gamma_abc_g1 (x gamma)  beta_tau_g1 by a^, alpha_tau_g1 by b^, tau_g1 by c^, of z^L and z^I
+  //   h_query (x delta)                 tau_g1 [0, 2n - 1) by srs_h_weights
+  // On the device: rho^j, one matvec of the three assignments z^I, z^L, z, one batch of nine inverse transforms, the H
+  // weights, and fifteen MSMs (more past SRS_VERIFY_MSM_MAX pairs).  The host compares the A and B sums and writes the
+  // four equations.  Nothing is written until every check passed.
+  // Timings (host clock around work that ends in a stream synchronise): h2d_ms = upload and point checks, witness_map_ms
+  // = the field work, msm_ms[0] / msm_ms[1] = the key-side / transcript-side MSMs, total_ms = the whole call.
+  int pk_verify_pairs(const g16_srs_desc* srs, const g16_pk_check_desc* pk, const uint64_t* rho_, uint32_t flags,
+                      uint64_t* pairs_g1, uint64_t* pairs_g2) override {
+    if (!srs || !pk || !rho_ || !pairs_g1 || !pairs_g2) return fail(G16_ERR_BAD_ARGUMENT, "null argument");
+    if (flags & ~(uint32_t)(G16_SER_VALIDATE | G16_PK_UNCONTRIBUTED))
+      return fail(G16_ERR_BAD_ARGUMENT, "g16_pk_verify_pairs takes G16_SER_VALIDATE and G16_PK_UNCONTRIBUTED only");
+    const Fr rho = load_fr(rho_);
+    if (rho.is_zero()) return fail(G16_ERR_BAD_ARGUMENT, "the challenge rho must be non-zero");
+    if (!have_circuit) return fail(G16_ERR_BAD_ARGUMENT, "g16_circuit_load must precede g16_pk_verify_pairs");
+    const uint64_t n = 1ull << L, nv = nvars(), hn = h_query_len(), ni = num_inputs, nw = num_witness;
+    const uint32_t nc = num_constraints;
+    const uint64_t* kp[PKV_MEMBERS] = {pk->a_query, pk->b_g1_query, pk->b_g2_query, pk->h_query, pk->l_query, pk->gamma_abc_g1,
+                                       pk->alpha_g1, pk->beta_g1,    pk->delta_g1,   pk->beta_g2, pk->gamma_g2, pk->delta_g2};
+    const uint64_t klen[PKV_MEMBERS] = {nv, nv, nv, hn, nw, ni, 1, 1, 1, 1, 1, 1};
+    for (int m = 0; m < PKV_MEMBERS; m++)
+      if (!kp[m] && klen[m]) return fail(G16_ERR_BAD_ARGUMENT, std::string("null pk member ") + pkv_member(m));
+    const uint64_t* sp[SRS_MEMBERS] = {srs->tau_g1, srs->tau_g2, srs->alpha_tau_g1, srs->beta_tau_g1, srs->beta_g2};
+    const uint64_t have[SRS_MEMBERS] = {srs->tau_g1_len, srs->tau_g2_len, srs->alpha_tau_g1_len, srs->beta_tau_g1_len, 1};
+    const uint64_t need[SRS_MEMBERS] = {2 * n - 1, n, n, n, 1};   // the prefixes g16_setup_from_srs reads
+    for (int m = 0; m < SRS_MEMBERS; m++) {
+      if (!sp[m]) return fail(G16_ERR_BAD_ARGUMENT, std::string("null srs member ") + srs_member(m));
+      if (have[m] < need[m])
+        return fail(G16_ERR_BAD_ARGUMENT, std::string(srs_member(m)) + " holds " + std::to_string(have[m]) +
+                                              " points, the circuit (domain 2^" + std::to_string(L) + ") needs at least " +
+                                              std::to_string(need[m]));
+    }
+    G16_NOT_BUSY();
+    G16_CUDA(cudaSetDevice(device));
+    int rc = ensure_circuit_domain();   // dom: the circuit's twiddles and n^-1
+    if (rc) return rc;
+    const auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point a) {
+      return (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count();
+    };
+    tm = g16_timings{};
+    cudaStream_t st = S0.st_main;
+    // --- upload and check every key member and transcript prefix; one error word ---
+    DevBuf kd[PKV_MEMBERS], sd[SRS_MEMBERS], err;
+    G16_CUDA(err.reserve(8));
+    G16_CUDA(cudaMemsetAsync(err.p, 0xff, 8, st));
+    unsigned long long* e = err.template as<unsigned long long>();
+    auto upload = [&](DevBuf& d, const uint64_t* p, uint64_t cnt, bool g2, uint32_t member) -> cudaError_t {
+      const size_t bytes = cnt * (g2 ? sizeof(A2) : sizeof(A1));
+      cudaError_t x = d.reserve(bytes + sizeof(A2));
+      if (x != cudaSuccess || !cnt) return x;
+      if ((x = cudaMemcpyAsync(d.p, p, bytes, cudaMemcpyHostToDevice, st)) != cudaSuccess) return x;
+      tm.h2d_bytes += bytes;
+      tm.launches++;
+      const uint32_t fl = flags & G16_SER_VALIDATE;
+      return g2 ? srs_check<CP, true>(st, d.p, (uint32_t)cnt, fl, member, e) : srs_check<CP, false>(st, d.p, (uint32_t)cnt, fl, member, e);
+    };
+    for (int m = 0; m < PKV_MEMBERS; m++) G16_CUDA(upload(kd[m], kp[m], klen[m], pkv_g2(m), m));
+    for (int m = 0; m < SRS_MEMBERS; m++)
+      G16_CUDA(upload(sd[m], sp[m], need[m], m == SRS_TAU_G2 || m == SRS_BETA_G2, PKV_SRS + m));
+    unsigned long long first_err = 0;
+    G16_CUDA(cudaMemcpyAsync(&first_err, err.p, 8, cudaMemcpyDeviceToHost, st));
+    G16_CUDA(cudaStreamSynchronize(st));
+    tm.d2h_bytes += 8;
+    if (first_err != ~0ull)
+      return fail(G16_ERR_INVALID_DATA, std::string(pkv_member((int)(first_err >> 48))) + "[" +
+                                            std::to_string((first_err >> 8) & ((1ull << 40) - 1)) + "]: " + ser_reason(first_err & 0xff));
+    tm.h2d_ms = ms_since(t0);
+    // --- the checks that need no MSM: affine limbs are canonical here, so equal points have equal limbs ---
+    auto same = [](const uint64_t* a, const uint64_t* b, size_t bytes) { return memcmp(a, b, bytes) == 0; };
+    auto is_inf = [](const uint64_t* a, size_t bytes) { return std::all_of(a, a + bytes / 8, [](uint64_t x) { return x == 0; }); };
+    if (is_inf(sp[SRS_TAU_G1], sizeof(A1))) return fail(G16_ERR_INVALID_DATA, "tau_g1[0]: point is the identity");
+    if (is_inf(sp[SRS_TAU_G2], sizeof(A2))) return fail(G16_ERR_INVALID_DATA, "tau_g2[0]: point is the identity");
+    if (!same(kp[PKV_ALPHA], sp[SRS_ALPHA], sizeof(A1)))
+      return fail(G16_ERR_INVALID_DATA, "alpha_g1: not alpha_tau_g1[0] of the transcript");
+    if (!same(kp[PKV_BETA], sp[SRS_BETA], sizeof(A1))) return fail(G16_ERR_INVALID_DATA, "beta_g1: not beta_tau_g1[0] of the transcript");
+    if (!same(kp[PKV_BETA2], sp[SRS_BETA_G2], sizeof(A2))) return fail(G16_ERR_INVALID_DATA, "beta_g2: not beta_g2 of the transcript");
+    for (int m : {PKV_DELTA1, PKV_DELTA2, PKV_GAMMA2})
+      if (is_inf(kp[m], pkv_g2(m) ? sizeof(A2) : sizeof(A1))) return fail(G16_ERR_INVALID_DATA, std::string(pkv_member(m)) + ": point is the identity");
+    if (!(flags & G16_PK_UNCONTRIBUTED) && same(kp[PKV_GAMMA2], kp[PKV_DELTA2], sizeof(A2)))
+      return fail(G16_ERR_INVALID_DATA, "gamma_g2 equals delta_g2: anyone can forge proofs under this key (G16_PK_UNCONTRIBUTED "
+                                        "accepts the uncontributed key of a ceremony)");
+    // --- field work: P = rho^j (j < max(nv, n)); Z = [z^I | z^L | z]; X = A, B, C times the three (9 vectors of n); T = their
+    // inverse transforms (a^I, a^L, a^, b^I, b^L, b^, c^I, c^L, c^); H = the H weights ---
+    auto t1 = std::chrono::steady_clock::now();
+    const unsigned long long nl0 = ntt_launches;
+    const bool circom = qap == G16_QAP_CIRCOM;
+    const uint64_t np = std::max(nv, n), nh = 2 * n - 1;
+    Fr tab[64];   // rho^(2^k), then omega_2n^-(2^k)
+    tab[0] = rho;
+    tab[32] = Fr::inv(fr_domain_root<Fr>(L + 1));
+    for (int k = 1; k < 32; k++) { tab[k] = Fr::sqr(tab[k - 1]); tab[32 + k] = Fr::sqr(tab[31 + k]); }
+    DevBuf dtab, dpow, dz, dx, dt, dh, df;
+    G16_CUDA(dtab.reserve(sizeof(tab)));
+    G16_CUDA(dpow.reserve(np * sizeof(Fr)));
+    G16_CUDA(dz.reserve(3 * nv * sizeof(Fr)));
+    G16_CUDA(dx.reserve(9 * n * sizeof(Fr)));
+    G16_CUDA(dt.reserve(9 * n * sizeof(Fr)));
+    G16_CUDA(dh.reserve(2 * n * sizeof(Fr)));
+    G16_CUDA(cudaMemcpyAsync(dtab.p, tab, sizeof(tab), cudaMemcpyHostToDevice, st));
+    tm.h2d_bytes += sizeof(tab);
+    const Fr* dtab_rho = dtab.template as<Fr>();
+    Fr *P = dpow.template as<Fr>(), *Z = dz.template as<Fr>(), *X = dx.template as<Fr>(), *T = dt.template as<Fr>();
+    Fr* H = dh.template as<Fr>();
+    G16_CUDA(srs_powers<Fr>(st, dtab_rho, Fr::one(), (uint32_t)np, P));
+    G16_CUDA(cudaMemsetAsync(Z, 0, 2 * nv * sizeof(Fr), st));
+    G16_CUDA(cudaMemcpyAsync(Z, P, ni * sizeof(Fr), cudaMemcpyDeviceToDevice, st));
+    if (nw) G16_CUDA(cudaMemcpyAsync(Z + nv + ni, P + ni, nw * sizeof(Fr), cudaMemcpyDeviceToDevice, st));
+    G16_CUDA(cudaMemcpyAsync(Z + 2 * nv, P, nv * sizeof(Fr), cudaMemcpyDeviceToDevice, st));
+    CsrDev cs[3];
+    csr_dev(cs);
+    r1cs_matvec<Fr>(st, cs, Z, nc, (uint32_t)ni, (uint32_t)n, X, X + 3 * n, X + 6 * n, 3, (uint32_t)nv, true);
+    const Fr zero = Fr::zero();
+    ntt_any(st, dom, true, X, X, T, NTT_LOAD_PLAIN, nullptr, nullptr, nullptr, zero, NTT_STORE_MUL_CONST, nullptr, dom.n_inv, 9);
+    if (!circom) {
+      G16_CUDA(srs_h_weights<Fr>(st, dtab_rho, Fr::one(), nullptr, (uint32_t)n, (uint32_t)nh, H));
+    } else {   // F = the unscaled inverse transform of rho^i (i < n) into df + n, df as the work buffer
+      G16_CUDA(df.reserve(2 * n * sizeof(Fr)));
+      Fr* F = df.template as<Fr>();
+      ntt_any(st, dom, true, P, F, F + n, NTT_LOAD_PLAIN, nullptr, nullptr, nullptr, zero, NTT_STORE_PLAIN, nullptr, zero);
+      G16_CUDA(srs_h_weights<Fr>(st, dtab_rho + 32, Fr::inv(fr_from_u64<Fr>(2 * n)), F + n, (uint32_t)n, (uint32_t)nh, H));
+    }
+    G16_CUDA(cudaGetLastError());
+    G16_CUDA(cudaStreamSynchronize(st));
+    dx.release();
+    df.release();
+    tm.launches += 3 + (ntt_launches - nl0);   // powers, matvec, H weights, the transforms
+    tm.witness_map_ms = ms_since(t1);
+    // --- MSMs: the key's sums under rho^j, then the transcript's under the weights ---
+    t1 = std::chrono::steady_clock::now();
+    MsmWorkspace<Fq> ws1;
+    MsmWorkspace<Fq2> ws2;
+    MsmCounters mc;
+    DevBuf dmask;
+    G16_CUDA(dmask.reserve(std::max(nv, 2 * n)));
+    uint8_t* mk = dmask.template as<uint8_t>();
+    auto g1sum = [&](DevBuf& b, const Fr* sc, uint64_t cnt, P1& acc) { return msm_device<Fq>(ws1, mc, false, b.template as<A1>(), sc, cnt, mk, acc); };
+    auto g2sum = [&](DevBuf& b, const Fr* sc, uint64_t cnt, P2& acc) { return msm_device<Fq2>(ws2, mc, true, b.template as<A2>(), sc, cnt, mk, acc); };
+    P1 kA = P1::inf(), kB1 = P1::inf(), kH = P1::inf(), kL = P1::inf(), kIC = P1::inf();
+    P2 kB2 = P2::inf();
+    if ((rc = g1sum(kd[PKV_A], P, nv, kA)) || (rc = g1sum(kd[PKV_B1], P, nv, kB1)) || (rc = g2sum(kd[PKV_B2], P, nv, kB2)) ||
+        (rc = g1sum(kd[PKV_H], P, hn, kH)) || (rc = g1sum(kd[PKV_L], P + ni, nw, kL)) || (rc = g1sum(kd[PKV_ABC], P, ni, kIC)))
+      return rc;
+    tm.msm_ms[0] = ms_since(t1);
+    tm.msm_pairs[0] = 3 * nv + hn + nw + ni;
+    t1 = std::chrono::steady_clock::now();
+    P1 tA = P1::inf(), tB1 = P1::inf(), tH = P1::inf(), tL = P1::inf(), tIC = P1::inf();
+    P2 tB2 = P2::inf();
+    DevBuf &t1d = sd[SRS_TAU_G1], &ad = sd[SRS_ALPHA], &bd = sd[SRS_BETA];
+    if ((rc = g1sum(t1d, T + 2 * n, n, tA)) || (rc = g1sum(t1d, T + 5 * n, n, tB1)) || (rc = g2sum(sd[SRS_TAU_G2], T + 5 * n, n, tB2)) ||
+        (rc = g1sum(bd, T + n, n, tL)) || (rc = g1sum(ad, T + 4 * n, n, tL)) || (rc = g1sum(t1d, T + 7 * n, n, tL)) ||
+        (rc = g1sum(bd, T, n, tIC)) || (rc = g1sum(ad, T + 3 * n, n, tIC)) || (rc = g1sum(t1d, T + 6 * n, n, tIC)) ||
+        (rc = g1sum(t1d, H, nh, tH)))
+      return rc;
+    tm.msm_ms[1] = ms_since(t1);
+    tm.msm_pairs[1] = 9 * n + nh;
+    tm.launches += mc.launches;
+    // --- the sums the call decides itself ---
+    const A1 sA[2] = {kA.to_affine(), tA.to_affine()}, sB1[2] = {kB1.to_affine(), tB1.to_affine()};
+    const A2 sB2[2] = {kB2.to_affine(), tB2.to_affine()};
+    const char* bad = memcmp(&sA[0], &sA[1], sizeof(A1))     ? "a_query"
+                      : memcmp(&sB1[0], &sB1[1], sizeof(A1)) ? "b_g1_query"
+                      : memcmp(&sB2[0], &sB2[1], sizeof(A2)) ? "b_g2_query"
+                                                             : nullptr;
+    if (bad) return fail(G16_ERR_INVALID_DATA, std::string(bad) + ": not the key of the resident circuit under this transcript");
+    // equation k: e(P_k, Q_k) = e(P'_k, Q'_k), written as P_0, P'_0, .., P_3, P'_3 and Q_0, Q'_0, .., Q_3, Q'_3
+    const A1 g1 = load_a1(sp[SRS_TAU_G1]), d1 = load_a1(kp[PKV_DELTA1]);
+    const A2 g2 = load_a2(sp[SRS_TAU_G2]), d2 = load_a2(kp[PKV_DELTA2]), gm2 = load_a2(kp[PKV_GAMMA2]);
+    const A1 ps[8] = {d1, g1, kH.to_affine(), tH.to_affine(), kL.to_affine(), tL.to_affine(), kIC.to_affine(), tIC.to_affine()};
+    const A2 qs[8] = {g2, d2, d2, g2, d2, g2, gm2, g2};
+    for (int i = 0; i < 8; i++) {
+      store_a1(pairs_g1 + (size_t)i * 2 * NQ64, ps[i]);
+      store_a2(pairs_g2 + (size_t)i * G2_64, qs[i]);
+    }
+    tm.total_ms = ms_since(t0);
+    return G16_OK;
+  }
   // CircomReduction::h_query_scalars(n - 1, tau, _, delta^-1): the odd entries 1, 3, .., 2n - 1 of the size-2n ifft of
   // v[i] = delta^-1 tau^i (i < 2n - 1), v[2n - 1] = 0.  With w = omega_2n, k = 2j + 1 and the geometric sum in closed form:
   //   out[j] = delta^-1 / (2n) * [ (tau^2n - 1) / (tau w^-k - 1) - tau^(2n-1) w^k ]

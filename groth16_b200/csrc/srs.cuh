@@ -1,7 +1,8 @@
 // srs.cuh -- proving keys from a powers-of-tau transcript (g16_setup_from_srs) and phase-2 delta contributions
 // (g16_setup_contribute): the group-valued inverse FFT, sparse sums of points, one scalar times many points, and the
 // transcript point checks; phase-1 contributions to a transcript (g16_srs_contribute): every point times its own power
-// of the secret; and the scalars of the transcript check (g16_srs_verify_pairs): one power of the challenge per point.
+// of the secret; the scalars of the transcript check (g16_srs_verify_pairs): one power of the challenge per point; and the
+// H-query weights of the key check (g16_pk_verify_pairs).
 //
 // Every kernel works on XYZZ points in global memory, one point (or one butterfly, or one chunk of a sum) per thread.  The
 // scalar multiplications are left-to-right double-and-add over the canonical scalar (XYZZ::mul_u32); a windowed form would
@@ -195,6 +196,22 @@ __global__ void __launch_bounds__(128) srs_powers_kernel(const FrF* tab, FrF c, 
   const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j < cnt) out[j] = srs_power(c, tab, j);
 }
+// The weights on tau_g1[0 .. 2n - 1) of the H-query check (g16_pk_verify_pairs), Montgomery form, k < cnt:
+//   f == nullptr (LibsnarkReduction, tab = rho^(2^b), c = 1): out[k] = -rho^k (k < n - 1), 0 (k = n - 1), rho^(k-n) (k >= n)
+//   otherwise    (CircomReduction, tab = w^(2^b) with w = omega_2n^-1, c = (2n)^-1): out[k] = c w^k f[k mod n]
+template <class FrF>
+__global__ void __launch_bounds__(128) srs_h_weights_kernel(const FrF* tab, FrF c, const FrF* f, uint32_t n, uint32_t cnt,
+                                                            FrF* out) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= cnt) return;
+  if (f) {
+    out[k] = FrF::mul(srs_power(c, tab, k), f[k & (n - 1)]);
+  } else if (k + 1 < n) {
+    out[k] = FrF::neg(srs_power(c, tab, k));
+  } else {
+    out[k] = k + 1 == n ? FrF::zero() : srs_power(c, tab, k - n);
+  }
+}
 // in-place bit-reversal permutation of 2^log_n points
 template <class F>
 __global__ void __launch_bounds__(128) srs_bitrev_kernel(XYZZ<F>* p, uint32_t n, int log_n) {
@@ -290,6 +307,11 @@ cudaError_t srs_powers(cudaStream_t st, const FrF* tab, FrF c, uint32_t cnt, FrF
   if (cnt) srs_powers_kernel<FrF><<<srs_blocks(cnt), 128, 0, st>>>(tab, c, cnt, out);
   return cudaGetLastError();
 }
+template <class FrF>
+cudaError_t srs_h_weights(cudaStream_t st, const FrF* tab, FrF c, const FrF* f, uint32_t n, uint32_t cnt, FrF* out) {
+  if (cnt) srs_h_weights_kernel<FrF><<<srs_blocks(cnt), 128, 0, st>>>(tab, c, f, n, cnt, out);
+  return cudaGetLastError();
+}
 // the unscaled inverse transform of 2^log_n points in place: out[j] = sum_i omega^(-ij) in[i]
 template <class F, class FrF>
 cudaError_t srs_ifft(cudaStream_t st, XYZZ<F>* p, int log_n, const FrF* tw_inv, unsigned long long* launches) {
@@ -335,6 +357,8 @@ cudaError_t srs_sum(cudaStream_t st, const XYZZ<F>* src, const uint32_t* d_idx, 
   X cudaError_t srs_check<CP, false>(cudaStream_t, const void*, uint32_t, uint32_t, uint32_t, unsigned long long*);  \
   X cudaError_t srs_check<CP, true>(cudaStream_t, const void*, uint32_t, uint32_t, uint32_t, unsigned long long*);   \
   X cudaError_t srs_powers<Fp<CP::FrP>>(cudaStream_t, const Fp<CP::FrP>*, Fp<CP::FrP>, uint32_t, Fp<CP::FrP>*);     \
+  X cudaError_t srs_h_weights<Fp<CP::FrP>>(cudaStream_t, const Fp<CP::FrP>*, Fp<CP::FrP>, const Fp<CP::FrP>*,       \
+                                           uint32_t, uint32_t, Fp<CP::FrP>*);                                       \
   G16_SRS_POINT_TEMPLATES(X, Fp<CP::FqP>, Fp<CP::FrP>)
 #endif
 

@@ -263,6 +263,63 @@ int g16_srs_contribute(g16_ctx* ctx, const g16_srs_desc* in, const uint64_t* tau
  * d2h_bytes = bytes copied each way, launches = kernels. */
 int g16_srs_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const uint64_t* g1, const uint64_t* g2, const uint64_t* rho,
                          uint32_t flags, uint64_t chunk_points, uint64_t* pairs_g1, uint64_t* pairs_g2);
+/* Phase 2 of the ceremony, the user's side (snarkjs `zkey verify`, without the contributions' proofs of knowledge): the GPU
+ * part of checking that `pk`, a proving key received from elsewhere, is the key of the resident circuit (under its
+ * reduction) made from the transcript `srs`, i.e. g16_setup(alpha, beta, gamma, delta, tau) for the transcript's tau, alpha,
+ * beta and some gamma, delta.  pk holds the members of g16_pk_export_desc, read-only, with the lengths g16_pk_export writes:
+ * a_query, b_g1_query, b_g2_query num_inputs + num_witness points, h_query n - 1 (G16_QAP_CIRCOM: n), l_query num_witness,
+ * gamma_abc_g1 num_inputs, the six single points one each (a member of no points may be null).  Transcript members may be
+ * longer than the circuit needs; only the prefixes g16_setup_from_srs reads are read (tau_g1 2n - 1 points, tau_g2,
+ * alpha_tau_g1, beta_tau_g1 n each, beta_g2).  rho (Montgomery Fr, non-zero) is a challenge the caller draws after the key
+ * and transcript are fixed.
+ * With z_j = rho^j (j < nv = num_inputs + num_witness) and g1 = tau_g1[0], g2 = tau_g2[0], the call forms
+ *   S_X(K) = sum_j rho^j X_j over a key member X (for l_query: sum_t rho^(num_inputs + t) l_query[t])
+ * and the same combination of the transcript, S_X(T), from field transforms of z as DESIGN.md section 16 gives (one MSM per
+ * transcript member; no group transform).  It decides itself, and refuses the key with G16_ERR_INVALID_DATA naming the
+ * member if one fails, in this order: tau_g1[0] and tau_g2[0] are not the identity; alpha_g1 = alpha_tau_g1[0], beta_g1 =
+ * beta_tau_g1[0], beta_g2 = the transcript's beta_g2 ("alpha_g1: not alpha_tau_g1[0] of the transcript"); delta_g1, delta_g2
+ * and gamma_g2 are not the identity; gamma_g2 != delta_g2 ("gamma_g2 equals delta_g2: ...": gamma = delta lets anyone forge
+ * proofs for any public input, and an uncontributed g16_setup_from_srs key has gamma = delta = 1 -- flag
+ * G16_PK_UNCONTRIBUTED accepts it, for the coordinator of a ceremony); S_X(K) = S_X(T) for a_query, b_g1_query and
+ * b_g2_query ("b_g2_query: not the key of the resident circuit under this transcript").  Then it writes eight affine G1 points
+ * P_0, P'_0, .., P_3, P'_3 to pairs_g1 and eight affine G2 points Q_0, Q'_0, .., Q_3, Q'_3 to pairs_g2; equation k holds iff
+ * e(P_k, Q_k) = e(P'_k, Q'_k):
+ *   k = 0  delta         (delta_g1, g2)          = (g1, delta_g2)
+ *   k = 1  h_query       (S_H(K), delta_g2)      = (S_H(T), g2)
+ *   k = 2  l_query       (S_L(K), delta_g2)      = (S_L(T), g2)
+ *   k = 3  gamma_abc_g1  (S_IC(K), gamma_g2)     = (S_IC(T), g2)
+ * The pairings are the caller's: this library has none.  If every point passes (with G16_SER_VALIDATE; without it the
+ * answer means nothing on a curve whose cofactor is not 1), the call accepts and all four equations hold, then with
+ * probability at least 1 - 6 N / r over rho (N = max(nv, n)) the key equals g16_setup(alpha, beta, gamma, delta, tau, g1, g2)
+ * point for point, for the transcript's tau, alpha, beta and some non-zero gamma != delta: a member that differs anywhere
+ * makes sum_j rho^j (K_j - K'_j) a non-zero polynomial in rho of degree below N that one of six equations forces to zero
+ * (Schwartz-Zippel).  It does not show that nobody knows delta: that needs the contributors' proofs of knowledge.  The
+ * transcript itself should have passed g16_srs_verify_pairs.
+ * Points: coordinates below q and on the curve, with G16_SER_VALIDATE also [r]P = O; the identity is valid in the key (an
+ * unused variable has it).  A refused point is G16_ERR_INVALID_DATA, g16_last_error() naming the first one, key members
+ * before transcript members, by member and index ("l_query[17]: point is not on the curve", "tau_g1[3]: ...").
+ * G16_ERR_BAD_ARGUMENT, decided before any point is read: a null pointer (pk members of no points excepted), flags other
+ * than G16_SER_VALIDATE | G16_PK_UNCONTRIBUTED, rho = 0, no resident circuit, a transcript member shorter than the
+ * circuit needs (naming the length it needs), a proof in flight.  Nothing is written to pairs_g1 / pairs_g2 unless the
+ * call returns G16_OK.  Needs a resident circuit and no key, and leaves the resident circuit, key and everything derived
+ * from them alone.  Afterwards g16_get_timings describes this call (every other field 0): total_ms = the whole call, h2d_ms
+ * = upload and point checks, witness_map_ms = the field work (powers of rho, the matrix products, the transforms),
+ * msm_ms[0] / msm_ms[1] = the key-side / transcript-side MSMs (host clock around work that ends in a stream synchronise),
+ * msm_pairs[0] / msm_pairs[1] = their points (3 nv + |h_query| + num_witness + num_inputs; 11 n - 1), h2d_bytes /
+ * d2h_bytes = bytes copied each way, launches = kernels. */
+enum { G16_PK_UNCONTRIBUTED = 4 };
+typedef struct {
+  const uint64_t* a_query;
+  const uint64_t* b_g1_query;
+  const uint64_t* b_g2_query;
+  const uint64_t* h_query;
+  const uint64_t* l_query;
+  const uint64_t* alpha_g1; const uint64_t* beta_g1; const uint64_t* delta_g1;
+  const uint64_t* beta_g2; const uint64_t* gamma_g2; const uint64_t* delta_g2;
+  const uint64_t* gamma_abc_g1;
+} g16_pk_check_desc;
+int g16_pk_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const g16_pk_check_desc* pk, const uint64_t* rho,
+                        uint32_t flags, uint64_t* pairs_g1, uint64_t* pairs_g2);
 
 /* ---- ark-serialized proving keys: `ProvingKey::serialize_{compressed,uncompressed}` / `deserialize_with_mode`
  * (data_structures.rs:125 derives them).  The bytes are a whole ProvingKey<E> as ark-serialize 0.5 writes it: vk {alpha_g1,

@@ -573,6 +573,93 @@ impl<E: SwPairing> B200Prover<E> {
         Ok(eqs.iter().all(|(p, q, p2, q2)| E::multi_pairing([*p, -*p2], [*q, *q2]).is_zero()))
     }
 
+    /// The GPU part of checking that `pk` is the key of the resident circuit made from the transcript `srs`
+    /// (g16_pk_verify_pairs, snarkjs `zkey verify` without the contributions' proofs of knowledge).  The library checks every
+    /// point (curve, with `validate` the subgroup), that alpha_g1, beta_g1 and beta_g2 are the transcript's, that delta and
+    /// gamma are not the identity, that gamma_g2 != delta_g2 (`uncontributed` accepts the initial key of a ceremony, where
+    /// gamma = delta = 1), and that the random combinations of a_query, b_g1_query and b_g2_query under the challenge `rho`
+    /// match the transcript's.  Returns the four equations (delta, h_query, l_query, gamma_abc_g1) as (P, Q, P', Q');
+    /// equation k holds iff e(P, Q) = e(P', Q').  A refusal is `InvalidData` (the message naming the member goes to
+    /// stderr); an argument error (a transcript too short for the circuit, rho = 0) is an `IoError` carrying it.
+    #[allow(clippy::type_complexity)]
+    pub fn key_verification_pairs(
+        &self,
+        pk: &ProvingKey<E>,
+        srs: &PowersOfTau<E>,
+        rho: E::ScalarField,
+        validate: Validate,
+        uncontributed: bool,
+    ) -> Result<[(Affine<E::G1Config>, Affine<E::G2Config>, Affine<E::G1Config>, Affine<E::G2Config>); 4], SerializationError>
+    {
+        let (t1, t2, a1, b1) =
+            (pack_points(&srs.tau_g1), pack_points(&srs.tau_g2), pack_points(&srs.alpha_tau_g1), pack_points(&srs.beta_tau_g1));
+        let bg2 = pack_points(core::slice::from_ref(&srs.beta_g2));
+        let sdesc = sys::g16_srs_desc {
+            tau_g1: t1.as_ptr(),
+            tau_g1_len: srs.tau_g1.len() as u64,
+            tau_g2: t2.as_ptr(),
+            tau_g2_len: srs.tau_g2.len() as u64,
+            alpha_tau_g1: a1.as_ptr(),
+            alpha_tau_g1_len: srs.alpha_tau_g1.len() as u64,
+            beta_tau_g1: b1.as_ptr(),
+            beta_tau_g1_len: srs.beta_tau_g1.len() as u64,
+            beta_g2: bg2.as_ptr(),
+        };
+        let (aq, bq1, bq2, hq, lq, abc) = (
+            pack_points(&pk.a_query),
+            pack_points(&pk.b_g1_query),
+            pack_points(&pk.b_g2_query),
+            pack_points(&pk.h_query),
+            pack_points(&pk.l_query),
+            pack_points(&pk.vk.gamma_abc_g1),
+        );
+        let (alpha_g1, beta_g1, delta_g1) =
+            (pack_points(&[pk.vk.alpha_g1]), pack_points(&[pk.beta_g1]), pack_points(&[pk.delta_g1]));
+        let (beta_g2, gamma_g2, delta_g2) =
+            (pack_points(&[pk.vk.beta_g2]), pack_points(&[pk.vk.gamma_g2]), pack_points(&[pk.vk.delta_g2]));
+        let kdesc = sys::g16_pk_check_desc {
+            a_query: aq.as_ptr(),
+            b_g1_query: bq1.as_ptr(),
+            b_g2_query: bq2.as_ptr(),
+            h_query: hq.as_ptr(),
+            l_query: lq.as_ptr(),
+            alpha_g1: alpha_g1.as_ptr(),
+            beta_g1: beta_g1.as_ptr(),
+            delta_g1: delta_g1.as_ptr(),
+            beta_g2: beta_g2.as_ptr(),
+            gamma_g2: gamma_g2.as_ptr(),
+            delta_g2: delta_g2.as_ptr(),
+            gamma_abc_g1: abc.as_ptr(),
+        };
+        let (w1, w2) = (point_limbs::<E::G1Config>(), point_limbs::<E::G2Config>());
+        let (mut o1, mut o2) = (vec![0u64; 8 * w1], vec![0u64; 8 * w2]);
+        let r = [rho];
+        let flags = if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 }
+            | if uncontributed { sys::G16_PK_UNCONTRIBUTED } else { 0 };
+        ser_status(unsafe {
+            sys::g16_pk_verify_pairs(self.ctx, &sdesc, &kdesc, scalars_ptr(&r), flags, o1.as_mut_ptr(), o2.as_mut_ptr())
+        })?;
+        let p = |i: usize| unpack_point::<E::G1Config>(&o1[i * w1..(i + 1) * w1]);
+        let q = |i: usize| unpack_point::<E::G2Config>(&o2[i * w2..(i + 1) * w2]);
+        Ok(core::array::from_fn(|k| (p(2 * k), q(2 * k), p(2 * k + 1), q(2 * k + 1))))
+    }
+
+    /// Checks that `pk` is the key of the resident circuit made from the transcript `srs`: `key_verification_pairs` under a
+    /// challenge drawn from `rng` (with `validate` = Yes and no uncontributed key), then each equation as
+    /// `E::multi_pairing([P, -P'], [Q, Q']).is_zero()`.  Ok(true): with probability at least 1 - 6 max(nv, n) / r the key is
+    /// the setup of the transcript's tau, alpha, beta with some gamma != delta.  Ok(false): an equation fails.  A key the
+    /// library refuses itself is `InvalidData`.  The transcript should have passed `verify_srs` first.
+    pub fn verify_key<R: RngCore>(&self, pk: &ProvingKey<E>, srs: &PowersOfTau<E>, rng: &mut R) -> Result<bool, SerializationError> {
+        let rho = loop {
+            let x = E::ScalarField::rand(rng);
+            if !x.is_zero() {
+                break x;
+            }
+        };
+        let eqs = self.key_verification_pairs(pk, srs, rho, Validate::Yes, false)?;
+        Ok(eqs.iter().all(|(p, q, p2, q2)| E::multi_pairing([*p, -*p2], [*q, *q2]).is_zero()))
+    }
+
     /// One phase-2 contribution to the resident key (g16_setup_contribute): delta_g1, delta_g2 times `delta`, the H and L
     /// queries times delta^-1.  delta = 0 is SynthesisError::UnexpectedIdentity.
     pub fn contribute_delta(&self, delta: E::ScalarField) -> R1CSResult<()> {

@@ -31,6 +31,8 @@ pub const G16_ASSIGNMENT_ON_DEVICE: u32 = 1;
 pub const G16_SERIAL_MSMS: u32 = 2;
 pub const G16_CHECK_WITNESS: u32 = 4;
 
+pub const G16_PK_UNCONTRIBUTED: u32 = 4;
+
 pub const G16_NONE: u64 = u64::MAX;
 
 #[repr(C)]
@@ -112,6 +114,22 @@ pub struct g16_pk_export_desc {
 }
 
 #[repr(C)]
+pub struct g16_pk_check_desc {
+    pub a_query: *const u64,
+    pub b_g1_query: *const u64,
+    pub b_g2_query: *const u64,
+    pub h_query: *const u64,
+    pub l_query: *const u64,
+    pub alpha_g1: *const u64,
+    pub beta_g1: *const u64,
+    pub delta_g1: *const u64,
+    pub beta_g2: *const u64,
+    pub gamma_g2: *const u64,
+    pub delta_g2: *const u64,
+    pub gamma_abc_g1: *const u64,
+}
+
+#[repr(C)]
 #[derive(Default, Clone, Copy)]
 pub struct g16_timings {
     pub total_ms: f32,
@@ -172,6 +190,7 @@ extern "C" {
     pub fn g16_srs_from_secrets(ctx: *mut g16_ctx, tau: *const u64, alpha: *const u64, beta: *const u64, g1: *const u64, g2: *const u64, out: *const g16_srs_out) -> c_int;
     pub fn g16_srs_contribute(ctx: *mut g16_ctx, srs_in: *const g16_srs_desc, tau: *const u64, alpha: *const u64, beta: *const u64, flags: u32, chunk_points: u64, out: *const g16_srs_out) -> c_int;
     pub fn g16_srs_verify_pairs(ctx: *mut g16_ctx, srs: *const g16_srs_desc, g1: *const u64, g2: *const u64, rho: *const u64, flags: u32, chunk_points: u64, pairs_g1: *mut u64, pairs_g2: *mut u64) -> c_int;
+    pub fn g16_pk_verify_pairs(ctx: *mut g16_ctx, srs: *const g16_srs_desc, pk: *const g16_pk_check_desc, rho: *const u64, flags: u32, pairs_g1: *mut u64, pairs_g2: *mut u64) -> c_int;
     pub fn g16_pk_load_serialized(ctx: *mut g16_ctx, bytes: *const u8, len: u64, flags: u32, rank: u32, world: u32, vk_out: *const g16_pk_export_desc) -> c_int;
     pub fn g16_pk_export_serialized(ctx: *mut g16_ctx, flags: u32, out: *mut u8, cap: u64, len_out: *mut u64) -> c_int;
     pub fn g16_prove(ctx: *mut g16_ctx, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32, proof_out: *mut u64) -> c_int;
