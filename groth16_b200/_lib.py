@@ -41,6 +41,19 @@ class SrsOut(C.Structure):
     _fields_ = SrsDesc._fields_
 
 
+class PkDeltaDesc(C.Structure):
+    _fields_ = [("h_query", u64p), ("h_len", C.c_uint64), ("l_query", u64p), ("l_len", C.c_uint64), ("delta_g1", u64p),
+                ("delta_g2", u64p)]
+
+
+class PkDeltaOut(C.Structure):
+    _fields_ = PkDeltaDesc._fields_
+
+
+class ContributionRecord(C.Structure):
+    _fields_ = [(n, u64p) for n in ("after_g1", "s_g1", "s_x_g1", "r_g2", "r_x_g2")]
+
+
 class Timings(C.Structure):
     _fields_ = [("total_ms", C.c_float), ("h2d_ms", C.c_float), ("witness_map_ms", C.c_float),
                 ("msm_ms", C.c_float * 5), ("msm_accum_ms", C.c_float * 5), ("host_finish_ms", C.c_float),
@@ -86,6 +99,10 @@ SIGNATURES = [
      + [C.c_void_p] * 2),
     ("g16_pk_verify_pairs", C.c_int, [C.c_void_p, C.POINTER(SrsDesc), C.POINTER(PkCheckDesc), C.c_void_p, C.c_uint32]
      + [C.c_void_p] * 2),
+    ("g16_pk_contribute", C.c_int, [C.c_void_p, C.POINTER(PkDeltaDesc), C.c_void_p, C.c_uint32, C.c_uint64,
+                                    C.POINTER(PkDeltaOut)]),
+    ("g16_contribution_chain_pairs", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ContributionRecord), C.c_uint32,
+                                               C.c_uint32, C.c_void_p, C.c_void_p]),
     ("g16_pk_load_serialized", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
                                          C.POINTER(PkExportDesc)]),
     ("g16_pk_export_serialized", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),

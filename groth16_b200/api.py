@@ -276,6 +276,101 @@ def pk_verify_args(pk: ProvingKey, srs: Srs, rho, r: int, g1_width: int, g2_widt
     return keys, arrs, rho
 
 
+PK_DELTA_MEMBERS = ("h_query", "l_query", "delta_g1", "delta_g2")
+
+
+def pk_contribute_args(pk: ProvingKey, delta, r: int, g1_width: int, g2_width: int, chunk_points: int = 0,
+                       in_place: bool = False) -> tuple:
+    """The arguments of Groth16.contribute_key as the library takes them: (h_query, l_query as (points, limbs) arrays and
+    delta_g1, delta_g2 as one point each, by name; delta mod r; chunk_points).  ValueError, before any device work: a member
+    missing or not made of whole points, h_query or l_query of 2^32 points or more, delta = 0 mod r (UnexpectedIdentity),
+    chunk_points outside [0, 2^64), and with `in_place` a member that cannot be written where it is (not a C-contiguous,
+    writable uint64 array)."""
+    held = dict(h_query=pk.h_query, l_query=pk.l_query, delta_g1=pk.delta_g1, delta_g2=pk.vk.delta_g2)
+    out = {}
+    for k, v in held.items():
+        w = g2_width if k == "delta_g2" else g1_width
+        if v is None:
+            raise ValueError(f"the key has no {k}")
+        a = np.ascontiguousarray(v, dtype=np.uint64)
+        if in_place and (a is not v or not a.flags["WRITEABLE"]):
+            raise ValueError(f"in_place needs the key's {k} to be a C-contiguous, writable uint64 array")
+        if a.ndim > 2 or a.size % w or (a.ndim == 2 and a.shape[1] != w):
+            raise ValueError(f"{k} of shape {a.shape} is not made of points of {w} limbs")
+        if k in ("delta_g1", "delta_g2"):
+            if a.size != w:
+                raise ValueError(f"{k} holds {a.size // w} points, it is one point")
+            out[k] = a.reshape(w)
+        else:
+            out[k] = a.reshape(-1, w)
+            if out[k].shape[0] >= 1 << 32:
+                raise ValueError(f"{k} holds {out[k].shape[0]} points, at most 2^32 - 1 are allowed")
+    delta = int(delta) % r
+    if delta == 0:
+        raise ValueError("delta must be non-zero mod r (UnexpectedIdentity)")
+    chunk_points = int(chunk_points)
+    if not 0 <= chunk_points < 1 << 64:
+        raise ValueError(f"chunk_points must be in [0, 2^64), not {chunk_points}")
+    return out, delta, chunk_points
+
+
+@dataclass
+class ContributionRecord:
+    """One contribution's public record (the public key of Bowe, Gabizon and Miers), affine Montgomery limbs: after_g1 =
+    x D for the running point D (phase 2: delta_g1; phase 1: tau_g1[1], alpha_tau_g1[0], beta_tau_g1[0]), s_g1 a point the
+    contributor chose, s_x_g1 = x s, r_x_g2 = x r.  r_g2 must be derived by the checker from the ceremony's transcript (a
+    hash to G2 of the contribution; the hash and the file format that binds it are the caller's) and never taken from the
+    contributor: an r whose discrete log is known makes the proof of knowledge empty."""
+    after_g1: np.ndarray
+    s_g1: np.ndarray
+    s_x_g1: np.ndarray
+    r_g2: np.ndarray
+    r_x_g2: np.ndarray
+
+
+RECORD_MEMBERS = ("after_g1", "s_g1", "s_x_g1", "r_g2", "r_x_g2")
+CHAIN_MAX = (1 << 30) - 1
+
+
+@dataclass
+class ChainPairs:
+    """g16_contribution_chain_pairs: 2 count equations.  Equation k holds iff e(g1[2k], g2[2k]) = e(g1[2k + 1], g2[2k + 1]):
+    k = 2i is record i's proof of knowledge (s_i, r_x_i) = (s_x_i, r_i), k = 2i + 1 its step (D_i, r_x_i) = (D_(i+1), r_i).
+    g1 is (4 count, G1 limbs) and g2 is (4 count, G2 limbs), affine Montgomery limbs."""
+    g1: np.ndarray
+    g2: np.ndarray
+
+    def __len__(self) -> int:
+        return self.g1.shape[0] // 2
+
+    def equation(self, k: int) -> tuple:
+        """(P_k, Q_k, P'_k, Q'_k) of equation k, as limb arrays"""
+        if not 0 <= k < len(self):
+            raise IndexError(f"equation {k} of {len(self)}")
+        return self.g1[2 * k], self.g2[2 * k], self.g1[2 * k + 1], self.g2[2 * k + 1]
+
+
+def chain_args(start_g1, end_g1, records: Sequence[ContributionRecord], g1_width: int, g2_width: int) -> tuple:
+    """The arguments of Groth16.contribution_chain_pairs as the library takes them: (start_g1, end_g1, and per record its
+    five members by name, each one point as a C-contiguous uint64 array).  ValueError, before any device work: no records
+    or more than 2^30 - 1, a point missing or not exactly one point of its group."""
+    n = len(records)
+    if not 1 <= n <= CHAIN_MAX:
+        raise ValueError(f"a chain has 1 to 2^30 - 1 records, not {n}")
+
+    def one(v, w, what):
+        if v is None:
+            raise ValueError(f"{what} is missing")
+        a = np.ascontiguousarray(v, dtype=np.uint64)
+        if a.size != w:
+            raise ValueError(f"{what} holds {a.size} limbs, one point is {w}")
+        return a.reshape(w)
+
+    recs = [{m: one(getattr(c, m), g2_width if m.endswith("g2") else g1_width, f"records[{i}].{m}") for m in RECORD_MEMBERS}
+            for i, c in enumerate(records)]
+    return one(start_g1, g1_width, "start_g1"), one(end_g1, g1_width, "end_g1"), recs
+
+
 @dataclass
 class WitnessReport:
     """g16_witness_report of one assignment, None where the library reports G16_NONE"""
@@ -613,6 +708,55 @@ class Groth16:
         flags = (_lib.SER_VALIDATE if validate else 0) | (_lib.PK_UNCONTRIBUTED if uncontributed else 0)
         _check(self._lib.g16_pk_verify_pairs(self._ctx, C.byref(s), C.byref(d), _ptr(r_), flags, _ptr(out1), _ptr(out2)))
         return KeyPairs(out1, out2)
+
+    def contribute_key(self, pk: ProvingKey, delta, validate: bool = False, chunk_points: int = 0,
+                       in_place: bool = False) -> ProvingKey:
+        """g16_pk_contribute: one phase-2 contribution delta (a Python int) to a key received from another party, on the GPU:
+        delta_g1 and delta_g2 times delta, every h_query and l_query point times delta^-1.  Returns a new ProvingKey whose
+        other members are pk's own arrays; with `in_place` the four members are written into pk's arrays (each then a
+        C-contiguous, writable uint64 array) and pk is returned.  `validate` adds the subgroup check of every point;
+        `chunk_points` caps the points per chunk (0: as many as the free device memory holds).  A refused point (delta_g1
+        or delta_g2 the identity among them) raises serialize.DeserializeError naming it, with nothing written.  Needs no
+        circuit or key and leaves the resident ones alone."""
+        ins, delta, chunk_points = pk_contribute_args(pk, delta, self.curve.r, 2 * self.nq, self.ng2, chunk_points, in_place)
+        outs = ins if in_place else {k: np.empty_like(v) for k, v in ins.items()}
+        d_in, d_out = _lib.PkDeltaDesc(), _lib.PkDeltaOut()
+        for d, arrs in ((d_in, ins), (d_out, outs)):
+            for k in ("h_query", "l_query"):
+                setattr(d, k, _u64p(arrs[k]) if arrs[k].size else None)
+                setattr(d, k.replace("_query", "_len"), arrs[k].shape[0])
+            d.delta_g1, d.delta_g2 = _u64p(arrs["delta_g1"]), _u64p(arrs["delta_g2"])
+        dl = np.ascontiguousarray(self.codec.fr.enc1(delta))
+        _check(self._lib.g16_pk_contribute(self._ctx, C.byref(d_in), _ptr(dl), _lib.SER_VALIDATE if validate else 0,
+                                           chunk_points, C.byref(d_out)))
+        if in_place:
+            return pk
+        vk = pk.vk
+        return ProvingKey(VerifyingKey(vk.alpha_g1, vk.beta_g2, vk.gamma_g2, outs["delta_g2"], vk.gamma_abc_g1), pk.beta_g1,
+                          outs["delta_g1"], pk.a_query, pk.b_g1_query, pk.b_g2_query, outs["h_query"], outs["l_query"])
+
+    def contribution_chain_pairs(self, start_g1, end_g1, records: Sequence[ContributionRecord],
+                                 validate: bool = True) -> ChainPairs:
+        """g16_contribution_chain_pairs: the proofs of knowledge of a chain of contributions, either phase.  With D_0 =
+        start_g1 (phase 2: the uncontributed key's delta_g1 = tau_g1[0]; phase 1: tau_g1[1], alpha_tau_g1[0] or
+        beta_tau_g1[0] of the transcript before the first contribution) and D_(i+1) = records[i].after_g1, it returns 2
+        len(records) equations (ChainPairs): with (P, Q, P', Q') = pairs.equation(k), the caller evaluates e(P, Q) = e(P',
+        Q') with its own pairing.  If all hold, end_g1 = (prod x_i) start_g1, and contributor i knew x_i provided each
+        records[i].r_g2 was derived by the checker from the ceremony's transcript (never taken from the contributor).
+        The library checks every point (canonical, on the curve, with `validate` in the prime-order subgroup, never the
+        identity) and that the last record's after_g1 is end_g1; a refusal raises serialize.DeserializeError naming the
+        record and member.  `validate` defaults to True: without the subgroup check the answer means nothing on a curve
+        whose cofactor is not 1.  Needs no circuit or key and leaves the resident ones alone."""
+        start, end, recs = chain_args(start_g1, end_g1, records, 2 * self.nq, self.ng2)
+        descs = (_lib.ContributionRecord * len(recs))()
+        for d, rc in zip(descs, recs):
+            for m in RECORD_MEMBERS:
+                setattr(d, m, _u64p(rc[m]))
+        out1 = np.zeros((4 * len(recs), 2 * self.nq), dtype=np.uint64)
+        out2 = np.zeros((4 * len(recs), self.ng2), dtype=np.uint64)
+        _check(self._lib.g16_contribution_chain_pairs(self._ctx, _ptr(start), _ptr(end), descs, len(recs),
+                                                      _lib.SER_VALIDATE if validate else 0, _ptr(out1), _ptr(out2)))
+        return ChainPairs(out1, out2)
 
     def _after_key_change(self, rc: int):
         """Status of g16_setup_from_srs / g16_setup_contribute: argument errors (G16_ERR_BAD_ARGUMENT,

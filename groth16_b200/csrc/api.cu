@@ -173,6 +173,17 @@ int g16_pk_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const g16_pk_chec
   CTX_OR_FAIL(ctx);
   return ctx->eng->pk_verify_pairs(srs, pk, rho, flags, pairs_g1, pairs_g2);
 }
+int g16_pk_contribute(g16_ctx* ctx, const g16_pk_delta_desc* in, const uint64_t* delta, uint32_t flags, uint64_t chunk_points,
+                      const g16_pk_delta_out* out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->pk_contribute(in, delta, flags, chunk_points, out);
+}
+int g16_contribution_chain_pairs(g16_ctx* ctx, const uint64_t* start_g1, const uint64_t* end_g1,
+                                 const g16_contribution_record* records, uint32_t count, uint32_t flags, uint64_t* pairs_g1,
+                                 uint64_t* pairs_g2) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->contribution_chain_pairs(start_g1, end_g1, records, count, flags, pairs_g1, pairs_g2);
+}
 int g16_pk_load_serialized(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                            const g16_pk_export_desc* vk_out) {
   CTX_OR_FAIL(ctx);

@@ -154,6 +154,10 @@ struct IEngine {
                                uint32_t flags, uint64_t chunk_points, uint64_t* pairs_g1, uint64_t* pairs_g2) = 0;
   virtual int pk_verify_pairs(const g16_srs_desc* srs, const g16_pk_check_desc* pk, const uint64_t* rho, uint32_t flags,
                               uint64_t* pairs_g1, uint64_t* pairs_g2) = 0;
+  virtual int pk_contribute(const g16_pk_delta_desc* in, const uint64_t* delta, uint32_t flags, uint64_t chunk_points,
+                            const g16_pk_delta_out* out) = 0;
+  virtual int contribution_chain_pairs(const uint64_t* start_g1, const uint64_t* end_g1, const g16_contribution_record* records,
+                                       uint32_t count, uint32_t flags, uint64_t* pairs_g1, uint64_t* pairs_g2) = 0;
   virtual int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                                  const g16_pk_export_desc* vk_out) = 0;
   virtual int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) = 0;
@@ -1393,8 +1397,7 @@ struct Engine : IEngine {
     }
     // an output range may be its own input range (in place) and must overlap no other input or output range
     auto overlap = [&](const void* a, int ma, const void* b, int mb) {
-      const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
-      return len[ma] && len[mb] && a0 < b0 + len[mb] * esz[mb] && b0 < a0 + len[ma] * esz[ma];
+      return srs_overlap((uintptr_t)a, len[ma] * esz[ma], (uintptr_t)b, len[mb] * esz[mb]);
     };
     for (int o = 0; o < SRS_MEMBERS; o++)
       for (int m = 0; m < SRS_MEMBERS; m++) {
@@ -1851,6 +1854,206 @@ struct Engine : IEngine {
     for (int i = 0; i < 8; i++) {
       store_a1(pairs_g1 + (size_t)i * 2 * NQ64, ps[i]);
       store_a2(pairs_g2 + (size_t)i * G2_64, qs[i]);
+    }
+    tm.total_ms = ms_since(t0);
+    return G16_OK;
+  }
+
+  // ---- phase-2 contributions to a key in host memory (g16_pk_contribute) and the proofs of knowledge of a chain of
+  // contributions (g16_contribution_chain_pairs) ----
+  enum { PKD_H = 0, PKD_L, PKD_DELTA1, PKD_DELTA2, PKD_MEMBERS };
+  static const char* pkd_member(int m) {
+    static const char* t[PKD_MEMBERS] = {"h_query", "l_query", "delta_g1", "delta_g2"};
+    return t[m];
+  }
+  // g16_pk_contribute: delta_g1, delta_g2 times delta; every h_query and l_query point times delta^-1.  Two passes over h_query
+  // and l_query in chunks of at most `cap` points through one device buffer, as g16_srs_contribute: every point (delta_g1 and
+  // delta_g2 too, the identity refused there) is uploaded and checked before anything is written to `out`, then each chunk is
+  // uploaded again, multiplied in place on the device (srs_scale_affine_kernel) and copied out.  The two single points are
+  // multiplied on the host, as g16_setup_contribute does.
+  // Timings (host clock around work that ends in a stream synchronise): h2d_ms = the check pass, msm_ms[0] / msm_ms[1] = the
+  // transform of h_query / l_query, total_ms = the whole call.
+  int pk_contribute(const g16_pk_delta_desc* in, const uint64_t* delta_, uint32_t flags, uint64_t chunk_points,
+                    const g16_pk_delta_out* out) override {
+    if (!in || !out || !delta_) return fail(G16_ERR_BAD_ARGUMENT, "null argument");
+    if (flags & ~(uint32_t)G16_SER_VALIDATE) return fail(G16_ERR_BAD_ARGUMENT, "g16_pk_contribute takes 0 or G16_SER_VALIDATE");
+    const uint64_t* src[PKD_MEMBERS] = {in->h_query, in->l_query, in->delta_g1, in->delta_g2};
+    uint64_t* dst[PKD_MEMBERS] = {out->h_query, out->l_query, out->delta_g1, out->delta_g2};
+    const uint64_t len[PKD_MEMBERS] = {in->h_len, in->l_len, 1, 1};
+    const uint64_t olen[PKD_MEMBERS] = {out->h_len, out->l_len, 1, 1};
+    const uint64_t esz[PKD_MEMBERS] = {sizeof(A1), sizeof(A1), sizeof(A1), sizeof(A2)};
+    for (int m = 0; m < PKD_MEMBERS; m++) {
+      const std::string name = pkd_member(m);
+      if (olen[m] != len[m])
+        return fail(G16_ERR_BAD_ARGUMENT, "out " + name + " holds " + std::to_string(olen[m]) + " points, in " + name + " " +
+                                              std::to_string(len[m]) + ": the lengths must be equal");
+      if (len[m] >> 32)
+        return fail(G16_ERR_BAD_ARGUMENT, name + " holds " + std::to_string(len[m]) + " points, at most 2^32 - 1 are allowed");
+      if (len[m] && (!src[m] || !dst[m])) return fail(G16_ERR_BAD_ARGUMENT, "null key member " + name);
+    }
+    // an output range may be its own input range (in place) and must overlap no other input or output range
+    auto overlap = [&](const void* a, int ma, const void* b, int mb) {
+      return srs_overlap((uintptr_t)a, len[ma] * esz[ma], (uintptr_t)b, len[mb] * esz[mb]);
+    };
+    for (int o = 0; o < PKD_MEMBERS; o++)
+      for (int m = 0; m < PKD_MEMBERS; m++) {
+        if (overlap(dst[o], o, src[m], m) && !(o == m && (const void*)dst[o] == (const void*)src[m]))
+          return fail(G16_ERR_BAD_ARGUMENT, std::string("out ") + pkd_member(o) + " overlaps in " + pkd_member(m) +
+                                                ": an output may only be the very same array as its own input");
+        if (m > o && overlap(dst[o], o, dst[m], m))
+          return fail(G16_ERR_BAD_ARGUMENT, std::string("out ") + pkd_member(o) + " overlaps out " + pkd_member(m));
+      }
+    const Fr d = load_fr(delta_);
+    if (d.is_zero()) return fail(G16_ERR_BAD_ARGUMENT, "delta must be invertible (UnexpectedIdentity)");
+    G16_NOT_BUSY();
+    G16_CUDA(cudaSetDevice(device));
+    const auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point a) {
+      return (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count();
+    };
+    tm = g16_timings{};
+    cudaStream_t st = S0.st_main;
+    size_t free_b = 0, total_b = 0;
+    G16_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const uint64_t cap = srs_chunk_cap(chunk_points, std::max(len[PKD_H], len[PKD_L]), free_b, sizeof(A1));
+    DevBuf buf, err;
+    G16_CUDA(buf.reserve(std::max<uint64_t>(cap * sizeof(A1), sizeof(A2))));
+    G16_CUDA(err.reserve(8));
+    // --- check pass: every point, chunk by chunk; the first bad one by member, then index ---
+    for (int m = 0; m < PKD_MEMBERS; m++) {
+      const bool single = m == PKD_DELTA1 || m == PKD_DELTA2;
+      const uint32_t fl = flags | (single ? (uint32_t)SRS_REFUSE_IDENTITY : 0u);
+      for (uint64_t i0 = 0; i0 < len[m];) {
+        const uint32_t cnt = srs_chunk_len(len[m], i0, cap);
+        G16_CUDA(cudaMemcpyAsync(buf.p, (const char*)src[m] + i0 * esz[m], cnt * esz[m], cudaMemcpyHostToDevice, st));
+        G16_CUDA(cudaMemsetAsync(err.p, 0xff, 8, st));
+        unsigned long long* e = err.template as<unsigned long long>();
+        G16_CUDA((m == PKD_DELTA2 ? srs_check<CP, true>(st, buf.p, cnt, fl, m, e) : srs_check<CP, false>(st, buf.p, cnt, fl, m, e)));
+        unsigned long long first_err = 0;
+        G16_CUDA(cudaMemcpyAsync(&first_err, err.p, 8, cudaMemcpyDeviceToHost, st));
+        G16_CUDA(cudaStreamSynchronize(st));
+        tm.h2d_bytes += cnt * esz[m];
+        tm.d2h_bytes += 8;
+        tm.launches++;
+        if (first_err != ~0ull)
+          return fail(G16_ERR_INVALID_DATA, std::string(pkd_member(m)) +
+                                                (single ? std::string()
+                                                        : "[" + std::to_string(i0 + ((first_err >> 8) & ((1ull << 40) - 1))) + "]") +
+                                                ": " + srs_reason(first_err & 0xff));
+        i0 += cnt;
+      }
+    }
+    tm.h2d_ms = ms_since(t0);
+    // --- transform pass: h_query and l_query times delta^-1, chunk by chunk ---
+    const Fr di = Fr::inv(d);
+    for (int m : {PKD_H, PKD_L}) {
+      const auto t1 = std::chrono::steady_clock::now();
+      for (uint64_t i0 = 0; i0 < len[m];) {
+        const uint32_t cnt = srs_chunk_len(len[m], i0, cap);
+        G16_CUDA(cudaMemcpyAsync(buf.p, (const char*)src[m] + i0 * esz[m], cnt * esz[m], cudaMemcpyHostToDevice, st));
+        G16_CUDA((srs_scale_affine<Fq, Fr>(st, buf.template as<A1>(), cnt, di)));
+        G16_CUDA(cudaMemcpyAsync((char*)dst[m] + i0 * esz[m], buf.p, cnt * esz[m], cudaMemcpyDeviceToHost, st));
+        tm.h2d_bytes += cnt * esz[m];
+        tm.d2h_bytes += cnt * esz[m];
+        tm.launches++;
+        i0 += cnt;
+      }
+      G16_CUDA(cudaStreamSynchronize(st));
+      tm.msm_ms[m] = ms_since(t1);
+    }
+    // delta_g1 and delta_g2 are one point each: on the host, as g16_setup_contribute does
+    uint32_t k[Fr::N];
+    fr_to_canon(d, k);
+    store_a1(dst[PKD_DELTA1], P1::from_affine(load_a1(src[PKD_DELTA1])).mul_u32(k, Fr::N).to_affine());
+    store_a2(dst[PKD_DELTA2], P2::from_affine(load_a2(src[PKD_DELTA2])).mul_u32(k, Fr::N).to_affine());
+    tm.total_ms = ms_since(t0);
+    return G16_OK;
+  }
+  // Members of a contribution record, in the order a refusal names them within one record.  G1 points go to one device
+  // buffer as start_g1, end_g1, then (after_g1, s_g1, s_x_g1) per record; G2 points to another as (r_g2, r_x_g2) per record.
+  enum { CR_AFTER = 0, CR_S, CR_SX, CR_R, CR_RX, CR_MEMBERS };
+  static const char* cr_member(int m) {
+    static const char* t[CR_MEMBERS] = {"after_g1", "s_g1", "s_x_g1", "r_g2", "r_x_g2"};
+    return t[m];
+  }
+  // g16_contribution_chain_pairs: every point uploaded once and checked by srs_check_kernel (the identity refused), the end
+  // compared with the last record's after_g1, then the 2 count equations written from the host copies.  The G1 and G2
+  // uploads have an error word each; the refusal names the earlier of the two bad points by record, then member.
+  // Timings (host clock around work that ends in a stream synchronise): h2d_ms = upload and checks, total_ms = the call.
+  int contribution_chain_pairs(const uint64_t* start_g1, const uint64_t* end_g1, const g16_contribution_record* rec, uint32_t count,
+                               uint32_t flags, uint64_t* pairs_g1, uint64_t* pairs_g2) override {
+    if (!start_g1 || !end_g1 || !rec || !pairs_g1 || !pairs_g2) return fail(G16_ERR_BAD_ARGUMENT, "null argument");
+    if (count == 0 || count >= (1u << 30))
+      return fail(G16_ERR_BAD_ARGUMENT, "count is " + std::to_string(count) + ": a chain has 1 to 2^30 - 1 records");
+    if (flags & ~(uint32_t)G16_SER_VALIDATE)
+      return fail(G16_ERR_BAD_ARGUMENT, "g16_contribution_chain_pairs takes 0 or G16_SER_VALIDATE");
+    for (uint32_t i = 0; i < count; i++) {
+      const uint64_t* p[CR_MEMBERS] = {rec[i].after_g1, rec[i].s_g1, rec[i].s_x_g1, rec[i].r_g2, rec[i].r_x_g2};
+      for (int m = 0; m < CR_MEMBERS; m++)
+        if (!p[m]) return fail(G16_ERR_BAD_ARGUMENT, "records[" + std::to_string(i) + "]." + cr_member(m) + " is null");
+    }
+    G16_NOT_BUSY();
+    G16_CUDA(cudaSetDevice(device));
+    const auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point a) {
+      return (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count();
+    };
+    tm = g16_timings{};
+    cudaStream_t st = S0.st_main;
+    const uint64_t n1 = 2 + 3ull * count, n2 = 2ull * count, w1 = 2 * NQ64, w2 = G2_64;
+    std::vector<uint64_t> h1(n1 * w1), h2(n2 * w2);   // the points as the ABI lays them out, then uploaded as they are
+    auto put = [](std::vector<uint64_t>& v, uint64_t at, const uint64_t* p, uint64_t w) { memcpy(v.data() + at * w, p, w * 8); };
+    put(h1, 0, start_g1, w1);
+    put(h1, 1, end_g1, w1);
+    for (uint32_t i = 0; i < count; i++) {
+      put(h1, 2 + 3ull * i, rec[i].after_g1, w1);
+      put(h1, 3 + 3ull * i, rec[i].s_g1, w1);
+      put(h1, 4 + 3ull * i, rec[i].s_x_g1, w1);
+      put(h2, 2ull * i, rec[i].r_g2, w2);
+      put(h2, 2ull * i + 1, rec[i].r_x_g2, w2);
+    }
+    DevBuf d1, d2, err;
+    G16_CUDA(d1.reserve(n1 * w1 * 8));
+    G16_CUDA(d2.reserve(n2 * w2 * 8));
+    G16_CUDA(err.reserve(16));
+    unsigned long long* e = err.template as<unsigned long long>();
+    const uint32_t fl = flags | SRS_REFUSE_IDENTITY;
+    G16_CUDA(cudaMemsetAsync(err.p, 0xff, 16, st));
+    G16_CUDA(cudaMemcpyAsync(d1.p, h1.data(), n1 * w1 * 8, cudaMemcpyHostToDevice, st));
+    G16_CUDA(cudaMemcpyAsync(d2.p, h2.data(), n2 * w2 * 8, cudaMemcpyHostToDevice, st));
+    G16_CUDA((srs_check<CP, false>(st, d1.p, (uint32_t)n1, fl, 0, e)));
+    G16_CUDA((srs_check<CP, true>(st, d2.p, (uint32_t)n2, fl, 0, e + 1)));
+    unsigned long long first_err[2] = {0, 0};
+    G16_CUDA(cudaMemcpyAsync(first_err, err.p, 16, cudaMemcpyDeviceToHost, st));
+    G16_CUDA(cudaStreamSynchronize(st));
+    tm.h2d_bytes = (n1 * w1 + n2 * w2) * 8;
+    tm.d2h_bytes = 16;
+    tm.launches = 2;
+    tm.h2d_ms = ms_since(t0);
+    // position of a bad point: (record, member) as a sortable key, start_g1 and end_g1 before every record
+    auto where = [](unsigned long long w, bool g2) -> uint64_t {
+      const uint64_t k = (w >> 8) & ((1ull << 40) - 1);
+      if (g2) return (k / 2 + 1) * CR_MEMBERS + CR_R + k % 2;
+      return k < 2 ? k : ((k - 2) / 3 + 1) * CR_MEMBERS + (k - 2) % 3;
+    };
+    if (first_err[0] != ~0ull || first_err[1] != ~0ull) {
+      const bool g2 = first_err[0] == ~0ull || (first_err[1] != ~0ull && where(first_err[1], true) < where(first_err[0], false));
+      const uint64_t at = where(first_err[g2], g2);
+      const std::string name = at < 2 ? std::string(at ? "end_g1" : "start_g1")
+                                       : "records[" + std::to_string(at / CR_MEMBERS - 1) + "]." + cr_member((int)(at % CR_MEMBERS));
+      return fail(G16_ERR_INVALID_DATA, name + ": " + srs_reason(first_err[g2] & 0xff));
+    }
+    // affine limbs are canonical here, so equal points have equal limbs
+    if (memcmp(end_g1, rec[count - 1].after_g1, w1 * 8))
+      return fail(G16_ERR_INVALID_DATA, "records[" + std::to_string(count - 1) + "].after_g1: not end_g1");
+    // equation 2i: (s_i, r_x_i) = (s_x_i, r_i); equation 2i + 1: (D_i, r_x_i) = (D_(i+1), r_i), D_0 = start_g1
+    for (uint64_t i = 0; i < count; i++) {
+      const uint64_t ps[4] = {3 + 3 * i, 4 + 3 * i, i ? 2 + 3 * (i - 1) : 0, 2 + 3 * i};   // indices into h1
+      const uint64_t qs[4] = {2 * i + 1, 2 * i, 2 * i + 1, 2 * i};                         // indices into h2
+      for (uint64_t j = 0; j < 4; j++) {
+        memcpy(pairs_g1 + (4 * i + j) * w1, h1.data() + ps[j] * w1, w1 * 8);
+        memcpy(pairs_g2 + (4 * i + j) * w2, h2.data() + qs[j] * w2, w2 * 8);
+      }
     }
     tm.total_ms = ms_since(t0);
     return G16_OK;

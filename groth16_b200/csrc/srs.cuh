@@ -1,8 +1,9 @@
 // srs.cuh -- proving keys from a powers-of-tau transcript (g16_setup_from_srs) and phase-2 delta contributions
 // (g16_setup_contribute): the group-valued inverse FFT, sparse sums of points, one scalar times many points, and the
 // transcript point checks; phase-1 contributions to a transcript (g16_srs_contribute): every point times its own power
-// of the secret; the scalars of the transcript check (g16_srs_verify_pairs): one power of the challenge per point; and the
-// H-query weights of the key check (g16_pk_verify_pairs).
+// of the secret; the scalars of the transcript check (g16_srs_verify_pairs): one power of the challenge per point; the
+// H-query weights of the key check (g16_pk_verify_pairs); and delta contributions to a key in host memory
+// (g16_pk_contribute): every point times the one scalar delta^-1.
 //
 // Every kernel works on XYZZ points in global memory, one point (or one butterfly, or one chunk of a sum) per thread.  The
 // scalar multiplications are left-to-right double-and-add over the canonical scalar (XYZZ::mul_u32); a windowed form would
@@ -60,6 +61,9 @@ struct SrsSumPlan {
 // A member of `len` points runs in chunks of at most `cap` points; the chunk starting at point i0 holds
 // srs_chunk_len(len, i0, cap) of them.  len < 2^32 and 1 <= cap < 2^32, so a chunk's count and every index fit in 32 bits.
 inline uint32_t srs_chunk_len(uint64_t len, uint64_t i0, uint64_t cap) { return (uint32_t)std::min<uint64_t>(cap, len - i0); }
+// Whether the byte ranges [a, a + na) and [b, b + nb) share a byte; an empty range shares none.  The contribution calls
+// refuse an output range that overlaps any input or output range other than its own input (in place).
+inline bool srs_overlap(uintptr_t a, uint64_t na, uintptr_t b, uint64_t nb) { return na && nb && a < b + nb && b < a + na; }
 // Points per chunk: as many points of `esz` bytes as `free_bytes` of device memory hold after a 512 MiB margin, and no more
 // than `chunk_points` (0: no cap of its own), `longest` (the longest member) or 2^32 - 1; at least 1.
 inline uint64_t srs_chunk_cap(uint64_t chunk_points, uint64_t longest, uint64_t free_bytes, uint64_t esz) {
@@ -190,6 +194,16 @@ __global__ void __launch_bounds__(128) srs_contribute_kernel(Affine<F>* p, uint3
   const XYZZ<F> r = srs_mul(XYZZ<F>::from_affine(p[j]), srs_power(c, tab, j));
   srs_store_affine(&r, p + j);
 }
+// One chunk of a delta contribution to a key in host memory (g16_pk_contribute), in place: p[j] *= s for the one scalar
+// s = delta^-1, affine in and out; the identity stays the identity.  Every thread has the same scalar, so each of its bits
+// costs the warp the same branch.
+template <class F, class FrF>
+__global__ void __launch_bounds__(128) srs_scale_affine_kernel(Affine<F>* p, uint32_t cnt, FrF s) {
+  const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= cnt) return;
+  const XYZZ<F> r = srs_mul(XYZZ<F>::from_affine(p[j]), s);
+  srs_store_affine(&r, p + j);
+}
 // The scalars of one chunk of a transcript check: out[j] = c rho^j (tab[k] = rho^(2^k), c = rho^i0), Montgomery form.
 template <class FrF>
 __global__ void __launch_bounds__(128) srs_powers_kernel(const FrF* tab, FrF c, uint32_t cnt, FrF* out) {
@@ -302,6 +316,11 @@ cudaError_t srs_contribute(cudaStream_t st, Affine<F>* p, uint32_t cnt, const Fr
   if (cnt) srs_contribute_kernel<F, FrF><<<srs_blocks(cnt), 128, 0, st>>>(p, cnt, tab, c);
   return cudaGetLastError();
 }
+template <class F, class FrF>
+cudaError_t srs_scale_affine(cudaStream_t st, Affine<F>* p, uint32_t cnt, FrF s) {
+  if (cnt) srs_scale_affine_kernel<F, FrF><<<srs_blocks(cnt), 128, 0, st>>>(p, cnt, s);
+  return cudaGetLastError();
+}
 template <class FrF>
 cudaError_t srs_powers(cudaStream_t st, const FrF* tab, FrF c, uint32_t cnt, FrF* out) {
   if (cnt) srs_powers_kernel<FrF><<<srs_blocks(cnt), 128, 0, st>>>(tab, c, cnt, out);
@@ -359,6 +378,7 @@ cudaError_t srs_sum(cudaStream_t st, const XYZZ<F>* src, const uint32_t* d_idx, 
   X cudaError_t srs_powers<Fp<CP::FrP>>(cudaStream_t, const Fp<CP::FrP>*, Fp<CP::FrP>, uint32_t, Fp<CP::FrP>*);     \
   X cudaError_t srs_h_weights<Fp<CP::FrP>>(cudaStream_t, const Fp<CP::FrP>*, Fp<CP::FrP>, const Fp<CP::FrP>*,       \
                                            uint32_t, uint32_t, Fp<CP::FrP>*);                                       \
+  X cudaError_t srs_scale_affine<Fp<CP::FqP>, Fp<CP::FrP>>(cudaStream_t, Affine<Fp<CP::FqP>>*, uint32_t, Fp<CP::FrP>); \
   G16_SRS_POINT_TEMPLATES(X, Fp<CP::FqP>, Fp<CP::FrP>)
 #endif
 

@@ -226,7 +226,8 @@ int g16_srs_from_secrets(g16_ctx* ctx, const uint64_t* tau, const uint64_t* alph
  * around work that ends in a stream synchronise), h2d_bytes / d2h_bytes = bytes copied each way, launches = kernels. */
 int g16_srs_contribute(g16_ctx* ctx, const g16_srs_desc* in, const uint64_t* tau, const uint64_t* alpha, const uint64_t* beta,
                        uint32_t flags, uint64_t chunk_points, const g16_srs_out* out);
-/* Phase 1 of the ceremony, the checker's side (snarkjs `powersoftau verify`, without the contributions' proofs of knowledge):
+/* Phase 1 of the ceremony, the checker's side (snarkjs `powersoftau verify`; the contributions' proofs of knowledge are
+ * g16_contribution_chain_pairs):
  * the GPU part of checking that `srs` is a powers-of-tau transcript T(tau, alpha, beta) over the agreed affine generators g1,
  * g2.  rho (Montgomery Fr, non-zero) is a challenge the caller draws after the transcript is fixed, which whoever made the
  * transcript cannot predict (a CSPRNG, or a hash of the transcript).  For a member X of N points let
@@ -263,7 +264,8 @@ int g16_srs_contribute(g16_ctx* ctx, const g16_srs_desc* in, const uint64_t* tau
  * d2h_bytes = bytes copied each way, launches = kernels. */
 int g16_srs_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const uint64_t* g1, const uint64_t* g2, const uint64_t* rho,
                          uint32_t flags, uint64_t chunk_points, uint64_t* pairs_g1, uint64_t* pairs_g2);
-/* Phase 2 of the ceremony, the user's side (snarkjs `zkey verify`, without the contributions' proofs of knowledge): the GPU
+/* Phase 2 of the ceremony, the user's side (snarkjs `zkey verify`; the contributions' proofs of knowledge are
+ * g16_contribution_chain_pairs): the GPU
  * part of checking that `pk`, a proving key received from elsewhere, is the key of the resident circuit (under its
  * reduction) made from the transcript `srs`, i.e. g16_setup(alpha, beta, gamma, delta, tau) for the transcript's tau, alpha,
  * beta and some gamma, delta.  pk holds the members of g16_pk_export_desc, read-only, with the lengths g16_pk_export writes:
@@ -293,7 +295,8 @@ int g16_srs_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const uint64_t* 
  * probability at least 1 - 6 N / r over rho (N = max(nv, n)) the key equals g16_setup(alpha, beta, gamma, delta, tau, g1, g2)
  * point for point, for the transcript's tau, alpha, beta and some non-zero gamma != delta: a member that differs anywhere
  * makes sum_j rho^j (K_j - K'_j) a non-zero polynomial in rho of degree below N that one of six equations forces to zero
- * (Schwartz-Zippel).  It does not show that nobody knows delta: that needs the contributors' proofs of knowledge.  The
+ * (Schwartz-Zippel).  It does not show that nobody knows delta: g16_contribution_chain_pairs from tau_g1[0] to delta_g1
+ * does.  The
  * transcript itself should have passed g16_srs_verify_pairs.
  * Points: coordinates below q and on the curve, with G16_SER_VALIDATE also [r]P = O; the identity is valid in the key (an
  * unused variable has it).  A refused point is G16_ERR_INVALID_DATA, g16_last_error() naming the first one, key members
@@ -320,6 +323,76 @@ typedef struct {
 } g16_pk_check_desc;
 int g16_pk_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const g16_pk_check_desc* pk, const uint64_t* rho,
                         uint32_t flags, uint64_t* pairs_g1, uint64_t* pairs_g2);
+/* Phase 2 of the ceremony, a contributor's side for a key it was sent (snarkjs `zkey contribute`): one contribution delta
+ * (Montgomery Fr, non-zero) to the delta-dependent members of a proving key held in host memory, written to `out`.
+ * delta_g1 and delta_g2 are multiplied by delta, every h_query and l_query point by delta^-1; the identity (all-zero limbs)
+ * stays the identity (an unused variable has it in l_query).  No other key member changes, so the call does not take them.
+ * On a key g16_setup(alpha, beta, gamma, delta0, tau) the result is g16_setup(alpha, beta, gamma, delta0 delta, tau) limb
+ * for limb, and on the key g16_setup_contribute(delta) would change it is what that call makes.  Lengths run from 0 to
+ * 2^32 - 1, out->h_len and out->l_len equal to the input's; a member of length 0 may be null; delta_g1 and delta_g2 are
+ * always read and written.  out->m may be the very same pointer as in->m (in place); any other overlap of an output range
+ * with an input or another output range is refused.  The result does not depend on chunk_points, on in place or not, or on
+ * flags.
+ * Two passes in chunks of at most chunk_points points (0: as many as the free device memory holds; any value is also capped
+ * by it), so a key larger than the device streams through: first every point is uploaded and checked (coordinates below q,
+ * on the curve; G16_SER_VALIDATE adds [r]P = O; delta_g1 and delta_g2 must not be the identity), and only when all have
+ * passed is each chunk of h_query and l_query uploaded again, multiplied on the GPU (one thread per point, all by delta^-1)
+ * and written to out; delta_g1 and delta_g2 are multiplied on the host.  A refused point returns G16_ERR_INVALID_DATA with
+ * g16_last_error() naming the first one ("l_query[70001]: point is not on the curve", "delta_g2: point is the identity")
+ * and nothing written to out, so an in-place key is intact.
+ * G16_ERR_BAD_ARGUMENT, decided before any point is read: a null pointer where a point or scalar is needed, flags other
+ * than 0 or G16_SER_VALIDATE, delta = 0 ("UnexpectedIdentity"), in and out lengths that differ, a length of 2^32 or more,
+ * overlapping ranges, a proof in flight.  Needs no circuit or key and leaves the resident ones and everything derived from
+ * them alone.  Afterwards g16_get_timings describes this call (every other field 0): total_ms = the whole call, h2d_ms =
+ * the check pass, msm_ms[0] / msm_ms[1] = the transform of h_query / l_query (host clock around work that ends in a
+ * stream synchronise), h2d_bytes / d2h_bytes = bytes copied each way, launches = kernels. */
+typedef struct {
+  const uint64_t* h_query; uint64_t h_len;
+  const uint64_t* l_query; uint64_t l_len;
+  const uint64_t* delta_g1; const uint64_t* delta_g2;
+} g16_pk_delta_desc;
+typedef struct {
+  uint64_t* h_query; uint64_t h_len;
+  uint64_t* l_query; uint64_t l_len;
+  uint64_t* delta_g1; uint64_t* delta_g2;
+} g16_pk_delta_out;
+int g16_pk_contribute(g16_ctx* ctx, const g16_pk_delta_desc* in, const uint64_t* delta, uint32_t flags, uint64_t chunk_points,
+                      const g16_pk_delta_out* out);
+/* Both phases, the checker's side: the proofs of knowledge of a chain of contributions (the public keys of Bowe, Gabizon
+ * and Miers, as snarkjs and bellman's phase2 publish them).  One contribution multiplies a running G1 point D by the
+ * contributor's secret x: in phase 2 D is delta_g1 and x is delta; in phase 1 there are three chains, tau_g1[1] with x =
+ * tau, alpha_tau_g1[0] with alpha, beta_tau_g1[0] with beta.  Contributor i publishes records[i]: after_g1 = D_(i+1) =
+ * x_i D_i, a G1 point s of its choice, s_x_g1 = x_i s, and r_x_g2 = x_i r_i, where r_i (r_g2) is a G2 point
+ * hashed from the contribution's transcript.
+ * r_i MUST be derived by the checker itself from the ceremony's transcript (the hash to G2 and the file format that binds
+ * it, such as snarkjs .zkey contribution sections or bellman's params, are the caller's; this library fixes no hash).  It
+ * must never be taken from the contributor: an r whose discrete log is known makes the proof of knowledge empty.
+ * With D_0 = start_g1, the call writes 2 count equations as 4 count affine G1 points P_0, P'_0, P_1, P'_1, .. to pairs_g1
+ * and as many affine G2 points Q_0, Q'_0, .. to pairs_g2; equation k holds iff e(P_k, Q_k) = e(P'_k, Q'_k):
+ *   k = 2i      proof of knowledge   (s_i, r_x_i)   = (s_x_i, r_i)
+ *   k = 2i + 1  step                 (D_i, r_x_i)   = (D_(i+1), r_i)
+ * If all hold, D_count = (prod x_i) D_0 with x_i the discrete log of r_x_i to the base r_i, and when r_i is a random-oracle
+ * output over the contribution's transcript, contributor i knew x_i; one honest contributor then makes the product unknown.
+ * In phase 2, D_0 is the uncontributed key's delta_g1 = tau_g1[0]; with g16_pk_verify_pairs on the final key, delta is
+ * that product.  The pairings are the caller's: this library has none.
+ * The call itself checks, in one upload of every point through the GPU point check: coordinates below q, on the curve,
+ * G16_SER_VALIDATE adding [r]P = O; no point is the identity; and records[count - 1].after_g1 = end_g1.  A refusal is
+ * G16_ERR_INVALID_DATA naming the first bad point by record, then member ("records[3].r_x_g2: point is the identity",
+ * "records[4].after_g1: not end_g1", "start_g1: point is not on the curve").  G16_ERR_BAD_ARGUMENT: a null pointer, count = 0
+ * or 2^30 or more, flags other than 0 or G16_SER_VALIDATE, a proof in flight.  Nothing is written unless the call returns
+ * G16_OK.  Runs no MSM; needs no circuit or key and leaves the resident ones alone.  Afterwards g16_get_timings describes
+ * this call (every other field 0): total_ms = the whole call, h2d_ms = upload and point checks, h2d_bytes / d2h_bytes =
+ * bytes copied each way, launches = kernels. */
+typedef struct {
+  const uint64_t* after_g1; /* D_(i+1) = x_i D_i */
+  const uint64_t* s_g1;     /* a G1 point the contributor chose */
+  const uint64_t* s_x_g1;   /* x_i s */
+  const uint64_t* r_g2;     /* hash to G2 of the contribution's transcript, recomputed by the checker */
+  const uint64_t* r_x_g2;   /* x_i r */
+} g16_contribution_record;
+int g16_contribution_chain_pairs(g16_ctx* ctx, const uint64_t* start_g1, const uint64_t* end_g1,
+                                 const g16_contribution_record* records, uint32_t count, uint32_t flags, uint64_t* pairs_g1,
+                                 uint64_t* pairs_g2);
 
 /* ---- ark-serialized proving keys: `ProvingKey::serialize_{compressed,uncompressed}` / `deserialize_with_mode`
  * (data_structures.rs:125 derives them).  The bytes are a whole ProvingKey<E> as ark-serialize 0.5 writes it: vk {alpha_g1,

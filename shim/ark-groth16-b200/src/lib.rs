@@ -211,6 +211,33 @@ pub struct PowersOfTau<E: SwPairing> {
     pub beta_g2: Affine<E::G2Config>,
 }
 
+/// One contribution's public record (the public key of Bowe, Gabizon and Miers, as snarkjs and bellman's phase2 publish it):
+/// `after_g1` = x D for the running point D (phase 2: delta_g1; phase 1: tau_g1[1], alpha_tau_g1[0], beta_tau_g1[0]),
+/// `s_x_g1` = x s for a G1 point `s` of the contributor's choice, `r_x_g2` = x r.  `r_g2` must be the checker's own hash to
+/// G2 of the contribution's transcript, never a point taken from the contributor: an r with a known discrete log makes the
+/// proof of knowledge empty.  The hash and the file format that binds it are the caller's.
+pub struct ContributionRecord<E: SwPairing> {
+    pub after_g1: Affine<E::G1Config>,
+    pub s_g1: Affine<E::G1Config>,
+    pub s_x_g1: Affine<E::G1Config>,
+    pub r_g2: Affine<E::G2Config>,
+    pub r_x_g2: Affine<E::G2Config>,
+}
+impl<E: SwPairing> ContributionRecord<E> {
+    /// The contributor's record for secret `x`: `after` is its new running point, `s` its chosen point, `r` the hash to G2
+    /// of its contribution's transcript; s_x_g1 = x s and r_x_g2 = x r are formed here.
+    pub fn make(x: E::ScalarField, after: Affine<E::G1Config>, s: Affine<E::G1Config>, r: Affine<E::G2Config>) -> Self {
+        let k = x.into_bigint();
+        ContributionRecord {
+            after_g1: after,
+            s_g1: s,
+            s_x_g1: Affine::<E::G1Config>::from(s.mul_bigint(k)),
+            r_g2: r,
+            r_x_g2: Affine::<E::G2Config>::from(r.mul_bigint(k)),
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // the prover: one context = one curve on one GPU with ONE circuit and ONE proving key resident
 // ---------------------------------------------------------------------------------------------------------------------
@@ -495,7 +522,8 @@ impl<E: SwPairing> B200Prover<E> {
     }
 
     /// The GPU part of checking a powers-of-tau transcript (g16_srs_verify_pairs, snarkjs `powersoftau verify` without the
-    /// proofs of knowledge): every point is checked (curve, with `validate` the subgroup, never the identity), tau_g1[0] must
+    /// proofs of knowledge, which are `contribution_chain_pairs`): every point is checked (curve, with `validate` the subgroup,
+    /// never the identity), tau_g1[0] must
     /// be `g1` and tau_g2[0] must be `g2`, and one MSM per member under the challenge `rho` (non-zero, drawn after the
     /// transcript is fixed) reduces each member's chain to one pairing equation.  Returns the five equations as
     /// (P, Q, P', Q'); equation k holds iff e(P, Q) = e(P', Q').  A refused point is `InvalidData` (the message naming
@@ -574,9 +602,9 @@ impl<E: SwPairing> B200Prover<E> {
     }
 
     /// The GPU part of checking that `pk` is the key of the resident circuit made from the transcript `srs`
-    /// (g16_pk_verify_pairs, snarkjs `zkey verify` without the contributions' proofs of knowledge).  The library checks every
-    /// point (curve, with `validate` the subgroup), that alpha_g1, beta_g1 and beta_g2 are the transcript's, that delta and
-    /// gamma are not the identity, that gamma_g2 != delta_g2 (`uncontributed` accepts the initial key of a ceremony, where
+    /// (g16_pk_verify_pairs, snarkjs `zkey verify`; the contributions' proofs of knowledge are `contribution_chain_pairs`).
+    /// The library checks every point (curve, with `validate` the subgroup), that alpha_g1, beta_g1 and beta_g2 are the
+    /// transcript's, that delta and gamma are not the identity, that gamma_g2 != delta_g2 (`uncontributed` accepts the initial key of a ceremony, where
     /// gamma = delta = 1), and that the random combinations of a_query, b_g1_query and b_g2_query under the challenge `rho`
     /// match the transcript's.  Returns the four equations (delta, h_query, l_query, gamma_abc_g1) as (P, Q, P', Q');
     /// equation k holds iff e(P, Q) = e(P', Q').  A refusal is `InvalidData` (the message naming the member goes to
@@ -668,6 +696,124 @@ impl<E: SwPairing> B200Prover<E> {
         }
         let d = [delta];
         status(unsafe { sys::g16_setup_contribute(self.ctx, scalars_ptr(&d)) })
+    }
+
+    /// One phase-2 contribution to a key received from another party (g16_pk_contribute, snarkjs `zkey contribute`):
+    /// delta_g1 and delta_g2 times `delta`, every h_query and l_query point times delta^-1 on the GPU, in chunks of at most
+    /// `chunk_points` points (0: as many as the device memory holds).  Every other member is copied from `pk`.  Every point is
+    /// checked first (curve, with `validate` the subgroup; delta_g1 and delta_g2 not the identity): a refused point is
+    /// `InvalidData` (the message naming member and index goes to stderr).  delta = 0 is an `IoError` carrying
+    /// "UnexpectedIdentity".  Needs no circuit or key and leaves the resident ones alone.
+    pub fn contribute_key(
+        &self,
+        pk: &ProvingKey<E>,
+        delta: E::ScalarField,
+        validate: Validate,
+        chunk_points: u64,
+    ) -> Result<ProvingKey<E>, SerializationError> {
+        // packed copies, transformed in place by the library
+        let (mut hq, mut lq) = (pack_points(&pk.h_query), pack_points(&pk.l_query));
+        let (mut d1, mut d2) = (pack_points(&[pk.delta_g1]), pack_points(&[pk.vk.delta_g2]));
+        let desc = sys::g16_pk_delta_desc {
+            h_query: hq.as_ptr(),
+            h_len: pk.h_query.len() as u64,
+            l_query: lq.as_ptr(),
+            l_len: pk.l_query.len() as u64,
+            delta_g1: d1.as_ptr(),
+            delta_g2: d2.as_ptr(),
+        };
+        let out = sys::g16_pk_delta_out {
+            h_query: hq.as_mut_ptr(),
+            h_len: pk.h_query.len() as u64,
+            l_query: lq.as_mut_ptr(),
+            l_len: pk.l_query.len() as u64,
+            delta_g1: d1.as_mut_ptr(),
+            delta_g2: d2.as_mut_ptr(),
+        };
+        let d = [delta];
+        let flags = if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 };
+        ser_status(unsafe { sys::g16_pk_contribute(self.ctx, &desc, scalars_ptr(&d), flags, chunk_points, &out) })?;
+        let w1 = point_limbs::<E::G1Config>();
+        let mut key = pk.clone();
+        key.h_query = hq.chunks(w1).map(|l| unpack_point(l)).collect();
+        key.l_query = lq.chunks(w1).map(|l| unpack_point(l)).collect();
+        key.delta_g1 = unpack_point(&d1);
+        key.vk.delta_g2 = unpack_point(&d2);
+        Ok(key)
+    }
+
+    /// The proofs of knowledge of a chain of contributions (g16_contribution_chain_pairs), phase 1 or phase 2: from the
+    /// running point `start` (phase 2: the uncontributed key's delta_g1 = tau_g1[0]) to `end` (the final key's delta_g1)
+    /// through `records`.  The library checks every point (curve, with `validate` the subgroup, never the identity) and that
+    /// the last record ends at `end`; a refusal is `InvalidData` (the message naming record and member goes to stderr).
+    /// Returns 2 records.len() equations as (P, Q, P', Q'), equation k holding iff e(P, Q) = e(P', Q'): 2i is record i's
+    /// proof of knowledge (s, r_x) = (s_x, r), 2i + 1 its step (D_i, r_x) = (D_(i+1), r).  Each record's `r_g2` must have
+    /// been recomputed by the caller from the ceremony's transcript.
+    #[allow(clippy::type_complexity)]
+    pub fn contribution_chain_pairs(
+        &self,
+        start: &Affine<E::G1Config>,
+        end: &Affine<E::G1Config>,
+        records: &[ContributionRecord<E>],
+        validate: Validate,
+    ) -> Result<Vec<(Affine<E::G1Config>, Affine<E::G2Config>, Affine<E::G1Config>, Affine<E::G2Config>)>, SerializationError> {
+        let (sp, ep) = (pack_points(core::slice::from_ref(start)), pack_points(core::slice::from_ref(end)));
+        let packed: Vec<[Vec<u64>; 5]> = records
+            .iter()
+            .map(|c| {
+                [
+                    pack_points(&[c.after_g1]),
+                    pack_points(&[c.s_g1]),
+                    pack_points(&[c.s_x_g1]),
+                    pack_points(&[c.r_g2]),
+                    pack_points(&[c.r_x_g2]),
+                ]
+            })
+            .collect();
+        let descs: Vec<sys::g16_contribution_record> = packed
+            .iter()
+            .map(|p| sys::g16_contribution_record {
+                after_g1: p[0].as_ptr(),
+                s_g1: p[1].as_ptr(),
+                s_x_g1: p[2].as_ptr(),
+                r_g2: p[3].as_ptr(),
+                r_x_g2: p[4].as_ptr(),
+            })
+            .collect();
+        let (w1, w2) = (point_limbs::<E::G1Config>(), point_limbs::<E::G2Config>());
+        let n = 4 * records.len();
+        let (mut o1, mut o2) = (vec![0u64; n * w1], vec![0u64; n * w2]);
+        let flags = if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 };
+        ser_status(unsafe {
+            sys::g16_contribution_chain_pairs(
+                self.ctx,
+                sp.as_ptr(),
+                ep.as_ptr(),
+                descs.as_ptr(),
+                records.len() as u32,
+                flags,
+                o1.as_mut_ptr(),
+                o2.as_mut_ptr(),
+            )
+        })?;
+        let p = |i: usize| unpack_point::<E::G1Config>(&o1[i * w1..(i + 1) * w1]);
+        let q = |i: usize| unpack_point::<E::G2Config>(&o2[i * w2..(i + 1) * w2]);
+        Ok((0..2 * records.len()).map(|k| (p(2 * k), q(2 * k), p(2 * k + 1), q(2 * k + 1))).collect())
+    }
+
+    /// Checks a chain of contributions: `contribution_chain_pairs` with `validate` = Yes, then each equation as
+    /// `E::multi_pairing([P, -P'], [Q, Q']).is_zero()`.  Ok(true): end = (prod x_i) start, and contributor i knew x_i when
+    /// its r_g2 is a random-oracle output over its contribution's transcript, so one honest contributor makes the product
+    /// unknown.  Ok(false): an equation fails.  In phase 2, run it from tau_g1[0] to the final key's delta_g1 together with
+    /// `verify_key` on the final key.
+    pub fn verify_contribution_chain(
+        &self,
+        start: &Affine<E::G1Config>,
+        end: &Affine<E::G1Config>,
+        records: &[ContributionRecord<E>],
+    ) -> Result<bool, SerializationError> {
+        let eqs = self.contribution_chain_pairs(start, end, records, Validate::Yes)?;
+        Ok(eqs.iter().all(|(p, q, p2, q2)| E::multi_pairing([*p, -*p2], [*q, *q2]).is_zero()))
     }
 
     /// `ProvingKey::serialize_with_mode(compress)` of the resident key, encoded on the GPU (g16_pk_export_serialized).  Only

@@ -130,6 +130,37 @@ pub struct g16_pk_check_desc {
 }
 
 #[repr(C)]
+pub struct g16_pk_delta_desc {
+    pub h_query: *const u64,
+    pub h_len: u64,
+    pub l_query: *const u64,
+    pub l_len: u64,
+    pub delta_g1: *const u64,
+    pub delta_g2: *const u64,
+}
+
+#[repr(C)]
+pub struct g16_pk_delta_out {
+    pub h_query: *mut u64,
+    pub h_len: u64,
+    pub l_query: *mut u64,
+    pub l_len: u64,
+    pub delta_g1: *mut u64,
+    pub delta_g2: *mut u64,
+}
+
+/// One contribution's public record; r_g2 is recomputed by the checker from the ceremony's transcript, never taken from
+/// the contributor.
+#[repr(C)]
+pub struct g16_contribution_record {
+    pub after_g1: *const u64,
+    pub s_g1: *const u64,
+    pub s_x_g1: *const u64,
+    pub r_g2: *const u64,
+    pub r_x_g2: *const u64,
+}
+
+#[repr(C)]
 #[derive(Default, Clone, Copy)]
 pub struct g16_timings {
     pub total_ms: f32,
@@ -191,6 +222,8 @@ extern "C" {
     pub fn g16_srs_contribute(ctx: *mut g16_ctx, srs_in: *const g16_srs_desc, tau: *const u64, alpha: *const u64, beta: *const u64, flags: u32, chunk_points: u64, out: *const g16_srs_out) -> c_int;
     pub fn g16_srs_verify_pairs(ctx: *mut g16_ctx, srs: *const g16_srs_desc, g1: *const u64, g2: *const u64, rho: *const u64, flags: u32, chunk_points: u64, pairs_g1: *mut u64, pairs_g2: *mut u64) -> c_int;
     pub fn g16_pk_verify_pairs(ctx: *mut g16_ctx, srs: *const g16_srs_desc, pk: *const g16_pk_check_desc, rho: *const u64, flags: u32, pairs_g1: *mut u64, pairs_g2: *mut u64) -> c_int;
+    pub fn g16_pk_contribute(ctx: *mut g16_ctx, input: *const g16_pk_delta_desc, delta: *const u64, flags: u32, chunk_points: u64, out: *const g16_pk_delta_out) -> c_int;
+    pub fn g16_contribution_chain_pairs(ctx: *mut g16_ctx, start_g1: *const u64, end_g1: *const u64, records: *const g16_contribution_record, count: u32, flags: u32, pairs_g1: *mut u64, pairs_g2: *mut u64) -> c_int;
     pub fn g16_pk_load_serialized(ctx: *mut g16_ctx, bytes: *const u8, len: u64, flags: u32, rank: u32, world: u32, vk_out: *const g16_pk_export_desc) -> c_int;
     pub fn g16_pk_export_serialized(ctx: *mut g16_ctx, flags: u32, out: *mut u8, cap: u64, len_out: *mut u64) -> c_int;
     pub fn g16_prove(ctx: *mut g16_ctx, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32, proof_out: *mut u64) -> c_int;
