@@ -66,6 +66,11 @@ class Config(C.Structure):
                                          "ba_inv_gcd", "acc_block", "sm_count", "rank", "world")] + [("reserved", C.c_int32 * 4)]
 
 
+class ZkeyInfo(C.Structure):
+    _fields_ = [("num_inputs", C.c_uint32), ("num_constraints", C.c_uint32), ("num_witness", C.c_uint32), ("log_n", C.c_uint32),
+                ("a_nnz", C.c_uint64), ("b_nnz", C.c_uint64)]
+
+
 class WitnessReport(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("first_unsatisfied", "num_unsatisfied", "first_malformed")]
 
@@ -105,6 +110,8 @@ SIGNATURES = [
                                                C.c_uint32, C.c_void_p, C.c_void_p]),
     ("g16_pk_load_serialized", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
                                          C.POINTER(PkExportDesc)]),
+    ("g16_zkey_load", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(PkExportDesc),
+                                C.POINTER(ZkeyInfo)]),
     ("g16_pk_export_serialized", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("g16_prove", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     ("g16_prove_partial", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),

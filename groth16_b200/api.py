@@ -60,6 +60,37 @@ def _check(rc: int):
     raise ValueError(msg)
 
 
+def _zkey_num_inputs(data: bytes, nq: int) -> int:
+    """nPublic + 1 from section 2 of a .zkey, found by walking the section table; 1 when the file is too broken to say
+    (the C side then refuses it before writing anything)"""
+    mv = memoryview(data)
+    if len(mv) < 12:
+        return 1
+    pos, nsec = 12, int.from_bytes(mv[8:12], "little")
+    for _ in range(nsec):
+        if len(mv) - pos < 12:
+            return 1
+        sid, size = int.from_bytes(mv[pos:pos + 4], "little"), int.from_bytes(mv[pos + 4:pos + 12], "little")
+        pos += 12
+        if sid == 2 and size >= 4:
+            n8q = int.from_bytes(mv[pos:pos + 4], "little")
+            if n8q != 8 * nq or size < 8 + n8q:
+                return 1
+            n8r = int.from_bytes(mv[pos + 4 + n8q:pos + 8 + n8q], "little")
+            f = pos + 8 + n8q + n8r
+            if size < f + 8 - pos:
+                return 1
+            return int.from_bytes(mv[f + 4:f + 8], "little") + 1
+        pos += size
+    return 1
+
+
+def _zkey_host_refusal() -> bool:
+    """the last g16_zkey_load failure was decided on the host, before the resident circuit and key were released"""
+    msg = _lib.last_error()
+    return not (msg.startswith("coefficient") or "(byte " in msg or "is not the domain of the circuit" in msg)
+
+
 def _ptr(a: Optional[np.ndarray]):
     if a is None:
         return None
@@ -107,6 +138,18 @@ class ConstraintMatrices:
             return rp, col, np.ascontiguousarray(val)
 
         return ConstraintMatrices(num_instance, num_witness, len(a_rows), csr(a_rows), csr(b_rows), csr(c_rows))
+
+
+@dataclass
+class ZkeyCircuit:
+    """The circuit g16_zkey_load derived from a .zkey and made resident (A and B on the GPU only; a .zkey has no C).  Its
+    sizes stand in for ConstraintMatrices wherever the resident circuit's sizes are needed."""
+    num_instance_variables: int
+    num_constraints: int
+    num_witness_variables: int
+    log_n: int
+    a_nnz: int
+    b_nnz: int
 
 
 @dataclass
@@ -813,6 +856,43 @@ class Groth16:
         vk = VerifyingKey(out["alpha_g1"][0], out["beta_g2"][0], out["gamma_g2"][0], out["delta_g2"][0], out["gamma_abc_g1"])
         vk.beta_g1, vk.delta_g1 = out["beta_g1"][0], out["delta_g1"][0]
         return vk
+
+    def load_zkey(self, data: bytes, validate: bool = True, rank: int = 0, world: int = 1) -> Tuple[VerifyingKey, ZkeyCircuit]:
+        """g16_zkey_load: make the circuit (A and B; under CircomReduction) and the proving key of a snarkjs .zkey resident in
+        one call, the GPU counterpart of ark-circom's read_zkey followed by Groth16<E, CircomReduction>.  Sets this
+        context's reduction to "circom".  Returns the verifying key (beta_g1 / delta_g1 on the side as attributes) and the
+        derived circuit sizes.  A malformed file raises serialize.DeserializeError naming the first bad item (the previous
+        circuit and key stay resident when the file's structure or header is refused, none when a coefficient or point is);
+        another curve's context raises ValueError."""
+        buf = np.frombuffer(data, dtype=np.uint8)
+        nq, ng2 = self.nq, self.ng2
+        z = lambda rows, w: np.zeros((rows, w), dtype=np.uint64)
+        # gamma_abc_g1 holds nPublic + 1 points: read nPublic from the header when it is there, the C side checks the rest
+        ni = _zkey_num_inputs(data, nq)
+        out = dict(alpha_g1=z(1, 2 * nq), beta_g1=z(1, 2 * nq), delta_g1=z(1, 2 * nq), beta_g2=z(1, ng2),
+                   gamma_g2=z(1, ng2), delta_g2=z(1, ng2), gamma_abc_g1=z(ni, 2 * nq))
+        d = _lib.PkExportDesc()
+        for k, v in out.items():
+            setattr(d, k, _u64p(v) if v.size else None)
+        info = _lib.ZkeyInfo()
+        flags = _lib.SER_VALIDATE if validate else 0
+        rc = self._lib.g16_zkey_load(self._ctx, buf.ctypes.data_as(C.c_void_p) if buf.size else None, buf.size, flags, rank,
+                                     world, C.byref(d), C.byref(info))
+        if rc not in (_lib.G16_OK, _lib.ERR_BAD_ARGUMENT, _lib.ERR_POLYNOMIAL_DEGREE_TOO_LARGE) and not _zkey_host_refusal():
+            self._matrices = None
+            self._pk_resident = False
+            self._pk_obj = None
+        _check(rc)
+        self.qap = "circom"
+        self._matrices = ZkeyCircuit(info.num_inputs, info.num_constraints, info.num_witness, info.log_n, info.a_nnz,
+                                     info.b_nnz)
+        self._pk_resident = True
+        self._pk_obj = None
+        self.world = world
+        vk = VerifyingKey(out["alpha_g1"][0], out["beta_g2"][0], out["gamma_g2"][0], out["delta_g2"][0],
+                          out["gamma_abc_g1"][:info.num_inputs])
+        vk.beta_g1, vk.delta_g1 = out["beta_g1"][0], out["delta_g1"][0]
+        return vk, self._matrices
 
     def export_proving_key_bytes(self, compress: bool = True) -> bytes:
         """g16_pk_export_serialized: the resident key (made by generate_parameters_with_qap) as ark-serialize writes it,

@@ -99,6 +99,10 @@ const char* g16_last_error(void) { return last_error_ref().c_str(); }
 
 #define CTX_OR_FAIL(ctx) \
   if (!(ctx) || !(ctx)->eng) return fail(G16_ERR_BAD_ARGUMENT, "null context")
+// the calls that read matrix C refuse a circuit loaded by g16_zkey_load, which has none
+#define NEEDS_C(ctx, cond)                        \
+  if ((cond) && (ctx)->eng->circuit_without_c)    \
+  return fail(G16_ERR_BAD_ARGUMENT, "the resident circuit came from a .zkey, which holds no C matrix")
 
 int g16_fq_limbs(const g16_ctx* ctx) { return (ctx && ctx->eng) ? ctx->eng->fq_limbs() : 0; }
 int g16_fr_limbs(const g16_ctx* ctx) { return (ctx && ctx->eng) ? ctx->eng->fr_limbs() : 0; }
@@ -139,6 +143,7 @@ int g16_pk_load(g16_ctx* ctx, const g16_pk_desc* pk, uint32_t rank, uint32_t wor
 int g16_setup(g16_ctx* ctx, const uint64_t* alpha, const uint64_t* beta, const uint64_t* gamma, const uint64_t* delta,
               const uint64_t* tau, const uint64_t* g1, const uint64_t* g2) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, true);
   return ctx->eng->setup(alpha, beta, gamma, delta, tau, g1, g2);
 }
 int g16_pk_export(g16_ctx* ctx, const g16_pk_export_desc* out) {
@@ -147,6 +152,7 @@ int g16_pk_export(g16_ctx* ctx, const g16_pk_export_desc* out) {
 }
 int g16_setup_from_srs(g16_ctx* ctx, const g16_srs_desc* srs, uint32_t flags) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, true);
   return ctx->eng->setup_from_srs(srs, flags);
 }
 int g16_setup_contribute(g16_ctx* ctx, const uint64_t* delta) {
@@ -171,6 +177,7 @@ int g16_srs_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const uint64_t* 
 int g16_pk_verify_pairs(g16_ctx* ctx, const g16_srs_desc* srs, const g16_pk_check_desc* pk, const uint64_t* rho, uint32_t flags,
                         uint64_t* pairs_g1, uint64_t* pairs_g2) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, true);
   return ctx->eng->pk_verify_pairs(srs, pk, rho, flags, pairs_g1, pairs_g2);
 }
 int g16_pk_contribute(g16_ctx* ctx, const g16_pk_delta_desc* in, const uint64_t* delta, uint32_t flags, uint64_t chunk_points,
@@ -189,16 +196,23 @@ int g16_pk_load_serialized(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uin
   CTX_OR_FAIL(ctx);
   return ctx->eng->pk_load_serialized(bytes, len, flags, rank, world, vk_out);
 }
+int g16_zkey_load(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
+                  const g16_pk_export_desc* vk_out, g16_zkey_info* info_out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->zkey_load(bytes, len, flags, rank, world, vk_out, info_out);
+}
 int g16_pk_export_serialized(g16_ctx* ctx, uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) {
   CTX_OR_FAIL(ctx);
   return ctx->eng->pk_export_serialized(flags, out, cap, len_out);
 }
 int g16_prove(g16_ctx* ctx, const uint64_t* r, const uint64_t* s, const uint64_t* full_assignment, uint32_t flags, uint64_t* proof_out) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, flags & G16_CHECK_WITNESS);
   return ctx->eng->prove(r, s, full_assignment, flags, proof_out);
 }
 int g16_prove_partial(g16_ctx* ctx, const uint64_t* r, const uint64_t* full_assignment, uint32_t flags, uint64_t* partial_out) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, flags & G16_CHECK_WITNESS);
   return ctx->eng->prove_partial(r, full_assignment, flags, partial_out);
 }
 int g16_prove_assemble(g16_ctx* ctx, const uint64_t* r, const uint64_t* s, const uint64_t* partials, uint32_t nparts, uint64_t* proof_out) {
@@ -211,6 +225,7 @@ int g16_prove_assemble_prepare(g16_ctx* ctx, const uint64_t* r, const uint64_t* 
 }
 int g16_prove_submit(g16_ctx* ctx, int slot, const uint64_t* r, const uint64_t* s, const uint64_t* full_assignment, uint32_t flags) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, flags & G16_CHECK_WITNESS);
   return ctx->eng->prove_submit(slot, r, s, full_assignment, flags);
 }
 int g16_prove_wait(g16_ctx* ctx, int slot, uint64_t* proof_out) {
@@ -220,10 +235,12 @@ int g16_prove_wait(g16_ctx* ctx, int slot, uint64_t* proof_out) {
 int g16_prove_batch(g16_ctx* ctx, uint32_t count, const uint64_t* r, const uint64_t* s, const uint64_t* full_assignments,
                     uint32_t group, uint32_t flags, uint64_t* proofs_out) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, flags & G16_CHECK_WITNESS);
   return ctx->eng->prove_batch(count, r, s, full_assignments, group, flags, proofs_out);
 }
 int g16_prove_partial_submit(g16_ctx* ctx, int slot, const uint64_t* r, const uint64_t* full_assignment, uint32_t flags) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, flags & G16_CHECK_WITNESS);
   return ctx->eng->partial_submit(slot, r, full_assignment, flags);
 }
 int g16_prove_partial_wait(g16_ctx* ctx, int slot, uint64_t* partial_out) {
@@ -232,11 +249,13 @@ int g16_prove_partial_wait(g16_ctx* ctx, int slot, uint64_t* partial_out) {
 }
 int g16_witness_map(g16_ctx* ctx, const uint64_t* full_assignment, uint32_t flags, uint64_t* h_out) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, flags & G16_CHECK_WITNESS);
   return ctx->eng->witness_map(full_assignment, flags, h_out);
 }
 int g16_check_witness(g16_ctx* ctx, uint32_t count, const uint64_t* full_assignments, uint32_t flags,
                       g16_witness_report* reports_out) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, true);
   return ctx->eng->check_witness(count, full_assignments, flags, reports_out);
 }
 int g16_get_timings(const g16_ctx* ctx, g16_timings* out) {
@@ -264,6 +283,7 @@ int g16_comm_init(g16_ctx* ctx, const uint8_t* id128, uint32_t rank, uint32_t wo
 }
 int g16_prove_sharded_submit(g16_ctx* ctx, int slot, const uint64_t* r, const uint64_t* s, const uint64_t* full_assignment, uint32_t flags) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, flags & G16_CHECK_WITNESS);
   return ctx->eng->sharded_submit(slot, r, s, full_assignment, flags);
 }
 int g16_prove_sharded_wait(g16_ctx* ctx, int slot, uint64_t* proof_out) {
@@ -272,6 +292,7 @@ int g16_prove_sharded_wait(g16_ctx* ctx, int slot, uint64_t* proof_out) {
 }
 int g16_prove_sharded(g16_ctx* ctx, const uint64_t* r, const uint64_t* s, const uint64_t* full_assignment, uint32_t flags, uint64_t* proof_out) {
   CTX_OR_FAIL(ctx);
+  NEEDS_C(ctx, flags & G16_CHECK_WITNESS);
   const int rc = ctx->eng->sharded_submit(0, r, s, full_assignment, flags);
   if (rc) return rc;
   return ctx->eng->sharded_wait(0, proof_out);

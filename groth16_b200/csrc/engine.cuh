@@ -31,6 +31,7 @@
 #include "ntt.cuh"
 #include "ser.cuh"
 #include "srs.cuh"
+#include "zkey.cuh"
 
 namespace g16 {
 
@@ -161,6 +162,8 @@ struct IEngine {
   virtual int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                                  const g16_pk_export_desc* vk_out) = 0;
   virtual int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) = 0;
+  virtual int zkey_load(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
+                        const g16_pk_export_desc* vk_out, g16_zkey_info* info_out) = 0;
   virtual int prove(const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags, uint64_t* proof) = 0;
   virtual int prove_partial(const uint64_t* r, const uint64_t* z, uint32_t flags, uint64_t* partial) = 0;
   virtual int prove_assemble(const uint64_t* r, const uint64_t* s, const uint64_t* partials, uint32_t nparts, uint64_t* proof) = 0;
@@ -181,6 +184,8 @@ struct IEngine {
   virtual int get_option(const char* key, long long* value) const = 0;
   virtual int get_config(g16_config* out) const = 0;
   g16_timings tm{};
+  // the resident circuit came from a .zkey: matrix C is resident empty, and the calls that read it refuse (api.cu)
+  bool circuit_without_c = false;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -842,6 +847,7 @@ struct Engine : IEngine {
     }
     drop_key();
     have_circuit = false;
+    circuit_without_c = false;
     for (int m = 0; m < 3; m++) {
       const uint32_t nnz = ms[m]->row_ptr[nc];
       h_rp[m].assign(ms[m]->row_ptr, ms[m]->row_ptr + nc + 1);
@@ -2117,6 +2123,8 @@ struct Engine : IEngine {
     cudaEvent_t ev_h2d[2] = {}, ev_dec[2] = {};
     uint8_t* host[2] = {};
     DevBuf dev[2], aux, err;
+    uint64_t chunks = 0, h2d_bytes = 0;   // chunks staged so far (buffer chunks & 1 is next), bytes copied up
+    unsigned long long launches = 0;      // kernels
     ~SerStaging() {
       if (st_dec) cudaStreamSynchronize(st_dec);
       if (st_copy) cudaStreamSynchronize(st_copy);
@@ -2129,6 +2137,108 @@ struct Engine : IEngine {
       if (st_copy) cudaStreamDestroy(st_copy);
     }
   };
+  // host-bound points in sg.aux: the seven single points, element 0 of a / b_g1 / b_g2, gamma_abc_g1
+  enum { AUX_A0 = 7, AUX_B10 = 8, AUX_B20 = 9, AUX_ABC = 10 };
+  static size_t ser_aux_bytes(uint64_t n_abc) { return AUX_ABC * sizeof(A2) + (size_t)n_abc * sizeof(A1); }
+  // streams, events, the error word (all ones: no error) and zeroed aux; two pinned and two device buffers of `stage` bytes
+  int ser_staging_init(SerStaging& sg, size_t stage, size_t aux_bytes) {
+    G16_CUDA(cudaStreamCreateWithFlags(&sg.st_copy, cudaStreamNonBlocking));
+    G16_CUDA(cudaStreamCreateWithFlags(&sg.st_dec, cudaStreamNonBlocking));
+    // reset on the decode stream itself: st_dec does not wait for the legacy default stream, so a plain cudaMemset there
+    // could land after the first decodes and wipe their points or their error
+    G16_CUDA(sg.aux.reserve(aux_bytes));
+    G16_CUDA(cudaMemsetAsync(sg.aux.p, 0, aux_bytes, sg.st_dec));
+    G16_CUDA(sg.err.reserve(8));
+    G16_CUDA(cudaMemsetAsync(sg.err.p, 0xff, 8, sg.st_dec));
+    for (int k = 0; k < 2; k++) {
+      G16_CUDA(cudaEventCreateWithFlags(&sg.ev_h2d[k], cudaEventDisableTiming));
+      G16_CUDA(cudaEventCreateWithFlags(&sg.ev_dec[k], cudaEventDisableTiming));
+      G16_CUDA(cudaHostAlloc((void**)&sg.host[k], stage + 1, cudaHostAllocDefault));
+      G16_CUDA(sg.dev[k].reserve(stage + 1));
+    }
+    return G16_OK;
+  }
+  // Copies bytes [src, src + n) of the host stream to dst (null: device staging buffer chunks & 1) through pinned buffer
+  // chunks & 1, so that the copy of chunk i + 1 overlaps the kernel of chunk i.  On return st_dec waits for the copy: the
+  // caller enqueues the chunk's kernel there, then ser_chunk_done.
+  int ser_chunk_upload(SerStaging& sg, const uint8_t* src, size_t n, void* dst) {
+    const int k = (int)(sg.chunks & 1);
+    if (sg.chunks >= 2) G16_CUDA(cudaEventSynchronize(sg.ev_h2d[k]));   // pinned buffer k is free again
+    memcpy(sg.host[k], src, n);
+    if (sg.chunks >= 2) G16_CUDA(cudaStreamWaitEvent(sg.st_copy, sg.ev_dec[k], 0));   // the kernel that read dev[k] is done
+    G16_CUDA(cudaMemcpyAsync(dst ? dst : sg.dev[k].p, sg.host[k], n, cudaMemcpyHostToDevice, sg.st_copy));
+    G16_CUDA(cudaEventRecord(sg.ev_h2d[k], sg.st_copy));
+    G16_CUDA(cudaStreamWaitEvent(sg.st_dec, sg.ev_h2d[k], 0));
+    sg.h2d_bytes += n;
+    return G16_OK;
+  }
+  int ser_chunk_done(SerStaging& sg) {
+    G16_CUDA(cudaEventRecord(sg.ev_dec[sg.chunks & 1], sg.st_dec));
+    sg.chunks++;
+    sg.launches++;
+    return G16_OK;
+  }
+  // Decodes the points of `plan` (MONT: the .zkey encoding, else the ark one `flags` selects) into this rank's bases of
+  // every query and the host-bound points of sg.aux, as g16_pk_load places them.  place = false only checks them.  A refused
+  // point lands in sg.err.
+  template <bool MONT>
+  int ser_decode_points(SerStaging& sg, const uint8_t* bytes, const SerItem it[SER_ITEMS], const std::vector<SerChunk>& plan,
+                        uint32_t flags, bool place) {
+    auto aux_at = [&](int slot) { return (char*)sg.aux.p + (size_t)slot * sizeof(A2); };
+    for (const SerChunk& c : plan) {
+      const SerItem& x = it[c.member];
+      int rc = ser_chunk_upload(sg, bytes + c.off, (size_t)c.count * x.psize, nullptr);
+      if (rc) return rc;
+      SerDest d;
+      d.rank = rank;
+      d.world = world;
+      d.aux_n = 1;
+      switch (c.member) {
+        case SER_GAMMA_ABC: d.aux = aux_at(AUX_ABC); d.aux_n = x.len; break;
+        case SER_A: d.aux = aux_at(AUX_A0); d.bases = q[M_A].bases.p; d.skip = 1; d.pairs = q[M_A].pairs; break;
+        case SER_B_G1: d.aux = aux_at(AUX_B10); d.bases = q[M_B1].bases.p; d.skip = 1; d.pairs = q[M_B1].pairs; break;
+        case SER_B_G2: d.aux = aux_at(AUX_B20); d.bases = q[M_B2].bases.p; d.skip = 1; d.pairs = q[M_B2].pairs; break;
+        case SER_H: d.aux_n = 0; d.bases = q[M_H].bases.p; d.pairs = q[M_H].pairs; break;
+        case SER_L: d.aux_n = 0; d.bases = q[M_L].bases.p; d.pairs = q[M_L].pairs; break;
+        default: d.aux = aux_at(c.member); break;   // single points: slots 0 .. 6 in stream order
+      }
+      if (!place) d = SerDest{};
+      const uint8_t* src = sg.dev[sg.chunks & 1].template as<uint8_t>();
+      unsigned long long* err = sg.err.template as<unsigned long long>();
+      const cudaError_t e = x.g2 ? ser_decode_enqueue<CP, true, MONT>(sg.st_dec, src, c.first, c.count, flags, c.off, d, err)
+                                 : ser_decode_enqueue<CP, false, MONT>(sg.st_dec, src, c.first, c.count, flags, c.off, d, err);
+      G16_CUDA(e);
+      if ((rc = ser_chunk_done(sg))) return rc;
+    }
+    return G16_OK;
+  }
+  // After the decodes: the single points from sg.aux into the key, commit_key, and the verifying key into vk (if non-null)
+  int ser_commit(SerStaging& sg, const g16_pk_export_desc* vk) {
+    const size_t aux_bytes = ser_aux_bytes(num_inputs);
+    std::vector<char> aux(aux_bytes);
+    G16_CUDA(cudaMemcpy(aux.data(), sg.aux.p, aux_bytes, cudaMemcpyDeviceToHost));
+    auto a1 = [&](int slot) { A1 r; memcpy(&r, aux.data() + (size_t)slot * sizeof(A2), sizeof(A1)); return r; };
+    auto a2 = [&](int slot) { A2 r; memcpy(&r, aux.data() + (size_t)slot * sizeof(A2), sizeof(A2)); return r; };
+    alpha_g1 = a1(SER_ALPHA_G1); beta_g1 = a1(SER_BETA_G1); delta_g1 = a1(SER_DELTA_G1);
+    beta_g2 = a2(SER_BETA_G2); delta_g2 = a2(SER_DELTA_G2);
+    int rc = commit_key(a1(AUX_A0), a1(AUX_B10), a2(AUX_B20), false);
+    if (rc) return rc;
+    if (vk) {
+      store_vk_points(vk, a2(SER_GAMMA_G2));
+      if (vk->gamma_abc_g1)
+        for (uint32_t i = 0; i < num_inputs; i++) {
+          A1 p;
+          memcpy(&p, aux.data() + AUX_ABC * sizeof(A2) + (size_t)i * sizeof(A1), sizeof(A1));
+          store_a1(vk->gamma_abc_g1 + (size_t)i * 2 * NQ64, p);
+        }
+    }
+    return G16_OK;
+  }
+  static size_t ser_stage_bytes(const SerItem it[SER_ITEMS], const std::vector<SerChunk>& plan) {
+    size_t stage = 0;
+    for (const SerChunk& c : plan) stage = std::max<size_t>(stage, (size_t)c.count * it[c.member].psize);
+    return stage;
+  }
   int pk_load_serialized(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rk, uint32_t wd,
                          const g16_pk_export_desc* vk) override {
     using Fmt = SerFormat<CP>;
@@ -2149,59 +2259,10 @@ struct Engine : IEngine {
     const uint64_t qlen[5] = {it[SER_H].len, it[SER_L].len, it[SER_A].len, it[SER_B_G1].len, it[SER_B_G2].len};
     int rc = begin_key(rk, wd, qlen);   // the same truncation and shards as g16_pk_load
     if (rc) return rc;
-    // host-bound points: the seven single points, element 0 of a / b_g1 / b_g2, gamma_abc_g1
-    enum { AUX_A0 = 7, AUX_B10 = 8, AUX_B20 = 9, AUX_ABC = 10 };
-    const size_t aux_bytes = AUX_ABC * sizeof(A2) + (size_t)num_inputs * sizeof(A1);
-    SerStaging sg;
-    G16_CUDA(cudaStreamCreateWithFlags(&sg.st_copy, cudaStreamNonBlocking));
-    G16_CUDA(cudaStreamCreateWithFlags(&sg.st_dec, cudaStreamNonBlocking));
-    // reset on the decode stream itself: st_dec does not wait for the legacy default stream, so a plain cudaMemset there
-    // could land after the first decodes and wipe their points or their error
-    G16_CUDA(sg.aux.reserve(aux_bytes));
-    G16_CUDA(cudaMemsetAsync(sg.aux.p, 0, aux_bytes, sg.st_dec));
-    G16_CUDA(sg.err.reserve(8));
-    G16_CUDA(cudaMemsetAsync(sg.err.p, 0xff, 8, sg.st_dec));
-    auto aux_at = [&](int slot) { return (char*)sg.aux.p + (size_t)slot * sizeof(A2); };
     const std::vector<SerChunk> plan = ser_plan(it, SER_CHUNK);
-    size_t stage = 0;
-    for (const SerChunk& c : plan) stage = std::max<size_t>(stage, (size_t)c.count * it[c.member].psize);
-    for (int k = 0; k < 2; k++) {
-      G16_CUDA(cudaEventCreateWithFlags(&sg.ev_h2d[k], cudaEventDisableTiming));
-      G16_CUDA(cudaEventCreateWithFlags(&sg.ev_dec[k], cudaEventDisableTiming));
-      G16_CUDA(cudaHostAlloc((void**)&sg.host[k], stage + 1, cudaHostAllocDefault));
-      G16_CUDA(sg.dev[k].reserve(stage + 1));
-    }
-    for (size_t ci = 0; ci < plan.size(); ci++) {
-      const SerChunk& c = plan[ci];
-      const SerItem& x = it[c.member];
-      const int k = (int)(ci & 1);
-      const size_t nbytes = (size_t)c.count * x.psize;
-      if (ci >= 2) G16_CUDA(cudaEventSynchronize(sg.ev_h2d[k]));   // staging buffer k is free again
-      memcpy(sg.host[k], bytes + c.off, nbytes);
-      if (ci >= 2) G16_CUDA(cudaStreamWaitEvent(sg.st_copy, sg.ev_dec[k], 0));   // the decode that read dev[k] is done
-      G16_CUDA(cudaMemcpyAsync(sg.dev[k].p, sg.host[k], nbytes, cudaMemcpyHostToDevice, sg.st_copy));
-      G16_CUDA(cudaEventRecord(sg.ev_h2d[k], sg.st_copy));
-      G16_CUDA(cudaStreamWaitEvent(sg.st_dec, sg.ev_h2d[k], 0));
-      SerDest d;
-      d.rank = rank;
-      d.world = world;
-      d.aux_n = 1;
-      switch (c.member) {
-        case SER_GAMMA_ABC: d.aux = aux_at(AUX_ABC); d.aux_n = x.len; break;
-        case SER_A: d.aux = aux_at(AUX_A0); d.bases = q[M_A].bases.p; d.skip = 1; d.pairs = q[M_A].pairs; break;
-        case SER_B_G1: d.aux = aux_at(AUX_B10); d.bases = q[M_B1].bases.p; d.skip = 1; d.pairs = q[M_B1].pairs; break;
-        case SER_B_G2: d.aux = aux_at(AUX_B20); d.bases = q[M_B2].bases.p; d.skip = 1; d.pairs = q[M_B2].pairs; break;
-        case SER_H: d.aux_n = 0; d.bases = q[M_H].bases.p; d.pairs = q[M_H].pairs; break;
-        case SER_L: d.aux_n = 0; d.bases = q[M_L].bases.p; d.pairs = q[M_L].pairs; break;
-        default: d.aux = aux_at(c.member); break;   // single points: slots 0 .. 6 in stream order
-      }
-      const uint8_t* src = sg.dev[k].template as<uint8_t>();
-      unsigned long long* err = sg.err.template as<unsigned long long>();
-      const cudaError_t e = x.g2 ? ser_decode_enqueue<CP, true>(sg.st_dec, src, c.first, c.count, flags, c.off, d, err)
-                                 : ser_decode_enqueue<CP, false>(sg.st_dec, src, c.first, c.count, flags, c.off, d, err);
-      G16_CUDA(e);
-      G16_CUDA(cudaEventRecord(sg.ev_dec[k], sg.st_dec));
-    }
+    SerStaging sg;
+    if ((rc = ser_staging_init(sg, ser_stage_bytes(it, plan), ser_aux_bytes(num_inputs)))) return rc;
+    if ((rc = ser_decode_points<false>(sg, bytes, it, plan, flags, true))) return rc;
     G16_CUDA(cudaStreamSynchronize(sg.st_dec));
     unsigned long long first_err = 0;
     G16_CUDA(cudaMemcpy(&first_err, sg.err.p, 8, cudaMemcpyDeviceToHost));
@@ -2209,23 +2270,147 @@ struct Engine : IEngine {
       const uint64_t off = first_err >> 8;
       return fail(G16_ERR_INVALID_DATA, ser_locate(it, off) + " (byte " + std::to_string(off) + "): " + ser_reason(first_err & 0xff));
     }
-    std::vector<char> aux(aux_bytes);
-    G16_CUDA(cudaMemcpy(aux.data(), sg.aux.p, aux_bytes, cudaMemcpyDeviceToHost));
-    auto a1 = [&](int slot) { A1 r; memcpy(&r, aux.data() + (size_t)slot * sizeof(A2), sizeof(A1)); return r; };
-    auto a2 = [&](int slot) { A2 r; memcpy(&r, aux.data() + (size_t)slot * sizeof(A2), sizeof(A2)); return r; };
-    alpha_g1 = a1(SER_ALPHA_G1); beta_g1 = a1(SER_BETA_G1); delta_g1 = a1(SER_DELTA_G1);
-    beta_g2 = a2(SER_BETA_G2); delta_g2 = a2(SER_DELTA_G2);
-    if ((rc = commit_key(a1(AUX_A0), a1(AUX_B10), a2(AUX_B20), false))) return rc;
-    if (vk) {
-      store_vk_points(vk, a2(SER_GAMMA_G2));
-      if (vk->gamma_abc_g1)
-        for (uint32_t i = 0; i < num_inputs; i++) {
-          A1 p;
-          memcpy(&p, aux.data() + AUX_ABC * sizeof(A2) + (size_t)i * sizeof(A1), sizeof(A1));
-          store_a1(vk->gamma_abc_g1 + (size_t)i * 2 * NQ64, p);
+    return ser_commit(sg, vk);
+  }
+
+  // ---- snarkjs .zkey files (zkey.cuh): the circuit's A and B and its key in one call ----
+  // Host: zkey_walk decides the section table, every size and the header before anything resident is released.  Device,
+  // on the staging streams: the coefficient section goes chunk by chunk into one device copy, each chunk decoded in place
+  // (zkey_coef_kernel); then the circuit is derived from the largest constraint index and the CSR arrays are built
+  // (zkey_csr_enqueue) while the points are decoded and placed like an ark key's.  Every refusal after the host checks
+  // leaves neither a circuit nor a key resident.
+  int zkey_load(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rk, uint32_t wd, const g16_pk_export_desc* vk,
+                g16_zkey_info* info) override {
+    if constexpr (CP::CURVE_ID != 0 && CP::CURVE_ID != 1) {
+      return fail(G16_ERR_BAD_ARGUMENT, "snarkjs .zkey files exist for BN254 and BLS12-381 only");
+    } else {
+      if ((!bytes && len) || wd == 0 || rk >= wd) return fail(G16_ERR_BAD_ARGUMENT, "bad bytes / rank / world");
+      if (flags & ~(uint32_t)G16_SER_VALIDATE) return fail(G16_ERR_BAD_ARGUMENT, "g16_zkey_load takes G16_SER_VALIDATE only");
+      if (vk && (vk->a_query || vk->b_g1_query || vk->b_g2_query || vk->h_query || vk->l_query))
+        return fail(G16_ERR_BAD_ARGUMENT, "vk_out receives the verifying key only: its query members must be NULL");
+      G16_NOT_BUSY();
+      ZkeyLayout z;
+      const std::string why = zkey_walk<CP>(bytes, len, z);
+      if (!why.empty()) return fail(G16_ERR_INVALID_DATA, why);
+      int Ln = 0;
+      while ((1u << Ln) < z.domain_size) Ln++;
+      int rc = check_log((uint32_t)Ln);
+      if (rc) return rc;
+      if (Ln + 1 > CP::FrP::TWO_ADICITY)
+        return fail(G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "CircomReduction needs a domain of twice the size, which exceeds the field's two-adicity (PolynomialDegreeTooLarge)");
+      G16_CUDA(cudaSetDevice(device));
+      const auto t0 = std::chrono::steady_clock::now();
+      const unsigned long long launches0 = ntt_launches + ctr.launches;
+      tm = g16_timings{};
+      // from here on a refusal leaves neither a circuit nor a key resident
+      drop_key();
+      have_circuit = false;
+      circuit_without_c = true;
+      for (int m = 0; m < 3; m++) { h_rp[m].clear(); h_col[m].clear(); h_val[m].clear(); }
+      const uint32_t ds = z.domain_size;
+      const std::vector<SerChunk> plan = ser_plan(z.it, SER_CHUNK);
+      SerStaging sg;
+      if ((rc = ser_staging_init(sg, std::max<size_t>(ser_stage_bytes(z.it, plan), (size_t)SER_CHUNK * z.rs),
+                                 ser_aux_bytes(z.npub + 1ull))))
+        return rc;
+      // coefficients: every record into one device copy, decoded in place chunk by chunk
+      DevBuf d_rec, d_counts, d_small;
+      G16_CUDA(d_rec.reserve((size_t)z.ncoefs * z.rs + 4));
+      G16_CUDA(d_counts.reserve((size_t)2 * ds * 4));
+      G16_CUDA(d_small.reserve(8));   // row_end, then pub_err
+      G16_CUDA(cudaMemsetAsync(d_counts.p, 0, (size_t)2 * ds * 4, sg.st_dec));
+      G16_CUDA(cudaMemsetAsync(d_small.p, 0, 4, sg.st_dec));
+      G16_CUDA(cudaMemsetAsync((char*)d_small.p + 4, 0xff, 4, sg.st_dec));
+      uint8_t* rec = d_rec.template as<uint8_t>();
+      uint32_t* counts = d_counts.template as<uint32_t>();
+      uint32_t* row_end = d_small.template as<uint32_t>();
+      uint32_t* pub_err = row_end + 1;
+      unsigned long long* err = sg.err.template as<unsigned long long>();
+      for (uint64_t f = 0; f < z.ncoefs; f += SER_CHUNK) {
+        const uint32_t cnt = (uint32_t)std::min<uint64_t>(SER_CHUNK, z.ncoefs - f);
+        if ((rc = ser_chunk_upload(sg, bytes + z.coef_off + f * z.rs, (size_t)cnt * z.rs, rec + f * z.rs))) return rc;
+        G16_CUDA(zkey_coef_enqueue<Fr>(sg.st_dec, rec + f * z.rs, cnt, z.rs, z.coef_off + f * z.rs, ds, z.nvars, counts, row_end, err));
+        if ((rc = ser_chunk_done(sg))) return rc;
+      }
+      uint32_t small[2];
+      unsigned long long coef_err = 0;
+      G16_CUDA(cudaStreamSynchronize(sg.st_dec));
+      G16_CUDA(cudaMemcpy(small, d_small.p, 8, cudaMemcpyDeviceToHost));
+      G16_CUDA(cudaMemcpy(&coef_err, sg.err.p, 8, cudaMemcpyDeviceToHost));
+      uint32_t nc = 0;
+      std::string derived;   // why the coefficients do not make a circuit of this file, decided once every item has passed
+      if (coef_err == ~0ull) derived = zkey_derive(z, small[0], &nc);
+      const bool place = coef_err == ~0ull && derived.empty();
+      uint64_t nnz[2] = {0, 0};
+      uint32_t nnz_u32[2] = {0, 0};
+      if (place) {
+        // the circuit: A and B in CSR, C resident empty, the CircomReduction domain
+        num_inputs = z.npub + 1; num_constraints = nc; num_witness = z.nvars - z.npub - 1; L = Ln; qap = G16_QAP_CIRCOM;
+        for (int m = 0; m < 3; m++) {
+          G16_CUDA(csr_rp[m].reserve((size_t)(nc + 1) * 4));
+          G16_CUDA(cudaMemsetAsync(csr_rp[m].p, 0, (size_t)(nc + 1) * 4, sg.st_dec));
         }
+        DevBuf block_tot;
+        G16_CUDA(block_tot.reserve(((size_t)nc + 1 + 1023) / 1024 * 4 + 4));
+        G16_CUDA(zkey_row_ptr_enqueue(sg.st_dec, counts, nc, z.npub, ds, csr_rp[0].template as<uint32_t>(),
+                                      csr_rp[1].template as<uint32_t>(), block_tot.template as<uint32_t>(), pub_err, &sg.launches));
+        for (int m = 0; m < 2; m++)   // the sizes of col / val: the last entry of each row_ptr
+          G16_CUDA(cudaMemcpyAsync(&nnz_u32[m], csr_rp[m].template as<uint32_t>() + nc, 4, cudaMemcpyDeviceToHost, sg.st_dec));
+        G16_CUDA(cudaStreamSynchronize(sg.st_dec));
+        for (int m = 0; m < 3; m++) {
+          const uint64_t e = m < 2 ? nnz_u32[m] : 0;
+          if (m < 2) nnz[m] = e;
+          G16_CUDA(csr_col[m].reserve((size_t)e * 4 + 4));
+          G16_CUDA(csr_val[m].reserve((size_t)e * sizeof(Fr) + sizeof(Fr)));
+        }
+        const ZkeyCsr ca{csr_rp[0].template as<uint32_t>(), csr_col[0].template as<uint32_t>(), csr_val[0].p};
+        const ZkeyCsr cb{csr_rp[1].template as<uint32_t>(), csr_col[1].template as<uint32_t>(), csr_val[1].p};
+        G16_CUDA(zkey_scatter_enqueue<Fr>(sg.st_dec, rec, z.ncoefs, SER_CHUNK, z.rs, nc, ds, counts, ca, cb, pub_err, &sg.launches));
+        G16_CUDA(cudaStreamSynchronize(sg.st_dec));
+        // the records and counts are done with: freed before begin_key reserves the bases and commit_key weighs the free
+        // memory (a 2^24 circuit's records take gigabytes)
+        d_rec.release();
+        d_counts.release();
+        G16_CUDA(cudaMemcpy(&small[1], pub_err, 4, cudaMemcpyDeviceToHost));
+        if (small[1] != UINT32_MAX) {
+          const uint32_t s = small[1] >> 1;
+          return fail(G16_ERR_INVALID_DATA, "coefficients: public-input row " + std::to_string(s) +
+                                                (small[1] & 1 ? " of B is not empty" : " of A is not {(" + std::to_string(s) + ", 1)}"));
+        }
+        G16_CUDA(S0.d_z.reserve((size_t)z.nvars * sizeof(Fr)));
+        if ((rc = ensure_circuit_domain())) return rc;
+        // the key, placed for this circuit
+        const uint64_t qlen[5] = {z.it[SER_H].len, z.it[SER_L].len, z.it[SER_A].len, z.it[SER_B_G1].len, z.it[SER_B_G2].len};
+        if ((rc = begin_key(rk, wd, qlen))) return rc;
+      }
+      const auto t2 = std::chrono::steady_clock::now();
+      // the points: placed when the circuit stands, otherwise only checked, so that the first bad item in the file is named
+      if ((rc = ser_decode_points<true>(sg, bytes, z.it, plan, flags, place))) return rc;
+      G16_CUDA(cudaStreamSynchronize(sg.st_dec));
+      unsigned long long first_err = 0;
+      G16_CUDA(cudaMemcpy(&first_err, sg.err.p, 8, cudaMemcpyDeviceToHost));
+      if (first_err != ~0ull) {
+        const uint64_t off = first_err >> 8;
+        const uint32_t code = first_err & 0xff;
+        if (off >= z.coef_off && off < z.coef_off + (uint64_t)z.ncoefs * z.rs)
+          return fail(G16_ERR_INVALID_DATA, zkey_coef_reason(bytes, z, off, code));
+        return fail(G16_ERR_INVALID_DATA, zkey_locate(z, off) + " (byte " + std::to_string(off) + "): " + ser_reason(code));
+      }
+      if (!derived.empty()) return fail(G16_ERR_INVALID_DATA, derived);
+      for (DevBuf& b : sg.dev) b.release();   // likewise the staging buffers, before commit_key weighs the free memory
+      have_circuit = true;
+      if ((rc = ser_commit(sg, vk))) { have_circuit = false; return rc; }
+      const auto t3 = std::chrono::steady_clock::now();
+      auto ms = [](auto a, auto b) { return std::chrono::duration<float, std::milli>(b - a).count(); };
+      tm.total_ms = ms(t0, t3);
+      tm.witness_map_ms = ms(t0, t2);
+      tm.h2d_ms = ms(t2, t3);
+      tm.h2d_bytes = sg.h2d_bytes;
+      tm.d2h_bytes = 8 + 8 + 4 + 8 + ser_aux_bytes(num_inputs);
+      tm.launches = sg.launches + (ntt_launches + ctr.launches - launches0);
+      if (info) *info = g16_zkey_info{num_inputs, num_constraints, num_witness, (uint32_t)L, nnz[0], nnz[1]};
+      return G16_OK;
     }
-    return G16_OK;
   }
   int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) override {
     using Fmt = SerFormat<CP>;

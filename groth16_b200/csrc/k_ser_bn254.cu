@@ -1,5 +1,7 @@
-// k_ser_bn254.cu -- proving-key decode / encode kernels (ser.cuh) of BN254
+// k_ser_bn254.cu -- proving-key decode / encode kernels (ser.cuh) and .zkey kernels (zkey.cuh) of BN254
 #include "ser.cuh"
+#include "zkey.cuh"
 namespace g16 {
 G16_SER_TEMPLATES(template, BN254_Params)
+G16_ZKEY_TEMPLATES(template, BN254_Params)
 }  // namespace g16

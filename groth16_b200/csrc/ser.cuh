@@ -295,6 +295,45 @@ G16_HD uint32_t ser_decode(const uint8_t* raw, uint32_t flags, Affine<SerField<C
   return SER_OK;
 }
 
+// snarkjs .zkey points (zkey.cuh): every coordinate n8q = NB little-endian bytes already in Montgomery form (R = 2^(8 NB),
+// which is the ABI's R), G1 x || y, G2 x.c0 || x.c1 || y.c0 || y.c1 on every curve; the identity is all-zero bytes.  No flag
+// bits and no multiplication by R^2; otherwise the decisions of ser_decode: canonical coordinates (< q), on the curve, and
+// with SER_VALIDATE [r]P = O.
+template <class CP, bool G2>
+G16_HD uint32_t ser_decode_mont(const uint8_t* raw, uint32_t flags, Affine<SerField<CP, G2>>& out) {
+  using Fq = Fp<typename CP::FqP>;
+  using F = SerField<CP, G2>;
+  using Fmt = SerFormat<CP>;
+  constexpr int NB = Fmt::NB, NC = G2 ? Fmt::G2_NC : 1;
+  Fq v[2 * NC];
+  bool any = false;
+#pragma unroll
+  for (int k = 0; k < 2 * NC; k++) {
+    v[k] = ser_read_fq<typename CP::FqP>(raw + k * NB, false);
+    any |= !v[k].is_zero();
+  }
+  if (!any) {
+    out = Affine<F>::inf();
+    return SER_OK;
+  }
+#pragma unroll
+  for (int k = 0; k < 2 * NC; k++)
+    if (!ser_lt_mod(v[k])) return SER_ERR_NONCANONICAL;
+  F x, y;
+  if constexpr (G2 && NC == 2) {
+    x = {v[0], v[1]};
+    y = {v[2], v[3]};
+  } else {
+    x = v[0];
+    y = v[1];
+  }
+  if (F::sqr(y) != F::add(F::mul(F::sqr(x), x), ser_b<CP, G2>())) return SER_ERR_OFF_CURVE;
+  out = Affine<F>{x, y};
+  if ((flags & SER_VALIDATE) && !(!G2 && Fmt::G1_COFACTOR_ONE) && !ser_in_subgroup<typename CP::FrP>(out))
+    return SER_ERR_SUBGROUP;
+  return SER_OK;
+}
+
 // the point's encoding, exactly ArkCodec.point
 template <class CP, bool G2>
 G16_HD void ser_encode(const Affine<SerField<CP, G2>>& p, uint32_t flags, uint8_t* out) {
@@ -349,7 +388,8 @@ struct SerDest {
 };
 
 #ifdef __CUDACC__
-template <class CP, bool G2>
+// MONT: the .zkey encoding of ser_decode_mont (flags holds SER_VALIDATE at most) instead of the ark encodings
+template <class CP, bool G2, bool MONT = false>
 __global__ void __launch_bounds__(128) ser_decode_kernel(const uint8_t* src, uint64_t first, uint32_t count, uint32_t flags,
                                                          uint64_t off0, SerDest d, unsigned long long* err) {
   using A = Affine<SerField<CP, G2>>;
@@ -357,7 +397,9 @@ __global__ void __launch_bounds__(128) ser_decode_kernel(const uint8_t* src, uin
   if (t >= count) return;
   const uint32_t psize = SerFormat<CP>::point_bytes(G2, flags & SER_COMPRESSED);
   A p;
-  const uint32_t code = ser_decode<CP, G2>(src + (uint64_t)t * psize, flags, p);
+  uint32_t code;
+  if constexpr (MONT) code = ser_decode_mont<CP, G2>(src + (uint64_t)t * psize, flags, p);
+  else code = ser_decode<CP, G2>(src + (uint64_t)t * psize, flags, p);
   if (code) {   // the smallest (byte offset, code) is the first bad point in stream order
     atomicMin(err, ((off0 + (uint64_t)t * psize) << 8) | code);
     return;
@@ -375,11 +417,11 @@ __global__ void __launch_bounds__(128) ser_encode_kernel(const Affine<SerField<C
   const uint32_t psize = SerFormat<CP>::point_bytes(G2, flags & SER_COMPRESSED);
   ser_encode<CP, G2>(src[t], flags, out + (uint64_t)t * psize);
 }
-template <class CP, bool G2>
+template <class CP, bool G2, bool MONT = false>
 cudaError_t ser_decode_enqueue(cudaStream_t st, const uint8_t* src, uint64_t first, uint32_t count, uint32_t flags,
                                uint64_t off0, SerDest d, unsigned long long* err) {
   if (!count) return cudaSuccess;
-  ser_decode_kernel<CP, G2><<<(count + 127) / 128, 128, 0, st>>>(src, first, count, flags, off0, d, err);
+  ser_decode_kernel<CP, G2, MONT><<<(count + 127) / 128, 128, 0, st>>>(src, first, count, flags, off0, d, err);
   return cudaGetLastError();
 }
 template <class CP, bool G2>

@@ -418,6 +418,53 @@ int g16_pk_load_serialized(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uin
                            const g16_pk_export_desc* vk_out);
 int g16_pk_export_serialized(g16_ctx* ctx, uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out);
 
+/* ---- snarkjs .zkey files: the circuit and its proving key in one call, the GPU counterpart of ark-circom's read_zkey followed
+ * by Groth16<E, CircomReduction>.  `bytes` is a whole Groth16 .zkey (circuit_final.zkey) of the context's curve: "zkey",
+ * version 1, nSections, then {id u32, size u64, body} records; sections 1 .. 9 exactly once each, in any order, ids >= 10
+ * (section 10: the MPC contributions) skipped.  1: protocol = 1 (Groth16).  2: n8q, q, n8r, r, nVars, nPublic, domainSize,
+ * alpha1, beta1, beta2, gamma2, delta1, delta2.  3: IC (nPublic + 1 G1) = gamma_abc_g1.  4: nCoefs, then {matrix (0 = A,
+ * 1 = B), constraint, signal, value} records, value the canonical c R^2 mod r.  5 / 6 / 7: A / B1 / B2 (nVars points) =
+ * a_query / b_g1_query / b_g2_query.  8: C (nVars - nPublic - 1 G1) = l_query.  9: H (domainSize G1) = h_query.  Integers
+ * are little-endian; a coordinate is n8q bytes in Montgomery form, which is this ABI's; G2 is x.c0 || x.c1 || y.c0 || y.c1;
+ * the identity is all-zero bytes.  snarkjs appends row nConstraints + s = {(s, 1)} to A for s = 0 .. nPublic; the call
+ * derives num_inputs = nPublic + 1, num_witness = nVars - nPublic - 1, num_constraints = (largest constraint index) -
+ * nPublic, checks that those rows are exactly the appended ones (B: empty) and drops them (CircomReduction appends them
+ * itself), and that domainSize is the smallest power of two >= num_constraints + num_inputs.
+ * One call makes the circuit resident under G16_QAP_CIRCOM with A and B built on the GPU (one thread per coefficient
+ * record decodes and counts, an exclusive scan gives row_ptr, a scatter fills col / val; the order of entries within a row
+ * is free, and no result depends on it or on the chunking), and makes the key resident with the rules of g16_pk_load
+ * (rank / world shards; every rank decodes and checks everything).  Every prover path and g16_witness_map then take them.
+ * flags: 0 or G16_SER_VALIDATE (adds [r]P = O of every point).  Always checked: coordinates below q, points on the curve;
+ * coefficients with matrix < 2, constraint < domainSize, signal < nVars, value < r.
+ *   Host checks, decided before anything resident is released (a refusal leaves the previous circuit and key resident):
+ *   G16_ERR_BAD_ARGUMENT for a null pointer, flags other than 0 or G16_SER_VALIDATE, a vk_out with query members, bad
+ *   rank / world, a proof in flight, and a BLS12-377 or BW6-761 context (snarkjs has neither curve; no byte is read);
+ *   G16_ERR_INVALID_DATA for the section table (magic, version, truncation, trailing bytes, a missing or duplicated
+ *   section), a section size that does not match the header, protocol != 1, n8q / q / n8r / r other than the context's
+ *   curve, nVars < nPublic + 1, a domainSize that is not a power of two; G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE for a domain
+ *   the CircomReduction cannot run.
+ *   Device checks: then the old circuit and key are dropped, as g16_pk_load_serialized drops the old key.  A coefficient or
+ *   point the GPU refuses, appended rows that are not the public-input rows, or a domainSize that is not the derived
+ *   circuit's return G16_ERR_INVALID_DATA and leave neither a circuit nor a key resident.
+ *   g16_last_error() names the first bad item in file order: "coefficient 1234: signal 70000 >= nVars 65536", "B2[17] (byte
+ *   n): point is not on the curve", "coefficients: public-input row 3 of A is not {(3, 1)}".
+ * A .zkey holds no C matrix: C is resident as an empty matrix, and the calls that read it refuse the circuit with
+ * G16_ERR_BAD_ARGUMENT ("the resident circuit came from a .zkey, which holds no C matrix"): g16_check_witness, the flag
+ * G16_CHECK_WITNESS on every path, g16_setup, g16_setup_from_srs and g16_pk_verify_pairs.  The CircomReduction witness map
+ * never reads C (also on the sharded path with "wm_split": chain c starts from a o b).  The next g16_circuit_load* clears
+ * the state.
+ * vk_out as in g16_pk_load_serialized (nullable; capacity num_inputs in gamma_abc_g1; query members NULL).  info_out
+ * (nullable) receives the derived sizes, log2 of the domain and the entries of A and B.  Afterwards g16_get_timings
+ * describes this call (every other field 0): total_ms = the whole call, witness_map_ms = coefficient upload, decode and CSR
+ * build, h2d_ms = upload and point checks (host clock around work that ends in a stream synchronise), h2d_bytes / d2h_bytes
+ * = bytes copied each way, launches = kernels. */
+typedef struct {
+  uint32_t num_inputs, num_constraints, num_witness, log_n;
+  uint64_t a_nnz, b_nnz;
+} g16_zkey_info;
+int g16_zkey_load(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
+                  const g16_pk_export_desc* vk_out, g16_zkey_info* info_out);
+
 /* ---- proving: Groth16::create_proof_with_reduction_and_matrices, prover.rs:26-51
  *      = witness_map_from_matrices (r1cs_to_qap.rs:172-235) + create_proof_with_assignment (prover.rs:54-132).
  * r, s: Montgomery Fr.  full_assignment: (num_inputs + num_witness) Montgomery Fr, instance first.

@@ -10,6 +10,7 @@
 //!   * ark-circom's `CircomReduction` (circom circuits, snarkjs-compatible keys)  -> [`GpuCircomReduction`] for
 //!     `ark_groth16::Groth16<E, GpuCircomReduction>` (setup and witness map), and [`B200Prover::new_with_qap`] with
 //!     `sys::G16_QAP_CIRCOM` for the whole proof
+//!   * ark-circom's `read_zkey` (snarkjs `.zkey` files) followed by `Groth16<E, CircomReduction>` -> [`B200Prover::load_zkey`]
 //! The MSMs have no hook inside ark-groth16 (src/prover.rs:66,74,262 call `msm_bigint` on `E::G1` / `E::G2` directly),
 //! hence the sibling prover type instead of a trait implementation.
 //!
@@ -77,6 +78,29 @@ fn status(rc: i32) -> R1CSResult<()> {
 /// gamma_abc_g1 / query length that does not fit the circuit, G16_ERR_MALFORMED_KEY) is `InvalidData`, whose message naming
 /// the member, index and reason goes to stderr; a CUDA failure or a bad argument is an `IoError` carrying the library's
 /// message, so that callers can tell a missing GPU from bad key data.
+/// nPublic + 1 from section 2 of a `.zkey` (n8q-byte base field), found by walking the section table; 1 when the file is
+/// too broken to say (g16_zkey_load then refuses it before writing anything).
+fn zkey_num_inputs(b: &[u8], n8q: usize) -> usize {
+    let u32_at = |o: usize| -> Option<usize> { b.get(o..o + 4).map(|s| u32::from_le_bytes([s[0], s[1], s[2], s[3]]) as usize) };
+    let u64_at = |o: usize| -> Option<usize> {
+        b.get(o..o + 8).map(|s| u64::from_le_bytes([s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7]]) as usize)
+    };
+    let mut pos = 12usize;
+    for _ in 0..u32_at(8).unwrap_or(0) {
+        let (Some(id), Some(size)) = (u32_at(pos), u64_at(pos + 4)) else { return 1 };
+        pos += 12;
+        if id == 2 {
+            if u32_at(pos) != Some(n8q) {
+                return 1;
+            }
+            let Some(n8r) = u32_at(pos + 4 + n8q) else { return 1 };
+            return u32_at(pos + 8 + n8q + n8r + 4).map_or(1, |p| p + 1);
+        }
+        pos = pos.saturating_add(size);
+    }
+    1
+}
+
 fn ser_status(rc: i32) -> Result<(), SerializationError> {
     if rc == sys::G16_OK {
         return Ok(());
@@ -384,6 +408,66 @@ impl<E: SwPairing> B200Prover<E> {
             )
         })?;
         let vk = me.load_proving_key_bytes(bytes, compress, validate, rank, world)?;
+        Ok((me, vk))
+    }
+
+    /// A prover for the circuit and proving key of a snarkjs Groth16 `.zkey` (circuit_final.zkey), both decoded and made
+    /// resident on the GPU in one call (g16_zkey_load): the GPU counterpart of ark-circom's `read_zkey` followed by
+    /// `Groth16<E, CircomReduction>`.  The circuit's A and B are built on the device (a `.zkey` has no C: the calls that
+    /// need it refuse), its sizes are derived from the file, and proofs run under `sys::G16_QAP_CIRCOM`.  Returns the
+    /// prover and the key's VerifyingKey.  BN254 and BLS12-381 only, the curves snarkjs writes; a malformed file is
+    /// `SerializationError::InvalidData` with the library's message.
+    pub fn load_zkey(device: i32, bytes: &[u8], validate: Validate, rank: u32, world: u32) -> Result<(Self, VerifyingKey<E>), SerializationError> {
+        let curve = curve_id::<E::ScalarField>().ok_or_else(|| {
+            SerializationError::IoError(ark_std::io::Error::new(ark_std::io::ErrorKind::Other, "libg16b200 does not support this curve"))
+        })?;
+        let mut ctx = core::ptr::null_mut();
+        ser_status(unsafe { sys::g16_ctx_create(curve, device, &mut ctx) })?;
+        let (fq_limbs, g2_limbs) = (unsafe { sys::g16_fq_limbs(ctx) } as usize, unsafe { sys::g16_g2_limbs(ctx) } as usize);
+        let (w1, w2) = (point_limbs::<E::G1Config>(), point_limbs::<E::G2Config>());
+        let (mut alpha_g1, mut beta_g1, mut delta_g1) = (ark_std::vec![0u64; w1], ark_std::vec![0u64; w1], ark_std::vec![0u64; w1]);
+        let (mut beta_g2, mut gamma_g2, mut delta_g2) = (ark_std::vec![0u64; w2], ark_std::vec![0u64; w2], ark_std::vec![0u64; w2]);
+        let mut abc = ark_std::vec![0u64; w1 * zkey_num_inputs(bytes, 8 * fq_limbs)];
+        let null = core::ptr::null_mut();
+        let desc = sys::g16_pk_export_desc {
+            a_query: null,
+            b_g1_query: null,
+            b_g2_query: null,
+            h_query: null,
+            l_query: null,
+            alpha_g1: alpha_g1.as_mut_ptr(),
+            beta_g1: beta_g1.as_mut_ptr(),
+            delta_g1: delta_g1.as_mut_ptr(),
+            beta_g2: beta_g2.as_mut_ptr(),
+            gamma_g2: gamma_g2.as_mut_ptr(),
+            delta_g2: delta_g2.as_mut_ptr(),
+            gamma_abc_g1: abc.as_mut_ptr(),
+        };
+        let flags = if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 };
+        let mut info = sys::g16_zkey_info::default();
+        let rc = unsafe { sys::g16_zkey_load(ctx, bytes.as_ptr(), bytes.len() as u64, flags, rank, world, &desc, &mut info) };
+        if rc != 0 {
+            let err = ser_status(rc);
+            unsafe { sys::g16_ctx_destroy(ctx) };
+            err?;
+        }
+        let me = Self {
+            ctx,
+            num_inputs: info.num_inputs as usize,
+            num_constraints: info.num_constraints as usize,
+            num_variables: (info.num_inputs + info.num_witness) as usize,
+            fq_limbs,
+            g2_limbs,
+            flags: Cell::new(0),
+            _e: PhantomData,
+        };
+        let vk = VerifyingKey {
+            alpha_g1: unpack_point(&alpha_g1),
+            beta_g2: unpack_point(&beta_g2),
+            gamma_g2: unpack_point(&gamma_g2),
+            delta_g2: unpack_point(&delta_g2),
+            gamma_abc_g1: abc.chunks(w1).take(info.num_inputs as usize).map(|l| unpack_point(l)).collect(),
+        };
         Ok((me, vk))
     }
 

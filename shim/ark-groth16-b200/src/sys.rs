@@ -37,6 +37,17 @@ pub const G16_NONE: u64 = u64::MAX;
 
 #[repr(C)]
 #[derive(Default, Clone, Copy, Debug, PartialEq, Eq)]
+pub struct g16_zkey_info {
+    pub num_inputs: u32,
+    pub num_constraints: u32,
+    pub num_witness: u32,
+    pub log_n: u32,
+    pub a_nnz: u64,
+    pub b_nnz: u64,
+}
+
+#[repr(C)]
+#[derive(Default, Clone, Copy, Debug, PartialEq, Eq)]
 pub struct g16_witness_report {
     pub first_unsatisfied: u64,
     pub num_unsatisfied: u64,
@@ -225,6 +236,7 @@ extern "C" {
     pub fn g16_pk_contribute(ctx: *mut g16_ctx, input: *const g16_pk_delta_desc, delta: *const u64, flags: u32, chunk_points: u64, out: *const g16_pk_delta_out) -> c_int;
     pub fn g16_contribution_chain_pairs(ctx: *mut g16_ctx, start_g1: *const u64, end_g1: *const u64, records: *const g16_contribution_record, count: u32, flags: u32, pairs_g1: *mut u64, pairs_g2: *mut u64) -> c_int;
     pub fn g16_pk_load_serialized(ctx: *mut g16_ctx, bytes: *const u8, len: u64, flags: u32, rank: u32, world: u32, vk_out: *const g16_pk_export_desc) -> c_int;
+    pub fn g16_zkey_load(ctx: *mut g16_ctx, bytes: *const u8, len: u64, flags: u32, rank: u32, world: u32, vk_out: *const g16_pk_export_desc, info_out: *mut g16_zkey_info) -> c_int;
     pub fn g16_pk_export_serialized(ctx: *mut g16_ctx, flags: u32, out: *mut u8, cap: u64, len_out: *mut u64) -> c_int;
     pub fn g16_prove(ctx: *mut g16_ctx, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32, proof_out: *mut u64) -> c_int;
     pub fn g16_prove_partial(ctx: *mut g16_ctx, r: *const u64, full_assignment: *const u64, flags: u32, partial_out: *mut u64) -> c_int;
