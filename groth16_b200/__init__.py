@@ -9,13 +9,13 @@ _os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
 from ._lib import CHECK_WITNESS, ERR_UNSATISFIED
 from .api import (KEY_EQUATIONS, ChainPairs, ConstraintMatrices, ContributionRecord, CudaError, Groth16, KeyPairs, MalformedKey,
-                  PolynomialDegreeTooLarge, Proof, ProvingKey, Srs, SrsPairs, SynthesisError, Unsatisfiable, VerifyingKey,
+                  PolynomialDegreeTooLarge, Proof, ProvingKey, R1csCircuit, Srs, SrsPairs, SynthesisError, Unsatisfiable, VerifyingKey,
                   WitnessReport, ZkeyCircuit)
 from .codec import CurveCodec, FieldCodec
 from .params import BLS12_377, BLS12_381, BN254, BW6_761, CURVES, get_curve
 
 __all__ = ["Groth16", "ConstraintMatrices", "ProvingKey", "VerifyingKey", "Proof", "Srs", "SrsPairs", "KeyPairs", "KEY_EQUATIONS",
-           "ContributionRecord", "ChainPairs", "ZkeyCircuit",
+           "ContributionRecord", "ChainPairs", "ZkeyCircuit", "R1csCircuit",
            "SynthesisError", "PolynomialDegreeTooLarge", "MalformedKey", "Unsatisfiable", "WitnessReport", "CHECK_WITNESS", "ERR_UNSATISFIED",
            "CudaError", "CurveCodec", "FieldCodec", "CURVES", "BW6_761", "BLS12_381",
            "BN254", "BLS12_377", "get_curve"]

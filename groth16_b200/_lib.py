@@ -71,6 +71,11 @@ class ZkeyInfo(C.Structure):
                 ("a_nnz", C.c_uint64), ("b_nnz", C.c_uint64)]
 
 
+class R1csInfo(C.Structure):
+    _fields_ = [("num_inputs", C.c_uint32), ("num_constraints", C.c_uint32), ("num_witness", C.c_uint32), ("log_n", C.c_uint32),
+                ("a_nnz", C.c_uint64), ("b_nnz", C.c_uint64), ("c_nnz", C.c_uint64)]
+
+
 class WitnessReport(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("first_unsatisfied", "num_unsatisfied", "first_malformed")]
 
@@ -112,6 +117,8 @@ SIGNATURES = [
                                          C.POINTER(PkExportDesc)]),
     ("g16_zkey_load", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(PkExportDesc),
                                 C.POINTER(ZkeyInfo)]),
+    ("g16_r1cs_load", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(R1csInfo)]),
+    ("g16_wtns_read", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("g16_pk_export_serialized", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("g16_prove", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     ("g16_prove_partial", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -149,6 +156,7 @@ ASSIGNMENT_ON_DEVICE = 1
 SERIAL_MSMS = 2
 CHECK_WITNESS = 4
 PK_UNCONTRIBUTED = 4   # a flag of g16_pk_verify_pairs
+ZKEY_KEY_ONLY = 16     # a flag of g16_zkey_load
 NONE = (1 << 64) - 1   # G16_NONE
 QAP_LIBSNARK = 0
 QAP_CIRCOM = 1

@@ -153,6 +153,20 @@ class ZkeyCircuit:
 
 
 @dataclass
+class R1csCircuit:
+    """The circuit g16_r1cs_load read from a circom .r1cs and made resident with all three matrices (on the GPU, and host
+    copies for the setup calls).  Its sizes stand in for ConstraintMatrices wherever the resident circuit's sizes are
+    needed."""
+    num_instance_variables: int
+    num_constraints: int
+    num_witness_variables: int
+    log_n: int
+    a_nnz: int
+    b_nnz: int
+    c_nnz: int
+
+
+@dataclass
 class VerifyingKey:
     alpha_g1: np.ndarray
     beta_g2: np.ndarray
@@ -893,6 +907,71 @@ class Groth16:
                           out["gamma_abc_g1"][:info.num_inputs])
         vk.beta_g1, vk.delta_g1 = out["beta_g1"][0], out["delta_g1"][0]
         return vk, self._matrices
+
+    def load_zkey_key(self, data: bytes, validate: bool = True, rank: int = 0, world: int = 1) -> VerifyingKey:
+        """g16_zkey_load with G16_ZKEY_KEY_ONLY: make only the proving key of a snarkjs .zkey resident, onto the resident
+        circuit (typically from load_r1cs, which keeps C), with the rules of load_proving_key.  Its coefficient section is not
+        read: whether the key belongs to the circuit is key_verification_pairs's question.  Needs a resident circuit under
+        qap="circom" (ValueError otherwise); sizes other than the circuit's raise MalformedKey and a malformed file
+        serialize.DeserializeError, both leaving the previous key resident; a refused point leaves no key."""
+        m = self._matrices
+        if m is None:
+            raise ValueError("load_r1cs or load_matrices must come first")
+        buf = np.frombuffer(data, dtype=np.uint8)
+        nq, ng2 = self.nq, self.ng2
+        z = lambda rows, w: np.zeros((rows, w), dtype=np.uint64)
+        out = dict(alpha_g1=z(1, 2 * nq), beta_g1=z(1, 2 * nq), delta_g1=z(1, 2 * nq), beta_g2=z(1, ng2),
+                   gamma_g2=z(1, ng2), delta_g2=z(1, ng2), gamma_abc_g1=z(m.num_instance_variables, 2 * nq))
+        d = _lib.PkExportDesc()
+        for k, v in out.items():
+            setattr(d, k, _u64p(v) if v.size else None)
+        flags = _lib.ZKEY_KEY_ONLY | (_lib.SER_VALIDATE if validate else 0)
+        rc = self._lib.g16_zkey_load(self._ctx, buf.ctypes.data_as(C.c_void_p) if buf.size else None, buf.size, flags, rank,
+                                     world, C.byref(d), None)
+        if rc == _lib.ERR_INVALID_DATA and "(byte " in _lib.last_error():
+            self._pk_resident = False
+            self._pk_obj = None
+        _check(rc)
+        self._pk_resident = True
+        self._pk_obj = None
+        self.world = world
+        vk = VerifyingKey(out["alpha_g1"][0], out["beta_g2"][0], out["gamma_g2"][0], out["delta_g2"][0], out["gamma_abc_g1"])
+        vk.beta_g1, vk.delta_g1 = out["beta_g1"][0], out["delta_g1"][0]
+        return vk
+
+    # ---- circom .r1cs circuits and .wtns witnesses, decoded on the GPU ----
+    def load_r1cs(self, data: bytes) -> R1csCircuit:
+        """g16_r1cs_load: make the circuit of a circom .r1cs resident with all three matrices, under this context's qap, as
+        load_matrices would the same terms (the GPU counterpart of ark-circom's R1CSFile + CircomCircuit).  Every call that
+        reads C (check_witness, CHECK_WITNESS, generate_parameters_from_srs, key_verification_pairs) then works.  A
+        malformed file raises serialize.DeserializeError naming the problem: the previous circuit and key stay resident
+        when the structure or header is refused, none when a term is."""
+        buf = np.frombuffer(data, dtype=np.uint8)
+        info = _lib.R1csInfo()
+        rc = self._lib.g16_r1cs_load(self._ctx, _lib.QAPS[self.qap], buf.ctypes.data_as(C.c_void_p) if buf.size else None,
+                                     buf.size, C.byref(info))
+        if rc == _lib.ERR_INVALID_DATA and "(byte " in _lib.last_error():
+            self._matrices = None
+            self._pk_resident = False
+            self._pk_obj = None
+        _check(rc)
+        self._matrices = R1csCircuit(info.num_inputs, info.num_constraints, info.num_witness, info.log_n, info.a_nnz,
+                                     info.b_nnz, info.c_nnz)
+        self._pk_resident = False
+        self._pk_obj = None
+        return self._matrices
+
+    def read_wtns(self, data: bytes) -> np.ndarray:
+        """g16_wtns_read: the witness of a circom .wtns as (n, nr) Montgomery limbs, usable directly as full_assignment.  A
+        malformed file or element raises serialize.DeserializeError naming it.  Needs no circuit; touches no resident state."""
+        buf = np.frombuffer(data, dtype=np.uint8)
+        ptr = buf.ctypes.data_as(C.c_void_p) if buf.size else None
+        n = C.c_uint64()
+        _check(self._lib.g16_wtns_read(self._ctx, ptr, buf.size, None, 0, C.byref(n)))
+        out = np.zeros((n.value, self.nr), dtype=np.uint64)
+        if n.value:
+            _check(self._lib.g16_wtns_read(self._ctx, ptr, buf.size, _ptr(out), n.value, C.byref(n)))
+        return out
 
     def export_proving_key_bytes(self, compress: bool = True) -> bytes:
         """g16_pk_export_serialized: the resident key (made by generate_parameters_with_qap) as ark-serialize writes it,

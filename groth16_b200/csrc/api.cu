@@ -99,7 +99,7 @@ const char* g16_last_error(void) { return last_error_ref().c_str(); }
 
 #define CTX_OR_FAIL(ctx) \
   if (!(ctx) || !(ctx)->eng) return fail(G16_ERR_BAD_ARGUMENT, "null context")
-// the calls that read matrix C refuse a circuit loaded by g16_zkey_load, which has none
+// the calls that read matrix C refuse a circuit loaded by g16_zkey_load, which has none (g16_r1cs_load loads one with C)
 #define NEEDS_C(ctx, cond)                        \
   if ((cond) && (ctx)->eng->circuit_without_c)    \
   return fail(G16_ERR_BAD_ARGUMENT, "the resident circuit came from a .zkey, which holds no C matrix")
@@ -200,6 +200,14 @@ int g16_zkey_load(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t fla
                   const g16_pk_export_desc* vk_out, g16_zkey_info* info_out) {
   CTX_OR_FAIL(ctx);
   return ctx->eng->zkey_load(bytes, len, flags, rank, world, vk_out, info_out);
+}
+int g16_r1cs_load(g16_ctx* ctx, int qap, const uint8_t* bytes, uint64_t len, g16_r1cs_info* info_out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->r1cs_load(qap, bytes, len, info_out);
+}
+int g16_wtns_read(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint64_t* out, uint64_t cap, uint64_t* count_out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->wtns_read(bytes, len, out, cap, count_out);
 }
 int g16_pk_export_serialized(g16_ctx* ctx, uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) {
   CTX_OR_FAIL(ctx);

@@ -32,6 +32,7 @@
 #include "ser.cuh"
 #include "srs.cuh"
 #include "zkey.cuh"
+#include "r1cs.cuh"
 
 namespace g16 {
 
@@ -164,6 +165,8 @@ struct IEngine {
   virtual int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) = 0;
   virtual int zkey_load(const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                         const g16_pk_export_desc* vk_out, g16_zkey_info* info_out) = 0;
+  virtual int r1cs_load(int qap, const uint8_t* bytes, uint64_t len, g16_r1cs_info* info_out) = 0;
+  virtual int wtns_read(const uint8_t* bytes, uint64_t len, uint64_t* out, uint64_t cap, uint64_t* count_out) = 0;
   virtual int prove(const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags, uint64_t* proof) = 0;
   virtual int prove_partial(const uint64_t* r, const uint64_t* z, uint32_t flags, uint64_t* partial) = 0;
   virtual int prove_assemble(const uint64_t* r, const uint64_t* s, const uint64_t* partials, uint32_t nparts, uint64_t* proof) = 0;
@@ -184,7 +187,7 @@ struct IEngine {
   virtual int get_option(const char* key, long long* value) const = 0;
   virtual int get_config(g16_config* out) const = 0;
   g16_timings tm{};
-  // the resident circuit came from a .zkey: matrix C is resident empty, and the calls that read it refuse (api.cu)
+  // the resident circuit came from a full .zkey load: matrix C is resident empty, and the calls that read it refuse (api.cu)
   bool circuit_without_c = false;
 };
 
@@ -2285,13 +2288,20 @@ struct Engine : IEngine {
       return fail(G16_ERR_BAD_ARGUMENT, "snarkjs .zkey files exist for BN254 and BLS12-381 only");
     } else {
       if ((!bytes && len) || wd == 0 || rk >= wd) return fail(G16_ERR_BAD_ARGUMENT, "bad bytes / rank / world");
-      if (flags & ~(uint32_t)G16_SER_VALIDATE) return fail(G16_ERR_BAD_ARGUMENT, "g16_zkey_load takes G16_SER_VALIDATE only");
+      if (flags & ~(uint32_t)(G16_SER_VALIDATE | G16_ZKEY_KEY_ONLY))
+        return fail(G16_ERR_BAD_ARGUMENT, "g16_zkey_load takes G16_SER_VALIDATE and G16_ZKEY_KEY_ONLY only");
       if (vk && (vk->a_query || vk->b_g1_query || vk->b_g2_query || vk->h_query || vk->l_query))
         return fail(G16_ERR_BAD_ARGUMENT, "vk_out receives the verifying key only: its query members must be NULL");
       G16_NOT_BUSY();
+      const bool key_only = flags & G16_ZKEY_KEY_ONLY;
+      flags &= ~(uint32_t)G16_ZKEY_KEY_ONLY;
+      if (key_only && (!have_circuit || qap != G16_QAP_CIRCOM))
+        return fail(G16_ERR_BAD_ARGUMENT, "G16_ZKEY_KEY_ONLY needs a resident circuit under G16_QAP_CIRCOM (a .zkey holds a "
+                                          "CircomReduction key)");
       ZkeyLayout z;
       const std::string why = zkey_walk<CP>(bytes, len, z);
       if (!why.empty()) return fail(G16_ERR_INVALID_DATA, why);
+      if (key_only) return zkey_key_only(bytes, z, flags, rk, wd, vk, info);
       int Ln = 0;
       while ((1u << Ln) < z.domain_size) Ln++;
       int rc = check_log((uint32_t)Ln);
@@ -2411,6 +2421,181 @@ struct Engine : IEngine {
       if (info) *info = g16_zkey_info{num_inputs, num_constraints, num_witness, (uint32_t)L, nnz[0], nnz[1]};
       return G16_OK;
     }
+  }
+  // G16_ZKEY_KEY_ONLY: the walked file's key onto the resident circuit (section 4 is not read).  The sizes are decided
+  // before begin_key drops the previous key; a refused point leaves the circuit and no key.
+  int zkey_key_only(const uint8_t* bytes, const ZkeyLayout& z, uint32_t flags, uint32_t rk, uint32_t wd, const g16_pk_export_desc* vk,
+                    g16_zkey_info* info) {
+    if ((uint64_t)z.nvars != nvars())
+      return fail(G16_ERR_MALFORMED_KEY, "section 2: nVars = " + std::to_string(z.nvars) + ", the resident circuit has " +
+                                             std::to_string(nvars()) + " variables");
+    if (z.npub + 1ull != num_inputs)
+      return fail(G16_ERR_MALFORMED_KEY, "section 2: nPublic + 1 = " + std::to_string(z.npub + 1ull) +
+                                             ", the resident circuit has " + std::to_string(num_inputs) + " instance variables");
+    if ((uint64_t)z.domain_size != 1ull << L)
+      return fail(G16_ERR_MALFORMED_KEY, "section 2: domainSize = " + std::to_string(z.domain_size) +
+                                             ", the resident circuit's domain is " + std::to_string(1ull << L));
+    G16_CUDA(cudaSetDevice(device));
+    const auto t0 = std::chrono::steady_clock::now();
+    tm = g16_timings{};
+    const uint64_t qlen[5] = {z.it[SER_H].len, z.it[SER_L].len, z.it[SER_A].len, z.it[SER_B_G1].len, z.it[SER_B_G2].len};
+    int rc = begin_key(rk, wd, qlen);
+    if (rc) return rc;
+    const std::vector<SerChunk> plan = ser_plan(z.it, SER_CHUNK);
+    SerStaging sg;
+    if ((rc = ser_staging_init(sg, ser_stage_bytes(z.it, plan), ser_aux_bytes(num_inputs)))) return rc;
+    if ((rc = ser_decode_points<true>(sg, bytes, z.it, plan, flags, true))) return rc;
+    G16_CUDA(cudaStreamSynchronize(sg.st_dec));
+    unsigned long long first_err = 0;
+    G16_CUDA(cudaMemcpy(&first_err, sg.err.p, 8, cudaMemcpyDeviceToHost));
+    if (first_err != ~0ull) {
+      const uint64_t off = first_err >> 8;
+      return fail(G16_ERR_INVALID_DATA, zkey_locate(z, off) + " (byte " + std::to_string(off) + "): " + ser_reason(first_err & 0xff));
+    }
+    for (DevBuf& b : sg.dev) b.release();
+    if ((rc = ser_commit(sg, vk))) return rc;
+    tm.total_ms = tm.h2d_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    tm.h2d_bytes = sg.h2d_bytes;
+    tm.d2h_bytes = 8 + ser_aux_bytes(num_inputs);
+    tm.launches = sg.launches;
+    const uint64_t nnz[2] = {h_rp[0].empty() ? 0 : h_rp[0].back(), h_rp[1].empty() ? 0 : h_rp[1].back()};
+    if (info) *info = g16_zkey_info{num_inputs, num_constraints, num_witness, (uint32_t)L, nnz[0], nnz[1]};
+    return G16_OK;
+  }
+
+  // ---- circom .r1cs circuits and .wtns witnesses (r1cs.cuh) ----
+  // Host: r1cs_walk decides the section table, the header, every term count, the three row_ptr arrays and the domain
+  // before anything resident is released; reading the counts is the format's only serial dependence.  Device, on the
+  // staging streams: the constraint section goes up in chunks of at most SER_CHUNK terms (and of at most the staging size in
+  // bytes), each decoded by one thread per term straight into the resident CSR arrays.  A refused term leaves neither a
+  // circuit nor a key resident.
+  int r1cs_load(int qp, const uint8_t* bytes, uint64_t len, g16_r1cs_info* info) override {
+    if (qp != G16_QAP_LIBSNARK && qp != G16_QAP_CIRCOM) return fail(G16_ERR_BAD_ARGUMENT, "unknown R1CS-to-QAP reduction");
+    if (!bytes) return fail(G16_ERR_BAD_ARGUMENT, "null bytes");
+    G16_NOT_BUSY();
+    const auto t0 = std::chrono::steady_clock::now();
+    R1csLayout z;
+    const std::string why = r1cs_walk<typename CP::FrP>(bytes, len, z);
+    if (!why.empty()) return fail(G16_ERR_INVALID_DATA, why);
+    int Ln = 0;
+    while ((1ull << Ln) < (uint64_t)z.m + z.num_inputs) Ln++;
+    int rc = check_log((uint32_t)Ln);
+    if (rc) return rc;
+    if (qp == G16_QAP_CIRCOM && Ln + 1 > CP::FrP::TWO_ADICITY)
+      return fail(G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "CircomReduction needs a domain of twice the size, which exceeds the field's two-adicity (PolynomialDegreeTooLarge)");
+    G16_CUDA(cudaSetDevice(device));
+    const auto t1 = std::chrono::steady_clock::now();
+    const unsigned long long launches0 = ntt_launches + ctr.launches;
+    tm = g16_timings{};
+    // from here on a refusal leaves neither a circuit nor a key resident
+    drop_key();
+    have_circuit = false;
+    circuit_without_c = false;
+    const uint32_t nc = z.m;
+    const uint64_t T = z.tp[nc];
+    R1csCsr csr;
+    for (int m = 0; m < 3; m++) {
+      const uint64_t nnz = z.rp[m][nc];
+      G16_CUDA(csr_rp[m].reserve((size_t)(nc + 1) * 4));
+      G16_CUDA(csr_col[m].reserve((size_t)nnz * 4 + 4));
+      G16_CUDA(csr_val[m].reserve((size_t)nnz * sizeof(Fr) + sizeof(Fr)));
+      G16_CUDA(cudaMemcpy(csr_rp[m].p, z.rp[m].data(), (size_t)(nc + 1) * 4, cudaMemcpyHostToDevice));
+      csr.row_ptr[m] = csr_rp[m].template as<uint32_t>();
+      csr.col[m] = csr_col[m].template as<uint32_t>();
+      csr.val[m] = csr_val[m].p;
+    }
+    DevBuf d_tp;
+    G16_CUDA(d_tp.reserve((size_t)(nc + 1) * 8));
+    G16_CUDA(cudaMemcpy(d_tp.p, z.tp.data(), (size_t)(nc + 1) * 8, cudaMemcpyHostToDevice));
+    const size_t stage = (size_t)SER_CHUNK * (z.ts + 12);   // SER_CHUNK terms and a count word per constraint among them
+    SerStaging sg;
+    if ((rc = ser_staging_init(sg, stage, 8))) return rc;
+    unsigned long long* err = sg.err.template as<unsigned long long>();
+    // the constraint holding term t: the last i with tp[i] <= t
+    auto constraint_of = [&](uint64_t t) {
+      return (uint32_t)(std::upper_bound(z.tp.begin(), z.tp.end(), t) - z.tp.begin() - 1);
+    };
+    auto term_off = [&](uint64_t t) { const uint32_t i = constraint_of(t); return r1cs_term_off(z, i, t - z.tp[i]); };
+    for (uint64_t a = 0; a < T;) {
+      // terms [a, b): SER_CHUNK of them unless their bytes (counts between them included) outgrow the staging buffers,
+      // which only runs of empty combinations can make them do
+      uint64_t b = std::min<uint64_t>(T, a + SER_CHUNK);
+      const uint64_t base = term_off(a);
+      while (b - a > 1 && term_off(b - 1) + z.ts - base > stage) b = a + (b - a) / 2;
+      const uint64_t span = term_off(b - 1) + z.ts - base;
+      if ((rc = ser_chunk_upload(sg, bytes + z.sec2_off + base, (size_t)span, nullptr))) return rc;
+      const uint8_t* chunk = sg.dev[sg.chunks & 1].template as<uint8_t>();
+      G16_CUDA(r1cs_term_enqueue<Fr>(sg.st_dec, chunk, base, z.sec2_off, a, (uint32_t)(b - a), constraint_of(a), constraint_of(b - 1),
+                                     d_tp.template as<uint64_t>(), z.ts, z.nwires, csr, err));
+      if ((rc = ser_chunk_done(sg))) return rc;
+      a = b;
+    }
+    G16_CUDA(cudaStreamSynchronize(sg.st_dec));
+    unsigned long long first_err = 0;
+    G16_CUDA(cudaMemcpy(&first_err, sg.err.p, 8, cudaMemcpyDeviceToHost));
+    if (first_err != ~0ull) return fail(G16_ERR_INVALID_DATA, r1cs_reason(bytes, z, first_err >> 8, (uint32_t)(first_err & 0xff)));
+    d_tp.release();
+    for (DevBuf& x : sg.dev) x.release();
+    // the host copies g16_setup and g16_setup_from_srs read: one download of the decoded CSR
+    uint64_t d2h = 8;
+    for (int m = 0; m < 3; m++) {
+      const uint32_t nnz = z.rp[m][nc];
+      h_col[m].resize(nnz);
+      h_val[m].resize(nnz);
+      if (nnz) {
+        G16_CUDA(cudaMemcpy(h_col[m].data(), csr_col[m].p, (size_t)nnz * 4, cudaMemcpyDeviceToHost));
+        G16_CUDA(cudaMemcpy(h_val[m].data(), csr_val[m].p, (size_t)nnz * sizeof(Fr), cudaMemcpyDeviceToHost));
+      }
+      d2h += (uint64_t)nnz * (4 + sizeof(Fr));
+      h_rp[m] = std::move(z.rp[m]);
+    }
+    num_inputs = z.num_inputs; num_constraints = nc; num_witness = z.num_witness; L = Ln; qap = qp;
+    G16_CUDA(S0.d_z.reserve((size_t)nvars() * sizeof(Fr)));
+    if ((rc = ensure_circuit_domain())) return rc;
+    G16_CUDA(cudaStreamSynchronize(S0.st_main));
+    have_circuit = true;
+    const auto t2 = std::chrono::steady_clock::now();
+    auto ms = [](auto x, auto y) { return std::chrono::duration<float, std::milli>(y - x).count(); };
+    tm.total_ms = ms(t0, t2);
+    tm.h2d_ms = ms(t0, t1);
+    tm.witness_map_ms = ms(t1, t2);
+    tm.h2d_bytes = sg.h2d_bytes + (uint64_t)(nc + 1) * (3 * 4 + 8);
+    tm.d2h_bytes = d2h;
+    tm.launches = sg.launches + (ntt_launches + ctr.launches - launches0);
+    if (info)
+      *info = g16_r1cs_info{num_inputs, num_constraints, num_witness, (uint32_t)L, h_rp[0][nc], h_rp[1][nc], h_rp[2][nc]};
+    return G16_OK;
+  }
+  int wtns_read(const uint8_t* bytes, uint64_t len, uint64_t* out, uint64_t cap, uint64_t* count) override {
+    if (!bytes || !count) return fail(G16_ERR_BAD_ARGUMENT, "null bytes / count_out");
+    WtnsLayout w;
+    const std::string why = wtns_walk<typename CP::FrP>(bytes, len, w);
+    if (!why.empty()) return fail(G16_ERR_INVALID_DATA, why);
+    *count = w.n;
+    if (!out) return G16_OK;
+    if (cap < w.n)
+      return fail(G16_ERR_BAD_ARGUMENT, "output buffer holds " + std::to_string(cap) + " elements, the witness has " + std::to_string(w.n));
+    if (!w.n) return G16_OK;
+    G16_CUDA(cudaSetDevice(device));
+    DevBuf d_out;
+    G16_CUDA(d_out.reserve((size_t)w.n * sizeof(Fr)));
+    SerStaging sg;
+    int rc = ser_staging_init(sg, (size_t)SER_CHUNK * w.n8, 8);
+    if (rc) return rc;
+    unsigned long long* err = sg.err.template as<unsigned long long>();
+    for (uint64_t e = 0; e < w.n; e += SER_CHUNK) {
+      const uint32_t cnt = (uint32_t)std::min<uint64_t>(SER_CHUNK, w.n - e);
+      const uint64_t off = w.off + e * w.n8;
+      if ((rc = ser_chunk_upload(sg, bytes + off, (size_t)cnt * w.n8, nullptr))) return rc;
+      G16_CUDA(wtns_elem_enqueue<Fr>(sg.st_dec, sg.dev[sg.chunks & 1].template as<uint8_t>(), off, e, cnt, d_out.p, err));
+      if ((rc = ser_chunk_done(sg))) return rc;
+    }
+    G16_CUDA(cudaStreamSynchronize(sg.st_dec));
+    unsigned long long first_err = 0;
+    G16_CUDA(cudaMemcpy(&first_err, sg.err.p, 8, cudaMemcpyDeviceToHost));
+    if (first_err != ~0ull) return fail(G16_ERR_INVALID_DATA, wtns_reason(w, first_err >> 8, (uint32_t)(first_err & 0xff)));
+    G16_CUDA(cudaMemcpy(out, d_out.p, (size_t)w.n * sizeof(Fr), cudaMemcpyDeviceToHost));
+    return G16_OK;
   }
   int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) override {
     using Fmt = SerFormat<CP>;

@@ -7,5 +7,6 @@ G16_NTT_TEMPLATES(extern template, Fp<BW6_FrP>)
 G16_MSM_TEMPLATES(extern template, Fp<BW6_FqP>, Fp<BW6_FrP>)
 G16_SER_TEMPLATES(extern template, BW6_Params)
 G16_SRS_TEMPLATES(extern template, BW6_Params)
+G16_R1CS_TEMPLATES(extern template, BW6_Params)
 IEngine* make_engine_bw6(int device, int* rc) { return make_engine<BW6_Params>(device, rc); }
 }  // namespace g16

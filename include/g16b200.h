@@ -464,6 +464,60 @@ typedef struct {
 } g16_zkey_info;
 int g16_zkey_load(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint32_t flags, uint32_t rank, uint32_t world,
                   const g16_pk_export_desc* vk_out, g16_zkey_info* info_out);
+/* G16_ZKEY_KEY_ONLY (flags of g16_zkey_load, with or without G16_SER_VALIDATE): only the key of the .zkey is made resident,
+ * onto the resident circuit, which stays as it is with its C matrix (the circom flow: g16_r1cs_load of circuit.r1cs, then
+ * the key of circuit_final.zkey).  The same section walk, header checks and point decode run; the key is placed with the
+ * rules of g16_pk_load (rank / world, vk_out).  Section 4 is not decoded: proofs use the resident A and B, and whether the
+ * key belongs to the resident circuit is g16_pk_verify_pairs's question, as after g16_pk_load.
+ *   Decided on the host, leaving the previous key resident: no resident circuit, or one under G16_QAP_LIBSNARK, is
+ *   G16_ERR_BAD_ARGUMENT (a snarkjs H query has domainSize points: a CircomReduction key); nVars other than num_inputs +
+ *   num_witness, nPublic + 1 other than num_inputs, or domainSize other than 2^log_n is G16_ERR_MALFORMED_KEY naming the
+ *   field.  A point the GPU refuses is G16_ERR_INVALID_DATA and leaves the circuit resident and no key.  info_out
+ *   (nullable) receives the resident circuit's sizes (a_nnz / b_nnz 0 for a circuit loaded by a full g16_zkey_load). */
+enum { G16_ZKEY_KEY_ONLY = 16 };
+
+/* ---- circom .r1cs circuits: all three matrices made resident, the GPU counterpart of ark-circom's R1CSFile followed by
+ * CircomCircuit.  `bytes` is a whole .r1cs (iden3 r1csfile): "r1cs", version u32 = 1, nSections u32, then {type u32, size
+ * u64, body} records in any order; integers little-endian.  Sections 1 and 2 exactly once each; 4 and 5 (custom gates,
+ * PLONK only) are refused; every other section (3: the wire-to-label map) is skipped.
+ *   1 (header, exactly 32 + n8 bytes): n8 u32, prime (n8 bytes), nWires u32, nPubOut u32, nPubIn u32, nPrvIn u32,
+ *     nLabels u64, mConstraints u32.
+ *   2 (constraints): mConstraints records of three linear combinations, A then B then C; each is nTerms u32 followed by
+ *     nTerms {wire u32, coefficient (n8 bytes, canonical: standard form, below r)}.  A constraint means A.w * B.w - C.w = 0.
+ * The circuit: num_inputs = 1 + nPubOut + nPubIn, num_witness = nWires - num_inputs, num_constraints = mConstraints,
+ * column = wire id (wire 0 is One, instance first), under the reduction `qap` with g16_circuit_load_qap's rules.  Terms are
+ * kept as the file has them, in file order (zero coefficients and repeated wires stay separate entries, as ark-circom
+ * pushes them); every result is a field sum, so all results equal those of the compacted matrices.
+ *   Host checks, decided before anything resident is released (a refusal leaves the previous circuit and key resident):
+ *   G16_ERR_BAD_ARGUMENT for null bytes, an unknown qap, a proof in flight; G16_ERR_INVALID_DATA for the section table
+ *   (magic, version, truncation, trailing bytes, section 1 or 2 missing or repeated, section 4 or 5), the header (its
+ *   size, n8 other than the context's scalar size, a prime other than its r, nWires < 1 + nPubOut + nPubIn + nPrvIn), a
+ *   constraint section whose size is not 12 mConstraints + (4 + n8) (all terms), and a matrix of 2^32 or more entries;
+ *   G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE for the domain.  g16_last_error() names what failed ("section 2 holds 1234 bytes,
+ *   its constraints need 1270", "section 1: prime is not the scalar field modulus of this curve").
+ *   Device checks: then the old circuit and key are dropped.  One GPU thread per term checks wire < nWires and coefficient
+ *   < r and writes c R at row_ptr[row] + its position (no atomics: the CSR is the file's order).  A refused term is
+ *   G16_ERR_INVALID_DATA naming the first in file order ("constraint 17, C term 2 (byte 123456): wire 70000 >= nWires
+ *   65536", "...: coefficient is not below r") and leaves neither a circuit nor a key resident.
+ * On success the circuit stands as after g16_circuit_load_qap: every call that reads C takes it.  info_out (nullable)
+ * receives the sizes, log2 of the domain and the entries of each matrix.  Afterwards g16_get_timings describes this call:
+ * total_ms = the whole call, h2d_ms = the host walk, witness_map_ms = upload, decode and the host copies, h2d_bytes /
+ * d2h_bytes, launches. */
+typedef struct {
+  uint32_t num_inputs, num_constraints, num_witness, log_n;
+  uint64_t a_nnz, b_nnz, c_nnz;
+} g16_r1cs_info;
+int g16_r1cs_load(g16_ctx* ctx, int qap, const uint8_t* bytes, uint64_t len, g16_r1cs_info* info_out);
+
+/* ---- circom / snarkjs .wtns witnesses, as this ABI's full assignment (ark-circom's read_witness).  `bytes` is a whole .wtns
+ * (iden3 wtnsfile): "wtns", version u32 = 2, nSections u32, then {type u32, size u64, body} records; sections 1 and 2
+ * exactly once each, others skipped.  1: n8 u32, prime (n8 bytes, the context's r), nWitness u32.  2: nWitness canonical
+ * n8-byte values.  out receives nWitness Montgomery Fr (g16_fr_limbs each), decoded on the GPU (one thread per element
+ * checks < r).  out == NULL writes the count only; cap (elements) below the count is G16_ERR_BAD_ARGUMENT with the count
+ * in *count_out.  A bad file is G16_ERR_INVALID_DATA naming the problem or the first bad element ("witness[17] (byte 80):
+ * not below r").  Needs no circuit and touches no resident state; element 0 and the length are g16_check_witness's
+ * question. */
+int g16_wtns_read(g16_ctx* ctx, const uint8_t* bytes, uint64_t len, uint64_t* out, uint64_t cap, uint64_t* count_out);
 
 /* ---- proving: Groth16::create_proof_with_reduction_and_matrices, prover.rs:26-51
  *      = witness_map_from_matrices (r1cs_to_qap.rs:172-235) + create_proof_with_assignment (prover.rs:54-132).

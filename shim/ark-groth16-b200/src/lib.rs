@@ -11,6 +11,8 @@
 //!     `ark_groth16::Groth16<E, GpuCircomReduction>` (setup and witness map), and [`B200Prover::new_with_qap`] with
 //!     `sys::G16_QAP_CIRCOM` for the whole proof
 //!   * ark-circom's `read_zkey` (snarkjs `.zkey` files) followed by `Groth16<E, CircomReduction>` -> [`B200Prover::load_zkey`]
+//!   * ark-circom's `R1CSFile` + `CircomCircuit` (circom `.r1cs` files, all three matrices) -> [`B200Prover::load_r1cs`], the
+//!     key of a `.zkey` onto it -> [`B200Prover::load_zkey_key`], and `read_witness` (`.wtns`) -> [`B200Prover::read_wtns`]
 //! The MSMs have no hook inside ark-groth16 (src/prover.rs:66,74,262 call `msm_bigint` on `E::G1` / `E::G2` directly),
 //! hence the sibling prover type instead of a trait implementation.
 //!
@@ -469,6 +471,89 @@ impl<E: SwPairing> B200Prover<E> {
             gamma_abc_g1: abc.chunks(w1).take(info.num_inputs as usize).map(|l| unpack_point(l)).collect(),
         };
         Ok((me, vk))
+    }
+
+    /// A prover for the circuit of a circom `.r1cs` (circuit.r1cs), read on the GPU with all three matrices
+    /// (g16_r1cs_load): the counterpart of ark-circom's `R1CSFile` followed by `CircomCircuit`, under the reduction `qap`.
+    /// No key is resident yet: follow with `load_zkey_key`, `load_proving_key` or `setup_from_srs`.  Every call that reads
+    /// C (`check_witness`, `set_check_witness`, `setup_from_srs`, `key_verification_pairs`) works on it.  A malformed file
+    /// is `SerializationError::InvalidData` with the library's message.
+    pub fn load_r1cs(device: i32, bytes: &[u8], qap: i32) -> Result<Self, SerializationError> {
+        let curve = curve_id::<E::ScalarField>().ok_or_else(|| {
+            SerializationError::IoError(ark_std::io::Error::new(ark_std::io::ErrorKind::Other, "libg16b200 does not support this curve"))
+        })?;
+        let mut ctx = core::ptr::null_mut();
+        ser_status(unsafe { sys::g16_ctx_create(curve, device, &mut ctx) })?;
+        let mut info = sys::g16_r1cs_info::default();
+        let rc = unsafe { sys::g16_r1cs_load(ctx, qap, bytes.as_ptr(), bytes.len() as u64, &mut info) };
+        if rc != 0 {
+            let err = ser_status(rc);
+            unsafe { sys::g16_ctx_destroy(ctx) };
+            err?;
+        }
+        Ok(Self {
+            ctx,
+            num_inputs: info.num_inputs as usize,
+            num_constraints: info.num_constraints as usize,
+            num_variables: (info.num_inputs + info.num_witness) as usize,
+            fq_limbs: unsafe { sys::g16_fq_limbs(ctx) } as usize,
+            g2_limbs: unsafe { sys::g16_g2_limbs(ctx) } as usize,
+            flags: Cell::new(0),
+            _e: PhantomData,
+        })
+    }
+
+    /// The proving key of a snarkjs `.zkey` onto the resident circuit (g16_zkey_load with `sys::G16_ZKEY_KEY_ONLY`), which
+    /// keeps its C matrix: the circom flow is `load_r1cs(circuit.r1cs, sys::G16_QAP_CIRCOM)` then this with
+    /// circuit_final.zkey.  The coefficient section is not read; whether the key belongs to the circuit is
+    /// `verify_key`'s question.  Sizes other than the circuit's are `InvalidData` with the previous key kept; a refused point
+    /// leaves no key.  Returns the key's VerifyingKey.
+    pub fn load_zkey_key(&self, bytes: &[u8], validate: Validate, rank: u32, world: u32) -> Result<VerifyingKey<E>, SerializationError> {
+        let (w1, w2) = (point_limbs::<E::G1Config>(), point_limbs::<E::G2Config>());
+        let (mut alpha_g1, mut beta_g1, mut delta_g1) = (ark_std::vec![0u64; w1], ark_std::vec![0u64; w1], ark_std::vec![0u64; w1]);
+        let (mut beta_g2, mut gamma_g2, mut delta_g2) = (ark_std::vec![0u64; w2], ark_std::vec![0u64; w2], ark_std::vec![0u64; w2]);
+        let mut abc = ark_std::vec![0u64; w1 * self.num_inputs];
+        let null = core::ptr::null_mut();
+        let desc = sys::g16_pk_export_desc {
+            a_query: null,
+            b_g1_query: null,
+            b_g2_query: null,
+            h_query: null,
+            l_query: null,
+            alpha_g1: alpha_g1.as_mut_ptr(),
+            beta_g1: beta_g1.as_mut_ptr(),
+            delta_g1: delta_g1.as_mut_ptr(),
+            beta_g2: beta_g2.as_mut_ptr(),
+            gamma_g2: gamma_g2.as_mut_ptr(),
+            delta_g2: delta_g2.as_mut_ptr(),
+            gamma_abc_g1: abc.as_mut_ptr(),
+        };
+        let flags = sys::G16_ZKEY_KEY_ONLY | if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 };
+        ser_status(unsafe {
+            sys::g16_zkey_load(self.ctx, bytes.as_ptr(), bytes.len() as u64, flags, rank, world, &desc, core::ptr::null_mut())
+        })?;
+        Ok(VerifyingKey {
+            alpha_g1: unpack_point(&alpha_g1),
+            beta_g2: unpack_point(&beta_g2),
+            gamma_g2: unpack_point(&gamma_g2),
+            delta_g2: unpack_point(&delta_g2),
+            gamma_abc_g1: abc.chunks(w1).map(|l| unpack_point(l)).collect(),
+        })
+    }
+
+    /// The full assignment of a circom / snarkjs `.wtns` (g16_wtns_read: elements checked below r and put in Montgomery form
+    /// on the GPU), usable directly as `full_assignment`.  Needs no circuit.  A malformed file or element is `InvalidData`.
+    pub fn read_wtns(&self, bytes: &[u8]) -> Result<Vec<E::ScalarField>, SerializationError> {
+        let mut n = 0u64;
+        ser_status(unsafe { sys::g16_wtns_read(self.ctx, bytes.as_ptr(), bytes.len() as u64, core::ptr::null_mut(), 0, &mut n) })?;
+        let mut out = ark_std::vec![E::ScalarField::zero(); n as usize];
+        if n > 0 {
+            // the ABI's Montgomery limbs are the field elements' memory image
+            ser_status(unsafe {
+                sys::g16_wtns_read(self.ctx, bytes.as_ptr(), bytes.len() as u64, out.as_mut_ptr() as *mut u64, n, &mut n)
+            })?;
+        }
+        Ok(out)
     }
 
     /// Replace the resident key by the ark-serialized ProvingKey in `bytes` (g16_pk_load_serialized).  A rejected key

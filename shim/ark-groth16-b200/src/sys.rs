@@ -35,6 +35,20 @@ pub const G16_PK_UNCONTRIBUTED: u32 = 4;
 
 pub const G16_NONE: u64 = u64::MAX;
 
+pub const G16_ZKEY_KEY_ONLY: u32 = 16;
+
+#[repr(C)]
+#[derive(Default, Clone, Copy, Debug, PartialEq, Eq)]
+pub struct g16_r1cs_info {
+    pub num_inputs: u32,
+    pub num_constraints: u32,
+    pub num_witness: u32,
+    pub log_n: u32,
+    pub a_nnz: u64,
+    pub b_nnz: u64,
+    pub c_nnz: u64,
+}
+
 #[repr(C)]
 #[derive(Default, Clone, Copy, Debug, PartialEq, Eq)]
 pub struct g16_zkey_info {
@@ -237,6 +251,8 @@ extern "C" {
     pub fn g16_contribution_chain_pairs(ctx: *mut g16_ctx, start_g1: *const u64, end_g1: *const u64, records: *const g16_contribution_record, count: u32, flags: u32, pairs_g1: *mut u64, pairs_g2: *mut u64) -> c_int;
     pub fn g16_pk_load_serialized(ctx: *mut g16_ctx, bytes: *const u8, len: u64, flags: u32, rank: u32, world: u32, vk_out: *const g16_pk_export_desc) -> c_int;
     pub fn g16_zkey_load(ctx: *mut g16_ctx, bytes: *const u8, len: u64, flags: u32, rank: u32, world: u32, vk_out: *const g16_pk_export_desc, info_out: *mut g16_zkey_info) -> c_int;
+    pub fn g16_r1cs_load(ctx: *mut g16_ctx, qap: c_int, bytes: *const u8, len: u64, info_out: *mut g16_r1cs_info) -> c_int;
+    pub fn g16_wtns_read(ctx: *mut g16_ctx, bytes: *const u8, len: u64, out: *mut u64, cap: u64, count_out: *mut u64) -> c_int;
     pub fn g16_pk_export_serialized(ctx: *mut g16_ctx, flags: u32, out: *mut u8, cap: u64, len_out: *mut u64) -> c_int;
     pub fn g16_prove(ctx: *mut g16_ctx, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32, proof_out: *mut u64) -> c_int;
     pub fn g16_prove_partial(ctx: *mut g16_ctx, r: *const u64, full_assignment: *const u64, flags: u32, partial_out: *mut u64) -> c_int;
