@@ -133,6 +133,7 @@ SIGNATURES = [
     ("g16_wtns_read", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("g16_ptau_read", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(SrsOut), C.POINTER(LagrangeOut), C.POINTER(PtauInfo)]),
     ("g16_setup_from_lagrange", C.c_int, [C.c_void_p, C.POINTER(SrsDesc), C.POINTER(LagrangeDesc), C.c_void_p, C.c_uint32]),
+    ("g16_ptau_prepare", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("g16_pk_export_serialized", C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("g16_prove", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     ("g16_prove_partial", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),

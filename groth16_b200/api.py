@@ -785,6 +785,30 @@ class Groth16:
             return self.generate_parameters_from_lagrange(None, p.srs, p.lagrange, rho, validate, export)
         return self.generate_parameters_from_srs(None, p.srs, validate, export)
 
+    def prepare_ptau(self, data, validate: bool = False, out=None):
+        """g16_ptau_prepare: snarkjs `powersoftau prepare phase2` on the GPU.  Returns the .ptau `data` with its Lagrange
+        sections 12..15 computed from the powers (those of a prepared input are recomputed), as bytes.  With `out`, a
+        writable uint8 buffer (an np.memmap of the target file, say) of at least the prepared size, writes into it instead
+        and returns the length, so a large file needs no second copy in RAM.  Every point of sections 2..5 is checked on the
+        GPU first (`validate`: also in the prime-order subgroup); a refused point or a malformed file raises
+        serialize.DeserializeError naming it, power + 1 above the scalar field's two-adicity PolynomialDegreeTooLarge, and a
+        level larger than the free device memory CudaError.  The file is not checked to be a powers-of-tau transcript
+        (srs_verification_pairs does that)."""
+        buf = np.frombuffer(data, dtype=np.uint8)
+        ptr = buf.ctypes.data_as(C.c_void_p) if buf.size else None
+        flags = _lib.SER_VALIDATE if validate else 0
+        n = C.c_uint64()
+        _check(self._lib.g16_ptau_prepare(self._ctx, ptr, buf.size, flags, None, 0, C.byref(n)))
+        if out is None:
+            res = np.empty(n.value, dtype=np.uint8)
+        else:
+            res = out if isinstance(out, np.ndarray) else np.frombuffer(out, dtype=np.uint8)
+            if res.dtype != np.uint8 or res.ndim != 1 or not res.flags.c_contiguous or not res.flags.writeable:
+                raise ValueError("out must be a writable, contiguous 1-D uint8 buffer")
+        _check(self._lib.g16_ptau_prepare(self._ctx, ptr, buf.size, flags, res.ctypes.data_as(C.c_void_p), res.size,
+                                          C.byref(n)))
+        return res.tobytes() if out is None else n.value
+
     def contribute_delta(self, delta, export: bool = True) -> Optional[ProvingKey]:
         """g16_setup_contribute: one phase-2 contribution delta (Python int) to the resident key made by
         generate_parameters_with_qap or generate_parameters_from_srs.  Returns the new key when `export`."""

@@ -220,6 +220,11 @@ int g16_setup_from_lagrange(g16_ctx* ctx, const g16_srs_desc* srs, const g16_lag
   NEEDS_C(ctx, true);
   return ctx->eng->setup_from_lagrange(srs, lag, rho, flags);
 }
+int g16_ptau_prepare(g16_ctx* ctx, const uint8_t* in, uint64_t in_len, uint32_t flags, uint8_t* out, uint64_t cap,
+                     uint64_t* len_out) {
+  CTX_OR_FAIL(ctx);
+  return ctx->eng->ptau_prepare(in, in_len, flags, out, cap, len_out);
+}
 int g16_pk_export_serialized(g16_ctx* ctx, uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) {
   CTX_OR_FAIL(ctx);
   return ctx->eng->pk_export_serialized(flags, out, cap, len_out);

@@ -14,6 +14,7 @@
 #include <cerrno>
 #include <chrono>
 #include <climits>
+#include <cmath>
 #include <cstdlib>
 #include <cstdio>
 #include <condition_variable>
@@ -171,6 +172,7 @@ struct IEngine {
   virtual int ptau_read(const uint8_t* bytes, uint64_t len, const g16_srs_out* srs_out, g16_lagrange_out* lag_out,
                         g16_ptau_info* info) = 0;
   virtual int setup_from_lagrange(const g16_srs_desc* srs, const g16_lagrange_desc* lag, const uint64_t* rho, uint32_t flags) = 0;
+  virtual int ptau_prepare(const uint8_t* in, uint64_t in_len, uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) = 0;
   virtual int prove(const uint64_t* r, const uint64_t* s, const uint64_t* z, uint32_t flags, uint64_t* proof) = 0;
   virtual int prove_partial(const uint64_t* r, const uint64_t* z, uint32_t flags, uint64_t* partial) = 0;
   virtual int prove_assemble(const uint64_t* r, const uint64_t* s, const uint64_t* partials, uint32_t nparts, uint64_t* proof) = 0;
@@ -1166,7 +1168,7 @@ struct Engine : IEngine {
       if (rho.is_zero()) return fail(G16_ERR_BAD_ARGUMENT, "the challenge rho must be non-zero");
     }
     G16_CUDA(cudaSetDevice(device));
-    int rc = ensure_circuit_domain();   // dom.tw_inv: the circuit's omega^-i
+    int rc = ensure_circuit_domain();   // dom.n_inv
     if (rc) return rc;
     const auto t0 = std::chrono::steady_clock::now();
     auto ms_since = [](std::chrono::steady_clock::time_point a) {
@@ -1216,8 +1218,18 @@ struct Engine : IEngine {
       // [tau^i], i < 2n - 1: 1/(2n) times the size-n transform of omega_2n^-i ([tau^i] - [tau^(i+n)]) (CircomReduction),
       // which lag's tau_g1_h holds (with h2n: plus (omega_2n^(2i+1) / 2n) [tau^(2n-1)], taken off here) ---
       const A1* t1p = up[SRS_TAU_G1].template as<A1>();
-      DevBuf hpts, dfr;
-      if (!lag) G16_CUDA(dfr.reserve(n * sizeof(Fr)));
+      DevBuf hpts, dfr, dtw;
+      // the transforms' scalars (srs_ifft): tw[b] = omega_n^-(2^b), tw[32] = n^-1
+      Fr tw[33];
+      tw[0] = Fr::inv(fr_domain_root<Fr>(L));
+      for (int b = 1; b < 32; b++) tw[b] = Fr::sqr(tw[b - 1]);
+      tw[32] = dom.n_inv;
+      if (!lag) {
+        G16_CUDA(dfr.reserve(n * sizeof(Fr)));
+        G16_CUDA(dtw.reserve(sizeof(tw)));
+        G16_CUDA(cudaMemcpyAsync(dtw.p, tw, sizeof(tw), cudaMemcpyHostToDevice, st));
+      }
+      const Fr* dtab = dtw.template as<Fr>();
       if (lptr[LAG_H] && !h2n) {
         G16_CUDA(cudaMemcpyAsync(q[M_H].bases.p, lup[LAG_H].p, n * sizeof(A1), cudaMemcpyDeviceToDevice, st));
       } else if (lptr[LAG_H]) {
@@ -1226,24 +1238,23 @@ struct Engine : IEngine {
         G16_CUDA(hpts.reserve(n * sizeof(P1)));
         if (!circom) {
           G16_CUDA(srs_diff<Fq>(st, t1p, (uint32_t)(2 * n - 1), (uint32_t)n, 0, (uint32_t)(n - 1), hpts.template as<P1>()));
-        } else {
-          G16_CUDA(srs_diff<Fq>(st, t1p, (uint32_t)(2 * n - 1), 0, (uint32_t)n, (uint32_t)n, hpts.template as<P1>()));
+          G16_CUDA(srs_affine<Fq>(st, hpts.template as<P1>(), (uint32_t)hn, q[M_H].bases.template as<A1>()));
+        } else {   // s_j = omega_2n^-j / 2n on [tau^j] - [tau^(j+n)], transformed straight into the H query's bases (hn = n)
           std::vector<Fr> s(n);
           const Fr w_inv = Fr::inv(fr_domain_root<Fr>(L + 1));
           Fr c = Fr::inv(fr_from_u64<Fr>(2 * n));
           for (uint64_t i = 0; i < n; i++) { s[i] = c; c = Fr::mul(c, w_inv); }
           G16_CUDA(cudaMemcpyAsync(dfr.p, s.data(), n * sizeof(Fr), cudaMemcpyHostToDevice, st));
-          G16_CUDA((srs_scale<Fq, Fr>(st, hpts.template as<P1>(), (uint32_t)n, dfr.template as<Fr>(), 1)));
-          G16_CUDA((srs_ifft<Fq, Fr>(st, hpts.template as<P1>(), L, dom.tw_inv, &ntt_launches)));
+          G16_CUDA((srs_ifft<Fq, Fr>(st, t1p, 2 * n - 1, n, L, dfr.template as<Fr>(), 1, dtab, L, hpts.template as<P1>(),
+                                     q[M_H].bases.template as<A1>(), &ntt_launches)));
           G16_CUDA(cudaStreamSynchronize(st));   // s is read by the copy above
         }
-        G16_CUDA(srs_affine<Fq>(st, hpts.template as<P1>(), (uint32_t)hn, q[M_H].bases.template as<A1>()));
       }
       G16_CUDA(cudaStreamSynchronize(st));
       hpts.release();
       tm.msm_ms[M_H] = ms_since(t1);
       // --- Lagrange points: [L_i], [alpha L_i], [beta L_i] in G1 (s1 = three blocks of n) and [L_i] in G2: lag's checked
-      // points, or the unscaled inverse transforms of the first n powers, then times n^-1 ---
+      // points, or the inverse transforms of the first n powers (srs_ifft, n^-1 applied as each point is loaded) ---
       t1 = std::chrono::steady_clock::now();
       DevBuf s1, s2;
       G16_CUDA(s1.reserve(3 * n * sizeof(P1)));
@@ -1257,15 +1268,11 @@ struct Engine : IEngine {
         G16_CUDA(cudaStreamSynchronize(st));
       } else {
         const int src1[3] = {SRS_TAU_G1, SRS_ALPHA, SRS_BETA};
-        for (int b = 0; b < 3; b++) {
-          G16_CUDA(srs_load<Fq>(st, up[src1[b]].template as<A1>(), (uint32_t)n, s1p + b * n));
-          G16_CUDA((srs_ifft<Fq, Fr>(st, s1p + b * n, L, dom.tw_inv, &ntt_launches)));
-        }
-        G16_CUDA(srs_load<Fq2>(st, up[SRS_TAU_G2].template as<A2>(), (uint32_t)n, s2p));
-        G16_CUDA((srs_ifft<Fq2, Fr>(st, s2p, L, dom.tw_inv, &ntt_launches)));
-        G16_CUDA(cudaMemcpyAsync(dfr.p, &dom.n_inv, sizeof(Fr), cudaMemcpyHostToDevice, st));
-        G16_CUDA((srs_scale<Fq, Fr>(st, s1p, (uint32_t)(3 * n), dfr.template as<Fr>(), 0)));
-        G16_CUDA((srs_scale<Fq2, Fr>(st, s2p, (uint32_t)n, dfr.template as<Fr>(), 0)));
+        for (int b = 0; b < 3; b++)
+          G16_CUDA((srs_ifft<Fq, Fr>(st, up[src1[b]].template as<A1>(), n, 0, L, dtab + 32, 0, dtab, L, s1p + b * n, nullptr,
+                                     &ntt_launches)));
+        G16_CUDA((srs_ifft<Fq2, Fr>(st, up[SRS_TAU_G2].template as<A2>(), n, 0, L, dtab + 32, 0, dtab, L, s2p, nullptr,
+                                    &ntt_launches)));
         G16_CUDA(cudaStreamSynchronize(st));
       }
       for (DevBuf& u : up) u.release();
@@ -2817,6 +2824,160 @@ struct Engine : IEngine {
         for (uint64_t i = 0; i < cnt; i++) memcpy(d + i * z.g1_bytes, src + 2 * i * z.g1_bytes, z.g1_bytes);
       }
     }
+    return G16_OK;
+  }
+  // g16_ptau_prepare (ptau.cuh): every Lagrange level of sections 2..5 by srs_ifft, member by member, one level at a time.
+  // Refusals before any point is read write nothing; then a check pass over every point of sections 2..5 (srs_check, the
+  // first bad one by member and index), and only after it the output: header and kept sections copied on the host, each
+  // level transformed on the device (1/2^k folded into the load, affine store fused into the last stage) and copied to
+  // its place.  Level 0 is X_0 itself.  Device memory: one member at a time, its points, one XYZZ buffer and one affine
+  // staging buffer for its top level.  Timings as g16_srs_contribute's: h2d_ms = the check pass, msm_ms[m] = member m.
+  int ptau_prepare(const uint8_t* in, uint64_t in_len, uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) override {
+    if (!in || !len_out) return fail(G16_ERR_BAD_ARGUMENT, "null in / len_out");
+    if (flags & ~(uint32_t)G16_SER_VALIDATE) return fail(G16_ERR_BAD_ARGUMENT, "g16_ptau_prepare takes 0 or G16_SER_VALIDATE");
+    G16_NOT_BUSY();
+    PtauLayout z;
+    BinSection sec[16];
+    std::string why = ptau_walk_header<CP>(in, in_len, z, sec);
+    if (!why.empty()) return fail(G16_ERR_INVALID_DATA, why);
+    const uint32_t two_adicity = (uint32_t)CP::FrP::TWO_ADICITY;
+    if (z.power + 1 > two_adicity)
+      return fail(G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "power " + std::to_string(z.power) + ": level power + 1 = " +
+                                                           std::to_string(z.power + 1) + " is above the scalar field's two-adicity " +
+                                                           std::to_string(two_adicity));
+    if (!(why = ptau_walk<CP>(in, in_len, z)).empty()) return fail(G16_ERR_INVALID_DATA, why);
+    const auto kept = ptau_kept_sections(in);
+    uint64_t kept_bytes = 0;
+    for (const auto& k : kept) kept_bytes += k.second;
+    const PtauPrepared pl = ptau_prepared_layout((uint32_t)kept.size(), kept_bytes, z.power, z.g1_bytes, z.g2_bytes);
+    *len_out = pl.size;
+    if (!out) return G16_OK;
+    if (cap < pl.size)
+      return fail(G16_ERR_BAD_ARGUMENT, "output buffer holds " + std::to_string(cap) + " bytes, the prepared file needs " +
+                                            std::to_string(pl.size));
+    if (srs_overlap((uintptr_t)in, in_len, (uintptr_t)out, pl.size)) return fail(G16_ERR_BAD_ARGUMENT, "out overlaps in");
+    G16_CUDA(cudaSetDevice(device));
+    const auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [](std::chrono::steady_clock::time_point a) {
+      return (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count();
+    };
+    tm = g16_timings{};
+    cudaStream_t st = S0.st_main;
+    const uint64_t esz[PTAU_MEMBERS] = {sizeof(A1), sizeof(A2), sizeof(A1), sizeof(A1)};
+    const uint64_t psz[PTAU_MEMBERS] = {sizeof(P1), sizeof(P2), sizeof(P1), sizeof(P1)};
+    // --- memory: member m needs its points, ptau_work_points(top) XYZZ and as many affine points on the device at once ---
+    size_t free_b = 0, total_b = 0;
+    G16_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    for (int m = 0; m < PTAU_MEMBERS; m++) {
+      const uint32_t top = ptau_top_level(m, z.power);
+      const double need = (double)z.len[m] * esz[m] + (double)(psz[m] + esz[m]) * (double)ptau_work_points(top);
+      if (need > (double)free_b)
+        return fail(G16_ERR_CUDA, std::string(srs_member(m)) + " level 2^" + std::to_string(top) + " needs " +
+                                      std::to_string((uint64_t)need) + " bytes of device memory, " + std::to_string(free_b) +
+                                      " are free");
+    }
+    // --- check pass: every point of sections 2..5 ---
+    DevBuf din, work, stage, err, dtab;
+    G16_CUDA(err.reserve(8));
+    for (int m = 0; m < PTAU_MEMBERS; m++) {
+      const uint64_t bytes = z.len[m] * esz[m];
+      G16_CUDA(din.reserve(bytes));
+      G16_CUDA(cudaMemcpyAsync(din.p, in + z.off[m], bytes, cudaMemcpyHostToDevice, st));
+      G16_CUDA(cudaMemsetAsync(err.p, 0xff, 8, st));
+      unsigned long long* e = err.template as<unsigned long long>();
+      const uint32_t cnt = (uint32_t)z.len[m];
+      G16_CUDA((m == PTAU_TAU_G2 ? srs_check<CP, true>(st, din.p, cnt, flags, m, e) : srs_check<CP, false>(st, din.p, cnt, flags, m, e)));
+      unsigned long long first_err = 0;
+      G16_CUDA(cudaMemcpyAsync(&first_err, err.p, 8, cudaMemcpyDeviceToHost, st));
+      G16_CUDA(cudaStreamSynchronize(st));
+      tm.h2d_bytes += bytes;
+      tm.d2h_bytes += 8;
+      tm.launches++;
+      if (first_err != ~0ull)
+        return fail(G16_ERR_INVALID_DATA, std::string(srs_member(m)) + "[" + std::to_string((first_err >> 8) & ((1ull << 40) - 1)) +
+                                              "]: " + ser_reason(first_err & 0xff));
+    }
+    tm.h2d_ms = ms_since(t0);
+    // --- output: header, kept sections, heads of 12..15 and every level 0 on the host ---
+    auto put32 = [&](uint64_t at, uint32_t v) { memcpy(out + at, &v, 4); };
+    auto put64 = [&](uint64_t at, uint64_t v) { memcpy(out + at, &v, 8); };
+    memcpy(out, "ptau", 4);
+    put32(4, 1);
+    put32(8, pl.nsec);
+    uint64_t pos = 12;
+    for (const auto& k : kept) { memcpy(out + pos, in + k.first, k.second); pos += k.second; }
+    for (int m = 0; m < PTAU_MEMBERS; m++) {
+      put32(pl.lag_off[m] - 12, 12 + m);
+      put64(pl.lag_off[m] - 8, pl.lag_pts[m] * esz[m]);
+      memcpy(out + pl.lag_off[m], in + z.off[m], esz[m]);
+    }
+    // --- transforms: level k of member m = srs_ifft of size 2^k over its first points, scaled by 1/2^k ---
+    const uint32_t tab_log = z.power + 1;
+    Fr tab[128];   // omega_N^-(2^b) (N = 2^tab_log) at b < 64, (1/2)^k at 64 + k
+    tab[0] = Fr::inv(fr_domain_root<Fr>((int)tab_log));
+    tab[64] = Fr::one();
+    const Fr half = Fr::inv(fr_from_u64<Fr>(2));
+    for (int b = 1; b < 64; b++) { tab[b] = Fr::sqr(tab[b - 1]); tab[64 + b] = Fr::mul(tab[63 + b], half); }
+    G16_CUDA(dtab.reserve(sizeof(tab)));
+    G16_CUDA(cudaMemcpyAsync(dtab.p, tab, sizeof(tab), cudaMemcpyHostToDevice, st));
+    tm.h2d_bytes += sizeof(tab);
+    const Fr* dt = dtab.template as<Fr>();
+    unsigned long long launches = 0;
+    // Levels 1 .. PTAU_SMALL_LEVELS of a member each run on a stream of their own, into their own slice of work and stage
+    // (level k at point 2^k - 1, as in the section): they are latency-bound, one thread's scalar multiplication per stage,
+    // and together they hold fewer butterflies than one wave.  The larger levels follow one by one on the main stream.
+    struct SideStreams {
+      cudaStream_t s[PTAU_SMALL_LEVELS] = {};
+      cudaEvent_t ev = nullptr;
+      ~SideStreams() {
+        for (cudaStream_t x : s) if (x) cudaStreamDestroy(x);
+        if (ev) cudaEventDestroy(ev);
+      }
+    } side;
+    for (cudaStream_t& x : side.s) G16_CUDA(cudaStreamCreateWithFlags(&x, cudaStreamNonBlocking));
+    G16_CUDA(cudaEventCreateWithFlags(&side.ev, cudaEventDisableTiming));
+    for (int m = 0; m < PTAU_MEMBERS; m++) {
+      const auto t1 = std::chrono::steady_clock::now();
+      const uint32_t top = ptau_top_level(m, z.power), small = std::min(top, PTAU_SMALL_LEVELS);
+      const uint64_t bytes = z.len[m] * esz[m], pts = ptau_work_points(top);
+      for (DevBuf* b : {&din, &work, &stage}) b->release();   // the peak is one member's
+      G16_CUDA(din.reserve(bytes));
+      G16_CUDA(work.reserve(psz[m] * pts));
+      G16_CUDA(stage.reserve(esz[m] * pts));
+      G16_CUDA(cudaMemcpyAsync(din.p, in + z.off[m], bytes, cudaMemcpyHostToDevice, st));
+      tm.h2d_bytes += bytes;
+      // level k on stream s, into the slices at point `at` of work and stage
+      auto level = [&](cudaStream_t s, uint32_t k, uint64_t at) -> cudaError_t {
+        if (m == PTAU_TAU_G2)
+          return srs_ifft<Fq2, Fr>(s, din.template as<A2>(), z.len[m], 0, (int)k, dt + 64 + k, 0, dt, (int)tab_log,
+                                   work.template as<P2>() + at, stage.template as<A2>() + at, &launches);
+        return srs_ifft<Fq, Fr>(s, din.template as<A1>(), z.len[m], 0, (int)k, dt + 64 + k, 0, dt, (int)tab_log,
+                                work.template as<P1>() + at, stage.template as<A1>() + at, &launches);
+      };
+      if (small) {
+        G16_CUDA(cudaEventRecord(side.ev, st));   // the member's points are on the device
+        for (uint32_t k = 1; k <= small; k++) {
+          G16_CUDA(cudaStreamWaitEvent(side.s[k - 1], side.ev, 0));
+          G16_CUDA(level(side.s[k - 1], k, ptau_level_start(k)));
+        }
+        for (uint32_t k = 1; k <= small; k++) G16_CUDA(cudaStreamSynchronize(side.s[k - 1]));
+        const uint64_t cnt = ptau_level_start(small + 1) - 1;   // levels 1 .. small, contiguous as in the section
+        G16_CUDA(cudaMemcpyAsync(out + pl.lag_off[m] + esz[m], stage.template as<uint8_t>() + esz[m], cnt * esz[m],
+                                 cudaMemcpyDeviceToHost, st));
+        tm.d2h_bytes += cnt * esz[m];
+      }
+      for (uint32_t k = small + 1; k <= top; k++) {
+        G16_CUDA(level(st, k, 0));
+        const uint64_t cnt = 1ull << k;
+        G16_CUDA(cudaMemcpyAsync(out + pl.lag_off[m] + ptau_level_start(k) * esz[m], stage.p, cnt * esz[m],
+                                 cudaMemcpyDeviceToHost, st));
+        tm.d2h_bytes += cnt * esz[m];
+      }
+      G16_CUDA(cudaStreamSynchronize(st));
+      tm.msm_ms[m] = ms_since(t1);
+    }
+    tm.launches += launches;
+    tm.total_ms = ms_since(t0);
     return G16_OK;
   }
   int pk_export_serialized(uint32_t flags, uint8_t* out, uint64_t cap, uint64_t* len_out) override {

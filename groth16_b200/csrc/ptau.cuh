@@ -1,7 +1,8 @@
 // ptau.cuh -- snarkjs .ptau powers-of-tau transcripts (iden3 binary container, as snarkjs `powersoftau` writes them): the
-// host walk of the section table and the header, and where each member and each level of Lagrange points lies.  Nothing is
-// decoded: the points are affine, Montgomery form and little-endian, which is this ABI's limb layout (as in a .zkey), so
-// they are copied as they are and checked by whichever call reads them.
+// host walk of the section table and the header, where each member and each level of Lagrange points lies, and the layout
+// of the prepared file g16_ptau_prepare writes.  Nothing is decoded: the points are affine, Montgomery form and
+// little-endian, which is this ABI's limb layout (as in a .zkey), so they are copied as they are and checked by whichever
+// call reads them.
 //
 // "ptau", version u32 = 1, nSections u32, then {id u32, size u64, body} records in any order; integers little-endian.  n8 is
 // the base-field byte size; a G1 point is x || y (n8 bytes each), a G2 point x.c0 || x.c1 || y.c0 || y.c1 (BW6-761: x || y
@@ -22,7 +23,10 @@
 // (BN254 at power 28) level power + 1 cannot exist and what snarkjs writes in section 12 there is unconfirmed: sections
 // 12..15 are then not interpreted, and the file reads as unprepared (its powers still serve).
 #pragma once
+#include <algorithm>
 #include <string>
+#include <utility>
+#include <vector>
 #include "r1cs.cuh"
 
 namespace g16 {
@@ -44,14 +48,13 @@ struct PtauLayout {
 // first point of level k in sections 12..15
 inline uint64_t ptau_level_start(uint32_t k) { return (1ull << k) - 1; }
 
-// Walks the section table and the header for the curve CP.  Returns "" and fills z, or why the file is refused (the first
-// problem found).
+// The first part of ptau_walk: the section table and section 1 alone.  Fills sec (ids 1..15), z.n8, z.power and
+// z.ceremony_power; no other section's size is compared yet.
 template <class CP>
-std::string ptau_walk(const uint8_t* b, uint64_t len, PtauLayout& z) {
+std::string ptau_walk_header(const uint8_t* b, uint64_t len, PtauLayout& z, BinSection* sec) {
   using FqP = typename CP::FqP;
   constexpr uint32_t N8 = 4 * FqP::N;
   z = PtauLayout{};
-  BinSection sec[16];
   const uint64_t need = bin_id(1) | bin_id(2) | bin_id(3) | bin_id(4) | bin_id(5) | bin_id(6);
   const uint64_t lag = bin_id(12) | bin_id(13) | bin_id(14) | bin_id(15);
   std::string why = bin_sections(b, len, "ptau", 1, need | lag, need, sec);
@@ -68,6 +71,16 @@ std::string ptau_walk(const uint8_t* b, uint64_t len, PtauLayout& z) {
   z.ceremony_power = r1_u32(h + 8 + N8);
   if (z.power > PTAU_MAX_POWER)
     return "section 1: power " + std::to_string(z.power) + " is above " + std::to_string(PTAU_MAX_POWER);
+  return "";
+}
+// Walks the section table and the header for the curve CP.  Returns "" and fills z, or why the file is refused (the first
+// problem found).
+template <class CP>
+std::string ptau_walk(const uint8_t* b, uint64_t len, PtauLayout& z) {
+  constexpr uint32_t N8 = 4 * CP::FqP::N;
+  BinSection sec[16];
+  std::string why = ptau_walk_header<CP>(b, len, z, sec);
+  if (!why.empty()) return why;
   z.g1_bytes = 2 * N8;
   z.g2_bytes = (uint32_t)sizeof(Affine<typename CP::G2F>);
   const uint64_t np = 1ull << z.power;
@@ -100,6 +113,53 @@ std::string ptau_walk(const uint8_t* b, uint64_t len, PtauLayout& z) {
   }
   z.prepared = true;
   return "";
+}
+
+// ---- prepared files (g16_ptau_prepare) ----------------------------------------------------------------------------------
+// The top level of member m: power + 1 for tauG1, power for the others.
+inline uint32_t ptau_top_level(int m, uint32_t power) { return power + (m == PTAU_TAU_G1); }
+// Levels 1 .. PTAU_SMALL_LEVELS of a member are transformed concurrently, each on its own stream and in its own slice of
+// the work buffers (level k at point 2^k - 1): together they hold 2^PTAU_SMALL_LEVELS - 1 butterflies, fewer than one wave
+// of the stage kernel on an H100 for either group.  The larger levels reuse the start of the buffers one at a time.
+constexpr uint32_t PTAU_SMALL_LEVELS = 14;
+// Points of each work buffer (XYZZ and affine staging) for a member whose top level is `top`.  Saturates far above any
+// device's memory (ptau_top_level <= PTAU_MAX_POWER + 1).
+inline uint64_t ptau_work_points(uint32_t top) {
+  return std::max<uint64_t>(1ull << top, ptau_level_start(std::min(top, PTAU_SMALL_LEVELS) + 1));
+}
+// The file g16_ptau_prepare writes: "ptau", version 1, nSections; the kept sections (every section of the input but
+// 12..15, byte for byte in input order: `kept` of them, `kept_bytes` with their 12-byte heads); then sections 12, 13, 14
+// and 15, each holding levels 0 .. ptau_top_level of its member.
+struct PtauPrepared {
+  uint32_t nsec = 0;
+  uint64_t size = 0;
+  uint64_t lag_off[PTAU_MEMBERS] = {};   // body offset of sections 12..15
+  uint64_t lag_pts[PTAU_MEMBERS] = {};   // their points: 2^(top + 1) - 1
+};
+inline PtauPrepared ptau_prepared_layout(uint32_t kept, uint64_t kept_bytes, uint32_t power, uint32_t g1_bytes, uint32_t g2_bytes) {
+  PtauPrepared p;
+  p.nsec = kept + PTAU_MEMBERS;
+  uint64_t pos = 12 + kept_bytes;
+  for (int m = 0; m < PTAU_MEMBERS; m++) {
+    p.lag_pts[m] = (2ull << ptau_top_level(m, power)) - 1;
+    p.lag_off[m] = pos + 12;
+    pos += 12 + p.lag_pts[m] * (m == PTAU_TAU_G2 ? g2_bytes : g1_bytes);
+  }
+  p.size = pos;
+  return p;
+}
+// The kept sections of a file ptau_walk accepted: {offset of the section's head, its bytes with the head}, in file order.
+inline std::vector<std::pair<uint64_t, uint64_t>> ptau_kept_sections(const uint8_t* b) {
+  std::vector<std::pair<uint64_t, uint64_t>> out;
+  const uint32_t nsec = r1_u32(b + 8);
+  uint64_t pos = 12;
+  for (uint32_t k = 0; k < nsec; k++) {
+    const uint32_t id = r1_u32(b + pos);
+    const uint64_t rec = 12 + r1_u64(b + pos + 4);
+    if (id < 12 || id > 15) out.push_back({pos, rec});
+    pos += rec;
+  }
+  return out;
 }
 
 }  // namespace g16

@@ -1,13 +1,13 @@
 // srs.cuh -- proving keys from a powers-of-tau transcript (g16_setup_from_srs) and phase-2 delta contributions
-// (g16_setup_contribute): the group-valued inverse FFT, sparse sums of points, one scalar times many points, and the
-// transcript point checks; phase-1 contributions to a transcript (g16_srs_contribute): every point times its own power
+// (g16_setup_contribute): the group-valued inverse FFT (also every Lagrange level of g16_ptau_prepare), sparse sums of
+// points, one scalar times many points, and the transcript point checks; phase-1 contributions to a transcript (g16_srs_contribute): every point times its own power
 // of the secret; the scalars of the transcript check (g16_srs_verify_pairs): one power of the challenge per point; the
 // H-query weights of the key check (g16_pk_verify_pairs); and delta contributions to a key in host memory
 // (g16_pk_contribute): every point times the one scalar delta^-1.
 //
 // Every kernel works on XYZZ points in global memory, one point (or one butterfly, or one chunk of a sum) per thread.  The
-// scalar multiplications are left-to-right double-and-add over the canonical scalar (XYZZ::mul_u32); a windowed form would
-// need a per-thread table of points in local or shared memory (DESIGN.md section 13).
+// scalar multiplications are left-to-right double-and-add over the canonical scalar (XYZZ::mul_u32), except the transform's
+// twiddle products on the groups srs_windowed names: a signed 4-bit window over a per-thread table (srs_mul_w4).
 #pragma once
 #include <cstdint>
 #include <vector>
@@ -128,6 +128,69 @@ G16_HD uint32_t srs_check_point(const Affine<SerField<CP, G2>>& p, uint32_t flag
     return SER_ERR_SUBGROUP;
   return SER_OK;
 }
+// ---- the group inverse transform: which butterfly each thread runs, and its twiddle -------------------------------------
+// i < 2^log_n reversed over log_n bits (log_n < 32)
+G16_HD uint32_t srs_bitrev(uint32_t i, int log_n) {
+  uint32_t r = 0;
+  for (int b = 0; b < log_n; b++, i >>= 1) r = (r << 1) | (i & 1u);
+  return r;
+}
+// Stage of span h = 2^log_h over n = 2^log_n points: n / 2 butterflies in G = n / 2h groups of h, group g joining points
+// 2hg + k and 2hg + k + h with twiddle k < h.  Thread t runs k = t / G, g = t mod G, so the G threads of one twiddle are
+// consecutive: a warp shares one twiddle wherever G >= 32, which is every stage but the last five (h >= n / 32).  There a
+// warp holds 32 / G twiddles, each shared by G lanes.
+G16_HD void srs_butterfly_at(uint32_t t, int log_n, int log_h, uint32_t& k, uint32_t& i0) {
+  const int log_g = log_n - 1 - log_h;
+  k = t >> log_g;
+  i0 = ((t & ((1u << log_g) - 1)) << (log_h + 1)) + k;
+}
+// The exponent e of twiddle k at span 2^log_h, omega_n^-(k n / 2h) = omega_N^-e with N = 2^tab_log >= n: e = k N / 2h.
+G16_HD uint64_t srs_twiddle_exp(uint32_t k, int log_h, int tab_log) { return (uint64_t)k << (tab_log - 1 - log_h); }
+
+// omega_N^-e in canonical form from tab[b] = omega_N^-(2^b) (Montgomery); out of line, so that its products are done
+// before the butterfly's points are live
+template <class FrF>
+G16_HD_NOINLINE FrF srs_twiddle(const FrF* tab, uint64_t e) { return FrF::from_mont(srs_power(FrF::one(), tab, e)); }
+// Signed fixed-window recoding of a canonical scalar k of nl 32-bit limbs: digits d_i in [-7, 8] with
+// k = sum_i d_i 16^i, i < 8 nl + 1.  Returns the digit count.
+G16_HD int srs_recode_w4(const uint32_t* k, int nl, int8_t* d) {
+  int carry = 0;
+  for (int i = 0; i < 8 * nl; i++) {
+    const int v = (int)((k[i >> 3] >> (4 * (i & 7))) & 15u) + carry;
+    carry = v > 8;
+    d[i] = (int8_t)(v - 16 * carry);
+  }
+  d[8 * nl] = (int8_t)carry;
+  return 8 * nl + 1;
+}
+// p times the canonical scalar k (nl limbs) by the signed 4-bit window: a table of 1P .. 8P per thread (local memory), then
+// per digit from the top four doublings and one addition of +-table[|d| - 1] (skipped for d = 0).  The operation sequence is
+// the same for every scalar but for zero digits and leading zero windows, about 64 additions against the ~128 of
+// XYZZ::mul_u32's double-and-add.
+template <class F>
+G16_HD_NOINLINE XYZZ<F> srs_mul_w4(const XYZZ<F>& p, const uint32_t* k, int nl) {
+  constexpr int MAXD = 8 * 12 + 1;   // up to 12 limbs (BW6-761's 377-bit scalars)
+  int8_t d[MAXD];
+  const int nd = srs_recode_w4(k, nl, d);
+  XYZZ<F> tab[8];
+  tab[0] = p;
+  for (int j = 1; j < 8; j++) { tab[j] = tab[j - 1]; tab[j].add(p); }
+  XYZZ<F> r = XYZZ<F>::inf();
+  int top = nd - 1;
+  while (top > 0 && d[top] == 0) top--;
+  for (int i = top; i >= 0; i--) {
+    if (i != top)
+      for (int b = 0; b < 4; b++) r.dbl_inplace();
+    const int a = d[i] < 0 ? -d[i] : d[i];
+    if (a) {
+      XYZZ<F> t = tab[a - 1];
+      if (d[i] < 0) t.negate();
+      r.add(t);
+    }
+  }
+  return r;
+}
+
 template <class F, class FrF>
 G16_HD XYZZ<F> srs_mul(const XYZZ<F>& p, const FrF& s_mont) {
   const FrF s = FrF::from_mont(s_mont);
@@ -226,32 +289,55 @@ __global__ void __launch_bounds__(128) srs_h_weights_kernel(const FrF* tab, FrF 
     out[k] = k + 1 == n ? FrF::zero() : srs_power(c, tab, k - n);
   }
 }
-// in-place bit-reversal permutation of 2^log_n points
-template <class F>
-__global__ void __launch_bounds__(128) srs_bitrev_kernel(XYZZ<F>* p, uint32_t n, int log_n) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n || log_n == 0) return;
-  const uint32_t r = __brev(i) >> (32 - log_n);
-  if (i < r) { const XYZZ<F> t = p[i]; p[i] = p[r]; p[r] = t; }
-}
-// One radix-2 decimation-in-time stage of the unscaled inverse transform over bit-reversed points: butterflies of span h,
-// (P, Q) -> (P + w^-k Q, P - w^-k Q) with w^-k = tw_inv[k n / 2h] (the circuit domain's omega^-i, i < n / 2); k = 0 skips
-// the multiplication.
+// The group inverse transform: load (bit reversal and scaling folded in), then one kernel per radix-2 stage.
+// work[i] = s_j X_j with j = rev(i), X_j = P(j) - P(j + d) (d = 0: X_j = P(j)), P(k) = in[k] for k < len and the identity
+// beyond, s_j = s[j * stride] (stride 0: one scalar for every point, uniform control flow; s == nullptr: no product).  The
+// transform is linear, so a scaling of its input is the scaling of its output.
 template <class F, class FrF>
-__global__ void __launch_bounds__(128) srs_butterfly_kernel(XYZZ<F>* p, uint32_t n, uint32_t h, const FrF* tw_inv) {
+__global__ void __launch_bounds__(128) srs_ifft_load_kernel(const Affine<F>* in, uint64_t len, uint64_t d, int log_n,
+                                                            const FrF* s, uint32_t stride, XYZZ<F>* work) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (1u << log_n)) return;
+  const uint32_t j = srs_bitrev(i, log_n);
+  XYZZ<F> x = j < len ? XYZZ<F>::from_affine(in[j]) : XYZZ<F>::inf();
+  if (d && j + d < len) x.madd(in[j + d], true);
+  if (s) x = srs_mul(x, s[(uint64_t)j * stride]);
+  work[i] = x;
+}
+// One radix-2 decimation-in-time stage of span h = 2^log_h over bit-reversed points: butterfly t (srs_butterfly_at) maps
+// (P, Q) -> (P + w^-k Q, P - w^-k Q) with w^-k = tab-power srs_twiddle_exp(k, log_h, tab_log) (tab[b] = omega_N^-(2^b),
+// N = 2^tab_log, any N >= n); k = 0 skips the product.  AFF (the last stage): both results go to out in canonical affine
+// form instead of back to p.  WIN: the twiddle product by the signed window (srs_mul_w4) instead of double-and-add.
+template <class F, class FrF, bool AFF, bool WIN>
+__global__ void __launch_bounds__(128) srs_ifft_stage_kernel(XYZZ<F>* p, int log_n, int log_h, const FrF* tab, int tab_log,
+                                                             Affine<F>* out) {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n / 2) return;
-  const uint32_t k = t & (h - 1);
-  const uint32_t i0 = (t - k) * 2 + k, i1 = i0 + h;
+  if (t >= (1u << (log_n - 1))) return;
+  uint32_t k, i0;
+  srs_butterfly_at(t, log_n, log_h, k, i0);
+  const uint32_t i1 = i0 + (1u << log_h);
   XYZZ<F> q = p[i1];
-  if (k) q = srs_mul(q, tw_inv[(uint64_t)k * (n / (2 * h))]);
-  XYZZ<F> lo = p[i0];
-  XYZZ<F> hi = lo;
-  lo.add(q);
-  q.negate();
-  hi.add(q);
-  p[i0] = lo;
-  p[i1] = hi;
+  if (k) {
+    const FrF w = srs_twiddle(tab, srs_twiddle_exp(k, log_h, tab_log));
+    q = WIN ? srs_mul_w4(q, w.v, FrF::N) : q.mul_u32(w.v, FrF::N);
+  }
+  if (AFF) {   // p is not written: P is read again for the second result rather than held across the first's inversion
+    XYZZ<F> r = p[i0];
+    r.add(q);
+    srs_store_affine(&r, out + i0);
+    r = p[i0];
+    q.negate();
+    r.add(q);
+    srs_store_affine(&r, out + i1);
+  } else {
+    XYZZ<F> lo = p[i0];
+    XYZZ<F> hi = lo;
+    lo.add(q);
+    q.negate();
+    hi.add(q);
+    p[i0] = lo;
+    p[i1] = hi;
+  }
 }
 // level 0 of a sparse sum: out[e] = coeff[e] * src[idx[e]], the product skipped when the coefficient is One
 template <class F, class FrF>
@@ -331,13 +417,34 @@ cudaError_t srs_h_weights(cudaStream_t st, const FrF* tab, FrF c, const FrF* f, 
   if (cnt) srs_h_weights_kernel<FrF><<<srs_blocks(cnt), 128, 0, st>>>(tab, c, f, n, cnt, out);
   return cudaGetLastError();
 }
-// the unscaled inverse transform of 2^log_n points in place: out[j] = sum_i omega^(-ij) in[i]
+// Whether the stages multiply by the twiddle with the signed window (srs_mul_w4) rather than double-and-add: in every stage,
+// for the groups whose window kernels compile without spills (coordinates of at most 64 bytes: BN254 G1 and G2, BLS12-381
+// and BLS12-377 G1).  Measured faster in both groups of BN254 and BLS12-381 (DESIGN.md section 21); the Fq2 points of the
+// BLS curves and BW6-761's points spill their 8-point table, so they keep double-and-add.
+template <class F>
+constexpr bool srs_windowed() { return sizeof(F) <= 64; }
+// The inverse transform of size n = 2^log_n (log_n < 32): Y_i = sum_{j<n} omega_n^(-ij) s_j X_j with X_j, s_j as
+// srs_ifft_load_kernel forms them from (in, len, d, s, stride).  tab (device): omega_N^-(2^b) for b < tab_log, N >= n.
+// Y goes to work (n XYZZ); with aff, the last stage writes Y in canonical affine form to aff instead (work then holds
+// the stage before it).  1 + log_n launches (2 for log_n = 0 with aff).
 template <class F, class FrF>
-cudaError_t srs_ifft(cudaStream_t st, XYZZ<F>* p, int log_n, const FrF* tw_inv, unsigned long long* launches) {
-  const uint32_t n = 1u << log_n;
-  srs_bitrev_kernel<F><<<srs_blocks(n), 128, 0, st>>>(p, n, log_n);
-  for (uint32_t h = 1; h < n; h *= 2) srs_butterfly_kernel<F, FrF><<<srs_blocks(n / 2), 128, 0, st>>>(p, n, h, tw_inv);
-  if (launches) *launches += 1 + log_n;
+cudaError_t srs_ifft(cudaStream_t st, const Affine<F>* in, uint64_t len, uint64_t d, int log_n, const FrF* s, uint32_t stride,
+                     const FrF* tab, int tab_log, XYZZ<F>* work, Affine<F>* aff, unsigned long long* launches) {
+  const uint64_t n = 1ull << log_n;
+  srs_ifft_load_kernel<F, FrF><<<srs_blocks(n), 128, 0, st>>>(in, len, d, log_n, s, stride, work);
+  for (int lh = 0; lh < log_n; lh++) {
+    const bool last = aff && lh == log_n - 1;
+    const unsigned b = srs_blocks(n / 2);
+    if constexpr (srs_windowed<F>()) {
+      if (last) srs_ifft_stage_kernel<F, FrF, true, true><<<b, 128, 0, st>>>(work, log_n, lh, tab, tab_log, aff);
+      else srs_ifft_stage_kernel<F, FrF, false, true><<<b, 128, 0, st>>>(work, log_n, lh, tab, tab_log, nullptr);
+    } else {
+      if (last) srs_ifft_stage_kernel<F, FrF, true, false><<<b, 128, 0, st>>>(work, log_n, lh, tab, tab_log, aff);
+      else srs_ifft_stage_kernel<F, FrF, false, false><<<b, 128, 0, st>>>(work, log_n, lh, tab, tab_log, nullptr);
+    }
+  }
+  if (aff && log_n == 0) srs_affine_kernel<F><<<1, 128, 0, st>>>(work, 1, aff);
+  if (launches) *launches += 1 + log_n + (aff && log_n == 0);
   return cudaGetLastError();
 }
 // One sparse sum.  src: the points, d_idx / d_coeff: the entries in column order, terms: cnt XYZZ of scratch, tmp: as many
@@ -369,7 +476,8 @@ cudaError_t srs_sum(cudaStream_t st, const XYZZ<F>* src, const uint32_t* d_idx, 
   X cudaError_t srs_affine<F>(cudaStream_t, const XYZZ<F>*, uint32_t, Affine<F>*);                                    \
   X cudaError_t srs_scale<F, FrF>(cudaStream_t, XYZZ<F>*, uint32_t, const FrF*, uint32_t);                            \
   X cudaError_t srs_contribute<F, FrF>(cudaStream_t, Affine<F>*, uint32_t, const FrF*, FrF);                          \
-  X cudaError_t srs_ifft<F, FrF>(cudaStream_t, XYZZ<F>*, int, const FrF*, unsigned long long*);                       \
+  X cudaError_t srs_ifft<F, FrF>(cudaStream_t, const Affine<F>*, uint64_t, uint64_t, int, const FrF*, uint32_t,        \
+                                 const FrF*, int, XYZZ<F>*, Affine<F>*, unsigned long long*);                         \
   X cudaError_t srs_sum<F, FrF>(cudaStream_t, const XYZZ<F>*, const uint32_t*, const FrF*, uint32_t, const SrsSumPlan&, \
                                 XYZZ<F>*, XYZZ<F>*, uint64_t*, uint64_t*, uint32_t, Affine<F>*);
 #define G16_SRS_TEMPLATES(X, CP)                                                                                     \

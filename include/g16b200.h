@@ -588,6 +588,34 @@ typedef struct {
 int g16_setup_from_lagrange(g16_ctx* ctx, const g16_srs_desc* srs, const g16_lagrange_desc* lag, const uint64_t* rho,
                             uint32_t flags);
 
+/* g16_ptau_prepare is snarkjs `powersoftau prepare phase2` on the GPU: `in` is a whole .ptau of the context's curve, and
+ * the output is the same file with sections 12..15 computed.  Level k of a member X holds the 2^k points (1/2^k)
+ * sum_{j<2^k} omega_k^(-ij) X_j, X_j the identity for j >= len(X); 13..15 hold levels 0 .. power, 12 levels 0 .. power + 1
+ * (the top one with the missing last power taken as the identity); level 0 is X_0.  The output is "ptau", version 1,
+ * nSections; every section of `in` except 12..15 byte for byte in input order (7 and unknown ids included); then sections
+ * 12, 13, 14 and 15.  Sections 12..15 of a prepared input are dropped and recomputed: the output never depends on them.
+ * Affine limbs are canonical, so the output is a function of the input alone.
+ * Size protocol as g16_pk_export_serialized: out = NULL writes the size to *len_out; cap below it is G16_ERR_BAD_ARGUMENT
+ * with the size in *len_out; out must not overlap in.
+ * Every point of sections 2..5 is checked on the GPU (canonical, on the curve, with G16_SER_VALIDATE also in the prime-order
+ * subgroup; the identity is accepted) before anything is transformed or written.  A refused point is G16_ERR_INVALID_DATA,
+ * g16_last_error() naming the first by member and index ("tau_g2[5]: point is not on the curve"), with nothing written to
+ * out.  The call does not check that the file is a powers-of-tau transcript: g16_srs_verify_pairs does that.
+ * Decided before any point is read, with nothing written:
+ *   G16_ERR_INVALID_DATA: anything g16_ptau_read's walk refuses.
+ *   G16_ERR_BAD_ARGUMENT: null in or len_out, flags other than 0 or G16_SER_VALIDATE, overlapping buffers, a proof in flight.
+ *   G16_ERR_POLYNOMIAL_DEGREE_TOO_LARGE: power + 1 above the scalar field's two-adicity (BN254 at power 28), decided from
+ *   section 1 before any other section's size is compared.
+ *   G16_ERR_CUDA: a member's top level does not fit in the free device memory (its points, 2^top XYZZ points and 2^top
+ *   affine points at once), g16_last_error() naming the member, the level, the bytes needed and the bytes free.
+ * Each level is transformed whole on the device, one member at a time: the peak is about 2^(power+1) XYZZ tauG1 points
+ * plus staging (BN254 at power 27: 32 GiB for that buffer).  No circuit or key is needed; the resident ones, and everything
+ * derived from them, are left alone.  Afterwards g16_get_timings describes this call: total_ms, h2d_ms = the check pass,
+ * msm_ms[0..3] = the transforms of tau_g1, tau_g2, alpha_tau_g1 and beta_tau_g1, h2d_bytes, d2h_bytes, launches; every
+ * other field 0. */
+int g16_ptau_prepare(g16_ctx* ctx, const uint8_t* in, uint64_t in_len, uint32_t flags, uint8_t* out, uint64_t cap,
+                     uint64_t* len_out);
+
 /* ---- proving: Groth16::create_proof_with_reduction_and_matrices, prover.rs:26-51
  *      = witness_map_from_matrices (r1cs_to_qap.rs:172-235) + create_proof_with_assignment (prover.rs:54-132).
  * r, s: Montgomery Fr.  full_assignment: (num_inputs + num_witness) Montgomery Fr, instance first.

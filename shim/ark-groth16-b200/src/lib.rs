@@ -1147,6 +1147,19 @@ impl<E: SwPairing> B200Prover<E> {
         Ok(eqs.iter().all(|(p, q, p2, q2)| E::multi_pairing([*p, -*p2], [*q, *q2]).is_zero()))
     }
 
+    /// snarkjs `powersoftau prepare phase2` on the GPU (g16_ptau_prepare): the `.ptau` file `bytes` with its Lagrange
+    /// sections 12..15 computed from the powers (those of a prepared input are recomputed).  Every point of sections 2..5 is
+    /// checked first, with `Validate::Yes` also in the prime-order subgroup; a refused point is `InvalidData`, the message
+    /// naming it.  The file is not checked to be a powers-of-tau transcript (`verify_srs` does that).
+    pub fn prepare_ptau(&self, bytes: &[u8], validate: Validate) -> Result<Vec<u8>, SerializationError> {
+        let flags = if matches!(validate, Validate::Yes) { sys::G16_SER_VALIDATE } else { 0 };
+        let mut n = 0u64;
+        ser_status(unsafe { sys::g16_ptau_prepare(self.ctx, bytes.as_ptr(), bytes.len() as u64, flags, core::ptr::null_mut(), 0, &mut n) })?;
+        let mut out = ark_std::vec![0u8; n as usize];
+        ser_status(unsafe { sys::g16_ptau_prepare(self.ctx, bytes.as_ptr(), bytes.len() as u64, flags, out.as_mut_ptr(), n, &mut n) })?;
+        Ok(out)
+    }
+
     /// `ProvingKey::serialize_with_mode(compress)` of the resident key, encoded on the GPU (g16_pk_export_serialized).  Only
     /// a key made by the library's own setup can be exported.
     pub fn export_proving_key_bytes(&self, compress: Compress) -> Result<Vec<u8>, SerializationError> {

@@ -289,6 +289,7 @@ extern "C" {
     pub fn g16_wtns_read(ctx: *mut g16_ctx, bytes: *const u8, len: u64, out: *mut u64, cap: u64, count_out: *mut u64) -> c_int;
     pub fn g16_ptau_read(ctx: *mut g16_ctx, bytes: *const u8, len: u64, srs_out: *const g16_srs_out, lag_out: *mut g16_lagrange_out, info: *mut g16_ptau_info) -> c_int;
     pub fn g16_setup_from_lagrange(ctx: *mut g16_ctx, srs: *const g16_srs_desc, lag: *const g16_lagrange_desc, rho: *const u64, flags: u32) -> c_int;
+    pub fn g16_ptau_prepare(ctx: *mut g16_ctx, input: *const u8, in_len: u64, flags: u32, out: *mut u8, cap: u64, len_out: *mut u64) -> c_int;
     pub fn g16_pk_export_serialized(ctx: *mut g16_ctx, flags: u32, out: *mut u8, cap: u64, len_out: *mut u64) -> c_int;
     pub fn g16_prove(ctx: *mut g16_ctx, r: *const u64, s: *const u64, full_assignment: *const u64, flags: u32, proof_out: *mut u64) -> c_int;
     pub fn g16_prove_partial(ctx: *mut g16_ctx, r: *const u64, full_assignment: *const u64, flags: u32, partial_out: *mut u64) -> c_int;
